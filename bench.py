@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- point-clouds/sec of the SECOND LiDAR-inference hot path on B200 (BASELINE.json metric).
+"""bench.py -- point-clouds/sec of the SECOND LiDAR-inference hot path on H100 (BASELINE.json metric).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b2second|reference] [--config car.fhd]
+                  [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the hot path (voxelize -> sparse middle -> BEV -> RPN -> decode/NMS) over one batch
@@ -15,10 +16,10 @@ Prints ONE JSON line (rank 0):
             the fused engine by b2second.fastpath.accelerate -- with HOST (pinned) clouds: H2D of the points and D2H of
             the detection records inside the timed region
   roofline  the dominant hand-written kernel, timed live with CUDA events (eager replay of the same pipeline):
-            k_conv3x3_tc2 (tcgen05 3x3 RPN layers; bound "tensor": algorithmic fp32 flops per launch / average
-            launch time against MEASURED_PEAKS.json bf16_tflops, with the 3xF16 ceiling spelled out; `traffic`
-            from the committed ncu capture), and as `second_kernel` the sparse middle layers (bound "hbm":
-            SURVEY.md §8d bytes / time against hbm_gbs)
+            k_conv3x3_tc2 (wgmma 3x3 RPN layers; bound "tensor": algorithmic fp32 flops per launch / average
+            launch time against MEASURED_PEAKS.json bf16_tflops, else the H100 SXM data-sheet figure, with the
+            3xF16 ceiling spelled out), and as `second_kernel` the sparse middle layers (bound "hbm": SURVEY.md §8d
+            bytes / time against hbm_gbs)
   configs   short runs of the other BASELINE.json configurations (car.lite, pointpillars xyres_16, all.fhd at 32
             frames split over the ranks, NuScenes at ~300 k points per cloud) and the bs=1 latency of the headline
             config, each with its stage split and RPN tensor rate
@@ -27,6 +28,10 @@ Prints ONE JSON line (rank 0):
 --impl reference: the reference arm = the reference's CPU implementation of the path.  spconv 1.x is not
   in the reference tree and cannot be installed (no network), so this is the oracle port timed with all host
   threads (DESIGN.md "reference arm").
+--dump-outputs DIR: after the timed steps, the detections of the last timed (resident) step are written as float32
+  .npy files: det_record (the packed per-frame records the engine hands to its caller) and, decoded from it,
+  box3d_lidar / scores / label_preds of all frames concatenated plus num_detections per frame.  Clouds and weights
+  are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -54,16 +59,18 @@ def parse():
     ap.add_argument("--impl", default="b2second", choices=["b2second", "reference"])
     ap.add_argument("--config", default="car.fhd")
     ap.add_argument("--batch", type=int, default=32,
-                    help="frames per GPU per step (serving batch; measured clouds/s at 8/16/32/64: 1950/2320/2460/2516)")
+                    help="frames per GPU per step (serving batch)")
     ap.add_argument("--points", type=int, default=29000, help="points per synthetic cloud (29k -> ~17k voxels)")
     ap.add_argument("--cpu-frames", type=int, default=24,
                     help="frames in the bounded CPU-baseline sample (~0.4 s each on 16 host threads -> ~10 s)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the short runs of the other BASELINE configs")
     ap.add_argument("--sparse", default="tc", choices=["tc", "fma"],
-                    help="sparse-conv inner product: tc = tcgen05 3xF16 split, fma = fp32 FMA tiles")
+                    help="sparse-conv inner product: tc = wgmma 3xF16 split, fma = fp32 FMA tiles")
     ap.add_argument("--rpn", default="auto", choices=["auto", "tc", "cudnn"],
-                    help="RPN implementation: tc = hand-written tcgen05 3xF16 implicit GEMM, cudnn = torch fp32")
+                    help="RPN implementation: tc = hand-written wgmma 3xF16 implicit GEMM, cudnn = torch fp32")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's detections to DIR/<name>.npy (float32)")
     return ap.parse_args()
 
 
@@ -110,7 +117,7 @@ def workload_desc(args, n_voxels=None):
          "parallelism": "frames sharded dp%d, one all-gather of detections" % args.gpus,
          "l2": "flushed between steps (512 MiB write), per-step CUDA events",
          "rpn": args.rpn, "sparse_conv": args.sparse,
-         "precision": "fp32-grade (tcgen05 kind::f16 on a 3-term fp16 hi/lo split, fp32 accumulation)"}
+         "precision": "fp32-grade (wgmma f16 on a 3-term fp16 hi/lo split, fp32 accumulation)"}
     if n_voxels is not None:
         d["active_voxels_per_cloud"] = n_voxels
     return d
@@ -142,13 +149,13 @@ def cpu_path_clouds_per_s(name, clouds, threads):
 
 CPU_KIND = ("port: mirror model (b2second.models, reference state-dict keys) on the oracle spconv package -- C voxelizer "
             "and NMS (single thread, as upstream) + torch-CPU sparse conv / RPN; the unmodified reference cannot run "
-            "here (spconv 1.x absent, /root/reference not on the GPU box)")
+            "here (spconv 1.x is not installable)")
 
 
 def cpu_threads():
     """torch-CPU intra-op threads for the CPU arm.  The sparse middle is thousands of tiny gather/mm/index_add
-    calls; on the 128-core GPU host, 128 intra-op threads made the same path ~200x SLOWER than 8-16 threads
-    (measured round 1), so the arm uses the thread count that the path can actually exploit."""
+    calls; on a many-core host, one intra-op thread per core makes the same path far slower than 8-16 threads, so
+    the arm uses the thread count that the path can actually exploit."""
     env = os.environ.get("B2S_CPU_THREADS")
     if env:
         return int(env)
@@ -224,6 +231,11 @@ class ClockSampler:
 
 
 # ------------------------------------------------------------------------------------------------ GPU arm
+# NVIDIA H100 SXM data sheet (700 W): dense BF16 tensor rate and HBM3 bandwidth; used when no measured peaks are given
+H100_BF16_TFLOPS = 989.0
+H100_HBM_GBS = 3350.0
+
+
 def _peaks():
     try:
         return json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))
@@ -266,7 +278,7 @@ def _rpn_tensor_rate(eng, stages, peaks):
     rpn_ms = stages.get("rpn", 0.0)
     if not rstats or rpn_ms <= 0:
         return None
-    bf16 = float(peaks.get("bf16_tflops", 1687.0))
+    bf16 = float(peaks.get("bf16_tflops", H100_BF16_TFLOPS))
     n_l = len(rstats)
     flops = sum(s["flops"] for s in rstats) / n_l
     launch_ms = rpn_ms / n_l
@@ -380,6 +392,7 @@ def run_gpu_arm(args):
         torch.cuda.profiler.stop()
         return
     ms_res = _timed(step_resident, args.steps, warm, flush, world, dev)
+    dumped = _snapshot_outputs(eng) if args.dump_outputs and rank == 0 else None   # before step_e2e reuses the buffers
     ms_e2e = _timed(step_e2e, args.steps, warm, flush, world, dev)
     clocks = sampler.stop() if rank == 0 else None
     eng.check_status()
@@ -416,7 +429,7 @@ def run_gpu_arm(args):
     conv_ms = sum(v for k, v in stages.items() if k.startswith("sparse_conv"))
     conv_bytes = sum(s["bytes"] for s in stats)
     conv_flops = sum(s["flops"] for s in stats)
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    hbm_peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     sparse_roof = {"kernel": "k_sparse_conv%s (all %d sparse layers of one step, %d frames)"
                              % ("_tc" if args.sparse == "tc" else "", len(stats), B),
                    "bound": "hbm", "achieved": conv_bytes / (conv_ms * 1e-3) / 1e9 if conv_ms > 0 else 0.0,
@@ -427,21 +440,14 @@ def run_gpu_arm(args):
     sparse_roof["frac"] = sparse_roof["achieved"] / hbm_peak
     rt = _rpn_tensor_rate(eng, stages, peaks)
     if rt is not None and stages.get("rpn", 0.0) >= 0.5 * conv_ms:
-        # dominant kernel = k_conv3x3_tc2 (dense RPN 3x3 layers, implicit GEMM on tcgen05, 3xF16 split for fp32-grade
+        # dominant kernel = k_conv3x3_tc2 (dense RPN 3x3 layers, implicit GEMM on wgmma, 3xF16 split for fp32-grade
         # results).  `achieved` counts ALGORITHMIC fp32 flops per launch (2*px*9*cin*cout) over the average launch
         # duration; the tensor pipe executes 3 fp16 MMAs per algorithmic MAC, so bf16_peak/3 is this arithmetic's
         # ceiling -- reported alongside.
-        traffic = None
-        try:   # dram read+write bytes per launch from the committed ncu --set full capture of this kernel
-            tj = json.load(open(os.path.join(REPO, "profiles", "r2_traffic.json")))
-            traffic = tj["k_conv3x3_tc2"]["dram_bytes_per_launch"] * B / tj["frames_in_capture"]
-        except Exception:
-            pass
         roofline = {"kernel": "k_conv3x3_tc2 (per launch; %d launches per step, %d frames)" % (rt["launches"], B),
                     "bound": "tensor", "achieved": rt["achieved"], "peak": rt["peak"], "unit": "TFLOP/s",
-                    "frac": rt["frac"], "traffic": traffic,
-                    "traffic_source": "profiles/r2_traffic.json (ncu --set full)" if traffic else None,
-                    "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst)" if peaks else "fallback",
+                    "frac": rt["frac"],
+                    "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst)" if peaks else "H100 SXM data sheet",
                     "algorithmic_flops_per_launch": rt["algorithmic_flops_per_launch"],
                     "algorithmic_bytes_per_launch": rt["algorithmic_bytes_per_launch_fp32"],
                     "bytes_moved_per_launch": rt["bytes_moved_per_launch"],
@@ -458,7 +464,7 @@ def run_gpu_arm(args):
                             "is why `frac` can exceed 1/3 -- tiles_computed_frac_per_layer says by how much",
                     "second_kernel": sparse_roof}
     else:
-        roofline = dict(sparse_roof, traffic=None, peak_source="measured" if peaks else "fallback")
+        roofline = dict(sparse_roof, peak_source="measured" if peaks else "H100 SXM data sheet")
     cpu_baseline = None
     if not args.no_cpu_baseline:
         threads = cpu_threads()
@@ -484,9 +490,25 @@ def run_gpu_arm(args):
             "clocks": clocks, "roofline": roofline, "stage_ms_eager": _group_stages(stages),
             "cpu_baseline": cpu_baseline, "configs": extra}
     print(json.dumps(line), flush=True)
+    if dumped is not None:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in dumped.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def _snapshot_outputs(eng):
+    """host copies of what the resident path's caller receives after the last timed step: the packed detection
+    records and their decoded per-frame fields (all frames concatenated), as float32"""
+    rec = eng.det_record.detach().float().cpu().numpy().copy()
+    dets = eng.detections(output="host")
+    out = {"det_record": rec,
+           "num_detections": np.array([d["scores"].shape[0] for d in dets], dtype=np.float32)}
+    for key in ("box3d_lidar", "scores", "label_preds"):
+        out[key] = np.concatenate([d[key].numpy().astype(np.float32) for d in dets], 0)
+    return out
 
 
 def main():

@@ -1,5 +1,5 @@
 /*
- * b2second.h -- C ABI of libb2second.so: the B200 (sm_100a) implementation of the native layer that
+ * b2second.h -- C ABI of libb2second.so: the H100 (sm_90a) implementation of the native layer that
  * second.pytorch reaches through the external `spconv` 1.x package on its LiDAR-inference hot path.
  *
  * Conventions
@@ -170,7 +170,7 @@ int b2s_sparse_conv(const float *feat_in, int cin, const float *weight, const in
                     const int *num_out_dev, int cap_out, const float *scale, const float *shift,
                     int relu, float *feat_out, int cout, void *stream);
 
-/* same contraction on the tensor pipe (tcgen05 kind::f16, 3xF16 hi/lo split, fp32-grade): Cin in {8,16,32,64}, Cout in
+/* same contraction on the tensor pipe (wgmma f16, 3xF16 hi/lo split, fp32-grade): Cin in {8,16,32,64}, Cout in
  * {16,32,64}, K <= 27 (b2s_sparse_conv_tc_supported).  Every fp32 operand x travels as two fp16 planes hi = fp16(x),
  * lo = fp16(x - hi); per K step the kernel issues A_hi*W_hi + A_hi*W_lo + A_lo*W_hi with fp32 accumulation.
  *   feat_hi/lo  rows of in_stride halves (>= Cin, multiple of 8; e.g. interleaved [row][hi Cin | lo Cin] with
@@ -232,8 +232,8 @@ int b2s_to_bev_tc(const float *feat, const b2s_half *feat_hi, const b2s_half *fe
 
 /* ---- dense RPN convolution on the tensor pipe (second/pytorch/models/rpn.py:467-497 blocks, :264-299 deblocks,
  *      :386-391 heads): 3x3 stride-1 pad-1 (taps=9) or 1x1 (taps=1) conv + per-channel scale/shift (+ReLU).
- * tcgen05 implicit GEMM (kind::f16), fp32-grade accuracy through the 3xF16 split (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi,
- * fp32 accumulation in TMEM, short chains drained with round-to-nearest adds).
+ * wgmma implicit GEMM (f16 operands), fp32-grade accuracy through the 3xF16 split (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi,
+ * fp32 accumulation in registers, short chains drained with round-to-nearest adds).
  *   in_hi/in_lo  [B, H+2, W+2, Cin]   NHWC + zero halo, fp16 hi/lo planes (Cin multiple of 64)
  *   w_hi/w_lo    [taps, n_pad, Cin]   tap = ky*3+kx, w[tap][co][ci] = W_torch[co][ci][ky][kx] * 2^s (s folded into
  *                                     `scale`); rows >= Cout zero; n_pad in {32, 64, 128}

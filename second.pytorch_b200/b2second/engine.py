@@ -10,7 +10,7 @@ buffers, so the whole frame batch is ONE CUDA graph:
   b2s_voxelize (+ fused SimpleVoxel mean)                     voxelnet.py:325-328, preprocess.py:303-315
      or, for an example that arrives already voxelised (the reference's own dict):
      b2s_hash_build + b2s_vfe_mean over the caller's voxels   voxel_encoder.py:220-225,246-255
-  per sparse layer: b2s_rulebook_{subm,conv} (cached per indice_key) + b2s_sparse_conv_tc (tcgen05, fp16 hi/lo
+  per sparse layer: b2s_rulebook_{subm,conv} (cached per indice_key) + b2s_sparse_conv_tc (wgmma, fp16 hi/lo
       planes flow from layer to layer) with BatchNorm1d/ReLU folded into the epilogue      middle.py:145-192
   b2s_pfn (PointPillars)                                       pointpillars.py:203-237
   b2s_to_bev_tc (NHWC + halo, fp16 hi/lo)                      middle.py:206-209 / pointpillars.py:444-476
@@ -78,14 +78,14 @@ class InferenceEngine:
         self.code = s.box_code_size
         self.use_graph = use_cuda_graph
         self._graphs = {}
-        # RPN: "tc" = hand-written tcgen05 implicit GEMM (csrc/conv_tc.cu, 3xF16), "cudnn" = torch/cuDNN fp32.
+        # RPN: "tc" = hand-written wgmma implicit GEMM (csrc/conv_tc.cu, 3xF16), "cudnn" = torch/cuDNN fp32.
         if rpn_impl == "auto":
             rpn_impl = "tc" if _tc.supported(s.rpn) else "cudnn"
         assert rpn_impl in ("tc", "cudnn")
         if rpn_impl == "tc" and not _tc.supported(s.rpn):
             raise ValueError("rpn_impl='tc': this RPN has a layer b2s_conv2d_tc_ex does not cover (channels % 64, kernel > 4)")
         self.rpn_impl = rpn_impl
-        assert sparse_impl in ("tc", "fma")       # sparse-conv inner product: tcgen05 3xF16 | fp32 FMA tiles
+        assert sparse_impl in ("tc", "fma")       # sparse-conv inner product: wgmma 3xF16 | fp32 FMA tiles
         self.sparse_impl = sparse_impl
         with torch.cuda.device(dev):
             self.status = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -534,7 +534,7 @@ class InferenceEngine:
         self._launch_nms(st)
 
     def _launch_tc_tail(self, feats, hilo):
-        """BEV (NHWC, halo, fp16 hi/lo) -> tcgen05 RPN layers -> packed heads -> decode/filter -> NMS."""
+        """BEV (NHWC, halo, fp16 hi/lo) -> wgmma RPN layers -> packed heads -> decode/filter -> NMS."""
         L, lib, s = self._L, self.lib, self.spec
         st = L.stream()
         fl = self.final_level
@@ -694,7 +694,7 @@ class InferenceEngine:
             if lyr.get("in_split") is not None:
                 n += 1                           # b2s_split_f16
         if self.rpn_impl == "tc":
-            n += len(self.tc_plan) - (1 if self.tc_tail_fused else 0)   # one tcgen05 kernel per RPN layer (fused tail: 1 for 2)
+            n += len(self.tc_plan) - (1 if self.tc_tail_fused else 0)   # one tensor-core kernel per RPN layer (fused tail: 1 for 2)
             if self.bg_idx:
                 # k_bg_layer per layer, k_bg_compact (+ k_bg_fill per layer unless the conv epilogue fills)
                 n += len(self.bg_idx) + 1 + (0 if self.bg_fused_fill else len(self.bg_idx))
@@ -720,7 +720,7 @@ class InferenceEngine:
         return out
 
     def rpn_layer_stats(self):
-        """per tcgen05 RPN layer: algorithmic fp32 flops (2*pixels*taps*cin*cout; the 3xF16 split issues 3x that on
+        """per tensor-core RPN layer: algorithmic fp32 flops (2*pixels*taps*cin*cout; the 3xF16 split issues 3x that on
         the tensor pipe) and bytes moved (fp16 hi/lo planes in and out + weights)."""
         if self.rpn_impl != "tc":
             return []

@@ -8,7 +8,7 @@
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kMaxBlocks = 148 * 8;   // bounded grids + grid-stride loops: cost follows the live row count
+constexpr int kMaxBlocks = 132 * 8;   // bounded grids + grid-stride loops: cost follows the live row count
 
 inline int bounded_grid(long long items)
 {

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libb2second.so (sm_100a).  See include/b2second.h for the ABI.
+// common.cuh -- shared helpers for libb2second.so (sm_90a).  See include/b2second.h for the ABI.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

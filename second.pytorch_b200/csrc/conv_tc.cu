@@ -1,28 +1,26 @@
-// conv_tc.cu -- dense RPN convolution as a tcgen05 implicit GEMM with fp32-grade accuracy (b2s_conv2d_tc).
+// conv_tc.cu -- dense RPN convolution as a wgmma implicit GEMM with fp32-grade accuracy (b2s_conv2d_tc).
 //
 // second.pytorch's RPNV2 (second/pytorch/models/rpn.py:467-497, forward :314-331,393-420) is a stack of
 // Conv2d(3x3, pad 1)+BatchNorm2d+ReLU blocks, 1x1 (de)conv blocks and 1x1 heads: 63.6 GFLOP/frame at car.fhd,
 // the FLOP majority of the frame.  cuDNN runs it in fp32 SIMT (the parity bar is fp32, TF32 is off).  Here it is
 //
-//     D[M = 128 pixels, N = Cout] += A[M, K = 64 channels of one tap] * B[N, K]^T        (tcgen05.mma, kind::f16)
+//     D[M = 128 pixels, N = Cout] += A[M, K = 64 channels of one tap] * B[N, K]^T        (wgmma, f16 -> f32)
 //
 // with the **3xF16 split** (tc_common.cuh) that keeps fp32-grade accuracy on the tensor pipe: every operand is stored
 // as hi = fp16(x) and lo = fp16(x - hi), and each K step issues
 //     A_lo*B_hi + A_hi*B_lo + A_hi*B_hi            (the dropped A_lo*B_lo term is ~2^-22 relative)
-// accumulating in fp32 in TMEM.
+// accumulating in fp32 registers.
 //
 // Layout: activations NHWC fp16 with a one-pixel zero halo, [B, H+2, W+2, C] (hi and lo planes), so every
 // filter tap is a plain shifted box and TMA (cp.async.bulk.tensor.4d, SWIZZLE_128B) fetches the
-// [8 rows x 16 cols x 64 channels] A tile of a tap directly into the K-major UMMA layout; image borders come
+// [8 rows x 16 cols x 64 channels] A tile of a tap directly into the K-major wgmma layout; image borders come
 // from the halo, partial tiles from TMA's out-of-bounds zero fill.  Weights are pre-arranged [tap][Cout][Cin].
 //
-// CTA = 8 warps, persistent over output tiles (static round robin):
-//   warp 0  TMA producer   : per K block (tap, 32-channel chunk) 4 bulk-tensor loads into a 3-stage smem ring
-//   warp 1  MMA issuer     : one elected lane issues 3 x 4 tcgen05.mma per K block, tcgen05.commit frees the stage
-//   warp 2  TMEM allocator : 4 accumulator slots x N columns
-//   warps 4-7 epilogue     : tcgen05.ld accumulator -> BN scale/shift -> ReLU -> hi/lo split -> NHWC stores
-// mbarrier pipelines: smem full/empty (TMA <-> MMA) and TMEM full/empty (MMA <-> epilogue), so the epilogue of
-// tile i overlaps the main loop of tile i+1.
+// CTA = 3 warpgroups, persistent over output tiles (static round robin):
+//   warp 0       TMA producer: per K block (tap, 64-channel chunk) 4 bulk-tensor loads into a STAGES-deep smem ring
+//   warpgroups 1, 2  consumers: warpgroup g issues the wgmmas of tile rows 64g .. 64g+63 and owns their accumulators;
+//                then BN scale/shift -> ReLU -> hi/lo split -> NHWC stores
+// The ring's full/empty mbarriers let the loads of the next K blocks (and of the next tile) run under the MMAs.
 //
 // Every mbarrier wait is bounded: on a (never expected) protocol error the kernel traps instead of hanging the GPU.
 #include <cuda_fp16.h>
@@ -33,7 +31,7 @@ namespace {
 
 using namespace b2s_tc;
 constexpr int TILE_H = 8, TILE_W = 16;   // BLOCK_M = 128 output pixels = 8 rows x 16 cols
-constexpr int kThreads = 256;
+constexpr int kThreads = 384;
 
 struct ConvParams {
     int B, H, W;             // the GEMM pixel grid: conv output pixels (for a k=s deconv sub-grid: the input pixels)
@@ -50,8 +48,8 @@ struct ConvParams {
     void *out_hi;            // fp16 hi plane, or (out_lo == NULL) the full fp32 result
     __half *out_lo;
     int *status;
-    int dbg;                 // B2S_CONV_DBG diagnostics (results wrong!): 1 = no lo loads, 2 = hi*hi MMA only, 4 = no drain
-    int chain;               // K blocks (tap x 64-channel chunk) per TMEM accumulation chain: 4 = 48 MMAs (B2S_CONV_CHAIN)
+    int dbg;                 // B2S_CONV_DBG diagnostics (results wrong!): 1 = no lo loads, 4 = no drain
+    int chain;               // K blocks (tap x 64-channel chunk) per accumulation chain: 4 = 48 MMAs (B2S_CONV_CHAIN)
 };
 
 template <int N, int STAGES>
@@ -62,22 +60,16 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ 
 {
     constexpr uint32_t B_TILE_BYTES = N * BLOCK_K * ELEM_BYTES;
     constexpr uint32_t STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-    // The tensor core's fp32 accumulate is not round-to-nearest: a long accumulation chain (432 MMAs for a
-    // 3x3x128 tap stack) showed a systematic ~2e-5 relative error (measured, round 1).  So the reduction is cut
-    // into short chains of p.chain K blocks (default 4 = 48 MMAs) into one of ACC_SLOTS TMEM accumulators, and the
-    // epilogue warps drain the partial sums into fp32 registers with round-to-nearest adds while the tensor core
-    // already works on the next chain.
-    constexpr int ACC_SLOTS = 4;
-    constexpr uint32_t TMEM_COLS = (ACC_SLOTS * N <= 32) ? 32 : (ACC_SLOTS * N <= 64) ? 64 : (ACC_SLOTS * N <= 128) ? 128
-                                   : (ACC_SLOTS * N <= 256) ? 256 : 512;
-    static_assert(N % 16 == 0 && N >= 16 && ACC_SLOTS * N <= 512, "UMMA N for M=128 / TMEM capacity");
+    constexpr int R = N / 2;                 // accumulator registers per thread (64 rows x N per warpgroup)
+    // The tensor core's fp32 accumulate is not round-to-nearest: one long accumulation chain (432 MMAs for a 3x3x128
+    // tap stack) carries a systematic ~2e-5 relative error.  So the reduction is cut into short chains of p.chain K
+    // blocks (default 4 = 48 MMAs), and each chain's partial sum is added to the running fp32 sum with round-to-nearest.
+    static_assert(N % 16 == 0 && N >= 16 && N <= 128, "wgmma N");
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    __shared__ __align__(8) uint64_t bar_full[STAGES], bar_empty[STAGES], bar_tfull[ACC_SLOTS], bar_tempty[ACC_SLOTS];
-    __shared__ uint32_t s_tmem_base;
+    __shared__ __align__(8) uint64_t bar_full[STAGES], bar_empty[STAGES];
     __shared__ float s_scale[N], s_shift[N];
-    __shared__ __align__(16) uint32_t s_stage[4][32 * 36];   // per epilogue warp: 32 px x 32 words transpose tile (padded rows)
 
     const int warp = warp_idx_uniform(), lane = threadIdx.x & 31;
     const int kchunks = p.Cin / BLOCK_K;
@@ -89,19 +81,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ 
         s_shift[c] = (p.shift && c < p.Cout) ? p.shift[c] : 0.f;
     }
     if (warp == 1 && lane == 0) {
-        for (int i = 0; i < STAGES; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 1); }
-        for (int i = 0; i < ACC_SLOTS; ++i) { mbar_init(&bar_tfull[i], 1); mbar_init(&bar_tempty[i], 4); }
+        for (int i = 0; i < STAGES; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)),
-                     "r"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = s_tmem_base;
 
     if (warp == 0) {
         // ===================== TMA producer =====================
@@ -137,170 +120,83 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ 
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        // whole warp walks the loops with warp-uniform values, one elected lane issues (tc_common.cuh)
-        {
-            constexpr uint32_t idesc = make_idesc_f16(N);
-            const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-            const uint32_t smem0 = smem_u32(smem);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-                // accumulation chains of p.chain K blocks (default 4 = 48 MMAs), whatever the tap / channel split
-                for (int kb0 = 0; kb0 < num_kb; kb0 += p.chain) {
-                    mbar_wait(&bar_tempty[acc], acc_phase ^ 1);     // epilogue has drained this accumulator
-                    tc_fence_after();
-                    const uint32_t tmem_d = tmem_u + (uint32_t)(acc * N);
-                    const int kb_chain = min(num_kb, kb0 + p.chain) - kb0;
-                    for (int chunk = 0; chunk < kb_chain; ++chunk) {
-                        mbar_wait(&bar_full[stage], phase);          // TMA bytes have landed
-                        tc_fence_after();
-                        const uint32_t sa = smem0 + (uint32_t)stage * STAGE_BYTES;
-                        const uint64_t a_hi = make_desc_sw128(sa), a_lo = make_desc_sw128(sa + A_TILE_BYTES);
-                        const uint64_t b_hi = make_desc_sw128(sa + 2 * A_TILE_BYTES);
-                        const uint64_t b_lo = make_desc_sw128(sa + 2 * A_TILE_BYTES + B_TILE_BYTES);
-                        if (elect_one_sync()) {
-#pragma unroll
-                            for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                                const uint64_t koff = (uint64_t)((k * UMMA_K * ELEM_BYTES) >> 4);   // +32 B per K step
-                                if (p.dbg & 2) {
-                                    umma_f16(tmem_d, a_hi + koff, b_hi + koff, idesc, (chunk | k) != 0);
-                                    continue;
-                                }
-                                umma_f16(tmem_d, a_lo + koff, b_hi + koff, idesc, (chunk | k) != 0);
-                                umma_f16(tmem_d, a_hi + koff, b_lo + koff, idesc, 1);
-                                umma_f16(tmem_d, a_hi + koff, b_hi + koff, idesc, 1);
-                            }
-                            umma_commit(&bar_empty[stage]);          // frees the smem stage when the MMAs retire
-                            if (chunk == kb_chain - 1) umma_commit(&bar_tfull[acc]);   // chain's partial sum complete
-                        }
-                        __syncwarp();
-                        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                    }
-                    if (++acc == ACC_SLOTS) { acc = 0; acc_phase ^= 1; }
-                }
-            }
-        }
     } else if (warp >= 4) {
-        // ===================== epilogue =====================
-        const int ew = warp - 4;                 // == warp % 4: the TMEM lane quarter this warp may read
-        int acc = 0;
-        uint32_t acc_phase = 0;
+        // ===================== consumers: MMA + epilogue =====================
+        const int cg = (warp >> 2) - 1;          // warpgroup 0 / 1: tile rows 64 cg .. 64 cg + 63
+        const int wl = warp & 3;
+        const uint32_t smem0 = smem_u32(smem);
+        const uint32_t a_off = (uint32_t)cg * 64u * 128u;
+        int stage = 0;
+        uint32_t phase = 0;
         for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
             int tw = tile % p.tiles_w;
             int th = (tile / p.tiles_w) % p.tiles_h;
             int b = tile / (p.tiles_w * p.tiles_h);
-            // drain the per-chain partial sums into fp32 registers (round-to-nearest adds)
-            float sum[N];
+            float sum[R], acc[R];
 #pragma unroll
-            for (int j = 0; j < N; ++j) sum[j] = 0.f;
+            for (int j = 0; j < R; ++j) sum[j] = 0.f;
+            // accumulation chains of p.chain K blocks (default 4 = 48 MMAs), whatever the tap / channel split
             for (int kb0 = 0; kb0 < num_kb; kb0 += p.chain) {
-                mbar_wait(&bar_tfull[acc], acc_phase);
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(acc * N);
+                const int kb_chain = min(num_kb, kb0 + p.chain) - kb0;
+                for (int chunk = 0; chunk < kb_chain; ++chunk) {
+                    mbar_wait(&bar_full[stage], phase);          // TMA bytes have landed
+                    const uint32_t sa = smem0 + (uint32_t)stage * STAGE_BYTES;
+                    const uint64_t a_hi = make_desc_sw128(sa + a_off), a_lo = make_desc_sw128(sa + A_TILE_BYTES + a_off);
+                    const uint64_t b_hi = make_desc_sw128(sa + 2 * A_TILE_BYTES);
+                    const uint64_t b_lo = make_desc_sw128(sa + 2 * A_TILE_BYTES + B_TILE_BYTES);
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+                        const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);   // +32 B per K step
+                        wgmma_ss<N>(acc, a_lo + koff, b_hi + koff, (chunk | k) != 0);
+                        wgmma_ss<N>(acc, a_hi + koff, b_lo + koff, 1);
+                        wgmma_ss<N>(acc, a_hi + koff, b_hi + koff, 1);
+                    }
+                    wgmma_commit();
+                    wgmma_wait_all();
+                    wgmma_fence_operands<R>(acc);
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&bar_empty[stage]);    // this warp's share of the stage has been read
+                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                }
+                // drain the chain's partial sum into the fp32 running sum (round-to-nearest adds)
                 if (!(p.dbg & 4)) {
 #pragma unroll
-                    for (int c0 = 0; c0 < N; c0 += 16) {
-                        uint32_t r[16];
-                        tmem_ld16(taddr + c0, r);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) sum[c0 + j] = __fadd_rn(sum[c0 + j], __uint_as_float(r[j]));
-                    }
+                    for (int j = 0; j < R; ++j) sum[j] = __fadd_rn(sum[j], acc[j]);
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&bar_tempty[acc]);
-                if (++acc == ACC_SLOTS) { acc = 0; acc_phase ^= 1; }
             }
-            // Coalesced stores.  In TMEM layout every lane owns one pixel (128 channels = 512 B), so a direct store is
-            // 32 lanes x 16 B at a 512-B stride: half-filled sectors, 32 L2 transactions per instruction -- measured as
-            // the dominant fixed cost of this kernel (B2S_CONV_DBG sweep, round 1).  Each warp therefore transposes
-            // 32 pixels x 32 channels through a 4.5 KB shared staging tile and writes whole 128-byte lines:
-            // instruction `it` covers pixels it*4 + lane/8, 16-byte chunk lane%8.
-            uint32_t *stg = s_stage[ew];
-            const int sp = lane >> 3, sq = lane & 7;
-            size_t gpix[8];
-            bool gok[8];
-#pragma unroll
-            for (int it = 0; it < 8; ++it) {
-                const int mm = ew * 32 + it * 4 + sp;
-                const int hh = th * TILE_H + mm / TILE_W, ww = tw * TILE_W + mm % TILE_W;
-                gok[it] = (hh < p.H) && (ww < p.W);
-                const int oh = hh * p.out_mul + p.off_h, ow = ww * p.out_mul + p.off_w;   // position in the output map
-                gpix[it] = p.out_padded ? ((size_t)b * (p.Hout + 2) + (oh + 1)) * (p.Wout + 2) + (ow + 1)
-                                        : ((size_t)b * p.Hout + oh) * p.Wout + ow;
-            }
+            // epilogue: this thread holds rows m0 = 64 cg + 16 wl + lane/4 and m0 + 8, and per 8-column block j the
+            // channel pair 8j + 2(lane % 4); a quad of lanes writes 16 (fp16 plane) or 32 (fp32) contiguous bytes
             bool range_bad = false;
-            // 32 channels per pass.  fp16 planes: the staging row of a pixel holds 16 words of hi pairs then 16 words of
-            // lo pairs; instruction `it` covers pixels it*4 + lane/8, lanes 0-3 of a group write the pixel's 64 hi bytes,
-            // lanes 4-7 its 64 lo bytes.  fp32 (heads): 32 floats per pixel, 8 x 16-byte chunks.
 #pragma unroll
-            for (int cc = 0; cc < N; cc += 32) {
-                __syncwarp();
-                if (p.out_lo) {
+            for (int rh = 0; rh < 2; ++rh) {
+                const int mm = cg * 64 + wl * 16 + (lane >> 2) + rh * 8;
+                const int hh = th * TILE_H + mm / TILE_W, ww = tw * TILE_W + mm % TILE_W;
+                if (hh >= p.H || ww >= p.W) continue;
+                const int oh = hh * p.out_mul + p.off_h, ow = ww * p.out_mul + p.off_w;   // position in the output map
+                const size_t gpix = p.out_padded ? ((size_t)b * (p.Hout + 2) + (oh + 1)) * (p.Wout + 2) + (ow + 1)
+                                                 : ((size_t)b * p.Hout + oh) * p.Wout + ow;
 #pragma unroll
-                    for (int c0 = 0; c0 < 32; c0 += 8) {
-                        uint32_t hw[4], lw[4];
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            float x0 = fmaf(sum[cc + c0 + 2 * j], s_scale[cc + c0 + 2 * j], s_shift[cc + c0 + 2 * j]);
-                            float x1 = fmaf(sum[cc + c0 + 2 * j + 1], s_scale[cc + c0 + 2 * j + 1], s_shift[cc + c0 + 2 * j + 1]);
-                            if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-                            range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
-                            const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
-                            hw[j] = __byte_perm(p0, p1, 0x5410);
-                            lw[j] = __byte_perm(p0, p1, 0x7632);
-                        }
-                        *reinterpret_cast<uint4 *>(stg + lane * 36 + c0 / 2) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                        *reinterpret_cast<uint4 *>(stg + lane * 36 + 16 + c0 / 2) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                    }
-                    __syncwarp();
-                    const int ch = cc + (sq & 3) * 8;                      // first of this lane's 8 channels
-                    if (ch < p.Cout) {
-                        __half *outp = (sq < 4) ? reinterpret_cast<__half *>(p.out_hi) : p.out_lo;
-#pragma unroll
-                        for (int it = 0; it < 8; ++it) {
-                            if (!gok[it]) continue;
-                            *reinterpret_cast<uint4 *>(outp + gpix[it] * p.out_stride + ch) =
-                                *reinterpret_cast<const uint4 *>(stg + (it * 4 + sp) * 36 + sq * 4);
-                        }
-                    }
-                } else {
-#pragma unroll
-                    for (int c0 = 0; c0 < 32; c0 += 4) {
-                        uint32_t v[4];
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            float x = fmaf(sum[cc + c0 + j], s_scale[cc + c0 + j], s_shift[cc + c0 + j]);
-                            if (p.relu) x = fmaxf(x, 0.f);
-                            v[j] = __float_as_uint(x);
-                        }
-                        *reinterpret_cast<uint4 *>(stg + lane * 36 + c0) = make_uint4(v[0], v[1], v[2], v[3]);
-                    }
-                    __syncwarp();
-                    if (cc + sq * 4 < p.Cout) {
-                        float *outp = reinterpret_cast<float *>(p.out_hi);
-#pragma unroll
-                        for (int it = 0; it < 8; ++it) {
-                            if (!gok[it]) continue;
-                            *reinterpret_cast<uint4 *>(outp + gpix[it] * p.out_stride + cc + sq * 4) =
-                                *reinterpret_cast<const uint4 *>(stg + (it * 4 + sp) * 36 + sq * 4);
-                        }
+                for (int j = 0; j < N / 8; ++j) {
+                    const int c = 8 * j + 2 * (lane & 3);
+                    if (c >= p.Cout) continue;                   // Cout is a multiple of 4: c + 1 < Cout too
+                    float x0 = fmaf(sum[4 * j + 2 * rh], s_scale[c], s_shift[c]);
+                    float x1 = fmaf(sum[4 * j + 2 * rh + 1], s_scale[c + 1], s_shift[c + 1]);
+                    if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                    if (p.out_lo) {
+                        range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
+                        const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
+                        *reinterpret_cast<uint32_t *>(reinterpret_cast<__half *>(p.out_hi) + gpix * p.out_stride + c) =
+                            __byte_perm(p0, p1, 0x5410);
+                        *reinterpret_cast<uint32_t *>(p.out_lo + gpix * p.out_stride + c) = __byte_perm(p0, p1, 0x7632);
+                    } else {
+                        *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out_hi) + gpix * p.out_stride + c) =
+                            make_float2(x0, x1);
                     }
                 }
             }
             if (__any_sync(0xffffffffu, range_bad) && lane == 0 && p.status) atomicOr(p.status, B2S_STATUS_F16_RANGE);
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
     }
 }
 

@@ -1,34 +1,22 @@
-// conv_tc2.cu -- 3x3 RPN convolution, second-generation tcgen05 kernel (weights-stationary orientation).
+// conv_tc2.cu -- 3x3 RPN convolution with vertical activation reuse (wgmma, sm_90a).
 //
-// Why a second kernel: k_conv_tc (conv_tc.cu) computes D[128 pixels, Cout] with both operands in shared memory.
-// A 128x128x8 tf32 MMA reads 4 KB of A and 4 KB of B from shared memory in its 64 tensor cycles -- exactly the
-// 128 B/clk the shared-memory data pipe can deliver -- so every TMA write into the ring (64 KB per K block) is
-// time the tensor pipe waits.  ncu (profiles/r1_tc_kernels_ncu_full.csv): tensor pipe 59.5 % active,
-// l1tex__data_pipe_tc_wavefronts_mem_shared 57.9 % + TMA writes + epilogue staging = the pipe is full.
+// Why a second kernel: k_conv_tc (conv_tc.cu) loads a fresh [8 x 16 pixel, 64 channel] activation tile for every
+// one of the 9 taps.  Here a stage is a 10-row x 16-col pixel tile (one 64-channel chunk, one horizontal tap offset
+// dx), and the three vertical taps dy = 0,1,2 are the SAME stage viewed dy pixel rows (= 2048 B = two whole 1024-byte
+// swizzle atoms) further down, so the wgmma descriptor just starts 2048*dy bytes later -- no swizzle-phase tricks.
+// Activation bytes written to shared memory drop 2.4x against k_conv_tc.
 //
-// This kernel removes shared-memory traffic per tensor cycle two ways:
-//   1. orientation swap, N = 256:  D^T[Cout = 128 (M, TMEM lanes), 256 pixels (N, TMEM columns)]
-//          += W[tap][Cout, 64 ch] (A)  *  X[256 pixels, 64 ch]^T (B)
-//      a 128x256x16 f16 MMA reads 4 + 8 KB in 128 tensor cycles = 96 B/clk;
-//   2. vertical reuse: the activation stage is an 18-row x 16-col pixel tile (one 64-channel chunk, one
-//      horizontal tap offset dx).  The three vertical taps dy = 0,1,2 are the SAME stage viewed 16 pixel rows
-//      (= 2048 B = two whole 1024-byte swizzle atoms) further down, so the UMMA descriptor just starts 2048*dy
-//      bytes later -- no swizzle-phase tricks.  Activation bytes written to shared memory drop 2.7x.
-// Per (dx, chunk) group: 72 KB activations + 3 x 32 KB weights written, 36 MMAs (4608 tensor cycles) -- the same
-// bytes and cycles as the 3xTF32 kernel of round 1, but a group now covers 64 channels instead of 32 (3xF16 split,
-// tc_common.cuh), so a 128-channel layer is 6 groups per tile instead of 12.
+// Work items are 16 x 16-pixel tiles (the granularity of the tile work list and of the background tiles, rpn_bg.cu);
+// a work item is computed as two 8 x 16 halves, one after the other (the lower half only when it has image rows).
+// A half is D[128 pixels, Cout = 128]: warpgroup g of the two consumer warpgroups owns pixel rows 4g .. 4g+3 of the
+// half, 64 pixels x 128 channels of fp32 accumulators plus the same again for the running sum, which is what the
+// register file holds at 384 threads per SM.
 //
-// Accumulation chains stay short (the tensor core's fp32 accumulate truncates: measured rms error grows linearly
-// with chain length, tools/bench_conv_tc.py): one chain = one (dx, chunk) group = 36 MMAs, drained by the
-// epilogue warps into fp32 registers with round-to-nearest adds; two 256-column TMEM accumulators ping-pong.
+// Accumulation chains stay short (the tensor core's fp32 accumulate truncates: the rms error grows linearly with chain
+// length): one chain = one (dx, chunk) group = 36 MMAs, added into fp32 registers with round-to-nearest adds.
 //
-// Epilogue without staging: a TMEM lane is an output CHANNEL here, so lane l of a warp holds channel 32q+l of
-// one pixel.  Lanes 2j / 2j+1 swap one value of a pixel pair (one shuffle of the packed hi|lo word), after which
-// every lane owns two adjacent channels of one pixel and stores a half2 per plane: a warp store writes
-// 2 pixels x 64 contiguous bytes.
-//
-// Warp roles (12 warps): 0 activation TMA producer, 1 MMA issuer, 2 TMEM allocator, 3 weight TMA producer,
-// 4-11 epilogue (lane quarter = warp % 4, pixel half = (warp - 4) / 4).
+// Warp roles (12 warps): 0 activation TMA producer, 3 weight TMA producer, 4-11 two consumer warpgroups (MMA,
+// epilogue, background tiles).
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -36,19 +24,18 @@
 namespace {
 
 using namespace b2s_tc;
-constexpr int T2_H = 16, T2_W = 16;                 // 256 output pixels per tile
-constexpr int HALO_H = T2_H + 2;                    // rows of the activation stage
-constexpr int N_PIX = T2_H * T2_W;                  // UMMA N
+constexpr int T2_H = 16, T2_W = 16;                 // work item: 256 output pixels
+constexpr int HALF_H = 8;                           // rows computed at once (BLOCK_M = 128 pixels)
+constexpr int HALO_H = HALF_H + 2;                  // rows of the activation stage
 constexpr int kThreads2 = 384;
-constexpr uint32_t X_PLANE_BYTES = HALO_H * T2_W * BLOCK_K * ELEM_BYTES;   // 36 KB (hi or lo)
-constexpr uint32_t X_STAGE_BYTES = 2 * X_PLANE_BYTES;             // 72 KB
+constexpr uint32_t X_PLANE_BYTES = HALO_H * T2_W * BLOCK_K * ELEM_BYTES;   // 20 KB (hi or lo)
+constexpr uint32_t X_STAGE_BYTES = 2 * X_PLANE_BYTES;             // 40 KB
 constexpr uint32_t W_PLANE_BYTES = 128 * BLOCK_K * ELEM_BYTES;             // 16 KB
-// Weight ring: 5 slots of ONE plane each (hi and lo alternate).  A K block issues its 8 W_hi MMAs first and frees
-// the hi slot, then its 4 W_lo MMAs -- so a slot is refilled two full K blocks (~3000 tensor cycles) before it is
-// needed.  (First version: 2 slots of hi+lo = one K block of lead -> the MMA issuer waited on weight loads,
-// 0.371 ms/layer; measured round 1.)
-constexpr int X_STAGES = 2, W_STAGES = 5, ACC2 = 2;
-constexpr uint32_t DY_BYTES = T2_W * BLOCK_K * ELEM_BYTES;                 // one pixel row of the tile = 2048 B
+// Weight ring of single planes: per dy the hi plane, then the lo plane.  Six slots = one whole (dx, chunk) group
+// of weights in flight while the previous one is multiplied.
+constexpr int X_STAGES = 2, W_STAGES = 6;
+constexpr uint32_t DY_BYTES = T2_W * BLOCK_K * ELEM_BYTES;                 // one pixel row of the stage = 2048 B
+static_assert(X_PLANE_BYTES % 1024 == 0, "stage planes are whole swizzle atoms");
 
 struct Conv2Params {
     int B, H, W, Cin, Cout, relu;
@@ -56,15 +43,12 @@ struct Conv2Params {
     const int *work_list, *work_count;   // optional (device): the tiles to compute, work_list[0 .. *work_count); tiles that
                                          // are not listed are "background" (b2s_rpn_bg_plan) and get their constant from
                                          // b2s_rpn_bg_fill.  NULL: every tile
-    const int *bg_list, *bg_count;       // optional (device): background tiles of this layer's output; the epilogue warps
+    const int *bg_list, *bg_count;       // optional (device): background tiles of this layer's output; the consumer warps
     const __half *bg_hi, *bg_lo;         // copy them from the layer's empty-frame response bg_hi/bg_lo [H+2, W+2, Cout]
-                                         // (one halo-padded frame) in the shadow of the MMA main loop
-    int last_half;                   // 1: the last tile row covers <= 8 image rows -> its MMAs run at N = 128 (upper half
-                                     // of the pixel tile only); H = 200 = 12.5 tiles of 16 rows saves 3.8 % of the MMA work
+                                         // (one halo-padded frame) between their work items
     int out_stride;
-    int dephase;                     // B2S_CONV2_DEPHASE: start delay step in cycles (CTA i waits (i & 3) steps)
     int dbg;                         // B2S_CONV2_DBG diagnostics (results wrong): 1 no activation loads, 2 no weight
-                                     // loads, 4 no TMEM drain, 8 no global stores
+                                     // loads, 4 no accumulator drain, 8 no global stores
     const float *scale, *shift;
     __half *out_hi, *out_lo;         // [B, H+2, W+2, out_stride] halo-padded fp16 planes (interior written)
     int *status;                     // bit B2S_STATUS_F16_RANGE raised when an activation exceeds the fp16 range
@@ -73,6 +57,12 @@ struct Conv2Params {
 // number of work items and the i-th tile of this launch (dense: identity)
 __device__ __forceinline__ int work_total(const Conv2Params &p) { return p.work_list ? min(*p.work_count, p.num_tiles) : p.num_tiles; }
 __device__ __forceinline__ int work_tile(const Conv2Params &p, int i) { return p.work_list ? __ldg(&p.work_list[i]) : i; }
+// 8-row halves of a tile that hold image rows (every role walks the same sequence)
+__device__ __forceinline__ int halves_of(const Conv2Params &p, int tile)
+{
+    const int th = (tile / p.tiles_w) % p.tiles_h;
+    return th * T2_H + HALF_H < p.H ? 2 : 1;
+}
 
 __global__ void __launch_bounds__(kThreads2, 1)
 k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
@@ -81,188 +71,89 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
 {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t *smem_x = smem;                                   // X_STAGES x 72 KB
+    uint8_t *smem_x = smem;                                   // X_STAGES x 40 KB
     uint8_t *smem_w = smem + X_STAGES * X_STAGE_BYTES;        // W_STAGES x 16 KB
-    __shared__ __align__(8) uint64_t bar_xfull[X_STAGES], bar_xempty[X_STAGES], bar_wfull[W_STAGES],
-        bar_wempty[W_STAGES], bar_tfull[ACC2], bar_tempty[ACC2];
-    __shared__ uint32_t s_tmem_base;
+    __shared__ __align__(8) uint64_t bar_xfull[X_STAGES], bar_xempty[X_STAGES], bar_wfull[W_STAGES], bar_wempty[W_STAGES];
+    __shared__ float s_scale[128], s_shift[128];
 
     const int warp = warp_idx_uniform(), lane = threadIdx.x & 31;
     const int kchunks = p.Cin / BLOCK_K;
     const int n_work = work_total(p);
 
+    if (threadIdx.x < 128) {
+        const int c = threadIdx.x;
+        s_scale[c] = (p.scale && c < p.Cout) ? p.scale[c] : 1.f;
+        s_shift[c] = (p.shift && c < p.Cout) ? p.shift[c] : 0.f;
+    }
     if (warp == 1 && lane == 0) {
-        for (int i = 0; i < X_STAGES; ++i) { mbar_init(&bar_xfull[i], 1); mbar_init(&bar_xempty[i], 1); }
-        for (int i = 0; i < W_STAGES; ++i) { mbar_init(&bar_wfull[i], 1); mbar_init(&bar_wempty[i], 1); }
-        for (int i = 0; i < ACC2; ++i) { mbar_init(&bar_tfull[i], 1); mbar_init(&bar_tempty[i], 8); }
+        for (int i = 0; i < X_STAGES; ++i) { mbar_init(&bar_xfull[i], 1); mbar_init(&bar_xempty[i], 8); }
+        for (int i = 0; i < W_STAGES; ++i) { mbar_init(&bar_wfull[i], 1); mbar_init(&bar_wempty[i], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)),
-                     "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = s_tmem_base;
 
     if (warp == 0) {
-        // ===================== activation producer: one 18x16-pixel x 32-channel stage per (dx, chunk) ==========
+        // ===================== activation producer: one 10x16-pixel x 64-channel stage per (half, dx, chunk) ======
         if (lane == 0) {
             int xs = 0;
             uint32_t xph = 0;
-            if (p.dephase > 0) {
-                // All CTAs run equal-length tiles in lock step, so their end-of-tile store bursts (256 KB per SM) hit
-                // L2 together; starting CTA i (i mod 4) quarter-tiles late spreads them out.  B2S_CONV2_DEPHASE
-                // = cycles per step (0 = off).
-                const long long t0 = clock64(), d = (long long)(blockIdx.x & 3) * p.dephase;
-                while (clock64() - t0 < d) { }
-            }
             for (int wi = blockIdx.x; wi < n_work; wi += gridDim.x) {
                 const int tile = work_tile(p, wi);
                 const int tw = tile % p.tiles_w, th = (tile / p.tiles_w) % p.tiles_h, b = tile / (p.tiles_w * p.tiles_h);
-                const int h0 = th * T2_H, w0 = tw * T2_W;
-                for (int dx = 0; dx < 3; ++dx)
-                    for (int chunk = 0; chunk < kchunks; ++chunk) {
-                        mbar_wait(&bar_xempty[xs], xph ^ 1);
-                        uint8_t *st = smem_x + (size_t)xs * X_STAGE_BYTES;
-                        if (p.dbg & 1) {                  // diagnostic: no activation loads (results wrong)
-                            mbar_arrive(&bar_xfull[xs]);
+                const int nh = halves_of(p, tile);
+                for (int hf = 0; hf < nh; ++hf) {
+                    const int h0 = th * T2_H + hf * HALF_H, w0 = tw * T2_W;
+                    for (int dx = 0; dx < 3; ++dx)
+                        for (int chunk = 0; chunk < kchunks; ++chunk) {
+                            mbar_wait(&bar_xempty[xs], xph ^ 1);
+                            uint8_t *st = smem_x + (size_t)xs * X_STAGE_BYTES;
+                            if (p.dbg & 1) {                  // diagnostic: no activation loads (results wrong)
+                                mbar_arrive(&bar_xfull[xs]);
+                                if (++xs == X_STAGES) { xs = 0; xph ^= 1; }
+                                continue;
+                            }
+                            mbar_arrive_expect_tx(&bar_xfull[xs], X_STAGE_BYTES);
+                            // padded coordinates: output (h, w) reads padded rows h..h+2 and cols w..w+2
+                            tma_load_4d(st, &map_x_hi, &bar_xfull[xs], chunk * BLOCK_K, w0 + dx, h0, b);
+                            tma_load_4d(st + X_PLANE_BYTES, &map_x_lo, &bar_xfull[xs], chunk * BLOCK_K, w0 + dx, h0, b);
                             if (++xs == X_STAGES) { xs = 0; xph ^= 1; }
-                            continue;
                         }
-                        mbar_arrive_expect_tx(&bar_xfull[xs], X_STAGE_BYTES);
-                        // padded coordinates: output (h, w) reads padded rows h..h+2 and cols w..w+2
-                        tma_load_4d(st, &map_x_hi, &bar_xfull[xs], chunk * BLOCK_K, w0 + dx, h0, b);
-                        tma_load_4d(st + X_PLANE_BYTES, &map_x_lo, &bar_xfull[xs], chunk * BLOCK_K, w0 + dx, h0, b);
-                        if (++xs == X_STAGES) { xs = 0; xph ^= 1; }
-                    }
+                }
             }
         }
     } else if (warp == 3) {
-        // ===================== weight producer: W[tap = dy*3+dx][128, 32 ch] hi/lo per K block ===================
+        // ===================== weight producer: W[tap = dy*3+dx][128, 64 ch] hi, then lo, per dy ===================
         if (lane == 0) {
             int ws = 0;
             uint32_t wph = 0;
-            for (int wi = blockIdx.x; wi < n_work; wi += gridDim.x)
-                for (int dx = 0; dx < 3; ++dx)
-                    for (int chunk = 0; chunk < kchunks; ++chunk)
-                        for (int dy = 0; dy < 3; ++dy)
-                            for (int pl = 0; pl < 2; ++pl) {           // hi plane, then lo plane
-                                mbar_wait(&bar_wempty[ws], wph ^ 1);
-                                if (p.dbg & 2) {          // diagnostic: no weight loads (results wrong)
-                                    mbar_arrive(&bar_wfull[ws]);
+            for (int wi = blockIdx.x; wi < n_work; wi += gridDim.x) {
+                const int nh = halves_of(p, work_tile(p, wi));
+                for (int hf = 0; hf < nh; ++hf)
+                    for (int dx = 0; dx < 3; ++dx)
+                        for (int chunk = 0; chunk < kchunks; ++chunk)
+                            for (int dy = 0; dy < 3; ++dy)
+                                for (int pl = 0; pl < 2; ++pl) {           // hi plane, then lo plane
+                                    mbar_wait(&bar_wempty[ws], wph ^ 1);
+                                    if (p.dbg & 2) {          // diagnostic: no weight loads (results wrong)
+                                        mbar_arrive(&bar_wfull[ws]);
+                                        if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
+                                        continue;
+                                    }
+                                    mbar_arrive_expect_tx(&bar_wfull[ws], W_PLANE_BYTES);
+                                    tma_load_3d(smem_w + (size_t)ws * W_PLANE_BYTES, pl ? &map_w_lo : &map_w_hi,
+                                                &bar_wfull[ws], chunk * BLOCK_K, 0, dy * 3 + dx);
                                     if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
-                                    continue;
                                 }
-                                mbar_arrive_expect_tx(&bar_wfull[ws], W_PLANE_BYTES);
-                                tma_load_3d(smem_w + (size_t)ws * W_PLANE_BYTES, pl ? &map_w_lo : &map_w_hi,
-                                            &bar_wfull[ws], chunk * BLOCK_K, 0, dy * 3 + dx);
-                                if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
-                            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        // The whole warp walks the loops (all values warp-uniform -> uniform registers); one elected lane issues
-        // the tcgen05 instructions.  See tc_common.cuh: an `if (lane == 0)` issuer costs ~190 cycles per MMA.
-        constexpr uint32_t idesc_full = make_idesc_f16(N_PIX), idesc_half = make_idesc_f16(N_PIX / 2);
-        const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint32_t sx0 = smem_u32(smem_x), sw0 = smem_u32(smem_w);
-        // Software-pipelined issue: the barrier of the NEXT burst's operands is waited for while the current burst
-        // still has MMAs to issue, so the tensor queue never runs dry between bursts.  (tests/cuda/mma_probe2.cu
-        // shows the pipe sustains 128 cycles per N=256 MMA on exactly this operand pattern; with a
-        // wait -> fence -> elect -> issue sequence between bursts the kernel measured 188.)
-        const int my_tiles = ((int)blockIdx.x < n_work) ? (n_work - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-        const int total_g = my_tiles * 3 * kchunks;
-        if (elect_one_sync() && total_g > 0) {
-            int xs = 0, ws = 0, acc = 0;
-            uint32_t xph = 0, wph = 0, aph = 0;
-            mbar_wait(&bar_tempty[0], 1);
-            mbar_wait(&bar_xfull[0], 0);
-            mbar_wait(&bar_wfull[0], 0);
-            tc_fence_after();
-            const int gpt = 3 * kchunks;                     // groups per tile
-            for (int gi = 0; gi < total_g; ++gi) {
-                const int tile = work_tile(p, (int)blockIdx.x + (gi / gpt) * (int)gridDim.x);
-                const bool half_tile = p.last_half && ((tile / p.tiles_w) % p.tiles_h) == p.tiles_h - 1;
-                const uint32_t idesc = half_tile ? idesc_half : idesc_full;
-                const uint32_t tmem_d = tmem_u + (uint32_t)(acc * N_PIX);
-                const uint32_t sx = sx0 + (uint32_t)xs * X_STAGE_BYTES;
-                for (int dy = 0; dy < 3; ++dy) {
-                    const uint64_t x_hi = make_desc_sw128(sx + dy * DY_BYTES);
-                    const uint64_t x_lo = make_desc_sw128(sx + X_PLANE_BYTES + dy * DY_BYTES);
-                    const uint64_t w_hi = make_desc_sw128(sw0 + (uint32_t)ws * W_PLANE_BYTES);
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) {
-                        const uint64_t koff = (uint64_t)((k * UMMA_K * ELEM_BYTES) >> 4);   // +32 B per K step
-                        umma_f16_afill(tmem_d, w_hi + koff, x_lo + koff, idesc, (dy | k) != 0);
-                        umma_f16_alast(tmem_d, w_hi + koff, x_hi + koff, idesc, 1);
-                    }
-                    // look ahead: the W_lo plane of this K block
-                    int wsn = ws + 1;
-                    uint32_t wphn = wph;
-                    if (wsn == W_STAGES) { wsn = 0; wphn ^= 1; }
-                    mbar_wait(&bar_wfull[wsn], wphn);
-                    tc_fence_after();
-                    {
-                        const uint64_t koff = (uint64_t)((3 * UMMA_K * ELEM_BYTES) >> 4);
-                        umma_f16_afill(tmem_d, w_hi + koff, x_lo + koff, idesc, 1);
-                        umma_f16_alast(tmem_d, w_hi + koff, x_hi + koff, idesc, 1);
-                    }
-                    umma_commit(&bar_wempty[ws]);
-                    ws = wsn; wph = wphn;
-                    const uint64_t w_lo = make_desc_sw128(sw0 + (uint32_t)ws * W_PLANE_BYTES);
-#pragma unroll
-                    for (int k = 0; k < 2; ++k) {
-                        const uint64_t koff = (uint64_t)((k * UMMA_K * ELEM_BYTES) >> 4);
-                        umma_f16(tmem_d, w_lo + koff, x_hi + koff, idesc, 1);
-                    }
-                    // look ahead: the next K block's W_hi plane, and at a group boundary the next accumulator and
-                    // activation stage
-                    wsn = ws + 1; wphn = wph;
-                    if (wsn == W_STAGES) { wsn = 0; wphn ^= 1; }
-                    const bool last = (gi == total_g - 1) && (dy == 2);
-                    if (!last) {
-                        mbar_wait(&bar_wfull[wsn], wphn);
-                        if (dy == 2) {
-                            const int accn = acc ^ 1, xsn = xs ^ 1;
-                            mbar_wait(&bar_tempty[accn], (accn == 0 ? (aph ^ 1) : aph) ^ 1);
-                            mbar_wait(&bar_xfull[xsn], xsn == 0 ? (xph ^ 1) : xph);
-                        }
-                        tc_fence_after();
-                    }
-#pragma unroll
-                    for (int k = 2; k < 4; ++k) {
-                        const uint64_t koff = (uint64_t)((k * UMMA_K * ELEM_BYTES) >> 4);
-                        umma_f16(tmem_d, w_lo + koff, x_hi + koff, idesc, 1);
-                    }
-                    umma_commit(&bar_wempty[ws]);
-                    if (dy == 2) {
-                        umma_commit(&bar_xempty[xs]);
-                        umma_commit(&bar_tfull[acc]);            // this group's partial sum is complete
-                    }
-                    ws = wsn; wph = wphn;
-                }
-                if (++xs == X_STAGES) { xs = 0; xph ^= 1; }
-                if (++acc == ACC2) { acc = 0; aph ^= 1; }
             }
         }
-        __syncwarp();
     } else if (warp >= 4) {
-        // ===================== epilogue =====================
-        const int q = warp & 3;                     // TMEM lane quarter this warp may read
-        const int half = (warp - 4) >> 2;           // pixel half: tile rows 8*half .. 8*half+7
-        const int c = q * 32 + lane;                // output channel of this thread
-        const bool c_ok = c < p.Cout;
-        const float sc = (p.scale && c_ok) ? p.scale[c] : 1.f;
-        const float sh = (p.shift && c_ok) ? p.shift[c] : 0.f;
-        int acc = 0;
-        uint32_t aph = 0;
-        // Background tiles (csrc/rpn_bg.cu) of this layer's output are filled by the epilogue warps, which otherwise
-        // spend most of a tile waiting for the tensor pipe: CTA c owns background tiles c, c + grid, ... and spreads
-        // them over its work items.  One load / store instruction of the 256 epilogue threads = one tile row of one
-        // plane (16 pixels x 256 B, contiguous) of the layer's empty-frame response, which stays L2 resident.
+        // ===================== consumers: MMA + epilogue + background tiles =====================
+        const int cg = (warp >> 2) - 1;             // warpgroup: pixel rows 4 cg .. 4 cg + 3 of the half
+        const int wl = warp & 3;
+        const uint32_t sx0 = smem_u32(smem_x), sw0 = smem_u32(smem_w);
+        // Background tiles (csrc/rpn_bg.cu) of this layer's output: CTA c owns background tiles c, c + grid, ... and
+        // spreads them over its work items.  One load / store instruction of the 256 consumer threads = one tile row of
+        // one plane (16 pixels x 256 B, contiguous) of the layer's empty-frame response, which stays L2 resident.
         const int n_bg = p.bg_list ? min(*p.bg_count, p.num_tiles) : 0;
         const int my_bg = ((int)blockIdx.x < n_bg) ? (n_bg - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
         const int my_work = ((int)blockIdx.x < n_work) ? (n_work - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
@@ -292,74 +183,87 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                 }
             }
         };
+        int xs = 0, ws = 0;
+        uint32_t xph = 0, wph = 0;
+        float sum[64], acc[64];
         for (int wi = blockIdx.x; wi < n_work; wi += gridDim.x) {
             const int tile = work_tile(p, wi);
             const int tw = tile % p.tiles_w, th = (tile / p.tiles_w) % p.tiles_h, b = tile / (p.tiles_w * p.tiles_h);
-            float sum[128];
+            const int nh = halves_of(p, tile);
+            for (int hf = 0; hf < nh; ++hf) {
 #pragma unroll
-            for (int j = 0; j < 128; ++j) sum[j] = 0.f;
-            const bool skip_half = p.last_half && th == p.tiles_h - 1 && half == 1;    // nothing was computed for it
-            for (int g = 0; g < 3 * kchunks; ++g) {
-                mbar_wait(&bar_tfull[acc], aph);
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * N_PIX + half * 128);
-                if (!(p.dbg & 4) && !skip_half) {
+                for (int j = 0; j < 64; ++j) sum[j] = 0.f;
+                for (int g = 0; g < 3 * kchunks; ++g) {
+                    mbar_wait(&bar_xfull[xs], xph);
+                    const uint32_t sx = sx0 + (uint32_t)xs * X_STAGE_BYTES + (uint32_t)(cg * 4) * DY_BYTES;
+#pragma unroll 1
+                    for (int dy = 0; dy < 3; ++dy) {
+                        int ws2 = ws + 1;
+                        uint32_t wph2 = wph;
+                        if (ws2 == W_STAGES) { ws2 = 0; wph2 ^= 1; }
+                        mbar_wait(&bar_wfull[ws], wph);
+                        mbar_wait(&bar_wfull[ws2], wph2);
+                        const uint64_t x_hi = make_desc_sw128(sx + dy * DY_BYTES);
+                        const uint64_t x_lo = make_desc_sw128(sx + X_PLANE_BYTES + dy * DY_BYTES);
+                        const uint64_t w_hi = make_desc_sw128(sw0 + (uint32_t)ws * W_PLANE_BYTES);
+                        const uint64_t w_lo = make_desc_sw128(sw0 + (uint32_t)ws2 * W_PLANE_BYTES);
+                        wgmma_fence();
 #pragma unroll
-                    for (int c0 = 0; c0 < 128; c0 += 16) {
-                        uint32_t r[16];
-                        tmem_ld16(taddr + c0, r);
-                        tmem_ld_wait();
+                        for (int k = 0; k < 4; ++k) {
+                            const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);   // +32 B per K step
+                            wgmma_ss<128>(acc, x_lo + koff, w_hi + koff, (dy | k) != 0);
+                            wgmma_ss<128>(acc, x_hi + koff, w_hi + koff, 1);
+                        }
 #pragma unroll
-                        for (int j = 0; j < 16; ++j) sum[c0 + j] = __fadd_rn(sum[c0 + j], __uint_as_float(r[j]));
+                        for (int k = 0; k < 4; ++k) {
+                            const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                            wgmma_ss<128>(acc, x_hi + koff, w_lo + koff, 1);
+                        }
+                        wgmma_commit();
+                        wgmma_wait_all();
+                        wgmma_fence_operands<64>(acc);
+                        __syncwarp();
+                        if (lane == 0) { mbar_arrive(&bar_wempty[ws]); mbar_arrive(&bar_wempty[ws2]); }
+                        ws = ws2 + 1; wph = wph2;
+                        if (ws == W_STAGES) { ws = 0; wph ^= 1; }
+                    }
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&bar_xempty[xs]);
+                    if (++xs == X_STAGES) { xs = 0; xph ^= 1; }
+                    if (!(p.dbg & 4)) {
+#pragma unroll
+                        for (int j = 0; j < 64; ++j) sum[j] = __fadd_rn(sum[j], acc[j]);
                     }
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&bar_tempty[acc]);
-                if (++acc == ACC2) { acc = 0; aph ^= 1; }
-            }
-            // BN scale/shift + ReLU + hi/lo fp16 split.  lane = channel; lanes 2j and 2j+1 exchange one packed (hi|lo)
-            // word per pixel pair so that each lane ends up with channels (2j, 2j+1) of ONE pixel: even lanes keep
-            // pixel cw, odd lanes pixel cw+1.  One half2 store per plane and lane = 2 x 64 contiguous bytes per warp.
-            const int hbase = th * T2_H + half * 8, wbase = tw * T2_W;
-            const int odd = lane & 1;
-            const int cpair = c & ~1;                                   // first channel of this lane's pair
-            const bool pair_ok = cpair < p.Cout;                         // Cout is even (host check)
-            bool range_bad = false;
+                // BN scale/shift + ReLU + hi/lo fp16 split.  This thread holds pixels m0 = 16 wl + lane/4 and m0 + 8 of
+                // the warpgroup's 64 (= rows 4 cg + m/16, column m % 16 of the half) and per 8-channel block j the
+                // channel pair 8j + 2(lane % 4): one 4-byte store per plane, a quad of lanes writes 16 contiguous bytes.
+                bool range_bad = false;
 #pragma unroll
-            for (int r = 0; r < 8; ++r) {
-                const int h = hbase + r;
-                if (h >= p.H) break;
-                const size_t rowpix = ((size_t)b * (p.H + 2) + (h + 1)) * (p.W + 2) + (wbase + 1);
-                __half *oh = p.out_hi + rowpix * p.out_stride + cpair;
-                __half *ol = p.out_lo + rowpix * p.out_stride + cpair;
+                for (int rh = 0; rh < 2; ++rh) {
+                    const int m = wl * 16 + (lane >> 2) + rh * 8;
+                    const int h = th * T2_H + hf * HALF_H + cg * 4 + m / T2_W, w = tw * T2_W + m % T2_W;
+                    if (h >= p.H || w >= p.W || (p.dbg & 8)) continue;
+                    const size_t pix = ((size_t)b * (p.H + 2) + (h + 1)) * (p.W + 2) + (w + 1);
+                    __half *oh = p.out_hi + pix * p.out_stride, *ol = p.out_lo + pix * p.out_stride;
 #pragma unroll
-                for (int cw = 0; cw < T2_W; cw += 2) {
-                    float x0 = fmaf(sum[r * 16 + cw], sc, sh), x1 = fmaf(sum[r * 16 + cw + 1], sc, sh);
-                    if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-                    range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
-                    const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
-                    const uint32_t recv = __shfl_xor_sync(0xffffffffu, odd ? p0 : p1, 1);
-                    // even lane: (own p0 = ch c, recv = ch c+1) of pixel cw; odd lane: (recv = ch c-1, own p1 = ch c) of cw+1
-                    const uint32_t a = odd ? recv : p0, bq = odd ? p1 : recv;
-                    const uint32_t hi2 = __byte_perm(a, bq, 0x5410), lo2 = __byte_perm(a, bq, 0x7632);
-                    const int col = cw + odd;
-                    if (pair_ok && wbase + col < p.W && !(p.dbg & 8)) {
-                        *reinterpret_cast<uint32_t *>(oh + (size_t)col * p.out_stride) = hi2;
-                        *reinterpret_cast<uint32_t *>(ol + (size_t)col * p.out_stride) = lo2;
+                    for (int j = 0; j < 16; ++j) {
+                        const int c = 8 * j + 2 * (lane & 3);
+                        if (c >= p.Cout) continue;                   // Cout is even (host check)
+                        float x0 = fmaf(sum[4 * j + 2 * rh], s_scale[c], s_shift[c]);
+                        float x1 = fmaf(sum[4 * j + 2 * rh + 1], s_scale[c + 1], s_shift[c + 1]);
+                        if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                        range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
+                        const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
+                        *reinterpret_cast<uint32_t *>(oh + c) = __byte_perm(p0, p1, 0x5410);
+                        *reinterpret_cast<uint32_t *>(ol + c) = __byte_perm(p0, p1, 0x7632);
                     }
                 }
+                if (range_bad && p.status) atomicOr(p.status, B2S_STATUS_F16_RANGE);
             }
-            if (range_bad && c_ok && p.status) atomicOr(p.status, B2S_STATUS_F16_RANGE);
             fill_bg(bg_quota);
         }
         fill_bg(my_bg);                                          // whatever is left (a CTA without work items: all of it)
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
     }
 }
 
@@ -392,20 +296,17 @@ int b2s_conv3x3_tc2(const __half *in_hi, const __half *in_lo, int B, int H, int 
     p.tiles_h = (H + T2_H - 1) / T2_H;
     p.tiles_w = (W + T2_W - 1) / T2_W;
     p.num_tiles = B * p.tiles_h * p.tiles_w;
-    p.last_half = (H % T2_H != 0 && H % T2_H <= T2_H / 2) ? 1 : 0;
     p.work_list = work_list; p.work_count = work_list ? work_count : nullptr;
     p.bg_list = bg_list; p.bg_count = bg_count; p.bg_hi = bg_hi; p.bg_lo = bg_lo;
     p.out_stride = out_stride;
     {
-        static int dbg = -1, deph = -1;
+        static int dbg = -1;
         if (dbg < 0) { const char *e = getenv("B2S_CONV2_DBG"); dbg = e ? atoi(e) : 0; }
-        if (deph < 0) { const char *e = getenv("B2S_CONV2_DEPHASE"); deph = e ? atoi(e) : 0; }
 #ifdef B2S_DIAG
         p.dbg = dbg;            // diagnostics that corrupt results exist only in `make DIAG=1` builds
 #else
         p.dbg = 0;
 #endif
-        p.dephase = deph;
     }
     p.scale = scale; p.shift = shift; p.out_hi = out_hi; p.out_lo = out_lo; p.status = status;
     const size_t smem = (size_t)X_STAGES * X_STAGE_BYTES + (size_t)W_STAGES * W_PLANE_BYTES + 1024;

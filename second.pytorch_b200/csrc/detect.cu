@@ -968,7 +968,7 @@ extern "C" int b2s_rotate_iou_eval(const float *boxes, int N, const float *query
     B2S_LAUNCH_OK();
     long long total = (long long)N * K;
     int blocks = b2s_cdiv(total, 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     k_rbbox_pairs<<<blocks, 256, 0, stream>>>(c, qc, nullptr, N, K, 0.f, criterion, out);
     B2S_LAUNCH_OK();
     return 0;
@@ -993,7 +993,7 @@ extern "C" int b2s_rbbox_overlap_host(const float *corners, const float *qcorner
     B2S_CUDA_OK(cudaMemcpy(si.p, standup_iou, sizeof(float) * (size_t)N * K, cudaMemcpyHostToDevice));
     long long total = (long long)N * K;
     int blocks = b2s_cdiv(total, 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     k_rbbox_pairs<<<blocks, 256>>>(c.as<float>(), qc.as<float>(), si.as<float>(), N, K, standup_thresh, criterion,
                                    o.as<float>());
     B2S_LAUNCH_OK();

@@ -137,7 +137,7 @@ extern "C" int b2s_transform_sweep(const float *points_in, int num_points, int f
     for (int i = 0; i < 9; ++i) m.r[i] = identity ? (i % 4 == 0 ? 1.0 : 0.0) : rotation_host[i];
     for (int i = 0; i < 3; ++i) m.t[i] = (identity || !translation_host) ? 0.0 : translation_host[i];
     int blocks = b2s_cdiv(num_points, kThreads);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     k_transform_sweep<<<blocks, kThreads, 0, stream>>>(points_in, num_points, feat_in, m, time_lag, identity, out);
     B2S_LAUNCH_OK();
     return 0;

@@ -140,7 +140,7 @@ extern "C" int b2s_rpn_bg_fill(const int *bg_list, const int *bg_count_dev, int 
                 "b2s_rpn_bg_fill: C must be a multiple of 8 whose chunk count divides 256");
     const int tiles_h = b2s_cdiv(H, TILE), tiles_w = b2s_cdiv(W, TILE);
     const int num_tiles = batch * tiles_h * tiles_w;
-    int blocks = num_tiles < 148 * 8 ? num_tiles : 148 * 8;
+    int blocks = num_tiles < 132 * 8 ? num_tiles : 132 * 8;
     k_bg_fill<<<blocks, 256, 0, stream>>>(bg_list, bg_count_dev, H, W, tiles_h, tiles_w, C,
                                           reinterpret_cast<const __half *>(f_hi), reinterpret_cast<const __half *>(f_lo),
                                           reinterpret_cast<__half *>(out_hi), reinterpret_cast<__half *>(out_lo), out_stride);

@@ -3,24 +3,19 @@
 //     heads = [conv_box | conv_cls | conv_dir_cls](y)   1x1, 128 -> <= 32 packed channels + bias  (rpn.py:386-420)
 // car.fhd / all.fhd: layer_nums [5], upsample_strides [1], num_upsample_filters [128].
 //
-// As two b2s_conv2d_tc launches y makes a round trip through HBM: 2 x 577 MB at 32 frames, the 1x1 stage was 0.41 ms of
-// a 5.4 ms step at 60-77 % of the HBM peak (profiles/, round 2).  Here y is produced into TMEM, gets its BN + ReLU +
-// hi/lo split in the epilogue warps' registers, goes BACK into tensor memory as packed fp16 pairs (tcgen05.st, lane =
-// pixel) and is the A operand of the second GEMM from there (tcgen05.mma with [a_tmem]): per 128-pixel tile the kernel
-// reads 64 KB of x and writes 16 KB of head records, instead of 208 KB of traffic.  Both weight sets (80 KB as hi/lo
-// planes) stay resident in shared memory and the rest of it is a 4-stage x ring (two tiles in flight).  (First version,
-// kept as B2S_RPN_TAIL_A=smem: y written to shared memory in the K-major SWIZZLE_128B layout -- that A tile costs 64 KB,
-// leaves an x ring of ONE tile, and the load latency of the next tile was exposed: 0.207 vs 0.172 ms.)  The MMA sequences, the epilogue arithmetic and the 3xF16 split are exactly those of k_conv_tc
+// As two b2s_conv2d_tc launches y makes a round trip through HBM (2 x 577 MB at 32 frames).  Here y never leaves the
+// SM: GEMM 1 accumulates it in the registers of the consumer warpgroup, BN + ReLU + the hi/lo split run on those
+// registers, and the packed fp16 pairs are directly the A operand of GEMM 2 (wgmma with A from registers: the
+// accumulator fragment of a 16-column block pair IS the A fragment of a 16-wide K step, no shuffle needed).  Per
+// 128-pixel tile the kernel reads 64 KB of x and writes 16 KB of head records, instead of 208 KB of traffic.  Both
+// weight sets (80 KB as hi/lo planes) stay resident in shared memory and the rest of it is a 4-slot x ring (two tiles
+// in flight).  The MMA sequences, the epilogue arithmetic and the 3xF16 split are exactly those of k_conv_tc
 // (conv_tc.cu) for the two layers, so the records are BIT-IDENTICAL to the two-launch path (tested).
 //
-// CTA = 8 warps, persistent over 8 x 16-pixel tiles:
-//   warp 0      TMA: weights once, then per tile the two 64-channel K blocks of x (hi + lo) into a 2-stage ring
-//   warp 1      MMA issuer (one elected lane): G1(i+1) is issued before G2(i), so the tensor pipe works on the next
-//               tile's first GEMM while the epilogue warps turn y(i) into the A operand
-//   warp 2      TMEM allocator (D1: 2 x 128 columns, D2: 32 columns)
-//   warps 4-11  epilogue, two groups of four (TMEM lane quarter = warp % 4): E1 = D1 -> BN/ReLU/split -> A2 (shared), group g
-//               takes the 64 channels of K block g; E2 = D2 -> + bias -> fp32 records (global), group g takes 16 columns.
-//               (With one group the epilogue was the longest stage of the per-tile chain.)
+// CTA = 3 warpgroups, persistent over 8 x 16-pixel tiles:
+//   warp 0            TMA: weights once, then per tile the two 64-channel K blocks of x (hi + lo) into the ring
+//   warpgroups 1, 2   consumers: warpgroup g owns tile pixels 64g .. 64g+63 through GEMM 1, the y epilogue, GEMM 2
+//                     and the record stores
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -32,9 +27,16 @@ constexpr int TILE_H = 8, TILE_W = 16;    // BLOCK_M = 128 pixels
 constexpr int C = 128;                    // channels of x and y
 constexpr int KB = C / BLOCK_K;           // 2 K blocks of 64 channels
 constexpr int N1 = 128;                   // GEMM 1 N (= channels of y)
-constexpr int kThreads = 384;              // 4 control warps + 2 x 4 epilogue warps
+constexpr int N2 = 32;                    // GEMM 2 N (packed head channels, zero padded)
+constexpr int kThreads = 384;             // 1 producer warpgroup + 2 consumer warpgroups
+constexpr int XS = 2 * KB;                // x ring slots (one K block of one tile each)
 constexpr uint32_t W1_KB_BYTES = 2 * N1 * BLOCK_K * ELEM_BYTES;        // hi + lo of one K block: 32 KB
+constexpr uint32_t W2_KB_BYTES = 2 * N2 * BLOCK_K * ELEM_BYTES;        // hi + lo of one K block of the head weights: 8 KB
 constexpr uint32_t X_STAGE_BYTES = 2 * A_TILE_BYTES;                   // hi + lo of one K block of x: 32 KB
+constexpr uint32_t OFF_W1 = 0, OFF_W2 = OFF_W1 + KB * W1_KB_BYTES, OFF_X = OFF_W2 + KB * W2_KB_BYTES;
+constexpr size_t SMEM_BYTES = OFF_X + XS * X_STAGE_BYTES + 1024;
+static_assert((OFF_W2 % 1024) == 0 && (OFF_X % 1024) == 0 && (W2_KB_BYTES / 2) % 1024 == 0,
+              "operand tiles are 1024-byte aligned (SWIZZLE_128B)");
 
 struct TailParams {
     int B, H, W, tiles_h, tiles_w, num_tiles;
@@ -44,45 +46,15 @@ struct TailParams {
     int *status;
 };
 
-// A operand of GEMM 2 straight from tensor memory (tcgen05.mma with [a_tmem]); 32 bits hold two consecutive channels
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t *r)
-{
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-                 ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
-}
-
-// ATM = false: y goes to SHARED memory as the K-major SWIZZLE_128B A tile of GEMM 2 (64 KB), the x ring holds one tile.
-// ATM = true : y goes back to TENSOR memory (fp16 hi/lo pairs, lane = pixel) and GEMM 2 reads its A operand from there; the
-//              64 KB of shared memory become two more x stages, so the next tile's x is in flight during the whole tile.
-template <int N2, bool ATM>
 __global__ void __launch_bounds__(kThreads, 1)
 k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
            const __grid_constant__ CUtensorMap map_w1_hi, const __grid_constant__ CUtensorMap map_w1_lo,
            const __grid_constant__ CUtensorMap map_w2_hi, const __grid_constant__ CUtensorMap map_w2_lo,
            const TailParams p)
 {
-    constexpr uint32_t W2_KB_BYTES = 2 * N2 * BLOCK_K * ELEM_BYTES;    // hi + lo of one K block of the head weights
-    constexpr uint32_t OFF_W1 = 0, OFF_W2 = OFF_W1 + KB * W1_KB_BYTES, OFF_X = OFF_W2 + KB * W2_KB_BYTES;
-    constexpr int XS = ATM ? 2 * KB : KB;                              // x ring stages (one K block of one tile each)
-    constexpr uint32_t OFF_A2 = OFF_X + KB * X_STAGE_BYTES;            // (!ATM) y as the A operand: KB x (hi 16 KB | lo 16 KB)
-    constexpr uint32_t TMEM_COLS = 512;                                // D1[0] at column 0, D1[1] at 128, D2 at 256 (N2)
-    constexpr uint32_t A2_HI_COL = 320, A2_LO_COL = 384;               // (ATM) y hi / lo: 32 columns per K block
-    static_assert(N2 % 16 == 0 && N2 >= 16 && N2 <= 64 && (OFF_W2 % 1024) == 0 && (OFF_X % 1024) == 0 && (OFF_A2 % 1024) == 0,
-                  "operand tiles are 1024-byte aligned (SWIZZLE_128B)");
-
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    __shared__ __align__(8) uint64_t bar_w, bar_xfull[XS], bar_xempty[XS], bar_d1full[2], bar_d1empty[2], bar_a2full,
-        bar_a2empty, bar_d2full, bar_d2empty;
-    __shared__ uint32_t s_tmem_base;
+    __shared__ __align__(8) uint64_t bar_w, bar_xfull[XS], bar_xempty[XS];
     __shared__ float s_scale1[N1], s_shift1[N1], s_scale2[N2], s_shift2[N2];
 
     const int warp = warp_idx_uniform(), lane = threadIdx.x & 31;
@@ -97,21 +69,10 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
     }
     if (warp == 1 && lane == 0) {
         mbar_init(&bar_w, 1);
-        for (int i = 0; i < XS; ++i) { mbar_init(&bar_xfull[i], 1); mbar_init(&bar_xempty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&bar_d1full[i], 1); mbar_init(&bar_d1empty[i], 8); }
-        mbar_init(&bar_a2full, 8); mbar_init(&bar_a2empty, 1);
-        mbar_init(&bar_d2full, 1); mbar_init(&bar_d2empty, 8);
+        for (int i = 0; i < XS; ++i) { mbar_init(&bar_xfull[i], 1); mbar_init(&bar_xempty[i], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)),
-                     "r"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = s_tmem_base;
     const int my_tiles = (int)blockIdx.x < p.num_tiles ? (p.num_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
 
     if (warp == 0) {
@@ -138,164 +99,92 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc1 = make_idesc_f16(N1), idesc2 = make_idesc_f16(N2);
-        const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint32_t smem0 = smem_u32(smem);
-        const int n_tiles_u = __shfl_sync(0xffffffffu, my_tiles, 0);
-        if (elect_one_sync() && n_tiles_u > 0) {
-            const uint32_t d2 = tmem_u + 256;
-            // per K step the three products of the 3xF16 split, in k_conv_tc's order: A_lo*B_hi, A_hi*B_lo, A_hi*B_hi
-            auto gemm = [&](uint32_t tmem_d, uint32_t a_base, uint32_t b_base, uint32_t b_plane_bytes, uint32_t idesc, int kb) {
-                const uint64_t a_hi = make_desc_sw128(a_base), a_lo = make_desc_sw128(a_base + A_TILE_BYTES);
-                const uint64_t b_hi = make_desc_sw128(b_base), b_lo = make_desc_sw128(b_base + b_plane_bytes);
-#pragma unroll
-                for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                    const uint64_t koff = (uint64_t)((k * UMMA_K * ELEM_BYTES) >> 4);
-                    umma_f16(tmem_d, a_lo + koff, b_hi + koff, idesc, (kb | k) != 0);
-                    umma_f16(tmem_d, a_hi + koff, b_lo + koff, idesc, 1);
-                    umma_f16(tmem_d, a_hi + koff, b_hi + koff, idesc, 1);
-                }
-            };
-            auto g1 = [&](int i) {           // D1[i & 1] = x(tile i) * W1^T
-                const uint32_t d1 = tmem_u + (uint32_t)(i & 1) * 128u;
-                mbar_wait(&bar_d1empty[i & 1], (uint32_t)((i >> 1) & 1) ^ 1u);      // E1(i-2) has read this accumulator
-                for (int kb = 0; kb < KB; ++kb) {
-                    const int u = i * KB + kb, slot = u % XS;
-                    mbar_wait(&bar_xfull[slot], (uint32_t)((u / XS) & 1));
-                    tc_fence_after();
-                    gemm(d1, smem0 + OFF_X + slot * X_STAGE_BYTES, smem0 + OFF_W1 + kb * W1_KB_BYTES, W1_KB_BYTES / 2, idesc1, kb);
-                    umma_commit(&bar_xempty[slot]);
-                }
-                umma_commit(&bar_d1full[i & 1]);
-            };
-            mbar_wait(&bar_w, 0);
-            tc_fence_after();
-            g1(0);
-            for (int i = 0; i < n_tiles_u; ++i) {
-                if (i + 1 < n_tiles_u) g1(i + 1);
-                // D2 = y(tile i) * W2^T, A operand written to shared memory by the epilogue warps
-                mbar_wait(&bar_d2empty, (uint32_t)(i & 1) ^ 1u);          // E2(i-1) has read D2
-                mbar_wait(&bar_a2full, (uint32_t)(i & 1));
-                tc_fence_after();
-                if constexpr (ATM) {
-                    for (int kb = 0; kb < KB; ++kb) {
-                        const uint32_t b_base = smem0 + OFF_W2 + kb * W2_KB_BYTES;
-                        const uint64_t b_hi = make_desc_sw128(b_base), b_lo = make_desc_sw128(b_base + W2_KB_BYTES / 2);
-#pragma unroll
-                        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                            const uint64_t koff = (uint64_t)((k * UMMA_K * ELEM_BYTES) >> 4);
-                            const uint32_t a_hi = tmem_u + A2_HI_COL + (uint32_t)(kb * (BLOCK_K / 2) + k * (UMMA_K / 2));
-                            const uint32_t a_lo = tmem_u + A2_LO_COL + (uint32_t)(kb * (BLOCK_K / 2) + k * (UMMA_K / 2));
-                            umma_f16_ts(d2, a_lo, b_hi + koff, idesc2, (kb | k) != 0);
-                            umma_f16_ts(d2, a_hi, b_lo + koff, idesc2, 1);
-                            umma_f16_ts(d2, a_hi, b_hi + koff, idesc2, 1);
-                        }
-                    }
-                } else {
-                    for (int kb = 0; kb < KB; ++kb)
-                        gemm(d2, smem0 + OFF_A2 + kb * X_STAGE_BYTES, smem0 + OFF_W2 + kb * W2_KB_BYTES, W2_KB_BYTES / 2, idesc2, kb);
-                }
-                umma_commit(&bar_a2empty);
-                umma_commit(&bar_d2full);
-            }
-        }
-        __syncwarp();
     } else if (warp >= 4) {
-        // ===================== epilogue =====================
-        const int ew = (warp - 4) & 3;                             // TMEM lane quarter; this thread owns tile pixel m
-        const int grp = (warp - 4) >> 2;                           // 0 / 1: which half of the channels / columns
-        static_assert(KB == 2 && N2 == 32, "two epilogue groups: one K block of y and 16 head columns each");
-        const int m = ew * 32 + lane;
-        const uint32_t row_off = (uint32_t)m * 128u, sw = (uint32_t)(m & 7);
+        // ===================== consumers =====================
+        const int cg = (warp >> 2) - 1;                          // tile pixels 64 cg .. 64 cg + 63
+        const int wl = warp & 3;
+        const uint32_t smem0 = smem_u32(smem);
+        const uint32_t a_off = (uint32_t)cg * 64u * 128u;
         bool range_bad = false;
-        int i = 0;
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++i) {
+        mbar_wait(&bar_w, 0);
+        int u = 0;
+        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
             const int tw = tile % p.tiles_w, th = (tile / p.tiles_w) % p.tiles_h, b = tile / (p.tiles_w * p.tiles_h);
-            // ---- E1: y = relu(D1 * scale1 + shift1) -> fp16 hi/lo -> the A tile of GEMM 2 (K-major, SWIZZLE_128B)
-            mbar_wait(&bar_d1full[i & 1], (uint32_t)((i >> 1) & 1));
-            tc_fence_after();
-            mbar_wait(&bar_a2empty, (uint32_t)(i & 1) ^ 1u);       // GEMM 2 of the previous tile has read the A tile
-            const uint32_t tlane = tmem_base + ((uint32_t)(ew * 32) << 16);
-            const uint32_t taddr = tlane + (uint32_t)(i & 1) * 128u;
-            {
-                const int kb = grp;
-                uint8_t *a2 = smem + OFF_A2 + kb * X_STAGE_BYTES;
+            // ---- GEMM 1: D1 = x * W1^T; per K step the three products of the 3xF16 split in k_conv_tc's order
+            float d1[N1 / 2];
+            for (int kb = 0; kb < KB; ++kb) {
+                const int slot = (u + kb) % XS;
+                mbar_wait(&bar_xfull[slot], (uint32_t)(((u + kb) / XS) & 1));
+                const uint32_t xa = smem0 + OFF_X + slot * X_STAGE_BYTES + a_off;
+                const uint32_t wb = smem0 + OFF_W1 + kb * W1_KB_BYTES;
+                const uint64_t a_hi = make_desc_sw128(xa), a_lo = make_desc_sw128(xa + A_TILE_BYTES);
+                const uint64_t b_hi = make_desc_sw128(wb), b_lo = make_desc_sw128(wb + W1_KB_BYTES / 2);
+                wgmma_fence();
 #pragma unroll
-                for (int c0 = 0; c0 < BLOCK_K; c0 += 16) {
-                    uint32_t r[16];
-                    uint32_t hi8[8], lo8[8];
-                    tmem_ld16(taddr + kb * BLOCK_K + c0, r);
-                    tmem_ld_wait();
+                for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+                    const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                    wgmma_ss<N1>(d1, a_lo + koff, b_hi + koff, (kb | k) != 0);
+                    wgmma_ss<N1>(d1, a_hi + koff, b_lo + koff, 1);
+                    wgmma_ss<N1>(d1, a_hi + koff, b_hi + koff, 1);
+                }
+                wgmma_commit();
+            }
+            wgmma_wait_all();
+            wgmma_fence_operands<N1 / 2>(d1);
+            __syncwarp();
+            if (lane == 0)
+                for (int kb = 0; kb < KB; ++kb) mbar_arrive(&bar_xempty[(u + kb) % XS]);
+            u += KB;
+            // ---- y = relu(D1 * scale1 + shift1) -> fp16 hi/lo pairs = the A fragments of GEMM 2.  K step s covers
+            // channels 16s .. 16s+15 = accumulator blocks 2s, 2s+1: a[0] = block 2s row r, a[1] = block 2s row r+8,
+            // a[2] / a[3] = block 2s+1 rows r / r+8.
+            uint32_t yh[N1 / 4], yl[N1 / 4];
 #pragma unroll
-                    for (int h8 = 0; h8 < 2; ++h8) {               // 8 channels = one 16-byte chunk of each plane
-                        uint32_t hw[4], lw[4];
+            for (int i = 0; i < N1 / 4; ++i) {
+                const int blk = i >> 1;                            // 8-column block of register pair i
+                const int c = 8 * blk + 2 * (lane & 3);
+                float x0 = fmaf(__fadd_rn(0.f, d1[2 * i]), s_scale1[c], s_shift1[c]);
+                float x1 = fmaf(__fadd_rn(0.f, d1[2 * i + 1]), s_scale1[c + 1], s_shift1[c + 1]);
+                x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f);
+                range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
+                const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
+                yh[i] = __byte_perm(p0, p1, 0x5410);
+                yl[i] = __byte_perm(p0, p1, 0x7632);
+            }
+            // ---- GEMM 2: D2 = y * W2^T (A from registers)
+            float d2[N2 / 2];
+            wgmma_fence();
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const int c = kb * BLOCK_K + c0 + h8 * 8 + 2 * j;
-                            float x0 = fmaf(__fadd_rn(0.f, __uint_as_float(r[h8 * 8 + 2 * j])), s_scale1[c], s_shift1[c]);
-                            float x1 = fmaf(__fadd_rn(0.f, __uint_as_float(r[h8 * 8 + 2 * j + 1])), s_scale1[c + 1], s_shift1[c + 1]);
-                            x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f);
-                            range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
-                            const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
-                            hw[j] = __byte_perm(p0, p1, 0x5410);
-                            lw[j] = __byte_perm(p0, p1, 0x7632);
-                        }
-                        if constexpr (ATM) {
+            for (int s = 0; s < C / MMA_K; ++s) {
+                const int kb = s / (BLOCK_K / MMA_K), k = s % (BLOCK_K / MMA_K);
+                const uint32_t wb = smem0 + OFF_W2 + kb * W2_KB_BYTES;
+                const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                const uint64_t b_hi = make_desc_sw128(wb) + koff, b_lo = make_desc_sw128(wb + W2_KB_BYTES / 2) + koff;
+                wgmma_rs<N2>(d2, &yl[4 * s], b_hi, s != 0);
+                wgmma_rs<N2>(d2, &yh[4 * s], b_lo, 1);
+                wgmma_rs<N2>(d2, &yh[4 * s], b_hi, 1);
+            }
+            wgmma_commit();
+            wgmma_wait_all();
+            wgmma_fence_operands<N2 / 2>(d2);
+            // ---- records = D2 * scale2 + shift2 (bias) -> fp32 [B, H, W, out_stride]
 #pragma unroll
-                            for (int j = 0; j < 4; ++j) { hi8[h8 * 4 + j] = hw[j]; lo8[h8 * 4 + j] = lw[j]; }
-                        } else {
-                            const uint32_t chunk = (uint32_t)(c0 / 8 + h8);
-                            const uint32_t off = row_off + ((chunk ^ sw) << 4);
-                            *reinterpret_cast<uint4 *>(a2 + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                            *reinterpret_cast<uint4 *>(a2 + A_TILE_BYTES + off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                        }
-                    }
-                    if constexpr (ATM) {         // 16 channels = 8 packed columns of each plane, this lane's row
-                        tmem_st8(tlane + A2_HI_COL + (uint32_t)(kb * (BLOCK_K / 2) + c0 / 2), hi8);
-                        tmem_st8(tlane + A2_LO_COL + (uint32_t)(kb * (BLOCK_K / 2) + c0 / 2), lo8);
-                    }
+            for (int rh = 0; rh < 2; ++rh) {
+                const int m = cg * 64 + wl * 16 + (lane >> 2) + rh * 8;
+                const int hh = th * TILE_H + m / TILE_W, ww = tw * TILE_W + m % TILE_W;
+                if (hh >= p.H || ww >= p.W) continue;
+                float *outp = p.out + (((size_t)b * p.H + hh) * p.W + ww) * p.out_stride;
+#pragma unroll
+                for (int j = 0; j < N2 / 8; ++j) {
+                    const int c = 8 * j + 2 * (lane & 3);
+                    if (c >= p.cout2) continue;                  // cout2 is a multiple of 4
+                    const float v0 = fmaf(__fadd_rn(0.f, d2[4 * j + 2 * rh]), s_scale2[c], s_shift2[c]);
+                    const float v1 = fmaf(__fadd_rn(0.f, d2[4 * j + 2 * rh + 1]), s_scale2[c + 1], s_shift2[c + 1]);
+                    *reinterpret_cast<float2 *>(outp + c) = make_float2(v0, v1);
                 }
             }
-            if constexpr (ATM) asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            tc_fence_before();
-            if constexpr (!ATM) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the MMA
-            __syncwarp();
-            if (lane == 0) { mbar_arrive(&bar_d1empty[i & 1]); mbar_arrive(&bar_a2full); }
-            // ---- E2: records = D2 * scale2 + shift2 (bias) -> fp32 [B, H, W, out_stride]
-            mbar_wait(&bar_d2full, (uint32_t)(i & 1));
-            tc_fence_after();
-            const int hh = th * TILE_H + m / TILE_W, ww = tw * TILE_W + m % TILE_W;
-            const bool ok = hh < p.H && ww < p.W;
-            float *outp = p.out + (((size_t)b * p.H + hh) * p.W + ww) * p.out_stride;
-            {
-                const int c0 = grp * 16;
-                uint32_t r[16];
-                tmem_ld16(tlane + 256 + c0, r);
-                tmem_ld_wait();
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    float v[4];
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const int c = c0 + q * 4 + j;
-                        v[j] = fmaf(__fadd_rn(0.f, __uint_as_float(r[q * 4 + j])), s_scale2[c], s_shift2[c]);
-                    }
-                    if (ok && c0 + q * 4 < p.cout2) *reinterpret_cast<float4 *>(outp + c0 + q * 4) = make_float4(v[0], v[1], v[2], v[3]);
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bar_d2empty);
         }
         if (__any_sync(0xffffffffu, range_bad) && lane == 0 && p.status) atomicOr(p.status, B2S_STATUS_F16_RANGE);
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
     }
 }
 
@@ -311,7 +200,7 @@ extern "C" int b2s_rpn_tail_tc(const b2s_half *in_hi, const b2s_half *in_lo, int
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     B2S_REQUIRE(Cin == C && Cmid == N1, "b2s_rpn_tail_tc: built for a 128 -> 128 deblock (got %d -> %d)", Cin, Cmid);
-    B2S_REQUIRE(n_pad2 == 32 && cout2 >= 4 && cout2 <= n_pad2 && cout2 % 4 == 0 && out_stride >= cout2 && out_stride % 4 == 0,
+    B2S_REQUIRE(n_pad2 == N2 && cout2 >= 4 && cout2 <= n_pad2 && cout2 % 4 == 0 && out_stride >= cout2 && out_stride % 4 == 0,
                 "b2s_rpn_tail_tc: up to 32 packed head channels (multiple of 4), out_stride a multiple of 4");
     B2S_REQUIRE(B >= 1 && H >= 1 && W >= 1 && ((uintptr_t)out & 15) == 0, "b2s_rpn_tail_tc: bad sizes / unaligned output");
     CUtensorMap x_hi, x_lo, m1_hi, m1_lo, m2_hi, m2_lo;
@@ -342,18 +231,10 @@ extern "C" int b2s_rpn_tail_tc(const b2s_half *in_hi, const b2s_half *in_lo, int
     p.cout2 = cout2; p.out_stride = out_stride;
     p.scale1 = scale1; p.shift1 = shift1; p.scale2 = scale2; p.shift2 = shift2;
     p.out = out; p.status = (int *)status_dev;
-    constexpr size_t smem = KB * (W1_KB_BYTES + 2 * 32 * BLOCK_K * ELEM_BYTES) + 2 * KB * X_STAGE_BYTES + 1024;
     const int num_sms = num_sms_current();
     const int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-    static int atm = -1;        // B2S_RPN_TAIL_A = tmem (default) | smem: where GEMM 2 reads y from (see k_rpn_tail)
-    if (atm < 0) { const char *e = getenv("B2S_RPN_TAIL_A"); atm = (e && e[0] == 's') ? 0 : 1; }
-    if (atm) {
-        B2S_SMEM_OPT_IN((k_rpn_tail<32, true>), smem);
-        k_rpn_tail<32, true><<<grid, kThreads, smem, stream>>>(x_hi, x_lo, m1_hi, m1_lo, m2_hi, m2_lo, p);
-    } else {
-        B2S_SMEM_OPT_IN((k_rpn_tail<32, false>), smem);
-        k_rpn_tail<32, false><<<grid, kThreads, smem, stream>>>(x_hi, x_lo, m1_hi, m1_lo, m2_hi, m2_lo, p);
-    }
+    B2S_SMEM_OPT_IN(k_rpn_tail, SMEM_BYTES);
+    k_rpn_tail<<<grid, kThreads, SMEM_BYTES, stream>>>(x_hi, x_lo, m1_hi, m1_lo, m2_hi, m2_lo, p);
     B2S_LAUNCH_OK();
     return 0;
 }

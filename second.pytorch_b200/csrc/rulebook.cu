@@ -28,7 +28,7 @@ namespace {
 
 constexpr int kThreads = 256;
 constexpr int kScanThreads = 1024;
-constexpr int kMaxBlocks = 148 * 8;
+constexpr int kMaxBlocks = 132 * 8;
 
 inline int bounded_grid(long long work_items, int threads)
 {

@@ -1,38 +1,32 @@
 // sparse_conv_tc.cu -- sparse convolution inner product on the tensor pipe (b2s_sparse_conv_tc, b2s_sparse_conv_tc_plan).
 //
-// Output-stationary like sparse_conv.cu (one CTA owns 128 output rows = one tcgen05 accumulator; nbr[o][k] names the
-// input row feeding output row o through kernel offset k), but the per-offset product
+// Output-stationary like sparse_conv.cu (one CTA owns 128 output rows at a time; nbr[o][k] names the input row feeding
+// output row o through kernel offset k), but the per-offset product
 //     D[128 rows, Cout] += A[128 gathered rows, 64 channels] * W[k][Cout, 64 channels]^T
-// is a tcgen05.mma (kind::f16) on the 3xF16 hi/lo split (tc_common.cuh), accumulating in TMEM.
+// is a wgmma (f16 -> f32) on the 3xF16 hi/lo split (tc_common.cuh), accumulating in registers.
 //
 // K block = one 128-byte-wide slice of the reduction (64 fp16 channels) = PACK = 64/Cin consecutive kernel offsets
 // side by side (Cin = 64: one offset; 32: 2; 16: 4; 8: 8; the weights arrive pre-packed as [K block][Cout][64], see
 // b2second/tc.py: pack_sparse_weights; a 3- or 4-feature input layer is zero-padded to 8 channels).
 //
-// Tile plan (round 2, sparse_plan.cu): tile_mask[tile] says which kernel offsets ANY of the tile's 128 rows needs; a K
-// block none of whose offsets is needed is skipped by every role (weights not loaded, rows not gathered, MMAs not
-// issued).  perm[] (optional) makes a tile = 128 rows with a similar neighbourhood shape, which roughly halves the
-// K blocks of the SECOND middle encoder.  A missing neighbour contributes exact zeros and the accumulation chains have
-// FIXED K-block boundaries (chain c = K blocks [c*CHAIN_KB, (c+1)*CHAIN_KB)), so the value of an output row does not
-// depend on which rows share its tile: planned, unplanned and round-1 results are bit-identical.
+// Tile plan (sparse_plan.cu): tile_mask[tile] says which kernel offsets ANY of the tile's 128 rows needs; a K block
+// none of whose offsets is needed is skipped by every role (weights not loaded, rows not gathered, MMAs not issued).
+// perm[] (optional) makes a tile = 128 rows with a similar neighbourhood shape, which roughly halves the K blocks of the
+// SECOND middle encoder.  A missing neighbour contributes exact zeros and the accumulation chains have FIXED K-block
+// boundaries (chain c = K blocks [c*CHAIN_KB, (c+1)*CHAIN_KB)), so the value of an output row does not depend on which
+// rows share its tile: planned and unplanned results are bit-identical.
 //
 // Warp roles (16 warps):
-//   warp 0      TMA producer for the weight tile of each K block (bulk tensor load, SWIZZLE_128B)
-//   warp 1      MMA issuer (one elected lane; see the comment at the role)
-//   warp 2      TMEM allocator
-//   warps 4-11  gather producers.  Gather warp w OWNS pipeline stage w % 4 and the tile's row half w / 4: it handles
+//   warps 0-7   gather producers.  Gather warp w OWNS pipeline stage w % 4 and the tile's row half w / 4: it handles
 //               every 4th K block, all 16-byte cp.async copies of its 64 rows (hi and lo planes) into the K-major
 //               SWIZZLE_128B A tile, zero-fill for missing neighbours, completion signalled on the stage's mbarrier
 //               with cp.async.mbarrier.arrive.noinc.  The neighbour-table entries of the NEXT owned K block are
 //               loaded (straight from global / L1) before the current one is waited for.
-//               History: in round 1 all 8 warps worked on EVERY K block (16 rows each) behind a shared-memory copy of
-//               the tile's table; that variant rebuilt with this round's copy loop is the OWN = 1 instantiation
-//               (1.5x slower than stage ownership).  A TMA tile::gather4 producer was tried in round 1
-//               (tests/cuda/gather4_probe.cu): 3x slower than cp.async.  What does and does not bound this kernel is
-//               in DESIGN.md section 7 (eleven measured variants, tools/experiments/README.md).
-//   warps 12-15 epilogue: drain per-chain partial sums from TMEM (round-to-nearest adds in registers, the
-//               tensor core's own accumulate is not RN -- see conv_tc.cu), BN scale/shift + ReLU, hi/lo split,
-//               coalesced row stores through a small staging tile
+//   warps 8-15  two consumer warpgroups: warpgroup g issues the wgmmas of tile rows 64g .. 64g+63 and owns their
+//               accumulators; per-chain partial sums go into fp32 running sums with round-to-nearest adds (the tensor
+//               core's own accumulate is not RN -- see conv_tc.cu), then BN scale/shift + ReLU, hi/lo split, stores.
+//               Lane 0 of warp 8 also issues the weight tile of each K block (bulk tensor load, SWIZZLE_128B) as soon as
+//               its stage is free, STAGES K blocks ahead of the MMAs.
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -40,38 +34,16 @@
 namespace {
 
 using namespace b2s_tc;
-// pipeline stages: 4 x (32 KB of gathered rows + 256 N bytes of weights).  Five stages for the narrow layers (N <= 32 fits)
-// were tried in round 2: not faster (the ring is not what bounds the kernel) and not validated -- kept at 4 everywhere.
-__host__ __device__ constexpr int stages_for(int /*n*/) { return 4; }
-// GW gather warps (warps 4 .. 4+GW-1), the epilogue is the 4 warps after them.  GW = 16 (24 warps) needs the register
-// file rebalanced between the roles with setmaxnreg (inside each role's branch, where ptxas honours it): 768 threads
-// start with 80 registers each; the gather warps drop to 64 and the epilogue warps (64 running sums + staging) rise to 144.
-// gather ownership: OWN = 4: warp w owns every 4th K block (pairs of warps share a K block, 64 rows each);
-//                   OWN = 1: all 8 warps work on every K block (16 rows each)
+// pipeline stages: 4 x (32 KB of gathered rows + 256 N bytes of weights)
+constexpr int STAGES = 4;
+// GW gather warps with stage ownership: warp w owns every OWN-th K block (pairs of warps share a K block, 64 rows each)
+constexpr int GW = 8, OWN = 4;
+constexpr int kThreads = 32 * (GW + 8);   // the gather warps, then two consumer warpgroups
 constexpr int GROUP = 3;                  // kernel offsets per accumulation chain (Cin = 64)
-constexpr int ACC_SLOTS = 4;
 
-__device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void *gsrc, uint32_t src_bytes)
-{
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_dst), "l"(gsrc), "r"(src_bytes) : "memory");
-}
 __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t *bar)
 {
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// non-blocking poll (mbarrier.test_wait never suspends the thread)
-__device__ __forceinline__ void mbar_wait_spin(uint64_t *bar, uint32_t parity)
-{
-    const uint32_t addr = smem_u32(bar);
-#pragma unroll 1
-    for (uint32_t it = 0; it < (1u << 30); ++it) {
-        uint32_t done;
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-        if (done) return;
-    }
-    __trap();
 }
 
 // warp-level wait: only lane 0 polls the barrier (32 lanes spinning on try_wait are 32 shared-memory operations per
@@ -86,13 +58,6 @@ __device__ __forceinline__ void mbar_wait_warp(uint64_t *bar, uint32_t parity, b
     }
 }
 
-#ifdef B2S_DIAG
-// make DIAG=1 + B2S_SP_ZSKIP bit 64: per-K-block clock64 stamps of every role of CTA 0 (K blocks 0..127), printed at exit
-__device__ long long g_trace[10][128];
-#define B2S_TRACE(ROLE, G) do { if ((p.flags & 64) && blockIdx.x == 0 && (G) < 128 && ((ROLE) < 5 || (threadIdx.x & 31) == 0)) g_trace[ROLE][G] = clock64(); } while (0)
-#else
-#define B2S_TRACE(ROLE, G) do { } while (0)
-#endif
 
 // read-only load the compiler may not move (volatile asm keeps its place among the other volatile asm statements: the
 // copies, the barrier operations).  The neighbour-table entries of the NEXT owned K block must be in flight while the
@@ -114,7 +79,7 @@ struct SpParams {
     const int *perm;             // tile position -> output row (NULL: identity)
     const unsigned *tile_mask;   // per 128-position tile: kernel offsets some row of the tile has (NULL: all)
     int cap_out, K, relu;
-    int flags;                   // B2S_SP_ZSKIP: bit 0 zero-slot skip (default on); 16 print the issuer's wait times
+    int flags;                   // B2S_SP_ZSKIP: bit 0 zero-slot skip (default on); 32 lane-0 polling with a sleeping wait
     const float *scale, *shift;
     void *out_hi;                // fp16 hi plane, or (out_lo == NULL) fp32 rows [cap_out, COUT]
     __half *out_lo;
@@ -138,16 +103,13 @@ __device__ __forceinline__ uint32_t kb_mask_of(uint32_t offsets, int num_kb)
     return m ? m : 1u;
 }
 
-// CIN in {8, 16, 32, 64}; COUT (= UMMA N) in {16, 32, 64}
-template <int CIN, int COUT, int OWN, int GW>
-__global__ void __launch_bounds__(32 * (4 + GW + 4), 1)
+// CIN in {8, 16, 32, 64}; COUT in {16, 32, 64}
+template <int CIN, int COUT>
+__global__ void __launch_bounds__(kThreads, 1)
 k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
                  const SpParams p)
 {
     constexpr int N = COUT;
-    constexpr int STAGES = stages_for(COUT);
-    static_assert(STAGES == 4, "only the 4-stage ring is validated");
-    static_assert(GW == 8 || GW == 16, "thread layout");
     constexpr int HALVES = GW / OWN;          // gather warps sharing one K block (each takes BLOCK_M / HALVES rows)
     constexpr int RI = BLOCK_M / HALVES / 4;  // 4-row copy iterations per gather warp and K block
     static_assert(GW % OWN == 0 && RI * 4 * HALVES == BLOCK_M && (OWN & (OWN - 1)) == 0 && RI * STAGES <= 128, "gather warp layout");
@@ -158,20 +120,17 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
     constexpr uint32_t CHAIN_BITS = (1u << CHAIN_KB) - 1u;
     constexpr uint32_t B_TILE_BYTES = N * BLOCK_K * ELEM_BYTES;
     constexpr uint32_t STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-    // B-operand concatenation: the stage holds W_hi (N rows) directly followed by W_lo (N rows), so ONE MMA with
-    // UMMA N = 2N computes A_hi*W_hi (accumulator columns [0,N)) and A_hi*W_lo (columns [N,2N)); a second MMA
-    // (UMMA N = N) adds A_lo*W_hi into columns [0,N).  8 instead of 12 MMAs per K block for the same products
-    // (tests/cuda/mma_probe2.cu: 448 instead of 576 tensor cycles at N = 64).  The epilogue adds the two halves.
-    constexpr int ACC_W = 2 * N;                              // accumulator slot width in TMEM columns
-    constexpr uint32_t TMEM_COLS = (ACC_SLOTS * ACC_W <= 128) ? 128 : (ACC_SLOTS * ACC_W <= 256) ? 256 : 512;
-    static_assert(N % 16 == 0 && ACC_SLOTS * ACC_W <= 512, "TMEM capacity");
+    // B-operand concatenation: the stage holds W_hi (N rows) directly followed by W_lo (N rows), so ONE wgmma with
+    // N' = 2N computes A_hi*W_hi (accumulator columns [0,N)) and A_hi*W_lo (columns [N,2N)); a second one (N' = N, the
+    // first half of the same accumulator registers) adds A_lo*W_hi into columns [0,N).  8 instead of 12 MMAs per K block
+    // for the same products.  The drain adds the two halves.
+    constexpr int R = N;                                      // accumulator registers per thread: 64 rows x 2N
+    static_assert(N % 16 == 0 && B_TILE_BYTES % 1024 == 0, "wgmma N / swizzle atoms");
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    __shared__ __align__(8) uint64_t bar_full[STAGES], bar_empty[STAGES], bar_tfull[ACC_SLOTS], bar_tempty[ACC_SLOTS];
-    __shared__ uint32_t s_tmem_base;
+    __shared__ __align__(8) uint64_t bar_full[STAGES], bar_empty[STAGES];
     __shared__ float s_scale[N], s_shift[N];
-    __shared__ __align__(16) uint32_t s_stage[4][32 * 36];   // per epilogue warp: 32 rows x 32 words transpose tile
 
     const int warp = warp_idx_uniform(), lane = threadIdx.x & 31;
     const int n_out = min(*p.n_out_dev, p.cap_out);
@@ -179,7 +138,7 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
     const int K = p.K;
     const int num_kb = (K + PACK - 1) / PACK;
     const int num_chains = (num_kb + CHAIN_KB - 1) / CHAIN_KB;
-    const bool poll1 = (p.flags & 32) != 0;                 // B2S_SP_ZSKIP bit 32: lane 0 polls with a sleeping wait (measured 1-3 % slower)
+    const bool poll1 = (p.flags & 32) != 0;                 // B2S_SP_ZSKIP bit 32: lane 0 polls with a sleeping wait
     const uint32_t all_offsets = K >= 32 ? 0xffffffffu : ((1u << K) - 1u);
     auto tile_kbm = [&](int tile) -> uint32_t {
         return kb_mask_of<PACK>(p.tile_mask ? __ldg(&p.tile_mask[tile]) & all_offsets : all_offsets, num_kb);
@@ -190,178 +149,19 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
         s_shift[threadIdx.x] = p.shift ? p.shift[threadIdx.x] : 0.f;
     }
     if (warp == 1 && lane == 0) {
-        for (int i = 0; i < STAGES; ++i) { mbar_init(&bar_full[i], 32 * HALVES + 1); mbar_init(&bar_empty[i], 1); }
-        for (int i = 0; i < ACC_SLOTS; ++i) { mbar_init(&bar_tfull[i], 1); mbar_init(&bar_tempty[i], 4); }
+        for (int i = 0; i < STAGES; ++i) { mbar_init(&bar_full[i], 32 * HALVES + 1); mbar_init(&bar_empty[i], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)),
-                     "r"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = s_tmem_base;
 
-    if (warp == 0) {
-        // ===================== weight TMA producer =====================
-        if (lane == 0 && (int)blockIdx.x < num_tiles) {
-            int stage = 0;
-            uint32_t phase = 0;
-            uint32_t kbm_next = tile_kbm(blockIdx.x);
-            int wg = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                uint32_t kbm = kbm_next;
-                if (tile + (int)gridDim.x < num_tiles) kbm_next = tile_kbm(tile + gridDim.x);
-                while (kbm) {
-                    const int kb = __ffs(kbm) - 1;
-                    kbm &= kbm - 1;
-                    mbar_wait(&bar_empty[stage], phase ^ 1);
-                    B2S_TRACE(0, wg);
-                    uint8_t *st = smem + (size_t)stage * STAGE_BYTES;
-#ifdef B2S_DIAG
-                    if (p.flags & 4) { mbar_arrive(&bar_full[stage]); if (++stage == STAGES) { stage = 0; phase ^= 1; } continue; }
-#endif
-                    mbar_arrive_expect_tx(&bar_full[stage], 2 * B_TILE_BYTES);
-                    tma_load_3d(st + 2 * A_TILE_BYTES, &map_w_hi, &bar_full[stage], 0, 0, kb);
-                    tma_load_3d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_w_lo, &bar_full[stage], 0, 0, kb);
-                    B2S_TRACE(1, wg);
-                    ++wg;
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        // ONE thread feeds the tensor pipe, and everything it executes besides the MMAs is serial latency during which
-        // the tensor queue drains.  (1) a K block is one asm sequence -- 8 MMAs, the commits and, issued after the first
-        // two MMAs but consumed after the commits, NON-BLOCKING tests of the next K block's full barrier and the next
-        // accumulator's empty barrier (blocking waits only when a test fails: a blocking wait placed between the MMA
-        // bursts cost ~200-400 cycles even on a long-complete barrier, clock64 trace of round 2); (2) the loop is
-        // unrolled over the pipeline stages so descriptors and barrier addresses are loop invariants; (3) per-tile
-        // bookkeeping (which K block closes an accumulation chain) is a mask computed once per tile.
-        // Tried and measured, not faster: two issuer threads alternating K blocks (hand-over by tcgen05.commit +
-        // fence: the commit -> mbarrier -> waiter latency, ~350 cycles, is paid per K block), software-pipelining the
-        // bookkeeping into the gap after the first two MMAs, 16 gather warps with setmaxnreg (B2S_SP_GW=16).
-        constexpr uint32_t idesc = make_idesc_f16(N), idesc2 = make_idesc_f16(2 * N);
-        const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint32_t smem0 = smem_u32(smem);
-        const int num_tiles_u = __shfl_sync(0xffffffffu, num_tiles, 0);
-        if (elect_one_sync() && blockIdx.x < (unsigned)num_tiles_u) {
-            // bit set = this K block is the last one of its accumulation chain present in the tile
-            auto chain_ends = [&](uint32_t kbm_) -> uint32_t {
-                uint32_t ce_ = 0;
-                for (int c = 0; c < num_chains; ++c) {
-                    const uint32_t m_ = kbm_ & (CHAIN_BITS << (c * CHAIN_KB));
-                    if (m_) ce_ |= 0x80000000u >> __clz(m_);
-                }
-                return ce_;
-            };
-            const uint32_t bar_full0 = smem_u32(&bar_full[0]), bar_empty0 = smem_u32(&bar_empty[0]);
-            const uint32_t bar_tfull0 = smem_u32(&bar_tfull[0]), bar_tempty0 = smem_u32(&bar_tempty[0]);
-            uint32_t phase = 0;                                 // parity of the full barriers in this round of the stages
-            uint32_t acc = 0, acc_phase = 0;
-            const bool timing = (p.flags & 16) != 0;
-            long long t_wait = 0, t_begin = clock64();
-            int n_kb = 0;
-            mbar_wait(&bar_tempty[0], 1);
-            mbar_wait(&bar_full[0], 0);
-            tc_fence_after();
-            int tile = blockIdx.x;
-            uint32_t kbm = tile_kbm(tile);
-            uint32_t ce = chain_ends(kbm);
-            bool last_tile = tile + (int)gridDim.x >= num_tiles_u;
-            uint32_t kbm_next = last_tile ? 0u : tile_kbm(tile + gridDim.x);
-            uint32_t fresh = 1;                                 // the next MMA opens an accumulation chain
-            for (;;) {
-#pragma unroll
-                for (int st = 0; st < STAGES; ++st) {
-                    const uint32_t low = kbm & (0u - kbm);
-                    kbm ^= low;
-                    const uint32_t chain_end = (ce & low) ? 1u : 0u;
-                    const bool tile_end = kbm == 0;
-                    const bool last = tile_end && last_tile;
-                    const uint32_t sa = smem0 + (uint32_t)st * STAGE_BYTES;
-                    const uint64_t a_hi = make_desc_sw128(sa), a_lo = make_desc_sw128(sa + A_TILE_BYTES);
-                    const uint64_t b_hl = make_desc_sw128(sa + 2 * A_TILE_BYTES);   // [W_hi; W_lo], 2N rows
-                    const uint32_t accn = (acc + 1) & (ACC_SLOTS - 1);
-                    const uint32_t acc_phase_n = acc_phase ^ (accn == 0 ? 1u : 0u);
-                    B2S_TRACE(2, n_kb);
-                    uint32_t r_full, r_tempty;
-                    // per K step: A_hi x [W_hi;W_lo] into columns [0,2N), A_lo x W_hi into [0,N)
-                    asm volatile(
-                        "{\n\t"
-                        ".reg .pred pacc, ptrue, pf, pt, pce;\n\t"
-                        ".reg .b64 ah, al, bb;\n\t"
-                        "setp.eq.b32 pacc, %6, 0;\n\t"
-                        "setp.eq.b32 ptrue, 0, 0;\n\t"
-                        "setp.ne.b32 pce, %13, 0;\n\t"
-                        "tcgen05.mma.cta_group::1.kind::f16 [%2], %3, %5, %8, pacc;\n\t"
-                        "tcgen05.mma.cta_group::1.kind::f16 [%2], %4, %5, %7, ptrue;\n\t"
-                        "mbarrier.test_wait.parity.shared::cta.b64 pf, [%9], %10;\n\t"
-                        "mbarrier.test_wait.parity.shared::cta.b64 pt, [%11], %12;\n\t"
-                        "add.u64 ah, %3, 2;\n\t add.u64 al, %4, 2;\n\t add.u64 bb, %5, 2;\n\t"
-                        "tcgen05.mma.cta_group::1.kind::f16 [%2], ah, bb, %8, ptrue;\n\t"
-                        "tcgen05.mma.cta_group::1.kind::f16 [%2], al, bb, %7, ptrue;\n\t"
-                        "add.u64 ah, %3, 4;\n\t add.u64 al, %4, 4;\n\t add.u64 bb, %5, 4;\n\t"
-                        "tcgen05.mma.cta_group::1.kind::f16 [%2], ah, bb, %8, ptrue;\n\t"
-                        "tcgen05.mma.cta_group::1.kind::f16 [%2], al, bb, %7, ptrue;\n\t"
-                        "add.u64 ah, %3, 6;\n\t add.u64 al, %4, 6;\n\t add.u64 bb, %5, 6;\n\t"
-                        "tcgen05.mma.cta_group::1.kind::f16 [%2], ah, bb, %8, ptrue;\n\t"
-                        "tcgen05.mma.cta_group::1.kind::f16 [%2], al, bb, %7, ptrue;\n\t"
-                        "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%14];\n\t"
-                        "@pce tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%15];\n\t"
-                        "selp.u32 %0, 1, 0, pf;\n\t"
-                        "selp.u32 %1, 1, 0, pt;\n\t"
-                        "}"
-                        : "=r"(r_full), "=r"(r_tempty)
-                        : "r"(tmem_u + acc * (uint32_t)ACC_W), "l"(a_hi), "l"(a_lo), "l"(b_hl), "r"(fresh), "r"(idesc), "r"(idesc2),
-                          "r"(bar_full0 + 8u * (uint32_t)((st + 1) % STAGES)), "r"(st + 1 == STAGES ? phase ^ 1u : phase),
-                          "r"(bar_tempty0 + 8u * accn), "r"(acc_phase_n ^ 1u), "r"(chain_end),
-                          "r"(bar_empty0 + 8u * (uint32_t)st), "r"(bar_tfull0 + 8u * acc)
-                        : "memory");
-                    static_assert(((UMMA_K * ELEM_BYTES) >> 4) == 2, "K-step advance of the descriptors inside the asm block");
-                    static_assert((ACC_SLOTS & (ACC_SLOTS - 1)) == 0, "accumulator ring index uses a mask");
-                    B2S_TRACE(4, n_kb);
-                    ++n_kb;
-                    fresh = chain_end;
-                    if (chain_end) { acc = accn; acc_phase = acc_phase_n; }
-                    if (last) goto issuer_done;
-                    if (!(r_full & (chain_end ? r_tempty : 1u))) {
-                        const long long w0 = timing ? clock64() : 0;
-                        if (!r_full) mbar_wait(&bar_full[(st + 1) % STAGES], st + 1 == STAGES ? phase ^ 1u : phase);
-                        if (chain_end && !r_tempty) mbar_wait(&bar_tempty[acc], acc_phase ^ 1u);
-                        if (timing) t_wait += clock64() - w0;
-                    }
-                    B2S_TRACE(3, n_kb - 1);
-                    tc_fence_after();
-                    if (tile_end) {
-                        tile += gridDim.x;
-                        kbm = kbm_next;
-                        ce = chain_ends(kbm);
-                        last_tile = tile + (int)gridDim.x >= num_tiles_u;
-                        if (!last_tile) kbm_next = tile_kbm(tile + gridDim.x);
-                    }
-                }
-                phase ^= 1u;
-            }
-        issuer_done:
-            if (timing && blockIdx.x == 0)
-                printf("[sparse_tc<%d,%d>] issuer: %d K blocks in %d tiles, total %lld cyc (%.0f/kb), blocking waits %lld (%.0f/kb)\n",
-                       CIN, COUT, n_kb, (num_tiles_u + (int)gridDim.x - 1) / (int)gridDim.x, clock64() - t_begin,
-                       (double)(clock64() - t_begin) / (n_kb + 1), t_wait, (double)t_wait / (n_kb + 1));
-        }
-        __syncwarp();
-    } else if (warp >= 4 && warp < 4 + GW) {
+    if (warp < GW) {
         // ===================== gather producers =====================
         // Lane mapping: one warp instruction covers 4 rows x 8 sixteen-byte chunks, so the 32 lanes write 4 whole
         // 128-byte smem rows (bank-conflict free under the 128B swizzle) and read 4 x 128 contiguous global bytes.
         // The loop body is written for instruction count: a gather warp is ONE instruction stream, ~8 cycles per
         // dependent instruction, and the first version of this loop (lambdas, branches around the copies) compiled to
         // ~740 instructions per K block for 32 copies -- the gather warps, not memory, bounded the kernel.
-        if constexpr (GW == 16) asm volatile("setmaxnreg.dec.sync.aligned.u32 64;");
-        const int gw = warp - 4;
+        const int gw = warp;
         const int my_own = gw % OWN;                           // this warp takes K blocks g with g % OWN == my_own
         const int half = gw / OWN;                             // rows half*(128/HALVES) .. of the tile
         const int sub = lane >> 3;                             // row within a group of 4
@@ -463,9 +263,7 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
             const uint32_t zeroed = (uint32_t)((my_stage < 4 ? zeroed_w0 : zeroed_w1) >> zsh) & ((1u << RI) - 1u);
             const uint32_t need = zskip_on ? (valid | (~zeroed & ((1u << RI) - 1u))) : 0xFFFFFFFFu;
             const uint32_t sa = sa0 + (uint32_t)my_stage * STAGE_BYTES;
-            if (half == 0) B2S_TRACE(5, g_cur);
             mbar_wait_warp(&bar_empty[my_stage], use_parity, poll1);
-            if (half == 0) B2S_TRACE(6, g_cur);
             if (lo_delta == (long long)(CIN * ELEM_BYTES)) {
                 // interleaved rows [hi Cin | lo Cin]: the lo copy is the hi address + an immediate
 #pragma unroll
@@ -499,7 +297,6 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
                 if (my_stage < 4) zeroed_w0 = (zeroed_w0 & clr) | set; else zeroed_w1 = (zeroed_w1 & clr) | set;
             }
             if (p.flags & 128) mbar_arrive(&bar_full[my_stage]); else cp_async_mbar_arrive_noinc(&bar_full[my_stage]);
-            if (half == 0) B2S_TRACE(7, g_cur);
             // ---- advance ----
             g_cur = e_owned;
             kb_cur = kb_nxt;
@@ -519,169 +316,123 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
 #undef B2S_LOAD_ROWS
 #undef B2S_LOAD_NBR
         asm volatile("cp.async.wait_all;" ::: "memory");
-    } else if (warp >= 4 + GW) {
-        // ===================== epilogue =====================
-        if constexpr (GW == 16) asm volatile("setmaxnreg.inc.sync.aligned.u32 144;");
-        const int ew = warp - (4 + GW);                // == warp % 4: TMEM lane quarter
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        const bool timing_e = (p.flags & 16) != 0 && blockIdx.x == 0 && ew == 0 && lane == 0;
-        long long te_wait = 0, te_drain = 0, te_store = 0, te_begin = clock64();
-        int te_chains = 0;
-        uint32_t kbm_next = (int)blockIdx.x < num_tiles ? tile_kbm(blockIdx.x) : 0u;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-            const uint32_t kbm = kbm_next;
-            if (tile + (int)gridDim.x < num_tiles) kbm_next = tile_kbm(tile + gridDim.x);
-            // output row of this lane's accumulator row (TMEM lane ew*32 + lane)
-            const int pos = tile * BLOCK_M + ew * 32 + lane;
-            int my_row = -1;
-            if (pos < n_out) my_row = p.perm ? __ldg(&p.perm[pos]) : pos;
-            float sum[N];
-#pragma unroll
-            for (int j = 0; j < N; ++j) sum[j] = 0.f;
-            for (int c = 0; c < num_chains; ++c) {
-                if (!(kbm & (CHAIN_BITS << (c * CHAIN_KB)))) continue;       // no K block of this chain was issued
-                const long long e0 = timing_e ? clock64() : 0;
-                mbar_wait_warp(&bar_tfull[acc], acc_phase, poll1);
-                tc_fence_after();
-                const long long e1 = timing_e ? clock64() : 0;
-                const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(acc * ACC_W);
-#pragma unroll
-                for (int c0 = 0; c0 < N; c0 += 16) {
-                    uint32_t ra[16], rb[16];
-                    tmem_ld16(taddr + c0, ra);            // A_hi*W_hi + A_lo*W_hi
-                    tmem_ld16(taddr + N + c0, rb);        // A_hi*W_lo
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        sum[c0 + j] = __fadd_rn(__fadd_rn(sum[c0 + j], __uint_as_float(ra[j])), __uint_as_float(rb[j]));
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&bar_tempty[acc]);
-                if (++acc == ACC_SLOTS) { acc = 0; acc_phase ^= 1; }
-                if (timing_e) { te_wait += e1 - e0; te_drain += clock64() - e1; ++te_chains; }
+    } else {
+        // ===================== consumers: MMA + epilogue =====================
+        const int cg = (warp - GW) >> 2;               // warpgroup: tile rows 64 cg .. 64 cg + 63
+        const int wl = warp & 3;
+        const uint32_t smem0 = smem_u32(smem);
+        const uint32_t a_off = (uint32_t)cg * 64u * 128u;
+        int stage = 0;
+        uint32_t phase = 0;
+        // Weight loads: lane 0 of the first consumer warp walks the CTA's K-block sequence STAGES K blocks ahead of the
+        // MMAs; a stage's weights are requested as soon as both warpgroups have released it.
+        const bool w_issuer = warp == GW && lane == 0 && (int)blockIdx.x < num_tiles;
+        int w_tile = (int)blockIdx.x, w_stage = 0;
+        uint32_t w_kbm = w_issuer ? tile_kbm(w_tile) : 0u, w_phase = 0;
+        auto issue_weights = [&]() {
+            if (w_kbm == 0) {
+                w_tile += gridDim.x;
+                if (w_tile >= num_tiles) return;
+                w_kbm = tile_kbm(w_tile);
             }
-            const long long es0 = timing_e ? clock64() : 0;
-            // coalesced stores: transpose 32 rows x CW channels through a padded shared tile so every store
-            // instruction writes whole contiguous row segments (a lane-per-row store is 16 B at a row stride).
-            // fp16 planes: a staged row = WP words of hi pairs, then (at word 16) WP words of lo pairs; the first CP
-            // lanes of a row group write the hi segment, the next CP lanes the lo segment.
-            constexpr int CW = N < 32 ? N : 32;                // channels per pass
-            uint32_t *stg = s_stage[ew];
-            bool range_bad = false;
-            if (p.out_lo) {
-                constexpr int WP = CW / 2;                     // words per plane and row
-                constexpr int CP = WP / 4;                     // 16-byte chunks per plane and row
-                constexpr int LPR = 2 * CP;                    // lanes per row
-                constexpr int RPI = 32 / LPR;                  // rows per store instruction
-                const int sp = lane / LPR, sq = lane % LPR;
-                __half *outp = (sq < CP) ? reinterpret_cast<__half *>(p.out_hi) : p.out_lo;
-                const int coff = (sq % CP) * 8;                // first of this lane's 8 channels inside the pass
+            const int kb = __ffs(w_kbm) - 1;
+            w_kbm &= w_kbm - 1;
+            mbar_wait(&bar_empty[w_stage], w_phase ^ 1);
+            uint8_t *st = smem + (size_t)w_stage * STAGE_BYTES;
+#ifdef B2S_DIAG
+            if (p.flags & 4) { mbar_arrive(&bar_full[w_stage]); if (++w_stage == STAGES) { w_stage = 0; w_phase ^= 1; } return; }
+#endif
+            mbar_arrive_expect_tx(&bar_full[w_stage], 2 * B_TILE_BYTES);
+            tma_load_3d(st + 2 * A_TILE_BYTES, &map_w_hi, &bar_full[w_stage], 0, 0, kb);
+            tma_load_3d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_w_lo, &bar_full[w_stage], 0, 0, kb);
+            if (++w_stage == STAGES) { w_stage = 0; w_phase ^= 1; }
+        };
+        if (w_issuer)
+            for (int i = 0; i < STAGES; ++i) issue_weights();
+        __syncwarp();
+        float acc[R], sum[R / 2];
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+            uint32_t kbm = tile_kbm(tile);
+            // bit set = this K block is the last one of its accumulation chain present in the tile
+            uint32_t ce = 0;
+            for (int c = 0; c < num_chains; ++c) {
+                const uint32_t m_ = kbm & (CHAIN_BITS << (c * CHAIN_KB));
+                if (m_) ce |= 0x80000000u >> __clz(m_);
+            }
 #pragma unroll
-                for (int cc = 0; cc < N; cc += CW) {
-                    __syncwarp();
+            for (int j = 0; j < R / 2; ++j) sum[j] = 0.f;
+            uint32_t fresh = 1;                                 // the next MMA opens an accumulation chain
+            while (kbm) {
+                const uint32_t low = kbm & (0u - kbm);
+                kbm ^= low;
+                mbar_wait_warp(&bar_full[stage], phase, poll1);
+                fence_proxy_async();                            // gathered rows were written by cp.async (generic proxy)
+                const uint32_t sa = smem0 + (uint32_t)stage * STAGE_BYTES;
+                const uint64_t a_hi = make_desc_sw128(sa + a_off), a_lo = make_desc_sw128(sa + A_TILE_BYTES + a_off);
+                const uint64_t b_hl = make_desc_sw128(sa + 2 * A_TILE_BYTES);   // [W_hi; W_lo], 2N rows
+                wgmma_fence();
 #pragma unroll
-                    for (int c0 = 0; c0 < CW; c0 += 8) {
-                        uint32_t hw[4], lw[4];
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            float x0 = fmaf(sum[cc + c0 + 2 * j], s_scale[cc + c0 + 2 * j], s_shift[cc + c0 + 2 * j]);
-                            float x1 = fmaf(sum[cc + c0 + 2 * j + 1], s_scale[cc + c0 + 2 * j + 1], s_shift[cc + c0 + 2 * j + 1]);
-                            if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-                            range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
-                            const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
-                            hw[j] = __byte_perm(p0, p1, 0x5410);
-                            lw[j] = __byte_perm(p0, p1, 0x7632);
-                        }
-                        *reinterpret_cast<uint4 *>(stg + lane * 36 + c0 / 2) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                        *reinterpret_cast<uint4 *>(stg + lane * 36 + 16 + c0 / 2) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                    }
-                    __syncwarp();
-#pragma unroll
-                    for (int it = 0; it < 32 / RPI; ++it) {
-                        const int rr = __shfl_sync(0xffffffffu, my_row, it * RPI + sp);
-                        if (rr >= 0)
-                            *reinterpret_cast<uint4 *>(outp + (size_t)rr * p.out_stride + cc + coff) =
-                                *reinterpret_cast<const uint4 *>(stg + (it * RPI + sp) * 36 + (sq < CP ? 0 : 16) + (sq % CP) * 4);
-                    }
+                for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+                    const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                    wgmma_ss<2 * N>(acc, a_hi + koff, b_hl + koff, (fresh && k == 0) ? 0u : 1u);
+                    wgmma_ss<N>(acc, a_lo + koff, b_hl + koff, 1);
                 }
-            } else {
-                constexpr int CH4 = CW / 4;                        // 16-byte chunks per row segment
-                constexpr int RPI = 32 / CH4;                      // rows per store instruction
-                const int sp = lane / CH4, sq = lane % CH4;
-                float *outp = reinterpret_cast<float *>(p.out_hi);
+                wgmma_commit();
+                wgmma_wait_all();
+                wgmma_fence_operands<R>(acc);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&bar_empty[stage]);
+                if (w_issuer) issue_weights();
+                __syncwarp();
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                fresh = (ce & low) ? 1u : 0u;
+                if (fresh) {
+                    // columns [0,N) hold A_hi*W_hi + A_lo*W_hi, the same columns of the second half A_hi*W_lo
 #pragma unroll
-                for (int cc = 0; cc < N; cc += CW) {
-                    __syncwarp();
+                    for (int j = 0; j < R / 2; ++j) sum[j] = __fadd_rn(__fadd_rn(sum[j], acc[j]), acc[R / 2 + j]);
+                }
+            }
+            // epilogue: rows m0 = 64 cg + 16 wl + lane/4 and m0 + 8 of the tile, per 8-column block j the channel pair
+            // 8j + 2(lane % 4); a quad of lanes writes 16 (fp16 planes) or 32 (fp32) contiguous bytes of a row
+            bool range_bad = false;
 #pragma unroll
-                    for (int c0 = 0; c0 < CW; c0 += 4) {
-                        uint32_t v[4];
+            for (int rh = 0; rh < 2; ++rh) {
+                const int pos = tile * BLOCK_M + cg * 64 + wl * 16 + (lane >> 2) + rh * 8;
+                if (pos >= n_out) continue;
+                const int row = p.perm ? __ldg(&p.perm[pos]) : pos;
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            float x = fmaf(sum[cc + c0 + j], s_scale[cc + c0 + j], s_shift[cc + c0 + j]);
-                            if (p.relu) x = fmaxf(x, 0.f);
-                            v[j] = __float_as_uint(x);
-                        }
-                        *reinterpret_cast<uint4 *>(stg + lane * 36 + c0) = make_uint4(v[0], v[1], v[2], v[3]);
-                    }
-                    __syncwarp();
-#pragma unroll
-                    for (int it = 0; it < 32 / RPI; ++it) {
-                        const int rr = __shfl_sync(0xffffffffu, my_row, it * RPI + sp);
-                        if (rr >= 0)
-                            *reinterpret_cast<uint4 *>(outp + (size_t)rr * N + cc + sq * 4) =
-                                *reinterpret_cast<const uint4 *>(stg + (it * RPI + sp) * 36 + sq * 4);
+                for (int j = 0; j < N / 8; ++j) {
+                    const int c = 8 * j + 2 * (lane & 3);
+                    float x0 = fmaf(sum[4 * j + 2 * rh], s_scale[c], s_shift[c]);
+                    float x1 = fmaf(sum[4 * j + 2 * rh + 1], s_scale[c + 1], s_shift[c + 1]);
+                    if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                    if (p.out_lo) {
+                        range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
+                        const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
+                        const size_t o = (size_t)row * p.out_stride + c;
+                        *reinterpret_cast<uint32_t *>(reinterpret_cast<__half *>(p.out_hi) + o) = __byte_perm(p0, p1, 0x5410);
+                        *reinterpret_cast<uint32_t *>(p.out_lo + o) = __byte_perm(p0, p1, 0x7632);
+                    } else {
+                        *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out_hi) + (size_t)row * N + c) = make_float2(x0, x1);
                     }
                 }
             }
             if (__any_sync(0xffffffffu, range_bad) && lane == 0 && p.status) atomicOr(p.status, B2S_STATUS_F16_RANGE);
-            if (timing_e) te_store += clock64() - es0;
         }
-        if (timing_e)
-            printf("[sparse_tc<%d,%d>] epilogue warp 0: %d chains, total %lld cyc, wait tfull %lld (%.0f/chain), drain %lld "
-                   "(%.0f/chain), output stage %lld\n", CIN, COUT, te_chains, clock64() - te_begin, te_wait,
-                   (double)te_wait / (te_chains + 1), te_drain, (double)te_drain / (te_chains + 1), te_store);
-    }
-    tc_fence_before();
-    __syncthreads();
-#ifdef B2S_DIAG
-    if ((p.flags & 64) && blockIdx.x == 0 && threadIdx.x == 0) {
-        const long long t0 = g_trace[2][0];
-        printf("[trace<%d,%d>] g: W(empty seen, tma issued) I(at waits, full seen, all waits done, MMAs+commits issued) G(at wait, empty seen, arrived)\n", CIN, COUT);
-        for (int g = 32; g < 96; ++g)
-            printf("[trace] %3d  W %7lld %7lld  I %7lld %7lld %7lld %7lld  G %7lld %7lld %7lld\n", g, g_trace[0][g] - t0, g_trace[1][g] - t0,
-                   g_trace[2][g] - t0, g_trace[2][g] - t0, g_trace[3][g] - t0, g_trace[4][g] - t0, g_trace[5][g] - t0, g_trace[6][g] - t0, g_trace[7][g] - t0);
-    }
-#endif
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
     }
 }
 
-template <int CIN, int COUT, int GW>
-int launch_gw(const CUtensorMap &w_hi, const CUtensorMap &w_lo, const SpParams &p, int num_sms, cudaStream_t stream)
-{
-    constexpr size_t stage = 2 * A_TILE_BYTES + 2 * (size_t)COUT * BLOCK_K * ELEM_BYTES;
-    size_t smem = stage * stages_for(COUT) + 1024;
-    B2S_SMEM_OPT_IN((k_sparse_conv_tc<CIN, COUT, 4, GW>), smem);
-    int tiles_cap = (p.cap_out + BLOCK_M - 1) / BLOCK_M;
-    int grid = tiles_cap < num_sms ? tiles_cap : num_sms;
-    k_sparse_conv_tc<CIN, COUT, 4, GW><<<grid, 32 * (4 + GW + 4), smem, stream>>>(w_hi, w_lo, p);
-    B2S_LAUNCH_OK();
-    return 0;
-}
 template <int CIN, int COUT>
 int launch(const CUtensorMap &w_hi, const CUtensorMap &w_lo, const SpParams &p, int num_sms, cudaStream_t stream)
 {
-#ifdef B2S_SP_GW16
-    // A/B build (make EXTRA=-DB2S_SP_GW16): B2S_SP_GW=16 runs 16 gather warps with setmaxnreg (measured: not faster)
-    static int gw = -1;
-    if (gw < 0) { const char *e = getenv("B2S_SP_GW"); gw = (e && atoi(e) == 16) ? 16 : 8; }
-    if (gw == 16) return launch_gw<CIN, COUT, 16>(w_hi, w_lo, p, num_sms, stream);
-#endif
-    return launch_gw<CIN, COUT, 8>(w_hi, w_lo, p, num_sms, stream);
+    constexpr size_t stage = 2 * A_TILE_BYTES + 2 * (size_t)COUT * BLOCK_K * ELEM_BYTES;
+    size_t smem = stage * STAGES + 1024;
+    B2S_SMEM_OPT_IN((k_sparse_conv_tc<CIN, COUT>), smem);
+    int tiles_cap = (p.cap_out + BLOCK_M - 1) / BLOCK_M;
+    int grid = tiles_cap < num_sms ? tiles_cap : num_sms;
+    k_sparse_conv_tc<CIN, COUT><<<grid, kThreads, smem, stream>>>(w_hi, w_lo, p);
+    B2S_LAUNCH_OK();
+    return 0;
 }
 
 }  // namespace
@@ -732,7 +483,7 @@ extern "C" int b2s_sparse_conv_tc_plan(const b2s_half *feat_hi, const b2s_half *
 #ifdef B2S_DIAG
         p.flags = fl;           // make DIAG=1: bit 2 no gather copies, 4 no weight loads, 8 no zero fills (results wrong)
 #else
-        p.flags = fl & (1 | 16 | 32);
+        p.flags = fl & (1 | 32);
 #endif
     }
     p.relu = relu; p.scale = scale; p.shift = shift; p.out_hi = out_hi; p.out_lo = reinterpret_cast<__half *>(out_lo);

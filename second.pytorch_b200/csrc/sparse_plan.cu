@@ -1,7 +1,7 @@
 // sparse_plan.cu -- tile plan of a sparse convolution (b2s_sparse_tile_plan): which kernel offsets a 128-row output
 // tile needs at all, and an order of the output rows that makes that set small.
 //
-// b2s_sparse_conv_tc is output-stationary: a CTA owns 128 output rows (one tcgen05 accumulator) and multiplies, per
+// b2s_sparse_conv_tc is output-stationary: a CTA owns 128 output rows (one accumulator tile) and multiplies, per
 // kernel offset k, the 128 gathered neighbour rows with W[k].  Only ~3.5-9 of the 27 neighbours of a row exist
 // (SURVEY.md App. D), so most gathered rows are zeros -- but an offset can only be SKIPPED when none of the tile's 128
 // rows has that neighbour.  In storage order that removes ~25 % of the (tile, offset) blocks (measured on the bench
@@ -193,7 +193,7 @@ extern "C" int b2s_sparse_tile_plan(const int *nbr, const unsigned *row_mask, in
         attr_done[dev & 63] = true;
     }
     int grid = b2s_cdiv(cap_out, kChunkRows);
-    if (grid > 148 * 2) grid = 148 * 2;
+    if (grid > 132 * 2) grid = 132 * 2;
     B2S_REQUIRE(nbr != nullptr || row_mask != nullptr, "b2s_sparse_tile_plan: nbr or row_mask required");
     k_tile_plan<<<grid, kThreads, smem, stream>>>(nbr, row_mask, num_out_dev, cap_out, g, sort ? 1 : 0, perm, tile_mask);
     B2S_LAUNCH_OK();

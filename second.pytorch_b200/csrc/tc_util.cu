@@ -48,7 +48,7 @@ __global__ void k_merge_f16(const __half *__restrict__ hi, const __half *__restr
 inline int grid_for(long long items)
 {
     long long b = (items + 255) / 256;
-    return (int)(b < 1 ? 1 : (b < 148 * 8 ? b : 148 * 8));
+    return (int)(b < 1 ? 1 : (b < 132 * 8 ? b : 132 * 8));
 }
 
 }  // namespace

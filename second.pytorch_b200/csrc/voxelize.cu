@@ -403,7 +403,7 @@ extern "C" int b2s_vfe_mean(const float *voxels, const int *num_points_per_voxel
                 vfe_num_features <= 8 && vfe_num_features <= F, "b2s_vfe_mean: bad feature counts");
     if (cap_rows <= 0) return 0;
     int blocks = b2s_cdiv(cap_rows, kThreads);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     k_vfe_mean<<<blocks, kThreads, 0, stream>>>(voxels, num_points_per_voxel, num_rows_dev, cap_rows, T, F, vfe_mode,
                                                 vfe_num_features, vfe_out);
     B2S_LAUNCH_OK();

@@ -317,7 +317,7 @@ class SparseConvolution(SparseModule):
         use_tc = (USE_TENSOR_CORES and cin_tc is not None
                   and bool(lib.b2s_sparse_conv_tc_supported(cin_tc, self.out_channels)))
         if use_tc:
-            # tensor pipe (tcgen05, 3xF16 split): fp16 hi/lo rows in, fp16 hi/lo rows out
+            # tensor pipe (wgmma, 3xF16 split): fp16 hi/lo rows in, fp16 hi/lo rows out
             if input._hilo is not None and input._hilo[0].shape[1] == cin_tc:
                 hi, lo, stride = input._hilo
             else:

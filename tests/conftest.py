@@ -1,4 +1,4 @@
-"""pytest wiring: `-m "not gpu"` runs on the CPU-only build container, `-m gpu` on a B200 box."""
+"""pytest wiring: `-m "not gpu"` runs on the CPU-only build container, `-m gpu` on an H100."""
 import os
 import sys
 
@@ -12,7 +12,7 @@ for p in (REPO, PKG):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

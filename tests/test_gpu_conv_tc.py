@@ -1,4 +1,4 @@
-"""GPU parity of the tensor-core RPN convolution (b2s_conv2d_tc, tcgen05 kind::f16 + 3xF16 hi/lo split) against torch
+"""GPU parity of the tensor-core RPN convolution (b2s_conv2d_tc, wgmma f16 + 3xF16 hi/lo split) against torch
 fp32 conv2d with TF32 disabled.  Bar: fp32-grade accuracy, |err| <= 2e-5 * max|ref| (plain fp16/TF32 would be ~1e-3)."""
 import ctypes
 

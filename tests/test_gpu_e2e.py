@@ -60,7 +60,7 @@ def test_module_path_matches_golden(product, name, seed, n, path):
 
 
 def _engine_cases():
-    """every fixture on the shipped configuration (tcgen05 RPN + tcgen05 sparse conv, CUDA graph); the seed-0 fixture
+    """every fixture on the shipped configuration (wgmma RPN + wgmma sparse conv, CUDA graph); the seed-0 fixture
     of every config additionally on the cross-check configurations (cuDNN RPN / FMA sparse conv, eager)."""
     out, ids = [], []
     for c in CASES:

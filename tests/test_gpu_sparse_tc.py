@@ -1,4 +1,4 @@
-"""GPU parity of the tensor-pipe sparse convolution (b2s_sparse_conv_tc, tcgen05 kind::f16 + 3xF16) against the CPU
+"""GPU parity of the tensor-pipe sparse convolution (b2s_sparse_conv_tc, wgmma f16 + 3xF16) against the CPU
 oracle's sparse conv (fp32).  Same rulebook (b2s_rulebook_*), same BN/ReLU epilogue; bar 2e-5 * max|ref| per layer."""
 import numpy as np
 import pytest
@@ -91,7 +91,7 @@ def test_sparse_conv_tc_matches_oracle(product, oracle, cin, cout, subm, n):
 
 @pytest.mark.timeout(180)
 def test_drop_in_sparse_sequential_runs_on_tensor_cores(product, oracle):
-    """spconv.SparseSequential in eval mode (the reference's middle_conv) on the tcgen05 kernel: hi/lo planes flow from
+    """spconv.SparseSequential in eval mode (the reference's middle_conv) on the wgmma kernel: hi/lo planes flow from
     layer to layer, .features materialises fp32 lazily, results match the oracle package layer stack."""
     from torch import nn
     torch.manual_seed(0)

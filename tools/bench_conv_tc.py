@@ -1,6 +1,6 @@
 """micro-benchmark of b2s_conv2d_tc alone (RPN 3x3 128->128 at car.fhd size), CUDA-event timed.
-B2S_CONV_DBG (diagnostic, wrong results; `make DIAG=1` builds only): 1 = no lo loads, 2 = hi*hi MMA only, 4 = no
-TMEM drain.  B2S_CONV_B = frames."""
+B2S_CONV_DBG (diagnostic, wrong results; `make DIAG=1` builds only): 1 = no lo loads, 4 = no accumulator
+drain.  B2S_CONV_B = frames."""
 import os
 import sys
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
