@@ -28,9 +28,13 @@
  *   b2s_to_bev          spconv.SparseConvTensor.dense() + view (middle.py:206-209) and
  *                       PointPillarsScatter.forward (second/pytorch/models/pointpillars.py:444-476)
  *   b2s_pfn             PillarFeatureNet.forward (pointpillars.py:203-237, single PFNLayer :51-65)
+ *   b2s_pfn_ex          the same, or PillarFeatureNetRadius.forward (pointpillars.py:240-325)
+ *   b2s_crop_nhwc       stage0[:, :, c:-c, c:-c] in VoxelNetNuscenesMultiHead.network_forward
+ *                       (second/pytorch/models/net_multi_head.py:155-160)
  *   b2s_decode_filter   box_coder.decode_torch + sigmoid + score threshold
  *                       (second/pytorch/models/voxelnet.py:413-414,444,560-576,
- *                        second/pytorch/core/box_torch_ops.py:56-102)
+ *                        second/pytorch/core/box_torch_ops.py:56-102); _segments: over the torch.cat of several
+ *                       heads' predictions (net_multi_head.py:163-172)
  *   b2s_nms             torch.topk + spconv.utils.rotate_non_max_suppression_cpu /
  *                       spconv.utils.non_max_suppression (box_torch_ops.py:454-515,
  *                       second/core/non_max_suppression/nms_cpu.py:20-31, nms_gpu.py:10-19)
@@ -305,6 +309,24 @@ int b2s_pfn(const float *points, int num_feat, const int *point_slots, const int
             float vx, float vy, float x_offset, float y_offset, float *out /*[cap_rows,Cout]*/,
             void *stream);
 
+/* decoration of the PFN input (b2s_pfn_ex): B2S_PFN_PLAIN = PillarFeatureNet, point features [x, y, z, r, ...] and the
+ * Linear has F+5 inputs; B2S_PFN_RADIUS = PillarFeatureNetRadius, point features [sqrt(x*x + y*y), z, r, ...] and F+4
+ * inputs.  Both append (xyz - mean xyz) and (xy - pillar centre).  b2s_pfn = b2s_pfn_ex(..., B2S_PFN_PLAIN, ...). */
+#define B2S_PFN_PLAIN 0
+#define B2S_PFN_RADIUS 1
+int b2s_pfn_ex(const float *points, int num_feat, const int *point_slots, const int *num_points_per_voxel,
+               const int *coors, const int *num_rows_dev, int cap_rows, int max_points,
+               const float *weight /*[Cout, F+5] or [Cout, F+4]*/, const float *scale, const float *shift, int cout,
+               float vx, float vy, float x_offset, float y_offset, int decoration, float *out /*[cap_rows,Cout]*/,
+               void *stream);
+
+/* ---- crop of a halo-padded NHWC map ----------------------------------------------------------------
+ * src [B, H+2, W+2, C] (fp16 hi/lo planes, one-pixel halo) -> dst [B, H-2*crop+2, W-2*crop+2, C]: the interior window
+ * rows [crop, H-crop), columns [crop, W-crop) of src, with dst's halo written as ZERO -- a conv on dst then sees the
+ * zero padding torch applies at the crop edge, not the neighbouring pixels of src.  C % 8 == 0, 16-byte aligned planes. */
+int b2s_crop_nhwc(const b2s_half *src_hi, const b2s_half *src_lo, int batch, int H, int W, int C, int crop,
+                  b2s_half *dst_hi, b2s_half *dst_lo, void *stream);
+
 /* ---- box decode + score filter ------------------------------------------------------------------ */
 /* Head tensors in the RPN's NCHW conv-output layout: box [B, A_loc*code, H, W], cls [B, A_loc*ncls, H, W],
  * dir [B, A_loc*nbins, H, W] (dir may be NULL).  anchors [A_loc*H*W, code] in (a_loc, y, x) order.
@@ -326,6 +348,26 @@ int b2s_decode_filter_strided(const float *box, const float *cls, const float *d
                               int code, int ncls, int nbins, float score_thresh, float *cand_box,
                               float *cand_score, int *cand_label, int *cand_dir, int *cand_anchor,
                               int *cand_count_dev, int cand_cap, unsigned *status_dev, void *stream);
+
+/* several head maps feeding ONE candidate list per frame (VoxelNetNuscenesMultiHead: the large head on the concat map,
+ * the small head on the cropped stage-0 map; net_multi_head.py:163-172 concatenates their predictions).  Segment s
+ * holds the global anchors [anchor_base, anchor_base + a_loc*H*W) in (a_loc, y, x) order; its tensors are addressed as
+ * in b2s_decode_filter_strided (dir may be NULL).  anchors [num_anchors, code] and anchors_mask [B, num_anchors] (may
+ * be NULL) are indexed by the GLOBAL anchor id, which is also what cand_anchor holds (the NMS tie-break key).
+ * Segments must not overlap; anchors no segment covers never become candidates.  One memset + one launch. */
+#define B2S_MAX_HEAD_SEGMENTS 4
+typedef struct b2s_head_segment {
+    const float *box, *cls, *dir;
+    long long box_batch_stride, cls_batch_stride, dir_batch_stride;
+    int ch_stride, pix_stride;
+    int a_loc, H, W;
+    int anchor_base;
+} b2s_head_segment;
+int b2s_decode_filter_segments(const b2s_head_segment *segments /*host[num_segments]*/, int num_segments,
+                               const float *anchors, const uint8_t *anchors_mask, int num_anchors, int batch, int code,
+                               int ncls, int nbins, float score_thresh, float *cand_box, float *cand_score,
+                               int *cand_label, int *cand_dir, int *cand_anchor, int *cand_count_dev, int cand_cap,
+                               unsigned *status_dev, void *stream);
 
 /* multi-class NMS branch (second/pytorch/models/voxelnet.py:458-547): one candidate list per (class, frame),
  * "virtual frame" v = c*batch + b (class-major): cand_* are [ncls*batch, cand_cap, ...], cand_count_dev [ncls*batch].

@@ -40,12 +40,14 @@ def _class_anchors(feature_size, cls, dtype=np.float32):
 
 
 def generate_anchors(cfg):
-    """-> float32 [A, 7+custom] for ``cfg.feature_map_size`` in the reference's order."""
+    """-> float32 [A, 7+custom] for ``cfg.feature_map_size`` in the reference's order.  A class with its own
+    ``feature_map_size`` (``cfg.class_feature_map_sizes``, the multi-head network) is laid out on that map."""
     fsize = cfg.feature_map_size
+    per_class = getattr(cfg, "class_feature_map_sizes", None) or [None] * len(cfg.classes)
     parts = []
-    for cls in cfg.classes:
+    for cls, fs in zip(cfg.classes, per_class):
         if cls.num_anchors_per_loc == 0:
             continue
-        a = _class_anchors(fsize, cls)
+        a = _class_anchors(fs if fs else fsize, cls)
         parts.append(a.reshape(-1, a.shape[-1]))
     return np.concatenate(parts, axis=0)

@@ -8,7 +8,8 @@ side needs neither protobuf nor the reference tree:
 * ``parse_prototxt`` / ``ModelConfig.from_prototxt`` read a reference-format ``.config`` file
   (only the ``model.second`` and ``eval_input_reader`` blocks are interpreted);
 * ``BUILTIN`` holds the five BASELINE.json configurations, written out by hand from the values in
-  SURVEY.md App. B (car.fhd, car.lite, all.fhd, pointpillars/car/xyres_16, nuscenes/all.pp.largea).
+  SURVEY.md App. B (car.fhd, car.lite, all.fhd, pointpillars/car/xyres_16, nuscenes/all.pp.largea);
+  ``EXTRA`` the further ones ``get_config`` knows (nuscenes/all.pp.mhead, a ``MultiHeadModelConfig``).
 """
 import re
 from dataclasses import dataclass, field
@@ -149,7 +150,13 @@ class ModelConfig:
             assert all(v == vals[0] for v in vals), "per-class %s must agree (second_builder.py:55-59)" % key
             return vals[0]
 
-        return ModelConfig(
+        kw = {}
+        cls = ModelConfig
+        if _one(m.get("network_class_name", ["VoxelNet"])) == "VoxelNetNuscenesMultiHead":
+            cls = MultiHeadModelConfig
+            kw["class_feature_map_sizes"] = [[int(v) for v in c[1].get("feature_map_size", [])] for c in classes]
+        return cls(
+            **kw,
             name=name,
             point_cloud_range=[float(v) for v in vg["point_cloud_range"]],
             voxel_size=[float(v) for v in vg["voxel_size"]],
@@ -193,6 +200,16 @@ class ModelConfig:
     def from_file(path, name=None):
         with open(path) as f:
             return ModelConfig.from_prototxt(f.read(), name or path)
+
+
+@dataclass
+class MultiHeadModelConfig(ModelConfig):
+    """``network_class_name: "VoxelNetNuscenesMultiHead"`` (second/pytorch/models/net_multi_head.py:121-176): an
+    RPNNoHead backbone with a DefaultHead on the concatenated map and a SmallObjectHead on the cropped stage-0 map.
+    Each class has its own anchor feature map (``class_settings.feature_map_size``, [1, H, W]); the classes of the
+    large head come first in the config."""
+    network_class: str = "VoxelNetNuscenesMultiHead"
+    class_feature_map_sizes: List[List[int]] = field(default_factory=list)
 
 
 def _one(v):
@@ -378,6 +395,40 @@ def _nusc_largea():
         direction_offset=0.78, nms_class_agnostic=True, eval_batch_size=1)
 
 
+def _nusc_mhead():
+    # second/configs/nuscenes/all.pp.mhead.config
+    def rng(z, r=50):
+        return [-r, -r, z, r, r, z]
+    big, small = [1, 100, 100], [1, 160, 160]
+    return MultiHeadModelConfig(
+        name="nuscenes.all.pp.mhead", point_cloud_range=[-50, -50, -5, 50, 50, 3],
+        voxel_size=[0.25, 0.25, 8], max_points_per_voxel=60, max_voxels=30000, num_point_features=4,
+        vfe_class="PillarFeatureNetRadius", vfe_num_filters=[64], vfe_with_distance=False,
+        middle_class="PointPillarsScatter", middle_num_input_features=64, middle_downsample_factor=1,
+        rpn_class="RPNNoHead", rpn_layer_nums=[3, 5, 5], rpn_layer_strides=[2, 2, 2],
+        rpn_num_filters=[64, 128, 256], rpn_upsample_strides=[0.5, 1, 2],
+        rpn_num_upsample_filters=[128, 128, 128], rpn_num_input_features=64,
+        classes=[
+            AnchorClass("bus", [2.94046906, 11.1885991, 3.47030982], [0, 1.57], anchor_ranges=rng(-0.0715754)),
+            AnchorClass("car", [1.95017717, 4.60718145, 1.72270761], [0, 1.57], anchor_ranges=rng(-0.93897414)),
+            AnchorClass("construction_vehicle", [2.73050468, 6.38352896, 3.13312415], [0, 1.57],
+                        anchor_ranges=rng(-0.08168083)),
+            AnchorClass("trailer", [3, 15, 3.8, 2, 3, 3.8], [0, 1.57], anchor_ranges=rng(0.22228277)),
+            AnchorClass("truck", [2.4560939, 6.73778078, 2.73004906], [0, 1.57], anchor_ranges=rng(-0.37937912)),
+            AnchorClass("barrier", [2.49008838, 0.48578221, 0.98297065], [0, 1.57], anchor_ranges=rng(-1.27247968, 40)),
+            AnchorClass("bicycle", [0.60058911, 1.68452161, 1.27192197], [0, 1.57], anchor_ranges=rng(-1.03743013, 40)),
+            AnchorClass("motorcycle", [0.76279481, 2.09973778, 1.44403034], [0, 1.57],
+                        anchor_ranges=rng(-0.99194854, 40)),
+            AnchorClass("pedestrian", [0.66344886, 0.7256437, 1.75748069], [0], anchor_ranges=rng(-0.73911038, 40)),
+            AnchorClass("traffic_cone", [0.39694519, 0.40359262, 1.06232151], [0], anchor_ranges=rng(-1.27868911, 40)),
+        ],
+        use_rotate_nms=False, use_multi_class_nms=False, nms_pre_max_size=1000, nms_post_max_size=300,
+        nms_score_threshold=0.05, nms_iou_threshold=0.5,
+        post_center_limit_range=[-59.6, -59.6, -10, 59.6, 59.6, 10], direction_limit_offset=0.0,
+        direction_offset=0.78, nms_class_agnostic=False, eval_batch_size=1,
+        class_feature_map_sizes=[big] * 5 + [small] * 5)
+
+
 BUILTIN = {
     "car.fhd": _car_fhd,
     "car.lite": _car_lite,
@@ -397,7 +448,18 @@ REFERENCE_FILES = {
 }
 
 
+# configs beyond the five BASELINE ones: get_config knows them, BUILTIN (what the BASELINE suites iterate) does not
+EXTRA = {
+    "nuscenes.all.pp.mhead": _nusc_mhead,
+}
+EXTRA_REFERENCE_FILES = {
+    "nuscenes.all.pp.mhead": "nuscenes/all.pp.mhead.config",
+}
+
+
 def get_config(name):
-    if name not in BUILTIN:
-        raise KeyError("unknown config %r (have %s)" % (name, sorted(BUILTIN)))
-    return BUILTIN[name]()
+    if name in BUILTIN:
+        return BUILTIN[name]()
+    if name in EXTRA:
+        return EXTRA[name]()
+    raise KeyError("unknown config %r (have %s)" % (name, sorted(BUILTIN) + sorted(EXTRA)))

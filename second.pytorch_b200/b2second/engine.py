@@ -12,11 +12,15 @@ buffers, so the whole frame batch is ONE CUDA graph:
      b2s_hash_build + b2s_vfe_mean over the caller's voxels   voxel_encoder.py:220-225,246-255
   per sparse layer: b2s_rulebook_{subm,conv} (cached per indice_key) + b2s_sparse_conv_tc (wgmma, fp16 hi/lo
       planes flow from layer to layer) with BatchNorm1d/ReLU folded into the epilogue      middle.py:145-192
-  b2s_pfn (PointPillars)                                       pointpillars.py:203-237
+  b2s_pfn (PointPillars) / b2s_pfn_ex (PillarFeatureNetRadius) pointpillars.py:203-237,240-325
   b2s_to_bev_tc (NHWC + halo, fp16 hi/lo)                      middle.py:206-209 / pointpillars.py:444-476
   RPN as a program of b2s_conv2d_tc_ex launches (tc.plan_rpn)  rpn.py:314-331,393-420,467-497
       (rpn_impl="cudnn" keeps the torch modules as a cross-check: fp32, TF32 off)
   b2s_decode_filter_strided + b2s_nms (+ direction/range epilogue)   voxelnet.py:377-645
+
+VoxelNetNuscenesMultiHead (net_multi_head.py:121-176) runs the same way with two head "segments": the large head's
+packed 1x1 convs on the concatenated map, and b2s_crop_nhwc of stage 0 -> three 3x3 convs -> the small head's packed
+1x1 convs; b2s_decode_filter_segments reads both records into ONE candidate list per frame, with global anchor ids.
 
 The network is read through ``b2second.spec.spec_from_module`` (attribute names of the reference), never through
 ``b2second.models`` classes or a ``ModelConfig``.
@@ -80,9 +84,9 @@ class InferenceEngine:
         self._graphs = {}
         # RPN: "tc" = hand-written wgmma implicit GEMM (csrc/conv_tc.cu, 3xF16), "cudnn" = torch/cuDNN fp32.
         if rpn_impl == "auto":
-            rpn_impl = "tc" if _tc.supported(s.rpn) else "cudnn"
+            rpn_impl = "tc" if _tc.supported(s.rpn, s.heads) else "cudnn"
         assert rpn_impl in ("tc", "cudnn")
-        if rpn_impl == "tc" and not _tc.supported(s.rpn):
+        if rpn_impl == "tc" and not _tc.supported(s.rpn, s.heads):
             raise ValueError("rpn_impl='tc': this RPN has a layer b2s_conv2d_tc_ex does not cover (channels % 64, kernel > 4)")
         self.rpn_impl = rpn_impl
         assert sparse_impl in ("tc", "fma")       # sparse-conv inner product: wgmma 3xF16 | fp32 FMA tiles
@@ -128,6 +132,7 @@ class InferenceEngine:
             if p["with_distance"]:
                 raise _spec.UnsupportedNetwork("PillarFeatureNet with_distance (off in every BASELINE config)")
             self.pfn_geom = (p["vx"], p["vy"], p["x_offset"], p["y_offset"])
+            self.pfn_deco = int(getattr(s, "pfn_decoration", 0))      # B2S_PFN_PLAIN / B2S_PFN_RADIUS
             self.feat_final_c = self.pfn_cout
             self.final_level = self.level0
             self.pfn_out = torch.zeros(cap0, self.pfn_cout, dtype=torch.float32, device=dev)
@@ -270,7 +275,8 @@ class InferenceEngine:
         rpn = self.spec.rpn
         if next(rpn.parameters()).device != dev:
             raise ValueError("the RPN's parameters must live on the engine's device")
-        plan = _tc.plan_rpn(rpn, H, W)
+        heads = getattr(self.spec, "heads", None)
+        plan = _tc.plan_rpn(rpn, H, W) if heads is None else _tc.plan_rpn_multihead(rpn, dict(heads), H, W)
         self.tc_prog = plan
         self.tc_plan = plan["ops"]
         # single-scale tail (one k = s = 1 deblock 128 -> 128 feeding the heads): one fused kernel, the deblock output
@@ -285,10 +291,18 @@ class InferenceEngine:
         self.tc_bufs = {"in": self.tc_bev}
         for name, (h, w, c) in plan["buffers"].items():
             self.tc_bufs[name] = plane(h, w, c)
-        hd = plan["heads"]
-        self.tc_head_stride = hd["stride"]
-        self.tc_heads = torch.zeros(B, hd["H"], hd["W"], self.tc_head_stride, dtype=torch.float32, device=dev)
-        self.tc_bufs["heads"] = (self.tc_heads, None)
+        if heads is not None:
+            # one packed fp32 record map per head segment [B, H, W, stride]
+            self.tc_seg_heads = {}
+            for sg in plan["segments"]:
+                t = torch.zeros(B, sg["H"], sg["W"], sg["stride"], dtype=torch.float32, device=dev)
+                self.tc_seg_heads[sg["name"]] = t
+                self.tc_bufs[sg["buffer"]] = (t, None)
+        else:
+            hd = plan["heads"]
+            self.tc_head_stride = hd["stride"]
+            self.tc_heads = torch.zeros(B, hd["H"], hd["W"], self.tc_head_stride, dtype=torch.float32, device=dev)
+            self.tc_bufs["heads"] = (self.tc_heads, None)
         self.tc_hw = (H, W)
         # background tiles (csrc/rpn_bg.cu): through the leading chain of 3x3 stride-1 layers, output tiles whose whole
         # receptive field is empty BEV are not computed but copied from the layer's response to an empty frame
@@ -338,6 +352,48 @@ class InferenceEngine:
             y = self.spec.rpn.conv_box(self._rpn_backbone(torch.zeros(1, self.bev_cd, H, W, device=self.dev)))
         return int(y.shape[2]), int(y.shape[3])
 
+    def _head_segments(self):
+        """multi-head network: [{"name", "H", "W", "a_loc", "base"}] in anchor order (large head first)."""
+        if self.rpn_impl == "tc":
+            segs = [{"name": g["name"], "H": g["H"], "W": g["W"], "a_loc": g["a_loc"]} for g in self.tc_prog["segments"]]
+        else:
+            D, H, W = self.final_level.shape
+            with torch.no_grad():
+                outs = self._rpn_multihead(torch.zeros(1, self.bev_cd, H, W, device=self.dev))
+            segs = [{"name": name, "H": int(o[0].shape[2]), "W": int(o[0].shape[3]), "a_loc": int(m._num_anchor_per_loc)}
+                    for (name, m), o in zip(self.spec.heads, outs)]
+        base = 0
+        for g in segs:
+            g["base"] = base
+            base += g["a_loc"] * g["H"] * g["W"]
+        want = self.spec.head_feature_map_sizes
+        got = [[g["H"], g["W"]] for g in segs]
+        if want is not None and got != [list(x) for x in want]:
+            raise _spec.UnsupportedNetwork("head maps %s do not match the per-class feature map sizes %s" % (got, want))
+        return segs
+
+    def _rpn_multihead(self, x):
+        """VoxelNetNuscenesMultiHead.network_forward after the scatter (net_multi_head.py:155-161) on the torch modules:
+        cuDNN cross-check path.  -> [(box, cls, dir) NCHW conv outputs] per head, large first."""
+        rpn = self.spec.rpn
+        ups, stage0 = [], None
+        for i in range(len(rpn.blocks)):
+            x = rpn.blocks[i](x)
+            if i == 0:
+                stage0 = x
+            if i - rpn._upsample_start_idx >= 0:
+                ups.append(rpn.deblocks[i - rpn._upsample_start_idx](x))
+        if len(ups) > 0:
+            x = torch.cat(ups, dim=1)
+        c = int(np.round(stage0.shape[2] * 0.1))
+        hd = dict(self.spec.heads)
+        small = hd["small"].net(stage0[:, :, c:-c, c:-c])
+        out = []
+        for m, feat in ((hd["large"], x), (hd["small"], small)):
+            out.append((m.conv_box(feat).contiguous(), m.conv_cls(feat).contiguous(),
+                        m.conv_dir_cls(feat).contiguous() if self.spec.use_direction_classifier else None))
+        return out
+
     def _rpn_backbone(self, x):
         """RPNNoHeadBase.forward (rpn.py:314-331) on the torch modules: cuDNN cross-check path only."""
         rpn = self.spec.rpn
@@ -352,9 +408,16 @@ class InferenceEngine:
 
     def _alloc_detect_buffers(self, cand_cap):
         s, dev = self.spec, self.dev
-        self.fH, self.fW = self._feature_hw()
-        self.a_loc = s.num_anchors_per_loc
-        self.A = self.a_loc * self.fH * self.fW
+        self.segments = None
+        if getattr(s, "heads", None) is None:
+            self.fH, self.fW = self._feature_hw()
+            self.a_loc = s.num_anchors_per_loc
+            self.A = self.a_loc * self.fH * self.fW
+        else:
+            self.segments = self._head_segments()
+            self.fH, self.fW = self.segments[0]["H"], self.segments[0]["W"]
+            self.a_loc = s.num_anchors_per_loc
+            self.A = sum(g["a_loc"] * g["H"] * g["W"] for g in self.segments)
         self.anchors = torch.zeros(self.A, self.code, dtype=torch.float32, device=dev)
         self._anchors_key = None
         try:
@@ -449,10 +512,16 @@ class InferenceEngine:
         if self.is_pillars:
             vx, vy, xo, yo = self.pfn_geom
             self._mark("pfn")
-            L.check(lib.b2s_pfn(L.ptr(pfn_points), self.F, L.ptr(pfn_slots), L.ptr(self.vox_num),
-                                L.ptr(self.vox_coors), L.ptr(self.num_voxels), self.level0.cap, self.T,
-                                L.ptr(self.pfn_w), L.ptr(self.pfn_scale), L.ptr(self.pfn_shift), self.pfn_cout,
-                                vx, vy, xo, yo, L.ptr(self.pfn_out), st), "b2s_pfn")
+            if self.pfn_deco == 0:
+                L.check(lib.b2s_pfn(L.ptr(pfn_points), self.F, L.ptr(pfn_slots), L.ptr(self.vox_num),
+                                    L.ptr(self.vox_coors), L.ptr(self.num_voxels), self.level0.cap, self.T,
+                                    L.ptr(self.pfn_w), L.ptr(self.pfn_scale), L.ptr(self.pfn_shift), self.pfn_cout,
+                                    vx, vy, xo, yo, L.ptr(self.pfn_out), st), "b2s_pfn")
+            else:
+                L.check(lib.b2s_pfn_ex(L.ptr(pfn_points), self.F, L.ptr(pfn_slots), L.ptr(self.vox_num),
+                                       L.ptr(self.vox_coors), L.ptr(self.num_voxels), self.level0.cap, self.T,
+                                       L.ptr(self.pfn_w), L.ptr(self.pfn_scale), L.ptr(self.pfn_shift), self.pfn_cout,
+                                       vx, vy, xo, yo, self.pfn_deco, L.ptr(self.pfn_out), st), "b2s_pfn_ex")
             feats, hilo = self.pfn_out, None
         else:
             feats, hilo = self.vfe_out, None          # hilo = (hi, lo, stride) once on the tensor pipe
@@ -521,6 +590,20 @@ class InferenceEngine:
         L.check(lib.b2s_to_bev(L.ptr(feats), L.ptr(fl.coors), L.ptr(fl.n_dev), fl.cap, self.feat_final_c, self.B,
                                D, H, W, L.ptr(self.bev), 0, st), "b2s_to_bev")
         self._mark("rpn")
+        if self.segments is not None:
+            outs = self._rpn_multihead(self.bev)
+            self._keep = outs
+            self._mark("decode_filter")
+            segs = []
+            for g, (box, cls, dirp) in zip(self.segments, outs):
+                HW = g["H"] * g["W"]
+                segs.append({"box": box.data_ptr(), "cls": cls.data_ptr(), "dir": dirp.data_ptr() if dirp is not None else None,
+                             "box_batch_stride": g["a_loc"] * self.code * HW, "cls_batch_stride": g["a_loc"] * s.num_class * HW,
+                             "dir_batch_stride": g["a_loc"] * s.num_direction_bins * HW, "ch_stride": HW, "pix_stride": 1,
+                             "a_loc": g["a_loc"], "H": g["H"], "W": g["W"], "anchor_base": g["base"]})
+            self._launch_decode_segments(segs, st)                                   # NCHW conv outputs
+            self._launch_nms(st)
+            return
         rpn = s.rpn
         x = self._rpn_backbone(self.bev)
         box = rpn.conv_box(x).contiguous()
@@ -561,6 +644,10 @@ class InferenceEngine:
                 self._mark("rpn_1x1")          # the 3x3 stack (k_conv3x3_tc2) is timed apart from the deblock/heads tail
                 marked_tail = True
             src, dst = self.tc_bufs[op["src"]], self.tc_bufs[op["dst"]]
+            if op["kind"] == "crop":                                  # small head input: stage 0 inside a zero halo
+                L.check(lib.b2s_crop_nhwc(L.ptr(src[0]), L.ptr(src[1]), self.B, op["Hin"], op["Win"], op["cin"],
+                                          op["crop"], L.ptr(dst[0]), L.ptr(dst[1]), st), "b2s_crop_nhwc")
+                continue
             cdst = dst[0].shape[-1]                                   # channels per pixel of the destination map
             esz = dst[0].element_size()
             o_hi = ctypes_ptr(dst[0].data_ptr() + esz * op["dst_coff"])
@@ -593,6 +680,20 @@ class InferenceEngine:
                 d["cout"], L.ptr(d["scale"]), L.ptr(d["shift"]), L.ptr(h["w_hi"]), L.ptr(h["w_lo"]), h["cout"], h["n_pad"],
                 L.ptr(h["scale"]), L.ptr(h["shift"]), L.ptr(self.tc_heads), self.tc_head_stride, L.ptr(self.status), st),
                 "b2s_rpn_tail_tc")
+        if self.segments is not None:
+            self._mark("decode_filter")
+            segs = []
+            for g, pg in zip(self.segments, self.tc_prog["segments"]):
+                t = self.tc_seg_heads[g["name"]]
+                esz, S, offs = t.element_size(), pg["stride"], pg["offsets"]
+                bs = g["H"] * g["W"] * S
+                segs.append({"box": t.data_ptr() + offs[0] * esz, "cls": t.data_ptr() + offs[1] * esz,
+                             "dir": t.data_ptr() + offs[2] * esz if s.use_direction_classifier else None,
+                             "box_batch_stride": bs, "cls_batch_stride": bs, "dir_batch_stride": bs, "ch_stride": 1,
+                             "pix_stride": S, "a_loc": g["a_loc"], "H": g["H"], "W": g["W"], "anchor_base": g["base"]})
+            self._launch_decode_segments(segs, st)                                   # packed NHWC head records
+            self._launch_nms(st)
+            return
         S = self.tc_head_stride
         self._mark("decode_filter")
         offs = self.tc_prog["heads"]["offsets"]
@@ -625,6 +726,15 @@ class InferenceEngine:
             self.code, s.num_class, s.num_direction_bins, self.score_thresh, L.ptr(self.cand_box),
             L.ptr(self.cand_score), L.ptr(self.cand_label), L.ptr(self.cand_dir), L.ptr(self.cand_anchor),
             L.ptr(self.cand_count), self.cand_cap, L.ptr(self.status), st), "b2s_decode_filter_strided")
+
+    def _launch_decode_segments(self, segs, st):
+        """several head maps -> one candidate list per frame (global anchor ids; the single-class NMS branch)."""
+        L, lib, s = self._L, self.lib, self.spec
+        L.check(lib.b2s_decode_filter_segments(
+            L.head_segments(segs), len(segs), L.ptr(self.anchors), L.ptr(self.anchors_mask) if self.use_mask else None,
+            self.A, self.B, self.code, s.num_class, s.num_direction_bins, self.score_thresh, L.ptr(self.cand_box),
+            L.ptr(self.cand_score), L.ptr(self.cand_label), L.ptr(self.cand_dir), L.ptr(self.cand_anchor),
+            L.ptr(self.cand_count), self.cand_cap, L.ptr(self.status), st), "b2s_decode_filter_segments")
 
     def _launch_nms(self, st):
         L, lib, s = self._L, self.lib, self.spec
@@ -682,7 +792,7 @@ class InferenceEngine:
         """how many of OUR kernels one pipeline pass launches (memsets and cuDNN kernels not counted)."""
         n = 7                                    # b2s_voxelize: insert, flag_scan, scan_sums, assign, fill, gather, finish
         if self.is_pillars:
-            n += 1                               # b2s_pfn
+            n += 1                               # b2s_pfn / b2s_pfn_ex
         for lyr in self.layers:
             if lyr["build_rb"]:
                 # subm_nbr / subm_ranked | mark, summary_scan, scan_sums, compact_words, nz_scan, scan_sums, emit,
@@ -694,7 +804,8 @@ class InferenceEngine:
             if lyr.get("in_split") is not None:
                 n += 1                           # b2s_split_f16
         if self.rpn_impl == "tc":
-            n += len(self.tc_plan) - (1 if self.tc_tail_fused else 0)   # one tensor-core kernel per RPN layer (fused tail: 1 for 2)
+            # one tensor-core kernel per RPN layer (fused tail: 1 for 2); the multi-head crop op is one b2s_crop_nhwc kernel
+            n += len(self.tc_plan) - (1 if self.tc_tail_fused else 0)
             if self.bg_idx:
                 # k_bg_layer per layer, k_bg_compact (+ k_bg_fill per layer unless the conv epilogue fills)
                 n += len(self.bg_idx) + 1 + (0 if self.bg_fused_fill else len(self.bg_idx))
@@ -702,7 +813,7 @@ class InferenceEngine:
             n += 1                               # b2s_merge_f16
         if self.mc:
             return n + 1 + 1 + 3 * (1 if self.mc_uniform else self.ncls) + 1      # ... + k_concat_classes
-        return n + 1 + 1 + 3                     # to_bev, decode_filter, nms: select_sort + iou_mask + reduce
+        return n + 1 + 1 + 3                     # to_bev, decode_filter(_segments), nms: select_sort + iou_mask + reduce
 
     def sparse_layer_stats(self):
         """sync; per sparse layer: rows in/out, pairs, algorithmic bytes and flops (SURVEY.md §8d formulas)."""

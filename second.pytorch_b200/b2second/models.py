@@ -7,9 +7,13 @@ contract and *state-dict keys*, so reference checkpoints load unchanged:
   VoxelNet.forward / network_forward / predict   second/pytorch/models/voxelnet.py:314-645
   SimpleVoxel / SimpleVoxelRadius                second/pytorch/models/voxel_encoder.py:206-255
   PillarFeatureNet / PFNLayer                    second/pytorch/models/pointpillars.py:22-65,153-237
+  PillarFeatureNetRadius                         second/pytorch/models/pointpillars.py:240-325
   PointPillarsScatter                            second/pytorch/models/pointpillars.py:420-476
   SpMiddleFHD / SpMiddleFHDLite                  second/pytorch/models/middle.py:110-210,417-483
   RPNV2 (RPNBase/RPNNoHeadBase)                  second/pytorch/models/rpn.py:202-420,467-497
+  RPNNoHead                                      second/pytorch/models/rpn.py:202-331,500-529
+  VoxelNetNuscenesMultiHead, SmallObjectHead,
+  DefaultHead                                    second/pytorch/models/net_multi_head.py:14-176
 
 Every module takes the ``spconv`` *backend module* it should build on: the product backend is
 ``second.pytorch_b200/spconv`` (CUDA, fails loudly without the extension); tests and the CPU
@@ -112,8 +116,46 @@ class PillarFeatureNet(nn.Module):
         return features.squeeze()
 
 
+class PillarFeatureNetRadius(nn.Module):
+    """PillarFeatureNet with the point's x, y replaced by its radius |xy|: F+4 Linear inputs."""
+
+    def __init__(self, num_input_features=4, num_filters=(64,), with_distance=False,
+                 voxel_size=(0.2, 0.2, 4), pc_range=(0, -40, -3, 70.4, 40, 1), **kw):
+        super().__init__()
+        assert len(num_filters) > 0
+        cin = num_input_features + 4 + (1 if with_distance else 0)
+        self._with_distance = with_distance
+        filters = [cin] + list(num_filters)
+        self.pfn_layers = nn.ModuleList([
+            PFNLayer(filters[i], filters[i + 1], last_layer=(i == len(filters) - 2))
+            for i in range(len(filters) - 1)])
+        self.vx = voxel_size[0]
+        self.vy = voxel_size[1]
+        self.x_offset = self.vx / 2 + pc_range[0]
+        self.y_offset = self.vy / 2 + pc_range[1]
+
+    def forward(self, features, num_voxels, coors):
+        dtype = features.dtype
+        points_mean = features[:, :, :3].sum(dim=1, keepdim=True) / num_voxels.type_as(features).view(-1, 1, 1)
+        f_cluster = features[:, :, :3] - points_mean
+        f_center = torch.zeros_like(features[:, :, :2])
+        f_center[:, :, 0] = features[:, :, 0] - (coors[:, 3].to(dtype).unsqueeze(1) * self.vx + self.x_offset)
+        f_center[:, :, 1] = features[:, :, 1] - (coors[:, 2].to(dtype).unsqueeze(1) * self.vy + self.y_offset)
+        radius = torch.norm(features[:, :, :2], p=2, dim=2, keepdim=True)
+        parts = [torch.cat([radius, features[:, :, 2:]], dim=2), f_cluster, f_center]
+        if self._with_distance:
+            parts.append(torch.norm(features[:, :, :3], 2, 2, keepdim=True))
+        features = torch.cat(parts, dim=-1)
+        T = features.shape[1]
+        mask = (num_voxels.int().unsqueeze(1) > torch.arange(T, dtype=torch.int, device=features.device).view(1, -1))
+        features = features * mask.unsqueeze(-1).type_as(features)
+        for pfn in self.pfn_layers:
+            features = pfn(features)
+        return features.squeeze()
+
+
 VFE_CLASSES = {"SimpleVoxel": SimpleVoxel, "SimpleVoxelRadius": SimpleVoxelRadius,
-               "PillarFeatureNet": PillarFeatureNet}
+               "PillarFeatureNet": PillarFeatureNet, "PillarFeatureNetRadius": PillarFeatureNetRadius}
 
 
 # ------------------------------------------------------------------------------- middle
@@ -191,7 +233,10 @@ MIDDLE_CLASSES = {"SpMiddleFHD": SpMiddleFHD, "SpMiddleFHDLite": SpMiddleFHDLite
 
 
 # ---------------------------------------------------------------------------------- RPN
-class RPNV2(nn.Module):
+class RPNNoHead(nn.Module):
+    """the RPN backbone without heads; forward returns ``stage{i}`` (block outputs), ``up{i}`` (deblock outputs) and
+    ``out`` (their concatenation), like RPNNoHeadBase.forward."""
+
     def __init__(self, num_class=2, layer_nums=(3, 5, 5), layer_strides=(2, 2, 2), num_filters=(128, 128, 256),
                  upsample_strides=(1, 2, 4), num_upsample_filters=(256, 256, 256), num_input_features=128,
                  num_anchor_per_loc=2, encode_background_as_zeros=True, use_direction_classifier=True,
@@ -203,6 +248,8 @@ class RPNV2(nn.Module):
         ratios = [upsample_strides[i] / np.prod(layer_strides[:i + self._upsample_start_idx + 1])
                   for i in range(len(upsample_strides))]
         assert all(r == ratios[0] for r in ratios)
+        self._num_filters = list(num_filters)
+        self._num_upsample_filters = list(num_upsample_filters)
         self._num_anchor_per_loc = num_anchor_per_loc
         self._num_direction_bins = num_direction_bins
         self._num_class = num_class
@@ -229,6 +276,30 @@ class RPNV2(nn.Module):
                 deblocks.append(nn.Sequential(up, _bn2d(num_upsample_filters[j]), nn.ReLU()))
         self.blocks = nn.ModuleList(blocks)
         self.deblocks = nn.ModuleList(deblocks)
+
+    def forward(self, x):
+        ups, res = [], {}
+        for i in range(len(self.blocks)):
+            x = self.blocks[i](x)
+            res["stage%d" % i] = x
+            if i - self._upsample_start_idx >= 0:
+                ups.append(self.deblocks[i - self._upsample_start_idx](x))
+        if len(ups) > 0:
+            x = torch.cat(ups, dim=1)
+        for i, up in enumerate(ups):
+            res["up%d" % i] = up
+        res["out"] = x
+        return res
+
+
+class RPNV2(RPNNoHead):
+    def __init__(self, num_class=2, layer_nums=(3, 5, 5), layer_strides=(2, 2, 2), num_filters=(128, 128, 256),
+                 upsample_strides=(1, 2, 4), num_upsample_filters=(256, 256, 256), num_input_features=128,
+                 num_anchor_per_loc=2, encode_background_as_zeros=True, use_direction_classifier=True,
+                 box_code_size=7, num_direction_bins=2):
+        super().__init__(num_class, layer_nums, layer_strides, num_filters, upsample_strides, num_upsample_filters,
+                         num_input_features, num_anchor_per_loc, encode_background_as_zeros, use_direction_classifier,
+                         box_code_size, num_direction_bins)
         final = sum(num_upsample_filters) if len(num_upsample_filters) else num_filters[-1]
         num_cls = num_anchor_per_loc * (num_class if encode_background_as_zeros else num_class + 1)
         self.conv_cls = nn.Conv2d(final, num_cls, 1)
@@ -261,6 +332,58 @@ class RPNV2(nn.Module):
         return ret
 
 
+RPN_CLASSES = {"RPNV2": RPNV2, "RPNNoHead": RPNNoHead}
+
+
+class DefaultHead(nn.Module):
+    """1x1 box / cls / dir convs; predictions flattened to [B, A_loc*H*W, k] in (a_loc, y, x) order."""
+
+    def __init__(self, num_filters, num_class, num_anchor_per_loc, box_code_size, num_direction_bins,
+                 use_direction_classifier, encode_background_as_zeros):
+        super().__init__()
+        self._num_anchor_per_loc = num_anchor_per_loc
+        self._num_direction_bins = num_direction_bins
+        self._num_class = num_class
+        self._use_direction_classifier = use_direction_classifier
+        self._box_code_size = box_code_size
+        num_cls = num_anchor_per_loc * (num_class if encode_background_as_zeros else num_class + 1)
+        self.conv_cls = nn.Conv2d(num_filters, num_cls, 1)
+        self.conv_box = nn.Conv2d(num_filters, num_anchor_per_loc * box_code_size, 1)
+        if use_direction_classifier:
+            self.conv_dir_cls = nn.Conv2d(num_filters, num_anchor_per_loc * num_direction_bins, 1)
+
+    def forward(self, x):
+        B = x.shape[0]
+        box_preds = self.conv_box(x)
+        cls_preds = self.conv_cls(x)
+        C, H, W = box_preds.shape[1:]
+        A = self._num_anchor_per_loc
+        box_preds = box_preds.view(-1, A, self._box_code_size, H, W).permute(0, 1, 3, 4, 2).contiguous()
+        cls_preds = cls_preds.view(-1, A, self._num_class, H, W).permute(0, 1, 3, 4, 2).contiguous()
+        ret = {"box_preds": box_preds.view(B, -1, self._box_code_size), "cls_preds": cls_preds.view(B, -1, self._num_class)}
+        if self._use_direction_classifier:
+            d = self.conv_dir_cls(x)
+            d = d.view(-1, A, self._num_direction_bins, H, W).permute(0, 1, 3, 4, 2).contiguous()
+            ret["dir_cls_preds"] = d.view(B, -1, self._num_direction_bins)
+        return ret
+
+
+class SmallObjectHead(DefaultHead):
+    """three Conv3x3 64 -> 64 (+BN, eps 1e-5, +ReLU) ahead of the 1x1 heads."""
+
+    def __init__(self, num_filters, num_class, num_anchor_per_loc, box_code_size, num_direction_bins,
+                 use_direction_classifier, encode_background_as_zeros):
+        super().__init__(64, num_class, num_anchor_per_loc, box_code_size, num_direction_bins,
+                         use_direction_classifier, encode_background_as_zeros)
+        self.net = nn.Sequential(
+            nn.Conv2d(num_filters, 64, 3, bias=False, padding=1), nn.BatchNorm2d(64), nn.ReLU(),
+            nn.Conv2d(64, 64, 3, bias=False, padding=1), nn.BatchNorm2d(64), nn.ReLU(),
+            nn.Conv2d(64, 64, 3, bias=False, padding=1), nn.BatchNorm2d(64), nn.ReLU())
+
+    def forward(self, x):
+        return super().forward(self.net(x))
+
+
 # ------------------------------------------------------------------------------ VoxelNet
 class _AnchorGeneratorInfo:
     def __init__(self, ac):
@@ -276,6 +399,9 @@ class MirrorTargetAssigner:
         self._cfg = cfg
         self._anchor_generators = [_AnchorGeneratorInfo(ac) for ac in cfg.classes]
         self._classes = [ac.class_name for ac in cfg.classes]
+        # per-class anchor feature maps (class_settings.feature_map_size); None: every class on cfg.feature_map_size
+        self._feature_map_sizes = [list(f) for f in cfg.class_feature_map_sizes] \
+            if getattr(cfg, "class_feature_map_sizes", None) else None
 
     @property
     def num_anchors_per_location(self):
@@ -284,13 +410,19 @@ class MirrorTargetAssigner:
     def generate_anchors(self, feature_map_size):
         a = generate_anchors(self._cfg)
         fm = [int(x) for x in feature_map_size]
-        assert a.shape[0] == self._cfg.num_anchors_per_loc * int(np.prod(fm)), "feature map size does not match the config"
+        if self._feature_map_sizes is None:
+            assert a.shape[0] == self._cfg.num_anchors_per_loc * int(np.prod(fm)), \
+                "feature map size does not match the config"
         return {"anchors": a}
 
+    def _class_hw(self, c):
+        fs = self._feature_map_sizes[c] if self._feature_map_sizes is not None else None
+        return int(np.prod(fs if fs else self._cfg.feature_map_size))
+
     def anchors_range(self, class_idx):
-        hw = int(np.prod(self._cfg.feature_map_size))
-        start = sum(g.num_anchors_per_localization for g in self._anchor_generators[:class_idx]) * hw
-        return start, start + self._anchor_generators[class_idx].num_anchors_per_localization * hw
+        start = sum(g.num_anchors_per_localization * self._class_hw(c)
+                    for c, g in enumerate(self._anchor_generators[:class_idx]))
+        return start, start + self._anchor_generators[class_idx].num_anchors_per_localization * self._class_hw(class_idx)
 
 
 class VoxelNet(nn.Module):
@@ -317,7 +449,7 @@ class VoxelNet(nn.Module):
             pc_range=self.voxel_generator.point_cloud_range)
         self.middle_feature_extractor = MIDDLE_CLASSES[cfg.middle_class](
             backend, cfg.dense_shape, num_input_features=cfg.middle_num_input_features)
-        self.rpn = RPNV2(
+        self.rpn = RPN_CLASSES[cfg.rpn_class](
             num_class=cfg.num_class, layer_nums=cfg.rpn_layer_nums, layer_strides=cfg.rpn_layer_strides,
             num_filters=cfg.rpn_num_filters, upsample_strides=cfg.rpn_upsample_strides,
             num_upsample_filters=cfg.rpn_num_upsample_filters, num_input_features=cfg.rpn_num_input_features,
@@ -531,6 +663,42 @@ def _voxelnet_finish_frame(self, sel_boxes, sel_scores, sel_labels, sel_dir, pos
             "label_preds": torch.zeros([0], dtype=torch.long, device=dev), "metadata": meta}
 
 
+class VoxelNetNuscenesMultiHead(VoxelNet):
+    """RPNNoHead backbone; a DefaultHead on the concatenated map for the large classes and a SmallObjectHead on the
+    stage-0 map cropped by round(0.1 H) on every side for the small ones.  The predictions are concatenated
+    (large first), which is the anchor order of the config (large classes listed first)."""
+    small_classes = ["pedestrian", "traffic_cone", "bicycle", "motorcycle", "barrier"]
+    large_classes = ["car", "truck", "trailer", "bus", "construction_vehicle"]
+
+    def __init__(self, cfg, backend):
+        super().__init__(cfg, backend)
+        assert cfg.num_class == 10 and isinstance(self.rpn, RPNNoHead) and not isinstance(self.rpn, RPNV2)
+        per_loc = {c.class_name: c.num_anchors_per_loc for c in cfg.classes}
+        head_kw = dict(num_class=cfg.num_class, encode_background_as_zeros=cfg.encode_background_as_zeros,
+                       use_direction_classifier=cfg.use_direction_classifier, box_code_size=cfg.box_code_size,
+                       num_direction_bins=cfg.num_direction_bins)
+        self.small_head = SmallObjectHead(num_filters=cfg.rpn_num_filters[0],
+                                          num_anchor_per_loc=sum(per_loc[c] for c in self.small_classes), **head_kw)
+        self.large_head = DefaultHead(num_filters=int(np.sum(cfg.rpn_num_upsample_filters)),
+                                      num_anchor_per_loc=sum(per_loc[c] for c in self.large_classes), **head_kw)
+
+    def network_forward(self, voxels, num_points, coors, batch_size):
+        voxel_features = self.voxel_feature_extractor(voxels, num_points, coors)
+        spatial_features = self.middle_feature_extractor(voxel_features, coors, batch_size)
+        rpn_out = self.rpn(spatial_features)
+        r1 = rpn_out["stage0"]
+        c = int(np.round(r1.shape[2] * 0.1))
+        small = self.small_head(r1[:, :, c:-c, c:-c])
+        large = self.large_head(rpn_out["out"])
+        res = {k: torch.cat([large[k], small[k]], dim=1) for k in ("box_preds", "cls_preds")}
+        if self._use_direction_classifier:
+            res["dir_cls_preds"] = torch.cat([large["dir_cls_preds"], small["dir_cls_preds"]], dim=1)
+        return res
+
+
+NETWORK_CLASSES = {"VoxelNet": VoxelNet, "VoxelNetNuscenesMultiHead": VoxelNetNuscenesMultiHead}
+
+
 VoxelNet._nms = _voxelnet_nms
 VoxelNet._predict_multiclass = _voxelnet_predict_multiclass
 VoxelNet._finish_frame = _voxelnet_finish_frame
@@ -541,7 +709,7 @@ def build_network(cfg, backend):
     if isinstance(cfg, str):
         from .config import get_config
         cfg = get_config(cfg)
-    return VoxelNet(cfg, backend)
+    return NETWORK_CLASSES[getattr(cfg, "network_class", "VoxelNet")](cfg, backend)
 
 
 # per-config constants for synthetic weights: head gain keeps box residuals O(0.3) (exp() stays finite),
@@ -556,6 +724,7 @@ SYNTH_INIT = {
     "all.fhd": dict(cls_bias=-1.526, head_gain=1.0),
     "pointpillars.car.xyres_16": dict(cls_bias=-3.421, head_gain=0.15),
     "nuscenes.all.pp.largea": dict(cls_bias=-3.888, head_gain=0.02),
+    "nuscenes.all.pp.mhead": dict(cls_bias=-3.9, head_gain=0.02),
 }
 
 
@@ -598,11 +767,13 @@ def seeded_init_(net, seed=0, cls_bias=None, head_gain=1.0, cls_sign=1.0):
         else:
             continue
         new[k] = t.to(v.dtype)
-    for hk in ("rpn.conv_cls.weight", "rpn.conv_box.weight", "rpn.conv_dir_cls.weight"):
-        if hk in new:
-            new[hk] = new[hk] * float(head_gain) * (float(cls_sign) if hk == "rpn.conv_cls.weight" else 1.0)
-    if cls_bias is not None and "rpn.conv_cls.bias" in new:
-        new["rpn.conv_cls.bias"] = torch.full_like(new["rpn.conv_cls.bias"], float(cls_bias))
+    for head in ("rpn", "small_head", "large_head"):      # the multi-head network's heads live beside the RPN
+        cls_w = head + ".conv_cls.weight"
+        for hk in (head + ".conv_cls.weight", head + ".conv_box.weight", head + ".conv_dir_cls.weight"):
+            if hk in new:
+                new[hk] = new[hk] * float(head_gain) * (float(cls_sign) if hk == cls_w else 1.0)
+        if cls_bias is not None and head + ".conv_cls.bias" in new:
+            new[head + ".conv_cls.bias"] = torch.full_like(new[head + ".conv_cls.bias"], float(cls_bias))
     merged = dict(sd)
     merged.update(new)
     net.load_state_dict(merged, strict=True)

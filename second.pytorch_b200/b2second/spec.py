@@ -9,9 +9,12 @@ the reference defines:
                       ``_nms_*``, ``_post_center_range``, ``_dir_offset`` ..., ``voxel_generator``, ``target_assigner``)
   SimpleVoxel(/Radius) second/pytorch/models/voxel_encoder.py:206-255 (``num_input_features``)
   PillarFeatureNet    second/pytorch/models/pointpillars.py:153-201 (``pfn_layers[i].linear/.norm``, ``vx vy x_offset y_offset``)
+  PillarFeatureNetRadius pointpillars.py:240-325 (same attributes; recognised, like every PFN, by its class name)
   SpMiddleFHD*        second/pytorch/models/middle.py:110-210 (``middle_conv`` = SparseSequential, ``sparse_shape``)
   PointPillarsScatter pointpillars.py:420-442 (``ny nx nchannels``)
   RPNV2               second/pytorch/models/rpn.py:202-420 (``blocks deblocks conv_box conv_cls conv_dir_cls _upsample_start_idx``)
+  VoxelNetNuscenesMultiHead  second/pytorch/models/net_multi_head.py:121-176 (``small_head.net/.conv_*``,
+                      ``large_head.conv_*``, an RPNNoHead ``rpn`` with ``blocks deblocks`` and no ``conv_box``)
 
 ``spec_from_module`` needs no CUDA and no ``spconv`` import: sparse conv layers are recognised by their
 attributes (``subm kernel_size stride padding dilation indice_key weight``), so a network built on ANY spconv
@@ -71,6 +74,13 @@ class NetSpec:
         if self.pfn is not None:
             sig["pfn"] = {k: (h(v) if isinstance(v, torch.Tensor) else v) for k, v in self.pfn.items()}
         sig["rpn"] = {k: h(v) for k, v in self.rpn.state_dict().items() if v.dtype.is_floating_point}
+        # keys only the radius PFN / the multi-head network have (the signature of every other network is unchanged)
+        if getattr(self, "pfn_decoration", 0):
+            sig["pfn_decoration"] = self.pfn_decoration
+        if getattr(self, "heads", None) is not None:
+            sig["heads"] = {name: {k: h(v) for k, v in m.state_dict().items() if v.dtype.is_floating_point}
+                            for name, m in self.heads}
+            sig["head_feature_map_sizes"] = self.head_feature_map_sizes
         return sig
 
 
@@ -97,7 +107,15 @@ def spec_from_module(net, max_voxels=None):
     # ---- VFE
     vfe = net.voxel_feature_extractor
     s.pfn = None
+    s.pfn_decoration = 0          # 0: PillarFeatureNet ([x, y, z, r, ...]), 1: PillarFeatureNetRadius ([|xy|, z, r, ...])
     if hasattr(vfe, "pfn_layers"):
+        name = type(vfe).__name__
+        # PillarFeatureNetRadiusHeight and PillarFeatureNetOld decorate differently (the latter overwrites x/y in place
+        # through a view, so its Linear sees the centre offsets twice): same attributes, other numbers
+        if name not in ("PillarFeatureNet", "PillarFeatureNetRadius"):
+            raise UnsupportedNetwork("voxel feature extractor %s (PillarFeatureNet and PillarFeatureNetRadius are "
+                                     "covered)" % name)
+        s.pfn_decoration = 1 if name == "PillarFeatureNetRadius" else 0
         s.vfe_kind = "pfn"
         if len(vfe.pfn_layers) != 1:
             raise UnsupportedNetwork("multi-layer PillarFeatureNet (every BASELINE config has num_filters=[64])")
@@ -109,7 +127,8 @@ def spec_from_module(net, max_voxels=None):
                  "cout": int(lyr.linear.weight.shape[0]), "vx": float(vfe.vx), "vy": float(vfe.vy),
                  "x_offset": float(vfe.x_offset), "y_offset": float(vfe.y_offset),
                  "with_distance": bool(getattr(vfe, "_with_distance", False))}
-        s.num_point_features = int(lyr.linear.weight.shape[1]) - 5 - (1 if s.pfn["with_distance"] else 0)
+        s.num_point_features = int(lyr.linear.weight.shape[1]) - (4 if s.pfn_decoration else 5) - \
+            (1 if s.pfn["with_distance"] else 0)
         s.vfe_num_features = s.num_point_features
     elif hasattr(vfe, "num_input_features") and not any(True for _ in vfe.parameters()):
         name = type(vfe).__name__
@@ -167,16 +186,21 @@ def spec_from_module(net, max_voxels=None):
         raise UnsupportedNetwork("PillarFeatureNet in front of a sparse middle extractor")
     # ---- RPN (layer plan is made by b2second.tc.plan_rpn from the module itself)
     rpn = net.rpn
-    for a in ("blocks", "deblocks", "conv_box", "conv_cls", "_upsample_start_idx", "_num_anchor_per_loc",
-              "_box_code_size", "_num_class"):
-        if not hasattr(rpn, a):
-            raise UnsupportedNetwork("RPN %s lacks attribute %s" % (type(rpn).__name__, a))
+    s.heads = None
+    s.head_feature_map_sizes = None
+    if hasattr(net, "small_head") or hasattr(net, "large_head"):
+        _multi_head(net, s)
+    else:
+        for a in ("blocks", "deblocks", "conv_box", "conv_cls", "_upsample_start_idx", "_num_anchor_per_loc",
+                  "_box_code_size", "_num_class"):
+            if not hasattr(rpn, a):
+                raise UnsupportedNetwork("RPN %s lacks attribute %s" % (type(rpn).__name__, a))
+        s.num_class = int(rpn._num_class)
+        s.box_code_size = int(rpn._box_code_size)
+        s.num_anchors_per_loc = int(rpn._num_anchor_per_loc)
+        s.use_direction_classifier = bool(getattr(rpn, "_use_direction_classifier", False))
+        s.num_direction_bins = int(getattr(rpn, "_num_direction_bins", 2))
     s.rpn = rpn
-    s.num_class = int(rpn._num_class)
-    s.box_code_size = int(rpn._box_code_size)
-    s.num_anchors_per_loc = int(rpn._num_anchor_per_loc)
-    s.use_direction_classifier = bool(getattr(rpn, "_use_direction_classifier", False))
-    s.num_direction_bins = int(getattr(rpn, "_num_direction_bins", 2))
     # ---- predict() parameters (voxelnet.py:104-143)
     if not getattr(net, "_encode_background_as_zeros", True) or not getattr(net, "_use_sigmoid_score", True):
         raise UnsupportedNetwork("softmax scores / background class (every BASELINE config: sigmoid, background as zeros)")
@@ -195,8 +219,70 @@ def spec_from_module(net, max_voxels=None):
     ta = getattr(net, "target_assigner", None)
     if ta is not None and hasattr(ta, "_anchor_generators"):
         s.class_anchor_counts = [int(g.num_anchors_per_localization) for g in ta._anchor_generators]
+    if s.heads is not None:
+        if s.multiclass_nms:
+            raise UnsupportedNetwork("the per-class NMS branch on the multi-head network")
+        _check_head_feature_maps(net, s)
     s.anchor_source = net
     return s
+
+
+def _head_module(m, what, with_net):
+    for a in ("conv_box", "conv_cls", "_num_anchor_per_loc", "_box_code_size", "_num_class") + (("net",) if with_net else ()):
+        if not hasattr(m, a):
+            raise UnsupportedNetwork("%s %s lacks attribute %s" % (what, type(m).__name__, a))
+    return m
+
+
+def _multi_head(net, s):
+    """VoxelNetNuscenesMultiHead (net_multi_head.py:121-176): large head (1x1 convs) on the RPN's concatenated map,
+    small head (3 x Conv3x3+BN+ReLU, then 1x1 convs) on stage 0 cropped by round(0.1 H); predictions concatenated
+    large first.  Any other arrangement is refused."""
+    rpn = net.rpn
+    if not (hasattr(net, "small_head") and hasattr(net, "large_head")):
+        raise UnsupportedNetwork("a multi-head network needs both small_head and large_head")
+    for a in ("blocks", "deblocks", "_upsample_start_idx"):
+        if not hasattr(rpn, a):
+            raise UnsupportedNetwork("RPN %s lacks attribute %s" % (type(rpn).__name__, a))
+    if hasattr(rpn, "conv_box") or hasattr(rpn, "conv_cls"):
+        raise UnsupportedNetwork("multi-head network whose RPN has heads of its own")
+    large = _head_module(net.large_head, "large_head", False)
+    small = _head_module(net.small_head, "small_head", True)
+    if hasattr(large, "net"):
+        raise UnsupportedNetwork("large_head with convolutions ahead of its 1x1 heads")
+    for a in ("_num_class", "_box_code_size", "_use_direction_classifier", "_num_direction_bins"):
+        if getattr(large, a, None) != getattr(small, a, None):
+            raise UnsupportedNetwork("the two heads disagree on %s" % a)
+    s.heads = [("large", large), ("small", small)]
+    s.num_class = int(large._num_class)
+    s.box_code_size = int(large._box_code_size)
+    s.num_anchors_per_loc = int(large._num_anchor_per_loc) + int(small._num_anchor_per_loc)
+    s.use_direction_classifier = bool(getattr(large, "_use_direction_classifier", False))
+    s.num_direction_bins = int(getattr(large, "_num_direction_bins", 2))
+
+
+def _check_head_feature_maps(net, s):
+    """the anchors of the target assigner's classes, in order, must be the large head's a_loc on one feature map followed
+    by the small head's on another (target_assigner.generate_anchors concatenates classes in config order)."""
+    ta = getattr(net, "target_assigner", None)
+    sizes = getattr(ta, "_feature_map_sizes", None)
+    counts = s.class_anchor_counts
+    if sizes is None or counts is None or len(sizes) != len(counts):
+        raise UnsupportedNetwork("multi-head network without per-class feature map sizes")
+    out, i = [], 0
+    for _, m in s.heads:
+        need, fs = int(m._num_anchor_per_loc), None
+        while need > 0 and i < len(counts):
+            f = [int(x) for x in sizes[i]]
+            if len(f) != 3 or f[0] != 1 or (fs is not None and f != fs):
+                raise UnsupportedNetwork("classes of one head on different feature maps (%s vs %s)" % (fs, f))
+            fs, need, i = f, need - counts[i], i + 1
+        if need != 0 or fs is None:
+            raise UnsupportedNetwork("per-class anchor counts do not add up to the heads' anchors per location")
+        out.append(fs[1:])
+    if i != len(counts):
+        raise UnsupportedNetwork("classes beyond the two heads' anchors")
+    s.head_feature_map_sizes = out
 
 
 def anchors_for(spec, feature_hw):

@@ -90,12 +90,16 @@ def _n_pad(cout):
     raise ValueError("Cout %d > 128 not supported by the tensor-core RPN" % cout)
 
 
-def supported(rpn):
-    """True when every layer of this RPNV2 maps onto b2s_conv2d_tc_ex (channels % 64 == 0, kernels <= 4x4)."""
+def supported(rpn, heads=None):
+    """True when every layer of this RPNV2 (or, with ``heads`` = the spec's [("large", m), ("small", m)], of this
+    multi-head network) maps onto b2s_conv2d_tc_ex (channels % 64 == 0, kernels <= 4x4)."""
     try:
-        plan_rpn(rpn, 64, 64, dry=True)
+        if heads is None:
+            plan_rpn(rpn, 64, 64, dry=True)
+        else:
+            plan_rpn_multihead(rpn, dict(heads), 64, 64, dry=True)
         return True
-    except (ValueError, AssertionError):
+    except (ValueError, AssertionError, AttributeError):
         return False
 
 
@@ -110,6 +114,79 @@ def plan_rpn(rpn, H, W, dry=False):
     Every op is one b2s_conv2d_tc_ex launch: conv k x k / stride / pad, or one (a, c) sub-grid of a k = s
     ConvTranspose2d; output channels are cut into slices of <= 128 (the kernel's n_pad) and `torch.cat` of the
     deblock outputs is a channel offset into the shared "cat" buffer."""
+    bufs, ops, emit, (cur, h, w), _ = _plan_backbone(rpn, H, W, dry)
+    heads = [rpn.conv_box, rpn.conv_cls] + ([rpn.conv_dir_cls] if rpn._use_direction_classifier else [])
+    offs, stride_s = _emit_heads(emit, heads, cur, "heads", h, w)
+    return {"buffers": bufs, "ops": ops, "in_channels": ops[0]["cin"],
+            "heads": {"offsets": offs, "stride": stride_s, "H": h, "W": w}}
+
+
+def plan_rpn_multihead(rpn, heads, H, W, dry=False):
+    """VoxelNetNuscenesMultiHead (second/pytorch/models/net_multi_head.py:121-176) on an H x W BEV map: the RPNNoHead
+    backbone up to the concatenated map, then
+      large head: its 1x1 box | cls | dir convs packed into one fp32 record per pixel of the concat map ("heads_large");
+      small head: a "crop" op (b2s_crop_nhwc: stage 0 cropped by c = round(0.1 H0) on every side into a zero-halo map),
+                  three Conv3x3 64 -> 64 + BN + ReLU, and its packed 1x1 heads ("heads_small").
+    ``heads`` = {"large": module, "small": module}.  Records wider than 128 channels are two launches (dst_coff 0 / 128).
+    -> {"buffers", "ops", "in_channels", "stage0", "crop", "segments": [{"name", "buffer", "offsets", "stride", "H", "W",
+    "a_loc"}, large first]} -- the order of the reference's torch.cat, hence of the anchors."""
+    bufs, ops, emit, (cur, h, w), (s0, h0, w0) = _plan_backbone(rpn, H, W, dry)
+    segs = []
+
+    def packed(m, src, name, hh, ww):
+        hd = [m.conv_box, m.conv_cls] + ([m.conv_dir_cls] if m._use_direction_classifier else [])
+        offs, stride_s = _emit_heads(emit, hd, src, "heads_" + name, hh, ww)
+        segs.append({"name": name, "buffer": "heads_" + name, "offsets": offs, "stride": stride_s, "H": hh, "W": ww,
+                     "a_loc": int(m._num_anchor_per_loc)})
+
+    large, small = heads["large"], heads["small"]
+    packed(large, cur, "large", h, w)
+    c0 = bufs[s0][2]
+    c = int(np.round(h0 * 0.1))
+    hc, wc = h0 - 2 * c, w0 - 2 * c
+    assert hc >= 1 and wc >= 1, "stage-0 map too small for the small head's crop"
+    bufs["crop"] = (hc, wc, c0)
+    ops.append({"kind": "crop", "src": s0, "dst": "crop", "crop": c, "cin": c0, "cout": c0, "Hin": h0, "Win": w0,
+                "Hg": hc, "Wg": wc, "Hout": hc, "Wout": wc, "kh": 0, "kw": 0, "taps": 0, "stride": 1, "pad": 0,
+                "n_pad": 0, "relu": False, "out_mul": 1, "off_h": 0, "off_w": 0, "dst_coff": 0, "planes": 2,
+                "padded": True, "shift": None, "v2": False})
+    mods = list(small.net.children())
+    assert len(mods) % 3 == 0
+    src = "crop"
+    for li in range(0, len(mods), 3):
+        conv, bn, relu = mods[li:li + 3]
+        assert isinstance(conv, nn.Conv2d) and conv.kernel_size == (3, 3) and conv.stride == (1, 1) and \
+            conv.padding == (1, 1) and conv.bias is None and conv.groups == 1
+        assert isinstance(bn, nn.BatchNorm2d) and isinstance(relu, nn.ReLU)
+        wt = conv.weight.detach()
+        wt = wt.permute(2, 3, 0, 1).reshape(9, wt.shape[0], wt.shape[1])
+        sc, sh = _fold_bn2d(bn)
+        dst = "small%s" % "ab"[(li // 3) % 2]
+        bufs[dst] = (hc, wc, wt.shape[1])
+        emit("head_conv", src, dst, wt, 3, 3, 1, 1, sc, sh, True, hc, wc, hc, wc, hc, wc)
+        src = dst
+    packed(small, src, "small", hc, wc)
+    return {"buffers": bufs, "ops": ops, "in_channels": ops[0]["cin"], "stage0": s0, "crop": c, "segments": segs}
+
+
+def _emit_heads(emit, heads, src, dst, h, w):
+    """box | cls | dir 1x1 convs packed into one fp32 record per pixel (bias as shift, padded to 4 channels);
+    -> (channel offsets of the heads in the record, record stride)."""
+    wt = torch.cat([hd.weight.detach()[:, :, 0, 0] for hd in heads], 0).unsqueeze(0)     # [1, sum Cout, Cin]
+    bias = torch.cat([hd.bias.detach() for hd in heads], 0).float().contiguous()
+    pad = (-wt.shape[1]) % 4
+    if pad:
+        wt = torch.cat([wt, torch.zeros(1, pad, wt.shape[2], device=wt.device, dtype=wt.dtype)], 1)
+        bias = torch.cat([bias, torch.zeros(pad, device=bias.device)])
+    stride_s = max(32, wt.shape[1])
+    emit("heads", src, dst, wt.contiguous(), 1, 1, 1, 0, None, bias, False, h, w, h, w, h, w, planes=1, padded=False)
+    offs = np.cumsum([0] + [hd.weight.shape[0] for hd in heads]).tolist()
+    return offs, stride_s
+
+
+def _plan_backbone(rpn, H, W, dry):
+    """blocks + deblocks of an RPN (RPNV2 or RPNNoHead) -> (buffers, ops, emit, (output buffer, h, w),
+    (stage-0 buffer, h, w))."""
     bufs, ops = {}, []
 
     def emit(kind, src, dst, w_t_co_ci, kh, kw, stride, pad, scale, shift, relu, hin, win, hg, wg, hout, wout,
@@ -139,6 +216,7 @@ def plan_rpn(rpn, H, W, dry=False):
             ops.append(d)
 
     cur, h, w = "in", H, W
+    stage0 = None
     ups = []                                   # (buffer, channels) of each deblock output, in order
     up_start = rpn._upsample_start_idx
     cat_hw = None
@@ -170,6 +248,8 @@ def plan_rpn(rpn, H, W, dry=False):
             emit("block", cur, dst, wt, 3, 3, st, 1, sc, sh, True, h, w, ho, wo, ho, wo)
             cur, h, w = dst, ho, wo
             li += 1
+        if bi == 0:
+            stage0 = (cur, h, w)
         j = bi - up_start
         if j >= 0:
             up, bn, relu = list(rpn.deblocks[j].children())
@@ -200,19 +280,7 @@ def plan_rpn(rpn, H, W, dry=False):
     if ups:
         bufs["cat"] = (cat_hw[0], cat_hw[1], sum(ups))
         cur, h, w = "cat", cat_hw[0], cat_hw[1]
-    # heads: box | cls | dir packed into one record per pixel, bias as shift
-    heads = [rpn.conv_box, rpn.conv_cls] + ([rpn.conv_dir_cls] if rpn._use_direction_classifier else [])
-    wt = torch.cat([hd.weight.detach()[:, :, 0, 0] for hd in heads], 0).unsqueeze(0)     # [1, sum Cout, Cin]
-    bias = torch.cat([hd.bias.detach() for hd in heads], 0).float().contiguous()
-    pad = (-wt.shape[1]) % 4
-    if pad:
-        wt = torch.cat([wt, torch.zeros(1, pad, wt.shape[2], device=wt.device, dtype=wt.dtype)], 1)
-        bias = torch.cat([bias, torch.zeros(pad, device=bias.device)])
-    stride_s = max(32, wt.shape[1])
-    emit("heads", cur, "heads", wt.contiguous(), 1, 1, 1, 0, None, bias, False, h, w, h, w, h, w, planes=1, padded=False)
-    offs = np.cumsum([0] + [hd.weight.shape[0] for hd in heads]).tolist()
-    return {"buffers": bufs, "ops": ops, "in_channels": ops[0]["cin"],
-            "heads": {"offsets": offs, "stride": stride_s, "H": h, "W": w}}
+    return bufs, ops, emit, (cur, h, w), stage0
 
 
 def fusable_tail(plan):

@@ -1,5 +1,5 @@
-// bev.cu -- sparse rows -> dense BEV map (b2s_to_bev) and the PointPillars feature net (b2s_pfn).
-// See include/b2second.h.  Pure HBM-bound data movement: zero-fill the dense map once, then one
+// bev.cu -- sparse rows -> dense BEV map (b2s_to_bev), the PointPillars feature net (b2s_pfn / b2s_pfn_ex) and the
+// crop of a halo-padded map into a zero-halo map (b2s_crop_nhwc).  See include/b2second.h.  Pure HBM-bound data movement: zero-fill the dense map once, then one
 // scattered write per (row, channel).
 #include <cuda_fp16.h>
 
@@ -73,7 +73,9 @@ __global__ void k_to_bev_tc(const float *__restrict__ feat, const __half *__rest
 // PointPillars PFN (single layer): one warp per pillar; lane l owns output channels l, l+32, ...
 // decorate each point with (xyz - mean xyz) and (xy - pillar centre), Linear(F+5 -> COUT), BN, ReLU,
 // max over the T slots (padded slots contribute relu(shift), exactly like the masked zero rows upstream).
-template <int COUT>
+// DECO = B2S_PFN_RADIUS (PillarFeatureNetRadius): the point's own features enter as [|xy|, z, r, ...] instead of
+// [x, y, z, r, ...], so the Linear has F+4 inputs.
+template <int COUT, int DECO>
 __global__ void __launch_bounds__(kThreads)
 k_pfn(const float *__restrict__ points, int F, const int *__restrict__ slots, const int *__restrict__ num,
       const int *__restrict__ coors, const int *__restrict__ n_dev, int cap_rows, int T,
@@ -81,7 +83,8 @@ k_pfn(const float *__restrict__ points, int F, const int *__restrict__ slots, co
       float vx, float vy, float xoff, float yoff, float *__restrict__ out)
 {
     constexpr int NCH = COUT / 32;
-    const int FIN = F + 5;
+    const int NRAW = DECO == B2S_PFN_RADIUS ? F - 1 : F;    // Linear inputs taken from the point itself
+    const int FIN = NRAW + 5;
     extern __shared__ float s_w[];  // [FIN][COUT] transposed weights
     for (int i = threadIdx.x; i < FIN * COUT; i += blockDim.x) {
         int c = i / FIN, f = i - c * FIN;  // weight is [COUT][FIN]
@@ -120,24 +123,77 @@ k_pfn(const float *__restrict__ points, int F, const int *__restrict__ slots, co
         const float *p = points + (size_t)__ldg(&sl[t]) * F;
         float feat[16];
 #pragma unroll
-        for (int f = 0; f < 8; ++f) feat[f] = (f < F) ? __ldg(&p[f]) : 0.f;
+        for (int f = 0; f < 9; ++f) feat[f] = (f < F) ? __ldg(&p[f]) : 0.f;
+        float raw[8];
+        if (DECO == B2S_PFN_RADIUS) {
+            // torch.norm(xy, p=2) with the multiply and add rounded separately, like the mean above
+            raw[0] = __fsqrt_rn(__fadd_rn(__fmul_rn(feat[0], feat[0]), __fmul_rn(feat[1], feat[1])));
+#pragma unroll
+            for (int f = 1; f < 8; ++f) raw[f] = feat[f + 1];
+        } else {
+#pragma unroll
+            for (int f = 0; f < 8; ++f) raw[f] = feat[f];
+        }
         float acc[NCH];
 #pragma unroll
         for (int j = 0; j < NCH; ++j) acc[j] = 0.f;
-        for (int f = 0; f < F; ++f)
+        for (int f = 0; f < NRAW; ++f)
 #pragma unroll
-            for (int j = 0; j < NCH; ++j) acc[j] = fmaf(feat[f], s_w[f * COUT + lane + 32 * j], acc[j]);
+            for (int j = 0; j < NCH; ++j) acc[j] = fmaf(raw[f], s_w[f * COUT + lane + 32 * j], acc[j]);
         float dec[5] = {__fsub_rn(feat[0], mx), __fsub_rn(feat[1], my), __fsub_rn(feat[2], mz),
                         __fsub_rn(feat[0], cx), __fsub_rn(feat[1], cy)};
 #pragma unroll
         for (int f = 0; f < 5; ++f)
 #pragma unroll
-            for (int j = 0; j < NCH; ++j) acc[j] = fmaf(dec[f], s_w[(F + f) * COUT + lane + 32 * j], acc[j]);
+            for (int j = 0; j < NCH; ++j) acc[j] = fmaf(dec[f], s_w[(NRAW + f) * COUT + lane + 32 * j], acc[j]);
 #pragma unroll
         for (int j = 0; j < NCH; ++j) best[j] = fmaxf(best[j], fmaxf(fmaf(acc[j], sc[j], sh[j]), 0.f));
     }
 #pragma unroll
     for (int j = 0; j < NCH; ++j) out[(size_t)row * COUT + lane + 32 * j] = best[j];
+}
+
+// interior window [c, H-c) x [c, W-c) of a halo-padded map [B, H+2, W+2, C] -> [B, Ho+2, Wo+2, C] whose halo is
+// written as zero; 16-byte vectors (C % 8 == 0)
+__global__ void k_crop_nhwc(const uint4 *__restrict__ src_hi, const uint4 *__restrict__ src_lo, int batch, int H, int W,
+                            int CV, int c, uint4 *__restrict__ dst_hi, uint4 *__restrict__ dst_lo)
+{
+    const int Ho = H - 2 * c, Wo = W - 2 * c;
+    const long long total = (long long)batch * (Ho + 2) * (Wo + 2) * CV;
+    for (long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x; gid < total;
+         gid += (long long)gridDim.x * blockDim.x) {
+        const int v = (int)(gid % CV);
+        long long px = gid / CV;
+        const int x = (int)(px % (Wo + 2));
+        px /= (Wo + 2);
+        const int y = (int)(px % (Ho + 2));
+        const int b = (int)(px / (Ho + 2));
+        uint4 hi = make_uint4(0u, 0u, 0u, 0u), lo = hi;
+        if (y >= 1 && y <= Ho && x >= 1 && x <= Wo) {
+            // dst interior pixel (y-1, x-1) = src pixel (y-1+c, x-1+c) = padded src (y+c, x+c)
+            const size_t s = (((size_t)b * (H + 2) + (y + c)) * (W + 2) + (x + c)) * CV + v;
+            hi = __ldg(&src_hi[s]);
+            lo = __ldg(&src_lo[s]);
+        }
+        dst_hi[gid] = hi;
+        dst_lo[gid] = lo;
+    }
+}
+
+template <int DECO>
+int pfn_launch(const float *points, int num_feat, const int *point_slots, const int *num_points_per_voxel,
+               const int *coors, const int *num_rows_dev, int cap_rows, int max_points, const float *weight,
+               const float *scale, const float *shift, int cout, float vx, float vy, float x_offset, float y_offset,
+               float *out, cudaStream_t stream)
+{
+    const int fin = num_feat + (DECO == B2S_PFN_RADIUS ? 4 : 5);
+    size_t smem = sizeof(float) * (size_t)fin * cout;
+    int warps_per_block = kThreads / 32;
+    k_pfn<64, DECO><<<b2s_cdiv(cap_rows, warps_per_block), kThreads, smem, stream>>>(
+        points, num_feat, point_slots, num_points_per_voxel, coors, num_rows_dev, cap_rows, max_points, weight,
+        scale, shift, vx, vy, x_offset, y_offset, out);
+    B2S_LAUNCH_OK();
+    return 0;
 }
 
 }  // namespace
@@ -186,16 +242,44 @@ extern "C" int b2s_pfn(const float *points, int num_feat, const int *point_slots
                        const float *shift, int cout, float vx, float vy, float x_offset, float y_offset,
                        float *out, void *stream_)
 {
+    return b2s_pfn_ex(points, num_feat, point_slots, num_points_per_voxel, coors, num_rows_dev, cap_rows, max_points,
+                      weight, scale, shift, cout, vx, vy, x_offset, y_offset, B2S_PFN_PLAIN, out, stream_);
+}
+
+extern "C" int b2s_pfn_ex(const float *points, int num_feat, const int *point_slots,
+                          const int *num_points_per_voxel, const int *coors, const int *num_rows_dev,
+                          int cap_rows, int max_points, const float *weight, const float *scale,
+                          const float *shift, int cout, float vx, float vy, float x_offset, float y_offset,
+                          int decoration, float *out, void *stream_)
+{
     cudaStream_t stream = (cudaStream_t)stream_;
     B2S_REQUIRE(num_feat >= 3 && num_feat <= 8, "b2s_pfn: num_feat must be 3..8");
     B2S_REQUIRE(cout == 64, "b2s_pfn: only Cout=64 (PillarFeatureNet num_filters=[64]) is built");
     B2S_REQUIRE(scale != nullptr && shift != nullptr, "b2s_pfn: scale/shift required (BN folded)");
+    B2S_REQUIRE(decoration == B2S_PFN_PLAIN || decoration == B2S_PFN_RADIUS,
+                "b2s_pfn_ex: decoration must be B2S_PFN_PLAIN (0) or B2S_PFN_RADIUS (1)");
     if (cap_rows == 0) return 0;
-    size_t smem = sizeof(float) * (size_t)(num_feat + 5) * cout;
-    int warps_per_block = kThreads / 32;
-    k_pfn<64><<<b2s_cdiv(cap_rows, warps_per_block), kThreads, smem, stream>>>(
-        points, num_feat, point_slots, num_points_per_voxel, coors, num_rows_dev, cap_rows, max_points, weight,
-        scale, shift, vx, vy, x_offset, y_offset, out);
+    if (decoration == B2S_PFN_RADIUS)
+        return pfn_launch<B2S_PFN_RADIUS>(points, num_feat, point_slots, num_points_per_voxel, coors, num_rows_dev,
+                                          cap_rows, max_points, weight, scale, shift, cout, vx, vy, x_offset, y_offset,
+                                          out, stream);
+    return pfn_launch<B2S_PFN_PLAIN>(points, num_feat, point_slots, num_points_per_voxel, coors, num_rows_dev, cap_rows,
+                                     max_points, weight, scale, shift, cout, vx, vy, x_offset, y_offset, out, stream);
+}
+
+extern "C" int b2s_crop_nhwc(const b2s_half *src_hi, const b2s_half *src_lo, int batch, int H, int W, int C, int crop,
+                             b2s_half *dst_hi, b2s_half *dst_lo, void *stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(batch >= 1 && H >= 1 && W >= 1 && crop >= 0 && H - 2 * crop >= 1 && W - 2 * crop >= 1,
+                "b2s_crop_nhwc: bad sizes (the window [crop, H-crop) x [crop, W-crop) must be non-empty)");
+    B2S_REQUIRE(C % 8 == 0 && ((uintptr_t)src_hi & 15) == 0 && ((uintptr_t)src_lo & 15) == 0 &&
+                    ((uintptr_t)dst_hi & 15) == 0 && ((uintptr_t)dst_lo & 15) == 0,
+                "b2s_crop_nhwc: C must be a multiple of 8 and the planes 16-byte aligned");
+    const long long total = (long long)batch * (H - 2 * crop + 2) * (W - 2 * crop + 2) * (C / 8);
+    k_crop_nhwc<<<bounded_grid(total), kThreads, 0, stream>>>(
+        reinterpret_cast<const uint4 *>(src_hi), reinterpret_cast<const uint4 *>(src_lo), batch, H, W, C / 8, crop,
+        reinterpret_cast<uint4 *>(dst_hi), reinterpret_cast<uint4 *>(dst_lo));
     B2S_LAUNCH_OK();
     return 0;
 }

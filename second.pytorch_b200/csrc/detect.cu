@@ -1,11 +1,13 @@
 // detect.cu -- SECOND predict step on the device (see include/b2second.h):
 //   b2s_decode_filter : box decode + sigmoid + score threshold over all anchors -> candidate list
+//                       (_strided: any head layout; _segments: several head maps into one list per frame)
 //   b2s_nms           : deterministic top-k (score desc, anchor asc) -> pairwise IoU bitmask
 //                       (rotated polygon clip, or stand-up boxes with the +1 convention)
 //                       -> greedy reduce in shared memory -> direction fix-up + range test
 //   b2s_nms_*_host    : numpy-facing spconv.utils signatures
 // Nothing here synchronises with the host (except the *_host wrappers, by contract).
 #include <math.h>
+#include <string.h>
 
 #include "common.cuh"
 
@@ -24,20 +26,14 @@ struct HeadStrides {
     int cs, ps;
 };
 
-__global__ void k_decode_filter(const float *__restrict__ box, const float *__restrict__ cls,
-                                const float *__restrict__ dir, HeadStrides hs, const float *__restrict__ anchors,
-                                const uint8_t *__restrict__ amask, int batch, int a_loc, int H, int W,
-                                int code, int ncls, int nbins, float thresh, float *cand_box,
-                                float *cand_score, int *cand_label, int *cand_dir, int *cand_anchor,
-                                int *cand_count, int cand_cap, unsigned *status)
+// one anchor: score = max over classes of the sigmoid (first class wins ties), threshold, append to frame b's list
+__device__ __forceinline__ void decode_filter_one(const float *__restrict__ box, const float *__restrict__ cls,
+                                                  const float *__restrict__ dir, const HeadStrides &hs,
+                                                  const float *__restrict__ an, int b, int al, int hw, int anchor_id,
+                                                  int code, int ncls, int nbins, float thresh, float *cand_box,
+                                                  float *cand_score, int *cand_label, int *cand_dir, int *cand_anchor,
+                                                  int *cand_count, int cand_cap, unsigned *status)
 {
-    const int HW = H * W;
-    const int A = a_loc * HW;
-    long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (gid >= (long long)batch * A) return;
-    const int b = (int)(gid / A), a = (int)(gid % A);
-    if (amask != nullptr && amask[gid] == 0) return;
-    const int al = a / HW, hw = a % HW;
     const size_t cs = (size_t)hs.cs, ps = (size_t)hs.ps;
     // class scores: the reference takes max/argmax over the SIGMOID scores (voxelnet.py:444,554-555), so
     // saturated or fp32-equal scores tie and the first class wins -- compare scores, not logits.
@@ -54,7 +50,6 @@ __global__ void k_decode_filter(const float *__restrict__ box, const float *__re
     const size_t slot = (size_t)b * cand_cap + pos;
     // box decode (second_box_decode): separate mul/add like the elementwise reference ops
     const float *bp = box + (size_t)b * hs.box_b + (size_t)al * code * cs + (size_t)hw * ps;
-    const float *an = anchors + (size_t)a * code;
     float t[kMaxCode], q[kMaxCode];
     for (int i = 0; i < code; ++i) { t[i] = __ldg(bp + (size_t)i * cs); q[i] = __ldg(&an[i]); }
     const float xa = q[0], ya = q[1], za = q[2], wa = q[3], la = q[4], ha = q[5], ra = q[6];
@@ -82,7 +77,55 @@ __global__ void k_decode_filter(const float *__restrict__ box, const float *__re
         }
     }
     cand_dir[slot] = dl;
-    cand_anchor[slot] = a;
+    cand_anchor[slot] = anchor_id;
+}
+
+__global__ void k_decode_filter(const float *__restrict__ box, const float *__restrict__ cls,
+                                const float *__restrict__ dir, HeadStrides hs, const float *__restrict__ anchors,
+                                const uint8_t *__restrict__ amask, int batch, int a_loc, int H, int W,
+                                int code, int ncls, int nbins, float thresh, float *cand_box,
+                                float *cand_score, int *cand_label, int *cand_dir, int *cand_anchor,
+                                int *cand_count, int cand_cap, unsigned *status)
+{
+    const int HW = H * W;
+    const int A = a_loc * HW;
+    long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= (long long)batch * A) return;
+    const int b = (int)(gid / A), a = (int)(gid % A);
+    if (amask != nullptr && amask[gid] == 0) return;
+    decode_filter_one(box, cls, dir, hs, anchors + (size_t)a * code, b, a / HW, a % HW, a, code, ncls, nbins, thresh,
+                      cand_box, cand_score, cand_label, cand_dir, cand_anchor, cand_count, cand_cap, status);
+}
+
+// several head maps (b2s_decode_filter_segments): segment s owns the global anchors [base_s, base_s + a_loc_s*H_s*W_s)
+struct Segments {
+    const float *box[B2S_MAX_HEAD_SEGMENTS], *cls[B2S_MAX_HEAD_SEGMENTS], *dir[B2S_MAX_HEAD_SEGMENTS];
+    HeadStrides hs[B2S_MAX_HEAD_SEGMENTS];
+    int a_loc[B2S_MAX_HEAD_SEGMENTS], H[B2S_MAX_HEAD_SEGMENTS], W[B2S_MAX_HEAD_SEGMENTS];
+    int base[B2S_MAX_HEAD_SEGMENTS];
+    int n;
+};
+
+__global__ void k_decode_filter_segments(Segments sg, const float *__restrict__ anchors,
+                                         const uint8_t *__restrict__ amask, int batch, int num_anchors, int code,
+                                         int ncls, int nbins, float thresh, float *cand_box, float *cand_score,
+                                         int *cand_label, int *cand_dir, int *cand_anchor, int *cand_count,
+                                         int cand_cap, unsigned *status)
+{
+    long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= (long long)batch * num_anchors) return;
+    const int b = (int)(gid / num_anchors), a = (int)(gid % num_anchors);
+    if (amask != nullptr && amask[gid] == 0) return;
+    int s = -1;
+#pragma unroll
+    for (int i = 0; i < B2S_MAX_HEAD_SEGMENTS; ++i)
+        if (i < sg.n && a >= sg.base[i] && a - sg.base[i] < sg.a_loc[i] * sg.H[i] * sg.W[i]) s = i;
+    if (s < 0) return;                                   // an anchor no segment covers (gaps are allowed)
+    const int HW = sg.H[s] * sg.W[s];
+    const int al = (a - sg.base[s]) / HW, hw = (a - sg.base[s]) % HW;
+    decode_filter_one(sg.box[s], sg.cls[s], sg.dir[s], sg.hs[s], anchors + (size_t)a * code, b, al, hw, a, code, ncls,
+                      nbins, thresh, cand_box, cand_score, cand_label, cand_dir, cand_anchor, cand_count, cand_cap,
+                      status);
 }
 
 // Per-class variant for the multi-class NMS branch (voxelnet.py:458-547): one candidate list per (class, frame) --
@@ -651,6 +694,46 @@ extern "C" int b2s_decode_filter_strided(const float *box, const float *cls, con
     return decode_filter_launch(box, cls, dir, hs, anchors, anchors_mask, batch, a_loc, H, W, code, ncls, nbins,
                                 score_thresh, cand_box, cand_score, cand_label, cand_dir, cand_anchor, cand_count_dev,
                                 cand_cap, status_dev, (cudaStream_t)stream_);
+}
+
+extern "C" int b2s_decode_filter_segments(const b2s_head_segment *segments, int num_segments, const float *anchors,
+                                          const uint8_t *anchors_mask, int num_anchors, int batch, int code, int ncls,
+                                          int nbins, float score_thresh, float *cand_box, float *cand_score,
+                                          int *cand_label, int *cand_dir, int *cand_anchor, int *cand_count_dev,
+                                          int cand_cap, unsigned *status_dev, void *stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(segments != nullptr && num_segments >= 1 && num_segments <= B2S_MAX_HEAD_SEGMENTS,
+                "b2s_decode_filter_segments: 1..4 segments");
+    B2S_REQUIRE(code >= 7 && code <= kMaxCode && ncls >= 1 && batch >= 1 && num_anchors >= 1 && cand_cap >= 1,
+                "b2s_decode_filter_segments: bad sizes");
+    Segments sg;
+    memset(&sg, 0, sizeof(sg));
+    sg.n = num_segments;
+    for (int i = 0; i < num_segments; ++i) {
+        const b2s_head_segment &g = segments[i];
+        B2S_REQUIRE(g.box != nullptr && g.cls != nullptr && g.a_loc >= 1 && g.H >= 1 && g.W >= 1 && g.anchor_base >= 0 &&
+                        (long long)g.anchor_base + (long long)g.a_loc * g.H * g.W <= num_anchors,
+                    "b2s_decode_filter_segments: segment %d lies outside [0, num_anchors) or has no box/cls tensor", i);
+        for (int j = 0; j < i; ++j) {
+            const b2s_head_segment &o = segments[j];
+            const long long lo = g.anchor_base > o.anchor_base ? g.anchor_base : o.anchor_base;
+            const long long e1 = (long long)g.anchor_base + (long long)g.a_loc * g.H * g.W;
+            const long long e2 = (long long)o.anchor_base + (long long)o.a_loc * o.H * o.W;
+            B2S_REQUIRE(lo >= (e1 < e2 ? e1 : e2), "b2s_decode_filter_segments: segments %d and %d overlap", j, i);
+        }
+        sg.box[i] = g.box; sg.cls[i] = g.cls; sg.dir[i] = g.dir;
+        sg.hs[i].box_b = g.box_batch_stride; sg.hs[i].cls_b = g.cls_batch_stride; sg.hs[i].dir_b = g.dir_batch_stride;
+        sg.hs[i].cs = g.ch_stride; sg.hs[i].ps = g.pix_stride;
+        sg.a_loc[i] = g.a_loc; sg.H[i] = g.H; sg.W[i] = g.W; sg.base[i] = g.anchor_base;
+    }
+    B2S_CUDA_OK(cudaMemsetAsync(cand_count_dev, 0, sizeof(int) * (size_t)batch, stream));
+    long long total = (long long)batch * num_anchors;
+    k_decode_filter_segments<<<b2s_cdiv(total, 256), 256, 0, stream>>>(
+        sg, anchors, anchors_mask, batch, num_anchors, code, ncls, nbins, score_thresh, cand_box, cand_score, cand_label,
+        cand_dir, cand_anchor, cand_count_dev, cand_cap, status_dev);
+    B2S_LAUNCH_OK();
+    return 0;
 }
 
 // multi-class NMS branch: per-(class, frame) candidate lists (class-major virtual frames, see k_decode_filter_mc).

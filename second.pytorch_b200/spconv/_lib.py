@@ -47,6 +47,9 @@ SIGNATURES = {
                            c_void_p]),
     "b2s_pfn": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
                         c_void_p, c_int, c_float, c_float, c_float, c_float, c_void_p, c_void_p]),
+    "b2s_pfn_ex": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                           c_void_p, c_int, c_float, c_float, c_float, c_float, c_int, c_void_p, c_void_p]),
+    "b2s_crop_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b2s_decode_filter": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                   c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                   c_int, c_void_p, c_void_p]),
@@ -78,6 +81,9 @@ SIGNATURES = {
                                           ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                           c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "b2s_decode_filter_segments": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                           c_void_p]),
     "b2s_decode_filter_multiclass": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_longlong, ctypes.c_longlong,
                                              ctypes.c_longlong, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                              c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -94,6 +100,22 @@ SIGNATURES = {
     "b2s_nms_aligned_host": (c_int, [c_void_p, c_int, c_float, c_float, c_int, c_void_p, c_int]),
     "b2s_nms_rotated_host": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p, c_int]),
 }
+
+
+class HeadSegment(ctypes.Structure):
+    """b2s_head_segment (include/b2second.h): one head map of b2s_decode_filter_segments."""
+    _fields_ = [("box", c_void_p), ("cls", c_void_p), ("dir", c_void_p), ("box_batch_stride", ctypes.c_longlong),
+                ("cls_batch_stride", ctypes.c_longlong), ("dir_batch_stride", ctypes.c_longlong), ("ch_stride", c_int),
+                ("pix_stride", c_int), ("a_loc", c_int), ("H", c_int), ("W", c_int), ("anchor_base", c_int)]
+
+
+def head_segments(segs):
+    """list of dicts with HeadSegment's field names (pointers as ints or None) -> ctypes array for the call."""
+    arr = (HeadSegment * len(segs))()
+    for i, d in enumerate(segs):
+        for k, v in d.items():
+            setattr(arr[i], k, v)
+    return arr
 
 
 def load():
