@@ -27,6 +27,9 @@
  *                       middle.py:146-191, folded into scale/shift/relu)
  *   b2s_to_bev          spconv.SparseConvTensor.dense() + view (middle.py:206-209) and
  *                       PointPillarsScatter.forward (second/pytorch/models/pointpillars.py:444-476)
+ *   b2s_sparse_conv_wgrad, b2s_rulebook_transpose, b2s_from_bev, b2s_split_f16_autoscale
+ *                       torch.ops.spconv.indice_conv_backward and the backward of dense() (training:
+ *                       second/pytorch/train.py through SubMConv3d / SparseConv3d)
  *   b2s_pfn             PillarFeatureNet.forward (pointpillars.py:203-237, single PFNLayer :51-65)
  *   b2s_pfn_ex          the same, or PillarFeatureNetRadius.forward (pointpillars.py:240-325)
  *   b2s_crop_nhwc       stage0[:, :, c:-c, c:-c] in VoxelNetNuscenesMultiHead.network_forward
@@ -218,12 +221,56 @@ int b2s_split_f16(const float *x, b2s_half *hi, b2s_half *lo, const int *num_row
                   int out_channels, int out_stride, void *stream);
 int b2s_merge_f16(const b2s_half *hi, const b2s_half *lo, float *x, const int *num_rows_dev, int cap_rows,
                   int row_floats, int in_stride, void *stream);
+/* b2s_split_f16 of x * 2^e with 2^e chosen on the device from max|x| over the live rows (the b2second.tc.pow2_scale
+ * rule: max|x| * 2^e in (2^12, 2^13]; 2^e = 1 when x is all zero or not finite) -- for gradients, which are often far
+ * below the fp16 normal range.  scale_dev [2] floats: [0] <- 2^-e (multiply the tensor-core result by it), [1] is
+ * workspace.  Two launches, no host sync. */
+int b2s_split_f16_autoscale(const float *x, b2s_half *hi, b2s_half *lo, const int *num_rows_dev, int cap_rows,
+                            int row_floats, int out_channels, int out_stride, float *scale_dev, void *stream);
+
+/* ---- sparse convolution backward (training) ------------------------------------------------------ */
+/* Input gradient (dgrad) is the forward contraction on a transposed table, computed by b2s_sparse_conv /
+ * b2s_sparse_conv_tc(_plan) with weights W'[k] = W[k]^T ([K, Cout, Cin]):
+ *   SubM (odd kernel): nbr is its own transpose under k <-> K-1-k, so use the same nbr and W'[k] = W[K-1-k]^T;
+ *   strided:           use nbrT from b2s_rulebook_transpose and W'[k] = W[k]^T. */
+/* nbrT[i][k] = o for nbr[o][k] = i, else -1: the input-side table of a strided conv (for one kernel offset an input row
+ * reaches at most one output row).  nbrT [cap_in, K] is filled with -1 first; entries naming a row >= cap_in are
+ * dropped and raise B2S_STATUS_ROWS_OVERFLOW (status_dev may be NULL). */
+int b2s_rulebook_transpose(const int *nbr, const int *num_out_dev, int cap_out, int K, int *nbrT, int cap_in,
+                           unsigned *status_dev, void *stream);
+/* Weight gradient dW[k] = sum_o in[nbr[o,k],:]^T dout[o,:] (fp32 FMA, any widths): dW [K, Cin, Cout] (the reference's
+ * weight layout viewed flat), times *scale_dev when scale_dev is not NULL (e.g. the 2^-e of a scaled dout).
+ * Deterministic (no float atomics): launch 1 writes one partial per 2048-row slab of output rows (rows ascending inside
+ * the slab) into the workspace, launch 2 adds the slabs in order. */
+size_t b2s_sparse_conv_wgrad_workspace_bytes(int cap_out, int K, int cin, int cout);
+int b2s_sparse_conv_wgrad(const float *feat_in, int cin, const float *dout, int cout, const int *nbr, int K,
+                          const int *num_out_dev, int cap_out, const float *scale_dev, float *dweight, void *workspace,
+                          size_t workspace_bytes, void *stream);
+/* the same contraction on the tensor pipe (wgmma f16, 3xF16 split: X_hi*dY_hi + X_hi*dY_lo + X_lo*dY_hi, fp32
+ * accumulation): Cin in {8, 16, 32, 64}, Cout in {16, 32, 64}, K <= 27 (the b2s_sparse_conv_tc_supported table).
+ *   feat_hi/lo   input rows as for b2s_sparse_conv_tc (in_stride halves, 16-byte aligned);
+ *   dout_hi/lo   dY rows (dout_stride halves), e.g. from b2s_split_f16_autoscale with its 2^-e passed as scale_dev;
+ *   perm / tile_mask  the forward's tile plan (b2s_sparse_tile_plan; either may be NULL): rows are reduced in perm order,
+ *                and 64-row chunks whose tile has none of a K block's offsets are skipped -- bit-identical with and
+ *                without tile_mask (same perm);
+ *   dweight      [K, Cin, Cout] fp32 (times *scale_dev when not NULL).  Deterministic: fixed chunk chains inside
+ *                2048-row slabs, slab partials (workspace) added in order by a second launch. */
+size_t b2s_sparse_conv_wgrad_tc_workspace_bytes(int cap_out, int K, int cin, int cout);
+int b2s_sparse_conv_wgrad_tc(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in, int cin,
+                             const b2s_half *dout_hi, const b2s_half *dout_lo, int dout_stride, int cout, const int *nbr,
+                             int K, const int *num_out_dev, int cap_out, const int *perm, const unsigned *tile_mask,
+                             const float *scale_dev, float *dweight, void *workspace, size_t workspace_bytes,
+                             void *stream);
 
 /* ---- dense BEV map ----------------------------------------------------------------------------- */
 #define B2S_LAYOUT_NCHW 0 /* out[b, c*D+z, y, x]  (== dense() [B,C,D,H,W] viewed [B,C*D,H,W]) */
 #define B2S_LAYOUT_NHWC 1 /* out[b, y, x, c*D+z] */
 int b2s_to_bev(const float *feat, const int *coors, const int *num_rows_dev, int cap_rows, int C,
                int batch, int D, int H, int W, float *out, int layout, void *stream);
+/* backward of b2s_to_bev: drows[r][c] = dmap at the position b2s_to_bev writes row r, channel c to (same layouts;
+ * 0 for rows whose coordinate lies outside the map) */
+int b2s_from_bev(const float *dmap, const int *coors, const int *num_rows_dev, int cap_rows, int C, int batch, int D,
+                 int H, int W, int layout, float *drows, void *stream);
 
 /* BEV map for the tensor-core RPN: NHWC with a one-pixel zero halo, [B, H+2, W+2, C*D], as two fp16 planes
  * hi = fp16(x), lo = fp16(x - hi) (the 3xF16 split b2s_conv2d_tc consumes).  Rows come as fp32 `feat` [rows, C]

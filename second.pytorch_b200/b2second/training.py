@@ -1,0 +1,27 @@
+"""Training through the CUDA ``spconv`` drop-in.
+
+Upstream ``spconv`` 1.x is mostly used to train: ``second/pytorch/train.py train`` runs ``SubMConv3d`` /
+``SparseConv3d`` forward and backward (``torch.ops.spconv.indice_conv_backward``).  The backward here is opt-in, the
+same way ``fastpath.accelerate(net)`` is the opt-in for the fused inference engine::
+
+    net = training.enable_sparse_backward(net)
+    net.train()
+    loss = criterion(net(example)); loss.backward()
+
+A marked sparse convolution in ``train()`` mode with grad enabled records autograd: its forward runs the inference
+kernels with fp32 output rows, its backward computes the input gradient on the same kernels over the transposed
+neighbour table (the tensor pipe where the widths allow, with the gradient split under an automatic power-of-two scale)
+and the weight gradient with ``b2s_sparse_conv_wgrad``.  BatchNorm1d and ReLU run as the torch modules that follow the
+conv.  ``eval()`` keeps the fused BN/ReLU inference path, marked or not; an unmarked conv in training mode still raises
+``NotImplementedError``.  Not covered: the fused engine, fp16/AMP, transposed / inverse sparse convs.
+"""
+
+
+def enable_sparse_backward(module):
+    """mark every ``spconv.SparseConvolution`` (the CUDA drop-in's) under ``module`` for training; returns ``module``."""
+    from . import loader
+    sp = loader.product_spconv()
+    for m in module.modules():
+        if isinstance(m, sp.SparseConvolution):
+            m._b2s_backward = True
+    return module

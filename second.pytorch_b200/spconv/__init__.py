@@ -103,30 +103,112 @@ class SparseConvTensor:
     def dense(self, channels_first=True):
         feats = self.features
         _lib.require_cuda(feats, "SparseConvTensor.features")
-        lib = _lib.load()
         feats = feats.contiguous().float()
+        if channels_first or self.spatial_shape[0] == 1:
+            layout = 0 if channels_first else 1
+            if feats.requires_grad and torch.is_grad_enabled():
+                return _DenseFunction.apply(feats, self, layout)     # training: the gradient flows back to the rows
+            return self._to_bev(feats, layout)
+        # channels_last with D>1: [B,D,H,W,C] is not a BEV layout; go through NCDHW once
+        return self.dense(True).permute(0, 2, 3, 4, 1).contiguous()
+
+    def _to_bev(self, feats, layout):
+        """fp32 rows -> [B,C,D,H,W] (layout 0) or [B,H,W,C] (layout 1, D == 1) through b2s_to_bev."""
+        lib = _lib.load()
         idx = self.indices.contiguous()
         n, C = feats.shape
         D, H, W = self.spatial_shape
         B = self.batch_size
         dev = feats.device
         n_dev = torch.tensor([n], dtype=torch.int32, device=dev)
-        if channels_first:
+        if layout == 0:
             out = torch.empty(B, C, D, H, W, dtype=torch.float32, device=dev)
-            layout = 0
         else:
             out = torch.empty(B, D, H, W, C, dtype=torch.float32, device=dev)
-            layout = 1
-        if channels_first or D == 1:
-            _lib.check(lib.b2s_to_bev(_lib.ptr(feats), _lib.ptr(idx), _lib.ptr(n_dev), n, C, B, D, H, W,
-                                      _lib.ptr(out), layout, _lib.stream()), "b2s_to_bev")
-            return out
-        # channels_last with D>1: [B,D,H,W,C] is not a BEV layout; go through NCDHW once
-        return self.dense(True).permute(0, 2, 3, 4, 1).contiguous()
+        _lib.check(lib.b2s_to_bev(_lib.ptr(feats), _lib.ptr(idx), _lib.ptr(n_dev), n, C, B, D, H, W,
+                                  _lib.ptr(out), layout, _lib.stream()), "b2s_to_bev")
+        return out
 
     @property
     def sparity(self):
         return self.indices.shape[0] / np.prod(self.spatial_shape) / self.batch_size
+
+
+class _DenseFunction(torch.autograd.Function):
+    """SparseConvTensor.dense() with its backward: the gradient of each row is gathered from the dense gradient at the
+    row's position (b2s_from_bev)."""
+
+    @staticmethod
+    def forward(ctx, feats, x, layout):
+        ctx.x, ctx.layout, ctx.shape = x, layout, feats.shape
+        return x._to_bev(feats, layout)
+
+    @staticmethod
+    def backward(ctx, grad):
+        x = ctx.x
+        n, C = ctx.shape
+        D, H, W = x.spatial_shape
+        grad = grad.contiguous().float()
+        drows = torch.empty(n, C, dtype=torch.float32, device=grad.device)
+        if n > 0:
+            lib = _lib.load()
+            n_dev = torch.tensor([n], dtype=torch.int32, device=grad.device)
+            _lib.check(lib.b2s_from_bev(_lib.ptr(grad), _lib.ptr(x.indices.contiguous()), _lib.ptr(n_dev), n, C,
+                                        x.batch_size, D, H, W, ctx.layout, _lib.ptr(drows), _lib.stream()),
+                       "b2s_from_bev")
+        return drows, None, None
+
+
+class _SparseConvFunction(torch.autograd.Function):
+    """one sparse convolution of the module path with its backward (torch.ops.spconv.indice_conv_backward upstream):
+      dX  the forward contraction over the transposed table with W'[k] = W[k]^T (SparseConvolution._dgrad),
+      dW  b2s_sparse_conv_wgrad_tc on the tensor pipe, else b2s_sparse_conv_wgrad,
+      db  dY summed over the rows.
+    Only the gradients autograd asks for are computed.  The weight is saved for backward, so autograd's version check
+    refuses a backward after an in-place change of the weight."""
+
+    @staticmethod
+    def forward(ctx, feats, weight, bias, conv, rb):
+        ctx.conv, ctx.rb = conv, rb
+        ctx.save_for_backward(feats, weight)
+        return conv._forward_rows(feats, rb)
+
+    @staticmethod
+    def backward(ctx, dy):
+        feats, weight = ctx.saved_tensors
+        conv, rb = ctx.conv, ctx.rb
+        dy = dy.contiguous().float()
+        split = _GradSplit(dy)
+        dx = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dx = conv._dgrad(dy, weight, rb, feats.shape[0], split)
+        if ctx.needs_input_grad[1]:
+            dw = conv._wgrad(feats, dy, rb, split).view_as(weight)
+        if ctx.needs_input_grad[2]:
+            db = dy.sum(0)
+        return dx, dw, db, None, None
+
+
+class _GradSplit:
+    """fp32 rows [n, c] as fp16 hi/lo planes of `channels` (>= c, zero padded) halves, scaled by a power of two picked on
+    the device (b2s_split_f16_autoscale), made on first use -- dY shared by the tensor-pipe dgrad and wgrad, and X for the
+    wgrad: (hi, lo, row stride in halves, 2^-e as a [1] device tensor)."""
+
+    def __init__(self, t, channels=None):
+        self.t, self.channels, self._planes = t, channels, None
+
+    def planes(self):
+        if self._planes is None:
+            t = self.t
+            n, c = t.shape
+            cp = self.channels or c
+            buf = torch.empty(max(n, 1), 2, cp, dtype=torch.float16, device=t.device)
+            sc = torch.empty(2, dtype=torch.float32, device=t.device)
+            lib = _lib.load()
+            _lib.check(lib.b2s_split_f16_autoscale(_lib.ptr(t), _lib.ptr(buf[:, 0]), _lib.ptr(buf[:, 1]), None, n, c, cp,
+                                                   2 * cp, _lib.ptr(sc), _lib.stream()), "b2s_split_f16_autoscale")
+            self._planes = (buf[:, 0], buf[:, 1], 2 * cp, sc[:1])
+        return self._planes
 
 
 class SparseModule(nn.Module):
@@ -280,13 +362,15 @@ class SparseConvolution(SparseModule):
 
     def forward(self, input, _epilogue=None):
         assert isinstance(input, SparseConvTensor)
-        if self.training and torch.is_grad_enabled() and self.weight.requires_grad:
-            # upstream implements indice_conv_backward; this drop-in covers the inference path only (SURVEY.md §8(f)4).
-            # A training-mode call that autograd would record must fail instead of silently returning gradient-free
-            # tensors.  (eval() with autograd enabled is the reference's own inference mode -- voxelnet.py:368-374 --
-            # and runs; so does anything under torch.no_grad().)
-            raise NotImplementedError("b2second spconv: training / autograd through sparse convolutions is not "
-                                      "implemented (inference drop-in); call net.eval() and run under torch.no_grad()")
+        record = self.training and torch.is_grad_enabled()
+        if record and self.weight.requires_grad and not self._b2s_backward:
+            # The backward (upstream's indice_conv_backward) is opt-in: b2second.training.enable_sparse_backward(net).
+            # Without it a training-mode call that autograd would record must fail instead of silently returning
+            # gradient-free tensors.  (eval() with autograd enabled is the reference's own inference mode --
+            # voxelnet.py:368-374 -- and runs; so does anything under torch.no_grad().)
+            raise NotImplementedError("b2second spconv: autograd through sparse convolutions is opt-in: call "
+                                      "b2second.training.enable_sparse_backward(net) to train, or net.eval() / "
+                                      "torch.no_grad() for inference")
         lib = _lib.load()
         K = int(np.prod(self.kernel_size))
         # a 1x1x1 stride-1 conv keeps the active set (upstream short-circuits it to a plain mm)
@@ -312,6 +396,12 @@ class SparseConvolution(SparseModule):
         out._hash = rb.out_hash
         out.indice_dict = input.indice_dict
         out.grid = input.grid
+        if record and self._b2s_backward:
+            # training (opt-in): fp32 output rows recorded by autograd; BN / ReLU run as the torch modules that follow
+            feats = input.features
+            _lib.require_cuda(feats, "SparseConvTensor.features")
+            out._features = _SparseConvFunction.apply(feats.contiguous().float(), self.weight, self.bias, self, rb)
+            return out
         from b2second import tc as _tc
         cin_tc = _tc.sparse_tc_cin(self.in_channels)
         use_tc = (USE_TENSOR_CORES and cin_tc is not None
@@ -359,6 +449,142 @@ class SparseConvolution(SparseModule):
                                            _lib.stream()), "b2s_sparse_conv")
         out._features = out_feats
         return out
+
+    # ---- training (b2second.training.enable_sparse_backward sets _b2s_backward) --------------------------------------
+    _b2s_backward = False
+
+    def _forward_rows(self, feats, rb):
+        """fp32 output rows [n_out, Cout] (+ bias) from fp32 input rows, on the kernel the inference path would pick
+        (tensor pipe with fp32 output, or b2s_sparse_conv)."""
+        lib = _lib.load()
+        K, n_in, n_out = rb.K, feats.shape[0], rb.num_out
+        dev = feats.device
+        shift = self.bias.detach().float().contiguous() if self.bias is not None else None
+        out = torch.empty(n_out, self.out_channels, dtype=torch.float32, device=dev)
+        if n_out == 0:
+            return out
+        cin_tc = self._wgrad_tc_cin(lib, K)
+        if cin_tc is not None:
+            buf = self._split_rows(feats, cin_tc)
+            hi, lo = buf[:, 0], buf[:, 1]
+            w_hi, w_lo, ws, inv = self._tc_weights(cin_tc)
+            status = torch.zeros(1, dtype=torch.int32, device=dev)
+            perm, tmask = ops.tile_plan(rb)
+            _lib.check(lib.b2s_sparse_conv_tc_plan(
+                _lib.ptr(hi), _lib.ptr(lo), 2 * cin_tc, buf.shape[0], cin_tc, _lib.ptr(w_hi), _lib.ptr(w_lo),
+                _lib.ptr(rb.nbr), K, _lib.ptr(rb.num_out_dev), n_out, _lib.ptr(perm), _lib.ptr(tmask), _lib.ptr(inv),
+                _lib.ptr(shift), 0, _lib.ptr(out), None, self.out_channels, self.out_channels, _lib.ptr(status),
+                _lib.stream()), "b2s_sparse_conv_tc_plan")
+            return out
+        w = self.weight.detach().float().contiguous().view(K, self.in_channels, self.out_channels)
+        _lib.check(lib.b2s_sparse_conv(_lib.ptr(feats), self.in_channels, _lib.ptr(w), _lib.ptr(rb.nbr), K,
+                                       _lib.ptr(rb.num_out_dev), n_out, None, _lib.ptr(shift), 0, _lib.ptr(out),
+                                       self.out_channels, _lib.stream()), "b2s_sparse_conv")
+        return out
+
+    def _wgrad_tc_cin(self, lib, K):
+        """channel count of the tensor-pipe forward / weight gradient (the input padded to 8), or None: fp32 kernels"""
+        from b2second import tc as _tc
+        cin_tc = _tc.sparse_tc_cin(self.in_channels)
+        if (USE_TENSOR_CORES and cin_tc is not None and K <= 27
+                and bool(lib.b2s_sparse_conv_tc_supported(cin_tc, self.out_channels))):
+            return cin_tc
+        return None
+
+    def _split_rows(self, feats, cin_tc):
+        """fp32 rows -> interleaved fp16 hi/lo planes [max(n, 1), 2, cin_tc] (b2s_split_f16, zero padded)"""
+        lib = _lib.load()
+        n = feats.shape[0]
+        buf = torch.empty(max(n, 1), 2, cin_tc, dtype=torch.float16, device=feats.device)
+        if n > 0:
+            _lib.check(lib.b2s_split_f16(_lib.ptr(feats), _lib.ptr(buf[:, 0]), _lib.ptr(buf[:, 1]), None, n,
+                                         self.in_channels, cin_tc, 2 * cin_tc, _lib.stream()), "b2s_split_f16")
+        return buf
+
+    def _dgrad_weights(self, w, flip):
+        """packed fp16 hi/lo planes of W'[k] = W[k]^T (flip: W[K-1-k]^T) for the tensor-pipe input gradient, with their
+        power-of-two scale; cached until the weight changes (one scale measurement per weight version)."""
+        from b2second import tc as _tc
+        key = (w.data_ptr(), w._version, str(w.device), flip)
+        cached = getattr(self, "_b2s_tc_wt", None)
+        if cached is None or cached[0] != key:
+            K = int(np.prod(self.kernel_size))
+            with torch.no_grad():
+                wt = w.detach().float().reshape(K, self.in_channels, self.out_channels)
+                wt = (wt.flip(0) if flip else wt).transpose(1, 2).contiguous()
+                wp = _tc.pack_sparse_weights(wt)
+                ws = _tc.pow2_scale(wp)
+                hi, lo = _tc.split_f16(wp, ws)
+            cached = (key, hi, lo, ws)
+            self._b2s_tc_wt = cached
+        return cached[1:]
+
+    def _dgrad(self, dy, weight, rb, n_in, split=None):
+        """input gradient [n_in, Cin] = the forward contraction of dY [n_out, Cout] over the transposed table with
+        W'[k] = W[k]^T.  A SubM table with odd kernel sizes is its own transpose under k <-> K-1-k (same table, same tile
+        plan, W'[k] = W[K-1-k]^T); any other table is transposed once (ops.transpose_rulebook)."""
+        from b2second import tc as _tc
+        lib = _lib.load()
+        K, cin, cout, n_out = rb.K, self.in_channels, self.out_channels, rb.num_out
+        dev = dy.device
+        if n_in == 0 or n_out == 0:
+            return torch.zeros(n_in, cin, dtype=torch.float32, device=dev)
+        flip = rb.subm and all(k % 2 == 1 for k in rb.ksize)
+        if flip:
+            table, n_dev, (perm, tmask) = rb.nbr, rb.num_out_dev, ops.tile_plan(rb)
+        else:
+            table, perm, tmask = ops.transpose_rulebook(rb, n_in), None, None
+            n_dev = torch.tensor([n_in], dtype=torch.int32, device=dev)
+        dx = torch.empty(n_in, cin, dtype=torch.float32, device=dev)
+        if (USE_TENSOR_CORES and K <= 27 and _tc.sparse_tc_cin(cout) == cout
+                and bool(lib.b2s_sparse_conv_tc_supported(cout, cin))):
+            # dY goes onto the tensor pipe scaled by a power of two picked on the device (gradients are often far below
+            # the fp16 normal range); the kernel's epilogue scale undoes both that and the weights' scale
+            w_hi, w_lo, ws = self._dgrad_weights(weight, flip)
+            g_hi, g_lo, g_stride, inv = (split or _GradSplit(dy)).planes()
+            scale = (inv / ws).expand(cin).contiguous()
+            status = torch.zeros(1, dtype=torch.int32, device=dev)
+            _lib.check(lib.b2s_sparse_conv_tc_plan(
+                _lib.ptr(g_hi), _lib.ptr(g_lo), g_stride, g_hi.shape[0], cout, _lib.ptr(w_hi), _lib.ptr(w_lo),
+                _lib.ptr(table), K, _lib.ptr(n_dev), n_in, _lib.ptr(perm), _lib.ptr(tmask), _lib.ptr(scale), None, 0,
+                _lib.ptr(dx), None, cin, cin, _lib.ptr(status), _lib.stream()), "b2s_sparse_conv_tc_plan")
+            return dx
+        w = weight.detach().float().reshape(K, cin, cout)
+        wt = (w.flip(0) if flip else w).transpose(1, 2).contiguous()        # [K, Cout, Cin]
+        _lib.check(lib.b2s_sparse_conv(_lib.ptr(dy), cout, _lib.ptr(wt), _lib.ptr(table), K, _lib.ptr(n_dev), n_in, None,
+                                       None, 0, _lib.ptr(dx), cin, _lib.stream()), "b2s_sparse_conv")
+        return dx
+
+    def _wgrad(self, feats, dy, rb, split=None):
+        """weight gradient [K, Cin, Cout] = sum over output rows of X[nbr[o,k]]^T dY[o]: b2s_sparse_conv_wgrad_tc on the
+        tensor pipe, b2s_sparse_conv_wgrad (fp32 FMA) otherwise.  On the tensor pipe both operands are split under their
+        own power-of-two scale (b2s_split_f16_autoscale): the forward's unscaled planes of X carry a small activation
+        with only 2^-25 absolute precision, which a weight gradient of few pairs would see; rows are reduced in the
+        forward's tile-plan order."""
+        lib = _lib.load()
+        K, cin, cout, n_out = rb.K, self.in_channels, self.out_channels, rb.num_out
+        dev = dy.device
+        cin_tc = self._wgrad_tc_cin(lib, K)
+        if cin_tc is not None and n_out > 0 and feats.shape[0] > 0:
+            x_hi, x_lo, x_stride, inv_x = _GradSplit(feats, cin_tc).planes()
+            g_hi, g_lo, g_stride, inv_g = (split or _GradSplit(dy)).planes()
+            scale = inv_x * inv_g                                      # powers of two: exact
+            perm, tmask = ops.tile_plan(rb)
+            dw = torch.empty(K, cin_tc, cout, dtype=torch.float32, device=dev)
+            ws_bytes = lib.b2s_sparse_conv_wgrad_tc_workspace_bytes(n_out, K, cin_tc, cout)
+            work = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+            _lib.check(lib.b2s_sparse_conv_wgrad_tc(
+                _lib.ptr(x_hi), _lib.ptr(x_lo), x_stride, x_hi.shape[0], cin_tc, _lib.ptr(g_hi), _lib.ptr(g_lo), g_stride,
+                cout, _lib.ptr(rb.nbr.contiguous()), K, _lib.ptr(rb.num_out_dev), n_out, _lib.ptr(perm), _lib.ptr(tmask),
+                _lib.ptr(scale), _lib.ptr(dw), _lib.ptr(work), ws_bytes, _lib.stream()), "b2s_sparse_conv_wgrad_tc")
+            return dw if cin_tc == cin else dw[:, :cin].contiguous()
+        dw = torch.empty(K, cin, cout, dtype=torch.float32, device=dev)
+        ws_bytes = lib.b2s_sparse_conv_wgrad_workspace_bytes(n_out, K, cin, cout)
+        work = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+        _lib.check(lib.b2s_sparse_conv_wgrad(_lib.ptr(feats), cin, _lib.ptr(dy), cout, _lib.ptr(rb.nbr.contiguous()), K,
+                                             _lib.ptr(rb.num_out_dev), n_out, None, _lib.ptr(dw), _lib.ptr(work), ws_bytes,
+                                             _lib.stream()), "b2s_sparse_conv_wgrad")
+        return dw
 
 
 class SparseConv3d(SparseConvolution):

@@ -63,6 +63,18 @@ SIGNATURES = {
                                         c_int, c_int, c_void_p, c_void_p]),
     "b2s_split_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b2s_merge_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "b2s_split_f16_autoscale": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                        c_void_p]),
+    "b2s_rulebook_transpose": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
+    "b2s_sparse_conv_wgrad_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "b2s_sparse_conv_wgrad": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                                      c_void_p, c_void_p, c_size_t, c_void_p]),
+    "b2s_sparse_conv_wgrad_tc_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "b2s_sparse_conv_wgrad_tc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
+                                         c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                         c_void_p, c_size_t, c_void_p]),
+    "b2s_from_bev":(c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                             c_void_p]),
     "b2s_to_bev_tc": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                               c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2s_rpn_bg_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
