@@ -21,12 +21,14 @@
 //               every 4th K block, all 16-byte cp.async copies of its 64 rows (hi and lo planes) into the K-major
 //               SWIZZLE_128B A tile, zero-fill for missing neighbours, completion signalled on the stage's mbarrier
 //               with cp.async.mbarrier.arrive.noinc.  The neighbour-table entries of the NEXT owned K block are
-//               loaded (straight from global / L1) before the current one is waited for.
+//               loaded (straight from global / L1) before the current one is waited for.  Lane 0 of the row-half-0
+//               warp of a K block also issues its weight tile (bulk tensor load, SWIZZLE_128B) once the stage is free.
 //   warps 8-15  two consumer warpgroups: warpgroup g issues the wgmmas of tile rows 64g .. 64g+63 and owns their
 //               accumulators; per-chain partial sums go into fp32 running sums with round-to-nearest adds (the tensor
 //               core's own accumulate is not RN -- see conv_tc.cu), then BN scale/shift + ReLU, hi/lo split, stores.
-//               Lane 0 of warp 8 also issues the weight tile of each K block (bulk tensor load, SWIZZLE_128B) as soon as
-//               its stage is free, STAGES K blocks ahead of the MMAs.
+//               Consumers only wait on full stages and release them: a consumer warp that also issued the weights
+//               would wait for the OTHER warpgroup to release each stage, tying the two together on every K block
+//               (that cost 25-35 % of the time of every layer but the last, 3x1x1 one, on H100).
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -264,6 +266,18 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
             const uint32_t need = zskip_on ? (valid | (~zeroed & ((1u << RI) - 1u))) : 0xFFFFFFFFu;
             const uint32_t sa = sa0 + (uint32_t)my_stage * STAGE_BYTES;
             mbar_wait_warp(&bar_empty[my_stage], use_parity, poll1);
+            // the K block's weights: its expect_tx arrival is the "+ 1" of the stage's bar_full count
+            if (half == 0 && lane == 0) {
+                uint8_t *st = smem + (size_t)my_stage * STAGE_BYTES;
+#ifdef B2S_DIAG
+                if (p.flags & 4) mbar_arrive(&bar_full[my_stage]); else
+#endif
+                {
+                    mbar_arrive_expect_tx(&bar_full[my_stage], 2 * B_TILE_BYTES);
+                    tma_load_3d(st + 2 * A_TILE_BYTES, &map_w_hi, &bar_full[my_stage], 0, 0, kb_cur);
+                    tma_load_3d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_w_lo, &bar_full[my_stage], 0, 0, kb_cur);
+                }
+            }
             if (lo_delta == (long long)(CIN * ELEM_BYTES)) {
                 // interleaved rows [hi Cin | lo Cin]: the lo copy is the hi address + an immediate
 #pragma unroll
@@ -324,32 +338,6 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
         const uint32_t a_off = (uint32_t)cg * 64u * 128u;
         int stage = 0;
         uint32_t phase = 0;
-        // Weight loads: lane 0 of the first consumer warp walks the CTA's K-block sequence STAGES K blocks ahead of the
-        // MMAs; a stage's weights are requested as soon as both warpgroups have released it.
-        const bool w_issuer = warp == GW && lane == 0 && (int)blockIdx.x < num_tiles;
-        int w_tile = (int)blockIdx.x, w_stage = 0;
-        uint32_t w_kbm = w_issuer ? tile_kbm(w_tile) : 0u, w_phase = 0;
-        auto issue_weights = [&]() {
-            if (w_kbm == 0) {
-                w_tile += gridDim.x;
-                if (w_tile >= num_tiles) return;
-                w_kbm = tile_kbm(w_tile);
-            }
-            const int kb = __ffs(w_kbm) - 1;
-            w_kbm &= w_kbm - 1;
-            mbar_wait(&bar_empty[w_stage], w_phase ^ 1);
-            uint8_t *st = smem + (size_t)w_stage * STAGE_BYTES;
-#ifdef B2S_DIAG
-            if (p.flags & 4) { mbar_arrive(&bar_full[w_stage]); if (++w_stage == STAGES) { w_stage = 0; w_phase ^= 1; } return; }
-#endif
-            mbar_arrive_expect_tx(&bar_full[w_stage], 2 * B_TILE_BYTES);
-            tma_load_3d(st + 2 * A_TILE_BYTES, &map_w_hi, &bar_full[w_stage], 0, 0, kb);
-            tma_load_3d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_w_lo, &bar_full[w_stage], 0, 0, kb);
-            if (++w_stage == STAGES) { w_stage = 0; w_phase ^= 1; }
-        };
-        if (w_issuer)
-            for (int i = 0; i < STAGES; ++i) issue_weights();
-        __syncwarp();
         float acc[R], sum[R / 2];
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             uint32_t kbm = tile_kbm(tile);
@@ -382,7 +370,6 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
                 wgmma_fence_operands<R>(acc);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&bar_empty[stage]);
-                if (w_issuer) issue_weights();
                 __syncwarp();
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 fresh = (ce & low) ? 1u : 0u;
