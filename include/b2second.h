@@ -38,6 +38,10 @@
  *                       (second/pytorch/models/voxelnet.py:413-414,444,560-576,
  *                        second/pytorch/core/box_torch_ops.py:56-102); _segments: over the torch.cat of several
  *                       heads' predictions (net_multi_head.py:163-172)
+ *   b2s_anchor_area_mask
+ *                       box_np_ops.sparse_sum_for_anchors_mask + cumsum(0).cumsum(1) +
+ *                       box_np_ops.fused_get_anchors_area + `> anchor_area_threshold`
+ *                       (second/data/preprocess.py:345-357, second/core/box_np_ops.py:917-946)
  *   b2s_nms             torch.topk + spconv.utils.rotate_non_max_suppression_cpu /
  *                       spconv.utils.non_max_suppression (box_torch_ops.py:454-515,
  *                       second/core/non_max_suppression/nms_cpu.py:20-31, nms_gpu.py:10-19)
@@ -373,6 +377,21 @@ int b2s_pfn_ex(const float *points, int num_feat, const int *point_slots, const 
  * zero padding torch applies at the crop edge, not the neighbouring pixels of src.  C % 8 == 0, 16-byte aligned planes. */
 int b2s_crop_nhwc(const b2s_half *src_hi, const b2s_half *src_lo, int batch, int H, int W, int C, int crop,
                   b2s_half *dst_hi, b2s_half *dst_lo, void *stream);
+
+/* ---- anchor-area mask (second/data/preprocess.py:345-357) ---------------------------------------- */
+/* mask_out [batch, num_anchors] uint8 = 1 where the anchor's BEV box holds more than `threshold` voxels.
+ * coors [cap, 4] (b, z, y, x), 16-byte aligned; the first min(*num_dev, cap) rows count (the voxels that survived the
+ * max_voxels cap), each once at (b, y, x) of a per-frame int32 count map [batch, ny, nx] (ny, nx = grid_size y, x).
+ * The map becomes its summed-area table (inclusive prefix sums along x, then y) and, for the box (x0, y0, x1, y1) of
+ * anchor_boxes [num_anchors, 4] int32 (16-byte aligned), area = S[y1,x1] - S[y1,x0] - S[y0,x1] + S[y0,x0]: the cells
+ * (x0, x1] x (y0, y1], as fused_get_anchors_area reads them.  Boxes must satisfy 0 <= x0 <= x1 < nx and
+ * 0 <= y0 <= y1 < ny (b2second/anchor_mask.py derives them on the host in float32).  Counts are integers below 2^24,
+ * so the result equals the reference's float32 map bit for bit.  count_map_ws: workspace of
+ * b2s_anchor_area_mask_workspace_bytes(batch, ny, nx) (host query) bytes.  One memset and four kernels. */
+size_t b2s_anchor_area_mask_workspace_bytes(int batch, int ny, int nx);
+int b2s_anchor_area_mask(const int *coors, const int *num_dev, int cap, int batch, int ny, int nx,
+                         const int *anchor_boxes, int num_anchors, float threshold, void *count_map_ws,
+                         size_t workspace_bytes, uint8_t *mask_out, void *stream);
 
 /* ---- box decode + score filter ------------------------------------------------------------------ */
 /* Head tensors in the RPN's NCHW conv-output layout: box [B, A_loc*code, H, W], cls [B, A_loc*ncls, H, W],

@@ -10,6 +10,7 @@ buffers, so the whole frame batch is ONE CUDA graph:
   b2s_voxelize (+ fused SimpleVoxel mean)                     voxelnet.py:325-328, preprocess.py:303-315
      or, for an example that arrives already voxelised (the reference's own dict):
      b2s_hash_build + b2s_vfe_mean over the caller's voxels   voxel_encoder.py:220-225,246-255
+  b2s_anchor_area_mask (only with anchor_area_threshold >= 0 and no example mask)   preprocess.py:345-357
   per sparse layer: b2s_rulebook_{subm,conv} (cached per indice_key) + b2s_sparse_conv_tc (wgmma, fp16 hi/lo
       planes flow from layer to layer) with BatchNorm1d/ReLU folded into the epilogue      middle.py:145-192
   b2s_pfn (PointPillars) / b2s_pfn_ex (PillarFeatureNetRadius) pointpillars.py:203-237,240-325
@@ -35,6 +36,7 @@ import os
 import numpy as np
 import torch
 
+from . import anchor_mask as _anchor_mask
 from . import spec as _spec
 from . import tc as _tc
 
@@ -57,7 +59,8 @@ class _Level:
 
 class InferenceEngine:
     def __init__(self, net, batch_size=1, max_points=None, max_voxels=None, row_cap_factor=2.0,
-                 cand_cap=None, use_cuda_graph=True, rpn_impl="auto", sparse_impl="tc", device=None):
+                 cand_cap=None, use_cuda_graph=True, rpn_impl="auto", sparse_impl="tc", device=None,
+                 anchor_area_threshold=None):
         import spconv as sp                      # the CUDA drop-in: fails loudly if the library is missing
         assert not getattr(sp, "__oracle__", False), "the engine is the product path; it never runs on the oracle"
         self.sp = sp
@@ -91,6 +94,8 @@ class InferenceEngine:
         self.rpn_impl = rpn_impl
         assert sparse_impl in ("tc", "fma")       # sparse-conv inner product: wgmma 3xF16 | fp32 FMA tiles
         self.sparse_impl = sparse_impl
+        # anchor-area mask of the reference's eval preprocessing (preprocess.py:345-357): None / negative = off
+        self.area_threshold = float(anchor_area_threshold) if _anchor_mask.enabled(anchor_area_threshold) else None
         with torch.cuda.device(dev):
             self.status = torch.zeros(1, dtype=torch.int32, device=dev)
             self._plan_middle(row_cap_factor)
@@ -98,6 +103,8 @@ class InferenceEngine:
             if rpn_impl == "tc":
                 self._alloc_tc_rpn()
             self._alloc_detect_buffers(cand_cap)
+            if self.area_threshold is not None:
+                self._alloc_area_mask()
 
     # ---------------------------------------------------------------- planning / allocation
     def _new_level(self, cap, shape, with_storage=True):
@@ -430,6 +437,7 @@ class InferenceEngine:
             self._anchors_key = "generated"
         self.anchors_mask = None                      # [B, A] uint8, allocated on first use
         self.use_mask = False
+        self._mask_src = None                         # None | "given" (the example's anchors_mask) | "area" (computed)
         self.cand_cap = int(cand_cap or min(self.A, 32768))
         B, cc, code = self.B, self.cand_cap, self.code
         # per-class NMS branch (voxelnet.py:458-547): one candidate list and one NMS per (class, frame) -- "virtual
@@ -478,6 +486,36 @@ class InferenceEngine:
         rng = s.post_center_range
         self.range_host = self._L.f6(rng) if len(rng) == 6 else None
 
+    def _alloc_area_mask(self):
+        """buffers of the computed anchor-area mask: the per-frame count map at voxel-grid resolution, the anchors'
+        integer BEV boxes (derived on the host whenever the anchor set changes) and the [B, A] mask decode reads."""
+        s = self.spec
+        self.am_ny, self.am_nx = int(s.grid_size[1]), int(s.grid_size[0])
+        self.am_ws_bytes = self.lib.b2s_anchor_area_mask_workspace_bytes(self.B, self.am_ny, self.am_nx)
+        self.am_ws = torch.empty(max(self.am_ws_bytes, 1), dtype=torch.uint8, device=self.dev)
+        self.am_boxes = torch.zeros(self.A, 4, dtype=torch.int32, device=self.dev)
+        if self.anchors_mask is None:
+            self.anchors_mask = torch.zeros(self.B, self.A, dtype=torch.uint8, device=self.dev)
+        self._mask_src, self.use_mask = "area", True
+        if self._anchors_key is not None:
+            self._set_area_boxes(self.anchors)
+
+    def _set_area_boxes(self, anchors):
+        """float32 host derivation of the boxes (b2second.anchor_mask); reads the anchors back once per anchor set."""
+        a = anchors.detach().reshape(-1, anchors.shape[-1]).float().cpu().numpy()
+        s = self.spec
+        boxes = _anchor_mask.anchor_boxes(a, s.voxel_size, s.point_cloud_range, s.grid_size)
+        self.am_boxes.copy_(torch.from_numpy(boxes))
+
+    def _launch_area_mask(self, st):
+        """count map of level 0's voxels -> summed-area table -> anchors_mask [B, A] (one memset, four kernels)."""
+        L, lv = self._L, self.level0
+        self._mark("anchor_mask")
+        L.check(self.lib.b2s_anchor_area_mask(
+            L.ptr(lv.coors), L.ptr(lv.n_dev), lv.cap, self.B, self.am_ny, self.am_nx, L.ptr(self.am_boxes), self.A,
+            self.area_threshold, L.ptr(self.am_ws), self.am_ws_bytes, L.ptr(self.anchors_mask), st),
+            "b2s_anchor_area_mask")
+
     @property
     def det(self):
         """[B, post_max, code+2] view of the detection records."""
@@ -509,6 +547,8 @@ class InferenceEngine:
                 L.check(lib.b2s_vfe_mean(L.ptr(self.in_voxels), L.ptr(self.vox_num), L.ptr(lv.n_dev), lv.cap, self.T,
                                          self.F, self.vfe_mode, self.vfe_nf, L.ptr(self.vfe_out), st), "b2s_vfe_mean")
             pfn_points, pfn_slots = self.in_voxels, self.in_slots
+        if self._mask_src == "area":
+            self._launch_area_mask(st)
         if self.is_pillars:
             vx, vy, xo, yo = self.pfn_geom
             self._mark("pfn")
@@ -791,6 +831,8 @@ class InferenceEngine:
     def kernel_launches_per_step(self):
         """how many of OUR kernels one pipeline pass launches (memsets and cuDNN kernels not counted)."""
         n = 7                                    # b2s_voxelize: insert, flag_scan, scan_sums, assign, fill, gather, finish
+        if self._mask_src == "area":
+            n += 4                               # b2s_anchor_area_mask: scatter, scan_rows, scan_cols, lookup
         if self.is_pillars:
             n += 1                               # b2s_pfn / b2s_pfn_ex
         for lyr in self.layers:
@@ -863,19 +905,20 @@ class InferenceEngine:
             "num_anchors=%d, but num_output=%d. please check size" % (a.shape[0], self.A)
         self.anchors.copy_(a, non_blocking=True)
         self._anchors_key = key
+        if self.area_threshold is not None:
+            self._set_area_boxes(a)            # one read-back per anchor set; the steady state does not sync
 
     def set_anchors_mask(self, mask):
-        """anchors_mask [B, A] (bool/uint8) or None (voxelnet.py:397-400,432-439)."""
+        """anchors_mask [B, A] (bool/uint8) or None (voxelnet.py:397-400,432-439).  With ``anchor_area_threshold``
+        set, None means the engine computes the mask; a given mask wins, as in the reference's example dict.
+        The three cases (no mask, given, computed) launch different sequences and keep separate CUDA graphs."""
         if mask is None:
-            if self.use_mask:
-                self.use_mask = False
-                self._graphs.clear()
+            self._mask_src = "area" if self.area_threshold is not None else None
+            self.use_mask = self._mask_src is not None
             return
         if self.anchors_mask is None:
             self.anchors_mask = torch.zeros(self.B, self.A, dtype=torch.uint8, device=self.dev)
-        if not self.use_mask:
-            self.use_mask = True
-            self._graphs.clear()               # the launch arguments change (NULL -> buffer)
+        self._mask_src, self.use_mask = "given", True
         self.anchors_mask.copy_(mask.reshape(self.B, self.A).to(torch.uint8), non_blocking=True)
 
     def load_points(self, frames):
@@ -1019,7 +1062,8 @@ class InferenceEngine:
                 with torch.no_grad():
                     self._launch(mode)
                 return self.det, self.det_count
-            g = self._graphs.get(mode)
+            key = (mode, self._mask_src)
+            g = self._graphs.get(key)
             if g is None:
                 with torch.no_grad():
                     side = torch.cuda.Stream()
@@ -1032,7 +1076,7 @@ class InferenceEngine:
                     g = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(g):
                         self._launch(mode)
-                    self._graphs[mode] = g
+                    self._graphs[key] = g
             g.replay()
         return self.det, self.det_count
 

@@ -19,6 +19,10 @@ runs as one CUDA graph per frame batch (``b2second.engine.InferenceEngine``).  A
 * ``sweeps``: per frame the NuScenes key-frame cloud + its sweeps with their ``sweep2lidar`` calibration, merged on
   the GPU (nuscenes_dataset.py:166-185) -- see ``InferenceEngine.load_sweeps``.
 
+``accelerate(net, anchor_area_threshold=t)`` (an engine keyword, like every other one ``FastPath`` forwards) makes the
+engine compute the reference preprocessing's ``anchors_mask`` (preprocess.py:345-357) on the GPU for any of these
+inputs that carries no ``anchors_mask`` of its own; the default (None) computes none.
+
 The list of result dicts holds GPU tensors like the reference's (``output="device"``); ``accelerate(net,
 output="host")`` returns CPU tensors through ONE pinned device-to-host copy of the detection records instead of one
 small copy per frame and field.

@@ -131,3 +131,30 @@ def crop_convex(points, planes):
     offs = torch.zeros(2, dtype=torch.int32, device=points.device)
     ConvexCrop(points.shape[0], points.device).crop_into(points, planes, out, offs, 0)
     return out, offs
+
+
+def anchor_area_mask(coordinates, batch_size, anchors, voxel_size, point_cloud_range, grid_size, threshold):
+    """the reference preprocessing's ``anchors_mask`` (second/data/preprocess.py:345-357) on the GPU, for callers who
+    build examples themselves: coordinates CUDA int [N, 4] (b, z, y, x) of the voxels that survived max_voxels;
+    anchors [A, >=7] (host or device; read on the host once to derive the integer boxes, b2second.anchor_mask);
+    grid_size (x, y, z).  -> CUDA bool [batch_size, A]: the anchor's BEV box holds more than ``threshold`` voxels."""
+    from . import anchor_mask
+    L, lib = _lib()
+    L.require_cuda(coordinates, "coordinates")
+    dev = coordinates.device
+    a = anchors.detach().cpu().numpy() if isinstance(anchors, torch.Tensor) else np.asarray(anchors)
+    boxes = torch.from_numpy(anchor_mask.anchor_boxes(a.reshape(-1, a.shape[-1]), voxel_size, point_cloud_range,
+                                                      grid_size)).to(dev)
+    B, A = int(batch_size), int(boxes.shape[0])
+    ny, nx = int(grid_size[1]), int(grid_size[0])
+    coors = coordinates.to(torch.int32).contiguous()
+    n = int(coors.shape[0])
+    n_dev = torch.tensor([n], dtype=torch.int32).to(dev)
+    ws_bytes = lib.b2s_anchor_area_mask_workspace_bytes(B, ny, nx)
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+    mask = torch.empty(B, A, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        L.check(lib.b2s_anchor_area_mask(L.ptr(coors) if n else None, L.ptr(n_dev), n, B, ny, nx, L.ptr(boxes), A,
+                                         float(threshold), L.ptr(ws), ws_bytes, L.ptr(mask), L.stream()),
+                "b2s_anchor_area_mask")
+    return mask.bool()

@@ -100,6 +100,9 @@ SIGNATURES = {
                                              ctypes.c_longlong, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                              c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                              c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "b2s_anchor_area_mask_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "b2s_anchor_area_mask": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_float, c_void_p,
+                                     c_size_t, c_void_p, c_void_p]),
     "b2s_concat_class_detections": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
                                             c_void_p]),
     "b2s_nms_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
