@@ -60,7 +60,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 200
+#define B2S_VERSION 201
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -152,8 +152,7 @@ size_t b2s_rulebook_conv_workspace_bytes(int batch, const int *out_shape /*host[
  * Builds the out-coordinate hash as well (hash_cap_out power of two >= 2*cap_out). */
 int b2s_rulebook_conv(const int *coors_in, const int *num_in_dev, int cap_in, int batch,
                       const int *in_shape, const int *out_shape, const int *ksize, const int *stride,
-                      const int *padding, const int *dilation, const unsigned long long *hash_keys_in,
-                      const int *hash_vals_in, int hash_cap_in, int *coors_out /*[cap_out,4]*/,
+                      const int *padding, const int *dilation, int *coors_out /*[cap_out,4]*/,
                       int *num_out_dev, int cap_out, int *nbr /*[cap_out,K]*/,
                       unsigned long long *hash_keys_out, int *hash_vals_out, int hash_cap_out,
                       void *workspace, size_t workspace_bytes, unsigned *row_mask /*[cap_out] or NULL*/,
@@ -318,8 +317,7 @@ int b2s_conv2d_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int batch, in
                      const int *work_count_dev,
                      const int *bg_list /*optional, with work_list: the background tiles of the output; the kernel's
                                           epilogue warps copy them from the layer's empty-frame response bg_hi/bg_lo
-                                          [Hout+2, Wout+2, Cout] while they wait for the tensor pipe (instead of a
-                                          separate b2s_rpn_bg_fill launch)*/,
+                                          [Hout+2, Wout+2, Cout] while they wait for the tensor pipe*/,
                      const int *bg_count_dev, const b2s_half *bg_hi, const b2s_half *bg_lo, unsigned *status_dev,
                      void *stream);
 
@@ -332,15 +330,11 @@ int b2s_conv2d_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int batch, in
  * b2s_rpn_bg_plan dilates the data mask through `num_layers` consecutive 3x3 stride-1 pad-1 layers and compacts, per
  * layer l, the 16x16 output tiles into
  *   work_lists[l*num_tiles ..]  tiles with a masked pixel (ascending), counts[2l] of them -> b2s_conv2d_tc_ex work_list
- *   bg_lists  [l*num_tiles ..]  background tiles,               counts[2l + 1] of them  -> bg_list / b2s_rpn_bg_fill
+ *   bg_lists  [l*num_tiles ..]  background tiles,               counts[2l + 1] of them  -> b2s_conv2d_tc_ex bg_list
  * with num_tiles = batch * ceil(H/16) * ceil(W/16), tile id = (b * tiles_h + th) * tiles_w + tw.
  * scratch: 2*batch*H*W bytes; tile_flags: num_layers*num_tiles ints. */
 int b2s_rpn_bg_plan(const uint8_t *occupancy /*[B,H,W]*/, int batch, int H, int W, int num_layers, uint8_t *scratch,
                     int *tile_flags, int *work_lists, int *bg_lists, int *counts, void *stream);
-/* copy the listed background tiles of a halo-padded NHWC map [B, H+2, W+2, out_stride] from the layer's empty-frame
- * response f_hi/f_lo [H+2, W+2, C] (fp16 hi/lo planes) */
-int b2s_rpn_bg_fill(const int *bg_list, const int *bg_count_dev, int batch, int H, int W, int C, const b2s_half *f_hi,
-                    const b2s_half *f_lo, b2s_half *out_hi, b2s_half *out_lo, int out_stride, void *stream);
 
 
 /* the tail of a single-scale RPNV2 in one kernel (csrc/rpn_tail.cu): y = relu(bn(deblock_1x1(x))) (128 -> 128) never

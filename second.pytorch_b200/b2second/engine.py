@@ -31,7 +31,6 @@ record the multi-GPU path all-gathers (SURVEY.md §8e); ``det`` and ``det_count`
 (``det_record [B, post_max*(code+2) + 1]``) so the all-gather needs no packing step.
 """
 import ctypes
-import os
 
 import numpy as np
 import torch
@@ -148,8 +147,6 @@ class InferenceEngine:
         level = self.level0
         rulebooks = {}
         max_ws = 0
-        thin_ok = os.environ.get("B2S_THIN_TC", "1") != "0"      # A/B switch: thin layers on the FMA core
-        plan_mode = int(os.environ.get("B2S_SP_PLAN", "4"))
         for j, ls in enumerate(s.layers):
             K = ls["K"]
             lyr = dict(ls)
@@ -166,8 +163,7 @@ class InferenceEngine:
                     # rulebook workspace, so this SubM table is built by rank lookups (b2s_rulebook_subm_ranked) and
                     # the level needs no hash table
                     prev = self.layers[-1] if self.layers else None
-                    lyr["ranked"] = bool(prev is not None and not prev["subm"] and prev["out_level"] is level
-                                         and os.environ.get("B2S_RB_RANKED", "1") != "0")
+                    lyr["ranked"] = bool(prev is not None and not prev["subm"] and prev["out_level"] is level)
                 else:
                     lyr["build_rb"] = False
                 lyr["rb"] = rulebooks[key]
@@ -185,21 +181,18 @@ class InferenceEngine:
                 max_ws = max(max_ws, self.lib.b2s_rulebook_conv_workspace_bytes(self.B, self._L.i3(out_shape)))
                 level = new
             # tile plan of the rulebook (csrc/sparse_plan.cu): which kernel offsets each 128-row tile needs, and an order
-            # of the rows that makes that set small.  B2S_SP_PLAN: 0 off, 1 masks only, 2 rows grouped for SubM
-            # rulebooks (shared by 2-3 layers) + masks for the strided ones, 3 rows grouped for every 27-offset rulebook,
-            # 4 (default) SubM rulebooks only (a strided conv uses its table once: the plan costs more than it saves)
+            # of the rows that makes that set small
             rb = lyr["rb"]
-            if "tile_mask" not in rb and plan_mode > 0 and (plan_mode != 4 or ls["subm"]):
+            if "tile_mask" not in rb and _tc.wants_tile_plan(ls["subm"], K):
                 cap_rb = lyr["out_level"].cap
                 rb["tile_mask"] = torch.zeros((cap_rb + 127) // 128, dtype=torch.int32, device=dev)
                 rb["row_mask"] = torch.zeros(cap_rb, dtype=torch.int32, device=dev)    # written by the rulebook builder
-                rb["sort"] = bool(K > 3 and (plan_mode == 3 or (plan_mode in (2, 4) and ls["subm"])))
-                rb["perm"] = torch.zeros(cap_rb, dtype=torch.int32, device=dev) if rb["sort"] else None
+                rb["perm"] = torch.zeros(cap_rb, dtype=torch.int32, device=dev)
             # tensor-pipe core (csrc/sparse_conv_tc.cu): the library says which (Cin, Cout) it was built for;
             # 3-/4-feature input layers are zero-padded to 8 channels.  Everything else: fp32 FMA core.
             cin_tc = _tc.sparse_tc_cin(ls["cin"])
             lyr["cin_tc"] = cin_tc
-            lyr["tc"] = bool(self.sparse_impl == "tc" and cin_tc is not None and (thin_ok or cin_tc >= 32) and
+            lyr["tc"] = bool(self.sparse_impl == "tc" and cin_tc is not None and
                              self.lib.b2s_sparse_conv_tc_supported(cin_tc, ls["cout"]))
             self.layers.append(lyr)
         # a level's coordinate hash is only built when some SubM rulebook still looks rows up by hash
@@ -287,8 +280,8 @@ class InferenceEngine:
         self.tc_prog = plan
         self.tc_plan = plan["ops"]
         # single-scale tail (one k = s = 1 deblock 128 -> 128 feeding the heads): one fused kernel, the deblock output
-        # never goes to HBM (csrc/rpn_tail.cu; bit-identical to the two launches).  B2S_RPN_TAIL=0: two launches.
-        self.tc_tail_fused = bool(os.environ.get("B2S_RPN_TAIL", "1") != "0" and _tc.fusable_tail(plan))
+        # never goes to HBM (csrc/rpn_tail.cu; bit-identical to the two launches)
+        self.tc_tail_fused = _tc.fusable_tail(plan)
         assert plan["in_channels"] == C, "BEV channels %d != RPN input %d" % (C, plan["in_channels"])
 
         def plane(h, w, c):
@@ -313,8 +306,7 @@ class InferenceEngine:
         self.tc_hw = (H, W)
         # background tiles (csrc/rpn_bg.cu): through the leading chain of 3x3 stride-1 layers, output tiles whose whole
         # receptive field is empty BEV are not computed but copied from the layer's response to an empty frame
-        self.bg_idx = _tc.background_layers(plan) if os.environ.get("B2S_RPN_BG", "1") != "0" else []
-        self.bg_fused_fill = os.environ.get("B2S_RPN_BG_FILL", "fused") == "fused"
+        self.bg_idx = _tc.background_layers(plan)
         if self.bg_idx:
             nl = len(self.bg_idx)
             self.bg_tiles = B * (-(-H // 16)) * (-(-W // 16))
@@ -583,7 +575,7 @@ class InferenceEngine:
                         L.check(lib.b2s_rulebook_conv(
                             L.ptr(lin.coors), L.ptr(lin.n_dev), lin.cap, self.B, L.i3(lin.shape), L.i3(lout.shape),
                             L.i3(lyr["kernel_size"]), L.i3(lyr["stride"]), L.i3(lyr["padding"]), L.i3(lyr["dilation"]),
-                            L.ptr(lin.keys), L.ptr(lin.vals), lin.hcap, L.ptr(lout.coors), L.ptr(lout.n_dev), lout.cap,
+                            L.ptr(lout.coors), L.ptr(lout.n_dev), lout.cap,
                             L.ptr(lyr["rb"]["nbr"]), L.ptr(lout.keys) if lyr["want_hash"] else None,
                             L.ptr(lout.vals) if lyr["want_hash"] else None, lout.hcap,
                             L.ptr(self.rb_ws), self.rb_ws_bytes, L.ptr(lyr["rb"].get("row_mask")), L.ptr(self.status), st),
@@ -592,7 +584,7 @@ class InferenceEngine:
                         rb = lyr["rb"]
                         L.check(lib.b2s_sparse_tile_plan(
                             L.ptr(rb["nbr"]), L.ptr(rb["row_mask"]), lyr["K"], L.i3(lyr["kernel_size"]), L.ptr(lout.n_dev), lout.cap,
-                            1 if rb["sort"] else 0, L.ptr(rb["perm"]), L.ptr(rb["tile_mask"]), st),
+                            1, L.ptr(rb["perm"]), L.ptr(rb["tile_mask"]), st),
                             "b2s_sparse_tile_plan")
                 self._mark("sparse_conv%d" % lyr["index"])
                 if lyr["tc"]:
@@ -697,12 +689,8 @@ class InferenceEngine:
                 bl = self.bg_idx.index(oi)
                 chi, clo = self.bg_field[bl]
                 work, work_n = L.ptr(self.bg_work[bl]), L.ptr(self.bg_counts[bl, 0:])
-                if self.bg_fused_fill:       # the conv kernel's epilogue warps store the constant into the background tiles
-                    bgl, bgn, bhi, blo = L.ptr(self.bg_list[bl]), L.ptr(self.bg_counts[bl, 1:]), L.ptr(chi), L.ptr(clo)
-                else:
-                    L.check(lib.b2s_rpn_bg_fill(L.ptr(self.bg_list[bl]), L.ptr(self.bg_counts[bl, 1:]), self.B,
-                                                op["Hout"], op["Wout"], op["cout"], L.ptr(chi), L.ptr(clo), o_hi, o_lo,
-                                                cdst, st), "b2s_rpn_bg_fill")
+                # the conv kernel's epilogue warps store the constant into the background tiles
+                bgl, bgn, bhi, blo = L.ptr(self.bg_list[bl]), L.ptr(self.bg_counts[bl, 1:]), L.ptr(chi), L.ptr(clo)
             L.check(lib.b2s_conv2d_tc_ex(
                 L.ptr(src[0]), L.ptr(src[1]), self.B, op["Hin"], op["Win"], op["cin"], L.ptr(op["w_hi"]),
                 L.ptr(op["w_lo"]), op["kh"], op["kw"], op["stride"], op["pad"], op["cout"], op["n_pad"],
@@ -849,8 +837,7 @@ class InferenceEngine:
             # one tensor-core kernel per RPN layer (fused tail: 1 for 2); the multi-head crop op is one b2s_crop_nhwc kernel
             n += len(self.tc_plan) - (1 if self.tc_tail_fused else 0)
             if self.bg_idx:
-                # k_bg_layer per layer, k_bg_compact (+ k_bg_fill per layer unless the conv epilogue fills)
-                n += len(self.bg_idx) + 1 + (0 if self.bg_fused_fill else len(self.bg_idx))
+                n += len(self.bg_idx) + 1        # k_bg_layer per layer, k_bg_compact
         elif getattr(self, "any_sparse_tc", False):
             n += 1                               # b2s_merge_f16
         if self.mc:

@@ -48,6 +48,13 @@ def sparse_tc_cin(cin):
     return None
 
 
+def wants_tile_plan(subm, K):
+    """whether a rulebook gets a tile plan (csrc/sparse_plan.cu: rows grouped by neighbourhood shape + per-tile offset
+    masks) for b2s_sparse_conv_tc_plan.  SubM rulebooks with more than 3 offsets do: an ``indice_key`` shares them
+    between layers.  A strided conv uses its table once, so the plan would cost more than it saves."""
+    return bool(subm and K > 3)
+
+
 def pack_sparse_weights(w):
     """spconv weight [K, Cin, Cout] -> the K-major B operand b2s_sparse_conv_tc expects (fp32, before the split).
     Cin is zero-padded to sparse_tc_cin(Cin).  Cin = 64: [K, Cout, 64].  Cin < 64: PACK = 64/Cin kernel offsets

@@ -48,8 +48,6 @@ struct ConvParams {
     void *out_hi;            // fp16 hi plane, or (out_lo == NULL) the full fp32 result
     __half *out_lo;
     int *status;
-    int dbg;                 // B2S_CONV_DBG diagnostics (results wrong!): 1 = no lo loads, 4 = no drain
-    int chain;               // K blocks (tap x 64-channel chunk) per accumulation chain: 4 = 48 MMAs (B2S_CONV_CHAIN)
 };
 
 template <int N, int STAGES>
@@ -62,8 +60,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ 
     constexpr uint32_t STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
     constexpr int R = N / 2;                 // accumulator registers per thread (64 rows x N per warpgroup)
     // The tensor core's fp32 accumulate is not round-to-nearest: one long accumulation chain (432 MMAs for a 3x3x128
-    // tap stack) carries a systematic ~2e-5 relative error.  So the reduction is cut into short chains of p.chain K
-    // blocks (default 4 = 48 MMAs), and each chain's partial sum is added to the running fp32 sum with round-to-nearest.
+    // tap stack) carries a systematic ~2e-5 relative error.  So the reduction is cut into short chains of CHAIN K
+    // blocks (tap x 64-channel chunk; 4 = 48 MMAs), and each chain's partial sum is added to the running fp32 sum with
+    // round-to-nearest.
+    constexpr int CHAIN = 4;
     static_assert(N % 16 == 0 && N >= 16 && N <= 128, "wgmma N");
 
     extern __shared__ uint8_t smem_raw[];
@@ -103,13 +103,6 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ 
                     const int dy = tap / p.kw, dx = tap - dy * p.kw;
                     mbar_wait(&bar_empty[stage], phase ^ 1);
                     uint8_t *st = smem + (size_t)stage * STAGE_BYTES;
-                    if (p.dbg & 1) {
-                        mbar_arrive_expect_tx(&bar_full[stage], A_TILE_BYTES + B_TILE_BYTES);
-                        tma_load_4d(st, &map_a_hi, &bar_full[stage], chunk * BLOCK_K, w0 + dx, h0 + dy, b);
-                        tma_load_3d(st + 2 * A_TILE_BYTES, &map_b_hi, &bar_full[stage], chunk * BLOCK_K, 0, tap);
-                        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                        continue;
-                    }
                     mbar_arrive_expect_tx(&bar_full[stage], STAGE_BYTES);
                     tma_load_4d(st, &map_a_hi, &bar_full[stage], chunk * BLOCK_K, w0 + dx, h0 + dy, b);
                     tma_load_4d(st + A_TILE_BYTES, &map_a_lo, &bar_full[stage], chunk * BLOCK_K, w0 + dx, h0 + dy, b);
@@ -135,9 +128,9 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ 
             float sum[R], acc[R];
 #pragma unroll
             for (int j = 0; j < R; ++j) sum[j] = 0.f;
-            // accumulation chains of p.chain K blocks (default 4 = 48 MMAs), whatever the tap / channel split
-            for (int kb0 = 0; kb0 < num_kb; kb0 += p.chain) {
-                const int kb_chain = min(num_kb, kb0 + p.chain) - kb0;
+            // accumulation chains of CHAIN K blocks, whatever the tap / channel split
+            for (int kb0 = 0; kb0 < num_kb; kb0 += CHAIN) {
+                const int kb_chain = min(num_kb, kb0 + CHAIN) - kb0;
                 for (int chunk = 0; chunk < kb_chain; ++chunk) {
                     mbar_wait(&bar_full[stage], phase);          // TMA bytes have landed
                     const uint32_t sa = smem0 + (uint32_t)stage * STAGE_BYTES;
@@ -160,10 +153,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ 
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
                 // drain the chain's partial sum into the fp32 running sum (round-to-nearest adds)
-                if (!(p.dbg & 4)) {
 #pragma unroll
-                    for (int j = 0; j < R; ++j) sum[j] = __fadd_rn(sum[j], acc[j]);
-                }
+                for (int j = 0; j < R; ++j) sum[j] = __fadd_rn(sum[j], acc[j]);
             }
             // epilogue: this thread holds rows m0 = 64 cg + 16 wl + lane/4 and m0 + 8, and per 8-column block j the
             // channel pair 8j + 2(lane % 4); a quad of lanes writes 16 (fp16 plane) or 32 (fp32) contiguous bytes
@@ -254,13 +245,8 @@ extern "C" int b2s_conv2d_tc_ex(const b2s_half *in_hi_, const b2s_half *in_lo_, 
                 "b2s_conv2d_tc: output positions outside the Hout x Wout map");
     const int num_sms = num_sms_current();
     // 3x3 stride 1 pad 1, n_pad 128, hi/lo halo-padded output on the same grid: the weights-stationary N=256
-    // kernel (conv_tc2.cu).  B2S_CONV_V2=0 falls back to k_conv_tc below.
-    static int use_v2 = -1;
-    if (use_v2 < 0) {
-        const char *e = getenv("B2S_CONV_V2");
-        use_v2 = (e && e[0] == '0') ? 0 : 1;
-    }
-    const bool v2 = use_v2 && kh == 3 && kw == 3 && stride == 1 && pad == 1 && n_pad == 128 && out_lo != nullptr &&
+    // kernel (conv_tc2.cu).  Every other shape runs k_conv_tc below.
+    const bool v2 = kh == 3 && kw == 3 && stride == 1 && pad == 1 && n_pad == 128 && out_lo != nullptr &&
                     out_padded && out_mul == 1 && off_h == 0 && off_w == 0 && Hg == Hin && Wg == Win && Hout == Hin &&
                     Wout == Win;
     B2S_REQUIRE(work_list == nullptr || (v2 && work_count_dev != nullptr),
@@ -297,18 +283,6 @@ extern "C" int b2s_conv2d_tc_ex(const b2s_half *in_hi_, const b2s_half *in_lo_, 
     p.num_tiles = B * p.tiles_h * p.tiles_w;
     p.Hout = Hout; p.Wout = Wout; p.out_mul = out_mul; p.off_h = off_h; p.off_w = off_w;
     p.out_padded = out_padded; p.out_stride = out_stride;
-    {
-        static int dbg = -1;
-        if (dbg < 0) { const char *e = getenv("B2S_CONV_DBG"); dbg = e ? atoi(e) : 0; }
-#ifdef B2S_DIAG
-        p.dbg = dbg;            // diagnostics that corrupt results exist only in `make DIAG=1` builds
-#else
-        p.dbg = 0;
-#endif
-        static int chain = -1;
-        if (chain < 0) { const char *e = getenv("B2S_CONV_CHAIN"); chain = e ? atoi(e) : 4; if (chain < 1) chain = 1; }
-        p.chain = chain;
-    }
     p.scale = scale; p.shift = shift; p.out_hi = out_hi; p.out_lo = out_lo; p.status = (int *)status_dev;
     switch (n_pad) {
         case 128: return launch<128, 3>(a_hi, a_lo, b_hi, b_lo, p, num_sms, stream);

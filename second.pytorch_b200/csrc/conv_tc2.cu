@@ -41,14 +41,12 @@ struct Conv2Params {
     int B, H, W, Cin, Cout, relu;
     int tiles_h, tiles_w, num_tiles;
     const int *work_list, *work_count;   // optional (device): the tiles to compute, work_list[0 .. *work_count); tiles that
-                                         // are not listed are "background" (b2s_rpn_bg_plan) and get their constant from
-                                         // b2s_rpn_bg_fill.  NULL: every tile
+                                         // are not listed are "background" (b2s_rpn_bg_plan) and get their constant
+                                         // through bg_list.  NULL: every tile
     const int *bg_list, *bg_count;       // optional (device): background tiles of this layer's output; the consumer warps
     const __half *bg_hi, *bg_lo;         // copy them from the layer's empty-frame response bg_hi/bg_lo [H+2, W+2, Cout]
                                          // (one halo-padded frame) between their work items
     int out_stride;
-    int dbg;                         // B2S_CONV2_DBG diagnostics (results wrong): 1 no activation loads, 2 no weight
-                                     // loads, 4 no accumulator drain, 8 no global stores
     const float *scale, *shift;
     __half *out_hi, *out_lo;         // [B, H+2, W+2, out_stride] halo-padded fp16 planes (interior written)
     int *status;                     // bit B2S_STATUS_F16_RANGE raised when an activation exceeds the fp16 range
@@ -107,11 +105,6 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                         for (int chunk = 0; chunk < kchunks; ++chunk) {
                             mbar_wait(&bar_xempty[xs], xph ^ 1);
                             uint8_t *st = smem_x + (size_t)xs * X_STAGE_BYTES;
-                            if (p.dbg & 1) {                  // diagnostic: no activation loads (results wrong)
-                                mbar_arrive(&bar_xfull[xs]);
-                                if (++xs == X_STAGES) { xs = 0; xph ^= 1; }
-                                continue;
-                            }
                             mbar_arrive_expect_tx(&bar_xfull[xs], X_STAGE_BYTES);
                             // padded coordinates: output (h, w) reads padded rows h..h+2 and cols w..w+2
                             tma_load_4d(st, &map_x_hi, &bar_xfull[xs], chunk * BLOCK_K, w0 + dx, h0, b);
@@ -134,11 +127,6 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                             for (int dy = 0; dy < 3; ++dy)
                                 for (int pl = 0; pl < 2; ++pl) {           // hi plane, then lo plane
                                     mbar_wait(&bar_wempty[ws], wph ^ 1);
-                                    if (p.dbg & 2) {          // diagnostic: no weight loads (results wrong)
-                                        mbar_arrive(&bar_wfull[ws]);
-                                        if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
-                                        continue;
-                                    }
                                     mbar_arrive_expect_tx(&bar_wfull[ws], W_PLANE_BYTES);
                                     tma_load_3d(smem_w + (size_t)ws * W_PLANE_BYTES, pl ? &map_w_lo : &map_w_hi,
                                                 &bar_wfull[ws], chunk * BLOCK_K, 0, dy * 3 + dx);
@@ -230,10 +218,8 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&bar_xempty[xs]);
                     if (++xs == X_STAGES) { xs = 0; xph ^= 1; }
-                    if (!(p.dbg & 4)) {
 #pragma unroll
-                        for (int j = 0; j < 64; ++j) sum[j] = __fadd_rn(sum[j], acc[j]);
-                    }
+                    for (int j = 0; j < 64; ++j) sum[j] = __fadd_rn(sum[j], acc[j]);
                 }
                 // BN scale/shift + ReLU + hi/lo fp16 split.  This thread holds pixels m0 = 16 wl + lane/4 and m0 + 8 of
                 // the warpgroup's 64 (= rows 4 cg + m/16, column m % 16 of the half) and per 8-channel block j the
@@ -243,7 +229,7 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                 for (int rh = 0; rh < 2; ++rh) {
                     const int m = wl * 16 + (lane >> 2) + rh * 8;
                     const int h = th * T2_H + hf * HALF_H + cg * 4 + m / T2_W, w = tw * T2_W + m % T2_W;
-                    if (h >= p.H || w >= p.W || (p.dbg & 8)) continue;
+                    if (h >= p.H || w >= p.W) continue;
                     const size_t pix = ((size_t)b * (p.H + 2) + (h + 1)) * (p.W + 2) + (w + 1);
                     __half *oh = p.out_hi + pix * p.out_stride, *ol = p.out_lo + pix * p.out_stride;
 #pragma unroll
@@ -299,15 +285,6 @@ int b2s_conv3x3_tc2(const __half *in_hi, const __half *in_lo, int B, int H, int 
     p.work_list = work_list; p.work_count = work_list ? work_count : nullptr;
     p.bg_list = bg_list; p.bg_count = bg_count; p.bg_hi = bg_hi; p.bg_lo = bg_lo;
     p.out_stride = out_stride;
-    {
-        static int dbg = -1;
-        if (dbg < 0) { const char *e = getenv("B2S_CONV2_DBG"); dbg = e ? atoi(e) : 0; }
-#ifdef B2S_DIAG
-        p.dbg = dbg;            // diagnostics that corrupt results exist only in `make DIAG=1` builds
-#else
-        p.dbg = 0;
-#endif
-    }
     p.scale = scale; p.shift = shift; p.out_hi = out_hi; p.out_lo = out_lo; p.status = status;
     const size_t smem = (size_t)X_STAGES * X_STAGE_BYTES + (size_t)W_STAGES * W_PLANE_BYTES + 1024;
     B2S_SMEM_OPT_IN(k_conv3x3_tc2, smem);

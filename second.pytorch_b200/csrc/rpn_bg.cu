@@ -1,4 +1,4 @@
-// rpn_bg.cu -- background-tile planning for the dense RPN (b2s_rpn_bg_plan, b2s_rpn_bg_fill).
+// rpn_bg.cu -- background-tile planning for the dense RPN (b2s_rpn_bg_plan).
 //
 // The BEV map that enters the RPN is mostly empty: 6-8 % of the 200 x 176 pixels of a synthetic KITTI cloud hold
 // data (real clouds: the camera-FOV wedge).  The output of layer l of a chain of 3x3 stride-1 pad-1 layers at pixel p
@@ -8,12 +8,10 @@
 // empty-frame response once per layer with the very kernel that runs the layer (so the values are bit-identical to
 // what the kernel would have produced) and keeps it as one halo-padded frame [H+2, W+2, C] of hi/lo planes.
 // Per step, the data mask is dilated by one pixel per layer (one tiny kernel per layer); a 16 x 16 output tile of
-// k_conv3x3_tc2 without a masked pixel is not computed -- it is copied from the empty-frame response (by the conv
-// kernel's own epilogue warps, or b2s_rpn_bg_fill) -- and the conv kernel walks the compacted list of the remaining
-// tiles, so the work stays balanced over the SMs.
+// k_conv3x3_tc2 without a masked pixel is not computed -- the conv kernel's own epilogue warps copy it from the
+// empty-frame response -- and the conv kernel walks the compacted list of the remaining tiles, so the work stays
+// balanced over the SMs.
 // Everything the reference computes is still produced; only the recomputation of a known field is skipped.
-#include <cuda_fp16.h>
-
 #include "common.cuh"
 
 namespace {
@@ -75,39 +73,6 @@ k_bg_compact(const int *__restrict__ tile_flag, int num_tiles, int *work_list, i
     }
 }
 
-// one block per background tile (grid-stride): thread = (pixel of a tile row, 16-byte channel chunk), so one load /
-// store instruction of the block moves one whole tile row of a plane (16 pixels x 256 B, contiguous in NHWC) from
-// the empty-frame response `f` [H+2, W+2, C] to the output map
-__global__ void __launch_bounds__(256)
-k_bg_fill(const int *__restrict__ bg_list, const int *__restrict__ bg_count, int H, int W, int tiles_h, int tiles_w, int C,
-          const __half *__restrict__ f_hi, const __half *__restrict__ f_lo, __half *__restrict__ out_hi,
-          __half *__restrict__ out_lo, int out_stride)
-{
-    const int n = *bg_count;
-    const int chunks = C / 8;                         // 16-byte chunks per pixel and plane
-    const int px_per_pass = 256 / chunks;             // pixels of a tile row covered per pass (C = 128: 16)
-    const int chunk = threadIdx.x % chunks, px = threadIdx.x / chunks;
-    for (int i = blockIdx.x; i < n; i += gridDim.x) {
-        const int tile = bg_list[i];
-        const int tw = tile % tiles_w, th = (tile / tiles_w) % tiles_h, b = tile / (tiles_w * tiles_h);
-        for (int r = 0; r < TILE; ++r) {
-            const int h = th * TILE + r;
-            if (h >= H) break;
-            for (int p0 = 0; p0 < TILE; p0 += px_per_pass) {
-                const int w = tw * TILE + p0 + px;
-                if (p0 + px < TILE && w < W) {
-                    const size_t fpix = (size_t)(h + 1) * (W + 2) + (w + 1);
-                    const size_t pix = (size_t)b * (H + 2) * (W + 2) + fpix;
-                    *reinterpret_cast<uint4 *>(out_hi + pix * out_stride + chunk * 8) =
-                        __ldg(reinterpret_cast<const uint4 *>(f_hi + fpix * C + chunk * 8));
-                    *reinterpret_cast<uint4 *>(out_lo + pix * out_stride + chunk * 8) =
-                        __ldg(reinterpret_cast<const uint4 *>(f_lo + fpix * C + chunk * 8));
-                }
-            }
-        }
-    }
-}
-
 }  // namespace
 
 extern "C" int b2s_rpn_bg_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, uint8_t *scratch,
@@ -127,23 +92,6 @@ extern "C" int b2s_rpn_bg_plan(const uint8_t *occupancy, int batch, int H, int W
         in = out;
     }
     k_bg_compact<<<num_layers, 1024, 0, stream>>>(tile_flags, num_tiles, work_lists, bg_lists, counts);
-    B2S_LAUNCH_OK();
-    return 0;
-}
-
-extern "C" int b2s_rpn_bg_fill(const int *bg_list, const int *bg_count_dev, int batch, int H, int W, int C,
-                               const b2s_half *f_hi, const b2s_half *f_lo, b2s_half *out_hi, b2s_half *out_lo,
-                               int out_stride, void *stream_)
-{
-    cudaStream_t stream = (cudaStream_t)stream_;
-    B2S_REQUIRE(C % 8 == 0 && C >= 8 && C <= 2048 && 256 % (C / 8) == 0 && out_stride >= C && out_stride % 8 == 0,
-                "b2s_rpn_bg_fill: C must be a multiple of 8 whose chunk count divides 256");
-    const int tiles_h = b2s_cdiv(H, TILE), tiles_w = b2s_cdiv(W, TILE);
-    const int num_tiles = batch * tiles_h * tiles_w;
-    int blocks = num_tiles < 132 * 8 ? num_tiles : 132 * 8;
-    k_bg_fill<<<blocks, 256, 0, stream>>>(bg_list, bg_count_dev, H, W, tiles_h, tiles_w, C,
-                                          reinterpret_cast<const __half *>(f_hi), reinterpret_cast<const __half *>(f_lo),
-                                          reinterpret_cast<__half *>(out_hi), reinterpret_cast<__half *>(out_lo), out_stride);
     B2S_LAUNCH_OK();
     return 0;
 }

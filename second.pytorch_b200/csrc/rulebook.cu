@@ -210,7 +210,7 @@ __global__ void k_nz_scan(int *nz_cnt /*in: counts, out: exclusive prefix inside
 // and pre-fills the rows' neighbour-table entries with -1.
 __global__ void k_conv_emit(const unsigned *__restrict__ bitmap, const int *__restrict__ nz_word,
                             const int *__restrict__ nz_prefix, const int *__restrict__ chunk_prefix,
-                            const int *__restrict__ nnz_dev, ConvGeom g, int cap_out, int *coors_out, int *nbr_fill,
+                            const int *__restrict__ nnz_dev, ConvGeom g, int cap_out, int *coors_out, int *nbr,
                             int *wrow0)
 {
     const int lane = threadIdx.x & 31;
@@ -229,12 +229,10 @@ __global__ void k_conv_emit(const unsigned *__restrict__ bitmap, const int *__re
             const unsigned wbits = __shfl_sync(0xffffffffu, bits, src);
             const int row0 = __shfl_sync(0xffffffffu, my_row0, src);
             const int word = __shfl_sync(0xffffffffu, my_word, src);
-            if (nbr_fill) {
-                // the rows of one bitmap word are consecutive: pre-fill their neighbour-table entries with -1
-                // (coalesced) for k_conv_scatter_nbr, instead of a capacity-sized memset
-                const int cnt = min(__popc(wbits), max(cap_out - row0, 0));
-                for (int q = lane; q < cnt * g.K; q += 32) nbr_fill[(size_t)row0 * g.K + q] = -1;
-            }
+            // the rows of one bitmap word are consecutive: pre-fill their neighbour-table entries with -1
+            // (coalesced) for k_conv_scatter_nbr, instead of a capacity-sized memset
+            const int cnt = min(__popc(wbits), max(cap_out - row0, 0));
+            for (int q = lane; q < cnt * g.K; q += 32) nbr[(size_t)row0 * g.K + q] = -1;
             if (wbits & (1u << lane)) {
                 int row = row0 + __popc(wbits & ((1u << lane) - 1u));
                 if (row < cap_out) {
@@ -252,40 +250,11 @@ __global__ void k_conv_emit(const unsigned *__restrict__ bitmap, const int *__re
     }
 }
 
-// one thread per (output row, k): neighbour lookup in the input hash
-__global__ void k_conv_nbr(const int *__restrict__ coors_out, const int *__restrict__ n_out_dev, int cap_out,
-                           ConvGeom g, const unsigned long long *__restrict__ keys_in,
-                           const int *__restrict__ vals_in, int mask_in, int *nbr, unsigned *row_mask)
-{
-    const int n = min(*n_out_dev, cap_out);
-    const long long total = (long long)n * g.K;
-    for (long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x; gid < total;
-         gid += (long long)gridDim.x * blockDim.x) {
-        int row = (int)(gid / g.K), k = (int)(gid % g.K);
-        int kk[3] = {k / (g.k[2] * g.k[1]), (k / g.k[2]) % g.k[1], k % g.k[2]};
-        int4 c = *reinterpret_cast<const int4 *>(coors_out + (size_t)row * 4);
-        int oc[3] = {c.y, c.z, c.w};
-        int ic[3];
-        bool ok = true;
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {
-            ic[j] = oc[j] * g.s[j] - g.p[j] + kk[j] * g.d[j];
-            if (ic[j] < 0 || ic[j] >= g.in_shape[j]) ok = false;
-        }
-        int r = -1;
-        if (ok)
-            r = b2s_hash_find(keys_in, vals_in, mask_in,
-                              b2s_flat_key(c.x, ic[0], ic[1], ic[2], g.in_shape[0], g.in_shape[1], g.in_shape[2]));
-        nbr[gid] = r;
-        if (row_mask && r >= 0) atomicOr(&row_mask[row], 1u << k);
-    }
-}
-
-// The same table built from the INPUT side: every input row visits the (<= ceil(k/s)^3) output cells it feeds,
-// ranks each cell in the occupancy bitmap (block prefix + word prefix + popcount of the lower bits = its output
+// Strided neighbour table, built from the INPUT side: every input row visits the (<= ceil(k/s)^3) output cells it
+// feeds, ranks each cell in the occupancy bitmap (block prefix + word prefix + popcount of the lower bits = its output
 // row, exactly what k_conv_emit assigns) and writes nbr[row_out][k] = row_in.  Work is proportional to the
-// (input, output) pairs instead of rows_out * K hash probes of which ~70 % miss (k_conv_nbr: 36 us vs the
-// level's 14 us mark pass, ncu launch list round 1); nbr is pre-filled with -1 by the caller.
+// (input, output) pairs instead of rows_out * K hash probes of which ~70 % miss (an output-side hash lookup took
+// 36 us vs the level's 14 us mark pass, ncu launch list round 1); nbr is pre-filled with -1 by k_conv_emit.
 __global__ void k_conv_scatter_nbr(const int *__restrict__ coors_in, const int *__restrict__ n_in_dev, int cap_in,
                                    ConvGeom g, const unsigned *__restrict__ bitmap,
                                    const int *__restrict__ wrow0, int cap_out, int *nbr, unsigned *row_mask)
@@ -479,8 +448,7 @@ extern "C" size_t b2s_rulebook_conv_workspace_bytes(int batch, const int *out_sh
 extern "C" int b2s_rulebook_conv(const int *coors_in, const int *num_in_dev, int cap_in, int batch,
                                  const int *in_shape, const int *out_shape, const int *ksize,
                                  const int *stride, const int *padding, const int *dilation,
-                                 const unsigned long long *hash_keys_in, const int *hash_vals_in,
-                                 int hash_cap_in, int *coors_out, int *num_out_dev, int cap_out, int *nbr,
+                                 int *coors_out, int *num_out_dev, int cap_out, int *nbr,
                                  unsigned long long *hash_keys_out, int *hash_vals_out, int hash_cap_out,
                                  void *workspace, size_t workspace_bytes, unsigned *row_mask, unsigned *status_dev,
                                  void *stream_)
@@ -529,11 +497,8 @@ extern "C" int b2s_rulebook_conv(const int *coors_in, const int *num_in_dev, int
     B2S_LAUNCH_OK();
     k_scan_sums<<<1, kScanThreads, 0, stream>>>(w.chunk_sums, 0, w.nnz, num_out_dev, cap_out, status_dev);
     B2S_LAUNCH_OK();
-    static int use_scatter = -1;   // B2S_RB_SCATTER=0: neighbour table by hash probes from the output side (k_conv_nbr)
-    if (use_scatter < 0) { const char *e = getenv("B2S_RB_SCATTER"); use_scatter = (e && e[0] == '0') ? 0 : 1; }
-    if (!hash_keys_in) use_scatter = 1;
     k_conv_emit<<<bounded_grid(w.nwords < (1ll << 22) ? w.nwords : (1ll << 22), kThreads), kThreads, 0, stream>>>(
-        w.bitmap, w.nz_word, w.nz_prefix, w.chunk_sums, w.nnz, g, cap_out, coors_out, use_scatter ? nbr : nullptr, w.wrow0);
+        w.bitmap, w.nz_word, w.nz_prefix, w.chunk_sums, w.nnz, g, cap_out, coors_out, nbr, w.wrow0);
     B2S_LAUNCH_OK();
     if (cap_out > 0) {
         if (want_hash) {
@@ -542,14 +507,11 @@ extern "C" int b2s_rulebook_conv(const int *coors_in, const int *num_in_dev, int
                 hash_vals_out, hash_cap_out - 1, status_dev);
             B2S_LAUNCH_OK();
         }
-        if (use_scatter && cap_in > 0) {
+        if (cap_in > 0) {
             k_conv_scatter_nbr<<<bounded_grid(cap_in, kThreads), kThreads, 0, stream>>>(
                 coors_in, num_in_dev, cap_in, g, w.bitmap, w.wrow0, cap_out, nbr, row_mask);
-        } else {
-            k_conv_nbr<<<bounded_grid((long long)cap_out * g.K, kThreads), kThreads, 0, stream>>>(
-                coors_out, num_out_dev, cap_out, g, hash_keys_in, hash_vals_in, hash_cap_in - 1, nbr, row_mask);
+            B2S_LAUNCH_OK();
         }
-        B2S_LAUNCH_OK();
     }
     return 0;
 }

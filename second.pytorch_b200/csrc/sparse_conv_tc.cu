@@ -48,19 +48,6 @@ __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t *bar)
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-// warp-level wait: only lane 0 polls the barrier (32 lanes spinning on try_wait are 32 shared-memory operations per
-// iteration competing with the copies for the LSU), the others are released through __syncwarp
-__device__ __forceinline__ void mbar_wait_warp(uint64_t *bar, uint32_t parity, bool lane0_only)
-{
-    if (lane0_only) {
-        if ((threadIdx.x & 31) == 0) mbar_wait_sleep(bar, parity);
-        __syncwarp();
-    } else {
-        mbar_wait(bar, parity);
-    }
-}
-
-
 // read-only load the compiler may not move (volatile asm keeps its place among the other volatile asm statements: the
 // copies, the barrier operations).  The neighbour-table entries of the NEXT owned K block must be in flight while the
 // current one is waited for and copied; as plain __ldg the compiler scheduled them next to their first use, and a third
@@ -81,7 +68,6 @@ struct SpParams {
     const int *perm;             // tile position -> output row (NULL: identity)
     const unsigned *tile_mask;   // per 128-position tile: kernel offsets some row of the tile has (NULL: all)
     int cap_out, K, relu;
-    int flags;                   // B2S_SP_ZSKIP: bit 0 zero-slot skip (default on); 32 lane-0 polling with a sleeping wait
     const float *scale, *shift;
     void *out_hi;                // fp16 hi plane, or (out_lo == NULL) fp32 rows [cap_out, COUT]
     __half *out_lo;
@@ -140,7 +126,6 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
     const int K = p.K;
     const int num_kb = (K + PACK - 1) / PACK;
     const int num_chains = (num_kb + CHAIN_KB - 1) / CHAIN_KB;
-    const bool poll1 = (p.flags & 32) != 0;                 // B2S_SP_ZSKIP bit 32: lane 0 polls with a sleeping wait
     const uint32_t all_offsets = K >= 32 ? 0xffffffffu : ((1u << K) - 1u);
     auto tile_kbm = [&](int tile) -> uint32_t {
         return kb_mask_of<PACK>(p.tile_mask ? __ldg(&p.tile_mask[tile]) & all_offsets : all_offsets, num_kb);
@@ -179,7 +164,6 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
         asm volatile("" : "+l"(src_base));                     // one 64-bit register (not base + lane part re-added per copy)
         const long long lo_delta = reinterpret_cast<const char *>(p.in_lo) - reinterpret_cast<const char *>(p.in_hi);
         const uint32_t row_bytes = (uint32_t)p.in_stride * ELEM_BYTES;       // rows_in * row_bytes < 2^32 (checked on the host)
-        const bool zskip_on = (p.flags & 1) != 0;
         const int grid = (int)gridDim.x;
         const int *__restrict__ nbr = p.nbr;
         const int pos0 = half * (BLOCK_M / HALVES) + sub;      // tile position of row slot i: pos0 + 4 i
@@ -263,20 +247,15 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
             const uint32_t use_parity = (((uint32_t)g_cur / STAGES) & 1u) ^ 1u;
             const int zsh = (my_stage & 3) * RI;
             const uint32_t zeroed = (uint32_t)((my_stage < 4 ? zeroed_w0 : zeroed_w1) >> zsh) & ((1u << RI) - 1u);
-            const uint32_t need = zskip_on ? (valid | (~zeroed & ((1u << RI) - 1u))) : 0xFFFFFFFFu;
+            const uint32_t need = valid | (~zeroed & ((1u << RI) - 1u));
             const uint32_t sa = sa0 + (uint32_t)my_stage * STAGE_BYTES;
-            mbar_wait_warp(&bar_empty[my_stage], use_parity, poll1);
+            mbar_wait(&bar_empty[my_stage], use_parity);
             // the K block's weights: its expect_tx arrival is the "+ 1" of the stage's bar_full count
             if (half == 0 && lane == 0) {
                 uint8_t *st = smem + (size_t)my_stage * STAGE_BYTES;
-#ifdef B2S_DIAG
-                if (p.flags & 4) mbar_arrive(&bar_full[my_stage]); else
-#endif
-                {
-                    mbar_arrive_expect_tx(&bar_full[my_stage], 2 * B_TILE_BYTES);
-                    tma_load_3d(st + 2 * A_TILE_BYTES, &map_w_hi, &bar_full[my_stage], 0, 0, kb_cur);
-                    tma_load_3d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_w_lo, &bar_full[my_stage], 0, 0, kb_cur);
-                }
+                mbar_arrive_expect_tx(&bar_full[my_stage], 2 * B_TILE_BYTES);
+                tma_load_3d(st + 2 * A_TILE_BYTES, &map_w_hi, &bar_full[my_stage], 0, 0, kb_cur);
+                tma_load_3d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_w_lo, &bar_full[my_stage], 0, 0, kb_cur);
             }
             if (lo_delta == (long long)(CIN * ELEM_BYTES)) {
                 // interleaved rows [hi Cin | lo Cin]: the lo copy is the hi address + an immediate
@@ -310,7 +289,7 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
                 const unsigned long long set = (unsigned long long)(~valid & ((1u << RI) - 1u)) << zsh;
                 if (my_stage < 4) zeroed_w0 = (zeroed_w0 & clr) | set; else zeroed_w1 = (zeroed_w1 & clr) | set;
             }
-            if (p.flags & 128) mbar_arrive(&bar_full[my_stage]); else cp_async_mbar_arrive_noinc(&bar_full[my_stage]);
+            cp_async_mbar_arrive_noinc(&bar_full[my_stage]);
             // ---- advance ----
             g_cur = e_owned;
             kb_cur = kb_nxt;
@@ -353,7 +332,7 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
             while (kbm) {
                 const uint32_t low = kbm & (0u - kbm);
                 kbm ^= low;
-                mbar_wait_warp(&bar_full[stage], phase, poll1);
+                mbar_wait(&bar_full[stage], phase);
                 fence_proxy_async();                            // gathered rows were written by cp.async (generic proxy)
                 const uint32_t sa = smem0 + (uint32_t)stage * STAGE_BYTES;
                 const uint64_t a_hi = make_desc_sw128(sa + a_off), a_lo = make_desc_sw128(sa + A_TILE_BYTES + a_off);
@@ -464,15 +443,6 @@ extern "C" int b2s_sparse_conv_tc_plan(const b2s_half *feat_hi, const b2s_half *
     p.in_stride = in_stride; p.out_stride = out_stride; p.status = (int *)status_dev;
     p.nbr = nbr; p.n_out_dev = num_out_dev; p.cap_out = cap_out; p.K = K;
     p.perm = perm; p.tile_mask = tile_mask;
-    {
-        static int fl = -1;
-        if (fl < 0) { const char *e = getenv("B2S_SP_ZSKIP"); fl = e ? atoi(e) : 1; }
-#ifdef B2S_DIAG
-        p.flags = fl;           // make DIAG=1: bit 2 no gather copies, 4 no weight loads, 8 no zero fills (results wrong)
-#else
-        p.flags = fl & (1 | 32);
-#endif
-    }
     p.relu = relu; p.scale = scale; p.shift = shift; p.out_hi = out_hi; p.out_lo = reinterpret_cast<__half *>(out_lo);
 #define B2S_TC_CASE(CI, CO) if (cin == CI && cout == CO) return launch<CI, CO>(m_hi, m_lo, p, num_sms, stream);
     B2S_TC_CASE(64, 64) B2S_TC_CASE(64, 32) B2S_TC_CASE(64, 16) B2S_TC_CASE(32, 64) B2S_TC_CASE(32, 32) B2S_TC_CASE(32, 16)

@@ -53,23 +53,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
     }
     __trap();
 }
-// the same wait with a suspend-time hint (the form CUTLASS's ClusterBarrier::wait uses): the thread sleeps in the
-// barrier unit instead of re-polling -- fewer shared-memory operations from many waiting warps, but a later wake-up.
-__device__ __forceinline__ void mbar_wait_sleep(uint64_t *bar, uint32_t parity)
-{
-    uint32_t addr = smem_u32(bar);
-#pragma unroll 1
-    for (uint32_t it = 0; it < (1u << 28); ++it) {
-        uint32_t done;
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done) : "r"(addr), "r"(parity), "r"(0x989680u) : "memory");
-        if (done) return;
-    }
-    __trap();
-}
 
 __device__ __forceinline__ void tma_load_4d(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1,
                                             int c2, int c3)

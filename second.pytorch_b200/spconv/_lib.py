@@ -36,8 +36,8 @@ SIGNATURES = {
                                   c_void_p, c_void_p, c_void_p]),
     "b2s_rulebook_conv_workspace_bytes": (c_size_t, [c_int, c_void_p]),
     "b2s_rulebook_conv": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                  c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
-                                  c_void_p, c_int, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
+                                  c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                  c_size_t, c_void_p, c_void_p, c_void_p]),
     "b2s_rulebook_subm_ranked": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
                                          c_void_p, c_void_p, c_void_p]),
     "b2s_rulebook_pairs": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
@@ -79,8 +79,6 @@ SIGNATURES = {
                               c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2s_rpn_bg_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                 c_void_p]),
-    "b2s_rpn_bg_fill": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                c_int, c_void_p]),
     "b2s_conv2d_tc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                               c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "b2s_conv2d_tc_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
@@ -148,7 +146,7 @@ def load():
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
-    if lib.b2s_version() < 200:
+    if lib.b2s_version() < 201:
         raise ImportError("libb2second.so is too old")
     _lib = lib
     return lib

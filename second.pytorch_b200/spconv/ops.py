@@ -45,7 +45,6 @@ def build_rulebook(x, ksize, stride, padding, dilation, subm):
     dev = idx.device
     n_in = idx.shape[0]
     K = int(np.prod(ksize))
-    keys, vals, cap = x._locator()
     n_in_dev = torch.tensor([n_in], dtype=torch.int32, device=dev)
     rb = Rulebook()
     rb.K = K
@@ -54,6 +53,7 @@ def build_rulebook(x, ksize, stride, padding, dilation, subm):
     rb.plan = None
     rb.nbrT = None
     if subm:
+        keys, vals, cap = x._locator()
         nbr = torch.empty(max(n_in, 1), K, dtype=torch.int32, device=dev)
         rb.row_mask = torch.empty(max(n_in, 1), dtype=torch.int32, device=dev)      # bit k: nbr[row][k] exists
         _lib.check(lib.b2s_rulebook_subm(_lib.ptr(idx), _lib.ptr(n_in_dev), n_in, _lib.i3(x.spatial_shape),
@@ -83,9 +83,8 @@ def build_rulebook(x, ksize, stride, padding, dilation, subm):
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
     _lib.check(lib.b2s_rulebook_conv(
         _lib.ptr(idx), _lib.ptr(n_in_dev), n_in, x.batch_size, _lib.i3(x.spatial_shape), oshape, _lib.i3(ksize),
-        _lib.i3(stride), _lib.i3(padding), _lib.i3(dilation), _lib.ptr(keys), _lib.ptr(vals), cap,
-        _lib.ptr(coors_out), _lib.ptr(num_out_dev), cap_out, _lib.ptr(nbr), _lib.ptr(keys_out), _lib.ptr(vals_out),
-        hash_cap_out, _lib.ptr(ws), ws_bytes, _lib.ptr(row_mask), _lib.ptr(status), _lib.stream()), "b2s_rulebook_conv")
+        _lib.i3(stride), _lib.i3(padding), _lib.i3(dilation), _lib.ptr(coors_out), _lib.ptr(num_out_dev), cap_out,
+        _lib.ptr(nbr), _lib.ptr(keys_out), _lib.ptr(vals_out), hash_cap_out, _lib.ptr(ws), ws_bytes, _lib.ptr(row_mask), _lib.ptr(status), _lib.stream()), "b2s_rulebook_conv")
     n_out, st = int(num_out_dev.item()), int(status.item())   # the one sync of the module-by-module path
     if st:
         raise RuntimeError("b2s_rulebook_conv: " + _lib.status_message(st))
@@ -101,10 +100,10 @@ def build_rulebook(x, ksize, stride, padding, dilation, subm):
 
 def tile_plan(rb):
     """tile plan of a rulebook for b2s_sparse_conv_tc_plan: (perm, tile_mask), built once per rulebook from the row masks
-    the builder wrote.  Rows are grouped for SubM rulebooks (an ``indice_key`` shares them between layers); a strided
-    conv uses its table once, so it gets no plan (None, None) -- the same policy as the fused engine."""
+    the builder wrote, or (None, None) where b2second.tc.wants_tile_plan says the rulebook gets none."""
+    from b2second import tc as _tc
     if rb.plan is None:
-        if not rb.subm or rb.K <= 3 or rb.num_out <= 0 or getattr(rb, "row_mask", None) is None:
+        if not _tc.wants_tile_plan(rb.subm, rb.K) or rb.num_out <= 0 or getattr(rb, "row_mask", None) is None:
             rb.plan = (None, None)
         else:
             lib = _lib.load()

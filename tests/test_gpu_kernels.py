@@ -350,11 +350,12 @@ def test_multiclass_nms_branch_on_the_fused_engine(product, name, agnostic):
 
 
 # ------------------------------------------------------------------------------------------------ RPN background tiles
-def test_rpn_background_plan_matches_numpy_and_engine_results_do_not_change(product, monkeypatch):
+def test_rpn_background_plan_matches_numpy_and_background_skip_is_bit_identical(product, monkeypatch):
     """b2s_rpn_bg_plan against its numpy restatement (tests/test_host_rpn_plan.py), and the fused engine with the
-    background-tile skip on vs off (tiles copied from the layer's empty-frame response by the conv kernel's epilogue warps,
-    or by b2s_rpn_bg_fill): bit-identical head tensors, candidates and detections."""
+    background-tile skip on vs off (tiles copied from the layer's empty-frame response by the conv kernel's epilogue
+    warps): bit-identical head tensors, candidates and detections."""
     import test_host_rpn_plan as hp
+    from b2second import tc
     from b2second.engine import InferenceEngine
     L = product._lib
     lib = L.load()
@@ -390,21 +391,19 @@ def test_rpn_background_plan_matches_numpy_and_engine_results_do_not_change(prod
     net = net.cuda()
     clouds = [torch.from_numpy(gu.make_cloud(name, s, n)).cuda() for s, n in ((0, 20000), (1, 29000))]
     res = {}
-    for mode, fill in (("1", "fused"), ("1", "separate"), ("0", "fused")):
-        monkeypatch.setenv("B2S_RPN_BG", mode)
-        monkeypatch.setenv("B2S_RPN_BG_FILL", fill)
-        eng = InferenceEngine(net, batch_size=2, max_points=30000, use_cuda_graph=(fill == "fused"))
-        assert bool(eng.bg_idx) == (mode == "1")
+    for bg_on in (True, False):
+        if not bg_on:                                        # the reference: no layer tracks background tiles
+            monkeypatch.setattr(tc, "background_layers", lambda plan: [])
+        eng = InferenceEngine(net, batch_size=2, max_points=30000, use_cuda_graph=True)
+        assert bool(eng.bg_idx) == bg_on
         eng.infer(clouds)
-        res[mode, fill] = (eng.detections(), eng.tc_heads.clone(), eng.cand_count.clone(),
-                           eng.bg_counts.clone() if eng.bg_idx else None, getattr(eng, "bg_tiles", 0))
-    off = res["0", "fused"]
-    for key in (("1", "fused"), ("1", "separate")):
-        on = res[key]
-        assert torch.equal(on[2], off[2])
-        skipped = on[3][:, 1].float() / on[4]
-        assert float(skipped.min()) > 0.3, skipped          # border tiles without data are background too
-        assert torch.equal(on[1], off[1]), key               # the copied field is what the kernel computes: bit-identical
-        for a, b in zip(on[0], off[0]):
-            assert a["box3d_lidar"].shape == b["box3d_lidar"].shape and a["box3d_lidar"].shape[0] > 0
-            assert torch.equal(a["box3d_lidar"], b["box3d_lidar"]) and torch.equal(a["scores"], b["scores"])
+        res[bg_on] = (eng.detections(), eng.tc_heads.clone(), eng.cand_count.clone(),
+                      eng.bg_counts.clone() if eng.bg_idx else None, getattr(eng, "bg_tiles", 0))
+    on, off = res[True], res[False]
+    assert torch.equal(on[2], off[2])
+    skipped = on[3][:, 1].float() / on[4]
+    assert float(skipped.min()) > 0.3, skipped              # border tiles without data are background too
+    assert torch.equal(on[1], off[1])                        # the copied field is what the kernel computes: bit-identical
+    for a, b in zip(on[0], off[0]):
+        assert a["box3d_lidar"].shape == b["box3d_lidar"].shape and a["box3d_lidar"].shape[0] > 0
+        assert torch.equal(a["box3d_lidar"], b["box3d_lidar"]) and torch.equal(a["scores"], b["scores"])
