@@ -60,7 +60,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 201
+#define B2S_VERSION 202
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -281,7 +281,7 @@ int b2s_from_bev(const float *dmap, const int *coors, const int *num_rows_dev, i
 int b2s_to_bev_tc(const float *feat, const b2s_half *feat_hi, const b2s_half *feat_lo, int feat_stride,
                   const int *coors, const int *num_rows_dev, int cap_rows, int C, int batch, int D, int H, int W,
                   b2s_half *out_hi, b2s_half *out_lo,
-                  uint8_t *occupancy /*optional [B,H,W]: 1 where a pixel received data (input of b2s_rpn_bg_plan)*/,
+                  uint8_t *occupancy /*optional [B,H,W]: 1 where a pixel received data (input of b2s_rpn_block_plan)*/,
                   void *stream);
 
 /* ---- dense RPN convolution on the tensor pipe (second/pytorch/models/rpn.py:467-497 blocks, :264-299 deblocks,
@@ -312,12 +312,12 @@ int b2s_conv2d_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int batch, in
                      int n_pad, const float *scale, const float *shift, int relu, int Hg, int Wg, void *out_hi,
                      b2s_half *out_lo, int Hout, int Wout, int out_padded, int out_stride, int out_mul, int off_h,
                      int off_w,
-                     const int *work_list /*optional (device): ids of the 16x16 output tiles to compute, from
-                                            b2s_rpn_bg_plan; only for the 3x3 stride-1 128-channel form; NULL: all*/,
+                     const int *work_list /*optional (device): ids of the 8x8 output blocks to compute, from
+                                            b2s_rpn_block_plan; only for the 3x3 stride-1 128-channel form; NULL: all*/,
                      const int *work_count_dev,
-                     const int *bg_list /*optional, with work_list: the background tiles of the output; the kernel's
-                                          epilogue warps copy them from the layer's empty-frame response bg_hi/bg_lo
-                                          [Hout+2, Wout+2, Cout] while they wait for the tensor pipe*/,
+                     const int *bg_list /*optional, with work_list: the background blocks of the output; the kernel's
+                                          fill warps copy them from the layer's empty-frame response bg_hi/bg_lo
+                                          [Hout+2, Wout+2, Cout] while its other warps compute the listed blocks*/,
                      const int *bg_count_dev, const b2s_half *bg_hi, const b2s_half *bg_lo, unsigned *status_dev,
                      void *stream);
 
@@ -327,12 +327,16 @@ int b2s_conv2d_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int batch, in
  * at p, a field that depends on the weights only (constant in the interior, different within l pixels of the border).
  * The caller computes that field once per layer by running the layer itself on an empty frame, and keeps it as one
  * halo-padded frame [H+2, W+2, C] of hi/lo planes.
- * b2s_rpn_bg_plan dilates the data mask through `num_layers` consecutive 3x3 stride-1 pad-1 layers and compacts, per
- * layer l, the 16x16 output tiles into
- *   work_lists[l*num_tiles ..]  tiles with a masked pixel (ascending), counts[2l] of them -> b2s_conv2d_tc_ex work_list
- *   bg_lists  [l*num_tiles ..]  background tiles,               counts[2l + 1] of them  -> b2s_conv2d_tc_ex bg_list
- * with num_tiles = batch * ceil(H/16) * ceil(W/16), tile id = (b * tiles_h + th) * tiles_w + tw.
- * scratch: 2*batch*H*W bytes; tile_flags: num_layers*num_tiles ints. */
+ * b2s_rpn_block_plan dilates the data mask through `num_layers` consecutive 3x3 stride-1 pad-1 layers and compacts,
+ * per layer l, the 8x8 output blocks into
+ *   work_lists[l*num_blocks ..]  blocks with a masked pixel (ascending), counts[2l] of them -> work_list
+ *   bg_lists  [l*num_blocks ..]  background blocks,               counts[2l + 1] of them  -> bg_list
+ * of b2s_conv2d_tc_ex, with num_blocks = batch * ceil(H/8) * ceil(W/8), block id = (b * blocks_h + bh) * blocks_w + bw.
+ * scratch: 2*batch*H*W bytes; block_flags: num_layers*num_blocks ints (1 = the block is computed).
+ * b2s_rpn_bg_plan is the same plan over 16x16 tiles (tile_flags / lists of num_tiles = batch * ceil(H/16) * ceil(W/16)
+ * entries, tile id = (b * tiles_h + th) * tiles_w + tw); its lists are not accepted by b2s_conv2d_tc_ex. */
+int b2s_rpn_block_plan(const uint8_t *occupancy /*[B,H,W]*/, int batch, int H, int W, int num_layers, uint8_t *scratch,
+                       int *block_flags, int *work_lists, int *bg_lists, int *counts, void *stream);
 int b2s_rpn_bg_plan(const uint8_t *occupancy /*[B,H,W]*/, int batch, int H, int W, int num_layers, uint8_t *scratch,
                     int *tile_flags, int *work_lists, int *bg_lists, int *counts, void *stream);
 

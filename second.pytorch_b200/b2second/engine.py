@@ -304,12 +304,12 @@ class InferenceEngine:
             self.tc_heads = torch.zeros(B, hd["H"], hd["W"], self.tc_head_stride, dtype=torch.float32, device=dev)
             self.tc_bufs["heads"] = (self.tc_heads, None)
         self.tc_hw = (H, W)
-        # background tiles (csrc/rpn_bg.cu): through the leading chain of 3x3 stride-1 layers, output tiles whose whole
-        # receptive field is empty BEV are not computed but copied from the layer's response to an empty frame
+        # background blocks (csrc/rpn_bg.cu): through the leading chain of 3x3 stride-1 layers, 8x8 output blocks whose
+        # whole receptive field is empty BEV are not computed but copied from the layer's response to an empty frame
         self.bg_idx = _tc.background_layers(plan)
         if self.bg_idx:
             nl = len(self.bg_idx)
-            self.bg_tiles = B * (-(-H // 16)) * (-(-W // 16))
+            self.bg_tiles = B * (-(-H // 8)) * (-(-W // 8))          # 8x8 blocks per layer
             self.bg_occ = torch.zeros(B, H, W, dtype=torch.uint8, device=dev)
             self.bg_scratch = torch.zeros(2, B, H, W, dtype=torch.uint8, device=dev)
             self.bg_flags = torch.zeros(nl, self.bg_tiles, dtype=torch.int32, device=dev)
@@ -666,9 +666,9 @@ class InferenceEngine:
                                       L.ptr(self.bg_occ) if self.bg_idx else None, st), "b2s_to_bev_tc")
         self._mark("rpn")
         if self.bg_idx:
-            L.check(lib.b2s_rpn_bg_plan(L.ptr(self.bg_occ), self.B, H, W, len(self.bg_idx), L.ptr(self.bg_scratch),
-                                        L.ptr(self.bg_flags), L.ptr(self.bg_work), L.ptr(self.bg_list),
-                                        L.ptr(self.bg_counts), st), "b2s_rpn_bg_plan")
+            L.check(lib.b2s_rpn_block_plan(L.ptr(self.bg_occ), self.B, H, W, len(self.bg_idx), L.ptr(self.bg_scratch),
+                                           L.ptr(self.bg_flags), L.ptr(self.bg_work), L.ptr(self.bg_list),
+                                           L.ptr(self.bg_counts), st), "b2s_rpn_block_plan")
         marked_tail = False
         n_ops = len(self.tc_plan) - (2 if self.tc_tail_fused else 0)
         for oi, op in enumerate(self.tc_plan[:n_ops]):
@@ -689,7 +689,7 @@ class InferenceEngine:
                 bl = self.bg_idx.index(oi)
                 chi, clo = self.bg_field[bl]
                 work, work_n = L.ptr(self.bg_work[bl]), L.ptr(self.bg_counts[bl, 0:])
-                # the conv kernel's epilogue warps store the constant into the background tiles
+                # the conv kernel's fill warps store the constant into the background blocks
                 bgl, bgn, bhi, blo = L.ptr(self.bg_list[bl]), L.ptr(self.bg_counts[bl, 1:]), L.ptr(chi), L.ptr(clo)
             L.check(lib.b2s_conv2d_tc_ex(
                 L.ptr(src[0]), L.ptr(src[1]), self.B, op["Hin"], op["Win"], op["cin"], L.ptr(op["w_hi"]),
@@ -870,7 +870,7 @@ class InferenceEngine:
             px = self.B * op["Hg"] * op["Wg"]
             px_in = self.B * op["Hin"] * op["Win"]
             out_b = 2 * 2 * px * cout if op["planes"] == 2 else 4 * px * cout
-            frac = 1.0                        # share of the 16x16 output tiles actually computed (the rest: background)
+            frac = 1.0                        # share of the 8x8 output blocks actually computed (the rest: background)
             if getattr(self, "bg_idx", None) and i in self.bg_idx:
                 frac = float(self.bg_counts[self.bg_idx.index(i), 0].item()) / self.bg_tiles
             out.append({"index": i, "kind": op["kind"], "v2": op["v2"], "cin": cin, "cout": cout, "taps": taps,

@@ -307,7 +307,7 @@ def fusable_tail(plan):
 
 def background_layers(plan):
     """indices of the leading ops of an RPN program that form a chain of 3x3 stride-1 pad-1 128-out layers starting at
-    the BEV input (the ops the weights-stationary kernel takes): background tiles are only tracked through those."""
+    the BEV input (the ops the weights-stationary kernel takes): background blocks are only tracked through those."""
     idx, src = [], "in"
     for i, op in enumerate(plan["ops"]):
         if op["v2"] and op["src"] == src and op["dst_coff"] == 0 and op["cout"] == op["n_pad"]:

@@ -58,7 +58,7 @@ __global__ void k_to_bev_tc(const float *__restrict__ feat, const __half *__rest
             continue;
         size_t CD = (size_t)C * D;
         size_t idx = (((size_t)q.x * (H + 2) + (q.z + 1)) * (W + 2) + (q.w + 1)) * CD + (size_t)c * D + q.y;
-        if (occ && c == 0) occ[((size_t)q.x * H + q.z) * W + q.w] = 1;      // the pixel holds data (b2s_rpn_bg_plan)
+        if (occ && c == 0) occ[((size_t)q.x * H + q.z) * W + q.w] = 1;      // the pixel holds data (b2s_rpn_block_plan)
         if (feat) {
             const uint32_t pk = b2s_tc::split_f16(__ldg(&feat[gid]));
             out_hi[idx] = __ushort_as_half((unsigned short)(pk & 0xFFFFu));

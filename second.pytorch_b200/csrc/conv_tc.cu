@@ -250,9 +250,9 @@ extern "C" int b2s_conv2d_tc_ex(const b2s_half *in_hi_, const b2s_half *in_lo_, 
                     out_padded && out_mul == 1 && off_h == 0 && off_w == 0 && Hg == Hin && Wg == Win && Hout == Hin &&
                     Wout == Win;
     B2S_REQUIRE(work_list == nullptr || (v2 && work_count_dev != nullptr),
-                "b2s_conv2d_tc: a tile work list is only taken by the 3x3 stride-1 128-channel kernel (16x16 tiles)");
+                "b2s_conv2d_tc: a block work list is only taken by the 3x3 stride-1 128-channel kernel (8x8 blocks)");
     B2S_REQUIRE(bg_list == nullptr || (work_list != nullptr && bg_count_dev != nullptr && bg_hi != nullptr && bg_lo != nullptr),
-                "b2s_conv2d_tc: a background-tile list needs the work list, its count and the constant's hi/lo planes");
+                "b2s_conv2d_tc: a background-block list needs the work list, its count and the constant's hi/lo planes");
     if (v2)
         return b2s_conv3x3_tc2(in_hi, in_lo, B, Hin, Win, Cin, w_hi, w_lo, Cout, scale, shift, relu,
                                reinterpret_cast<__half *>(out_hi), out_lo, out_stride, work_list, work_count_dev, bg_list,

@@ -1,4 +1,4 @@
-// rpn_bg.cu -- background-tile planning for the dense RPN (b2s_rpn_bg_plan).
+// rpn_bg.cu -- background planning for the dense RPN: b2s_rpn_block_plan (8 x 8 blocks), b2s_rpn_bg_plan (16 x 16).
 //
 // The BEV map that enters the RPN is mostly empty: 6-8 % of the 200 x 176 pixels of a synthetic KITTI cloud hold
 // data (real clouds: the camera-FOV wedge).  The output of layer l of a chain of 3x3 stride-1 pad-1 layers at pixel p
@@ -7,29 +7,35 @@
 // different within l pixels of the image border, where the zero padding is felt).  The engine computes that
 // empty-frame response once per layer with the very kernel that runs the layer (so the values are bit-identical to
 // what the kernel would have produced) and keeps it as one halo-padded frame [H+2, W+2, C] of hi/lo planes.
-// Per step, the data mask is dilated by one pixel per layer (one tiny kernel per layer); a 16 x 16 output tile of
-// k_conv3x3_tc2 without a masked pixel is not computed -- the conv kernel's own epilogue warps copy it from the
-// empty-frame response -- and the conv kernel walks the compacted list of the remaining tiles, so the work stays
-// balanced over the SMs.
+// Per step, the data mask is dilated by one pixel per layer (one tiny kernel per layer); an 8 x 8 output block of
+// k_conv3x3_tc2 (the 64 pixels of one consumer warpgroup's accumulator tile) without a masked pixel is not computed --
+// the conv kernel's fill warps copy it from the empty-frame response -- and the conv kernel walks the compacted list
+// of the remaining blocks, so the work stays balanced over the SMs.
 // Everything the reference computes is still produced; only the recomputation of a known field is skipped.
 #include "common.cuh"
 
 namespace {
 
-constexpr int TILE = 16;          // must equal conv_tc2.cu T2_H / T2_W
+constexpr int REGION = 16;        // pixels per edge of the square handled by one CTA (one thread per pixel)
+constexpr int COMPACT_PER_THREAD = 4;
 
-// one block per (frame, tile): out(p) = OR of `in` over the 3x3 window of p (outside the image: 0);
-// tile flag = OR of out over the tile's in-image pixels
-__global__ void __launch_bounds__(TILE * TILE)
-k_bg_layer(const uint8_t *__restrict__ in, int H, int W, int tiles_h, int tiles_w, uint8_t *__restrict__ out,
-           int *__restrict__ tile_flag)
+// one block per (frame, 16 x 16 region): out(p) = OR of `in` over the 3x3 window of p (outside the image: 0);
+// flag of each tile x tile block of the region (tile = 8 or 16) = OR of out over the block's in-image pixels
+__global__ void __launch_bounds__(REGION * REGION)
+k_bg_layer(const uint8_t *__restrict__ in, int H, int W, int tile, int regions_h, int regions_w, int tiles_h,
+           int tiles_w, uint8_t *__restrict__ out, int *__restrict__ tile_flag)
 {
-    const int tile = blockIdx.x;
-    const int tw = tile % tiles_w, th = (tile / tiles_w) % tiles_h, b = tile / (tiles_w * tiles_h);
-    const int h = th * TILE + (threadIdx.x >> 4), w = tw * TILE + (threadIdx.x & 15);
-    int v = 0;
+    const int region = blockIdx.x;
+    const int rw = region % regions_w, rh = (region / regions_w) % regions_h, b = region / (regions_w * regions_h);
+    const int r = threadIdx.x >> 4, c = threadIdx.x & 15;
+    const int h = rh * REGION + r, w = rw * REGION + c;
+    const int per_edge = REGION / tile;
+    __shared__ int s_any[4];
+    if (threadIdx.x < 4) s_any[threadIdx.x] = 0;
+    __syncthreads();
     if (h < H && w < W) {
         const uint8_t *f = in + (size_t)b * H * W;
+        int v = 0;
 #pragma unroll
         for (int dy = -1; dy <= 1; ++dy)
 #pragma unroll
@@ -38,12 +44,17 @@ k_bg_layer(const uint8_t *__restrict__ in, int H, int W, int tiles_h, int tiles_
                 v |= (y < 0 || y >= H || x < 0 || x >= W) ? 0 : (int)f[(size_t)y * W + x];
             }
         out[((size_t)b * H + h) * W + w] = (uint8_t)(v != 0);
+        if (v) s_any[(r / tile) * per_edge + c / tile] = 1;
     }
-    const int any = __syncthreads_or(v);
-    if (threadIdx.x == 0) tile_flag[tile] = any ? 1 : 0;
+    __syncthreads();
+    if ((int)threadIdx.x < per_edge * per_edge) {
+        const int th = rh * per_edge + (int)threadIdx.x / per_edge, tw = rw * per_edge + (int)threadIdx.x % per_edge;
+        if (th < tiles_h && tw < tiles_w) tile_flag[((size_t)b * tiles_h + th) * tiles_w + tw] = s_any[threadIdx.x];
+    }
 }
 
-// one block per layer: stable compaction of the tile ids into work (flag 1) and background (flag 0) lists
+// one block per layer: stable compaction of the tile ids into work (flag 1) and background (flag 0) lists; each
+// thread takes COMPACT_PER_THREAD consecutive ids per pass
 __global__ void __launch_bounds__(1024)
 k_bg_compact(const int *__restrict__ tile_flag, int num_tiles, int *work_list, int *bg_list, int *counts)
 {
@@ -53,18 +64,26 @@ k_bg_compact(const int *__restrict__ tile_flag, int num_tiles, int *work_list, i
     __shared__ int s_carry;
     if (threadIdx.x == 0) s_carry = 0;
     __syncthreads();
-    for (int base = 0; base < num_tiles; base += 1024) {
-        const int i = base + threadIdx.x;
-        const int f = i < num_tiles ? flag[i] : 0;
+    for (int base = 0; base < num_tiles; base += 1024 * COMPACT_PER_THREAD) {
+        const int i0 = base + (int)threadIdx.x * COMPACT_PER_THREAD;
+        int f[COMPACT_PER_THREAD], n = 0;
+#pragma unroll
+        for (int k = 0; k < COMPACT_PER_THREAD; ++k) {
+            f[k] = i0 + k < num_tiles ? flag[i0 + k] : 0;
+            n += f[k];
+        }
         int total;
-        const int ex = b2s_block_exscan(f, &total);
-        const int carry = s_carry;
-        if (i < num_tiles) {
-            if (f) work[carry + ex] = i;
-            else bg[i - (carry + ex)] = i;            // background tiles before i: i - (#work tiles before i)
+        const int ex = b2s_block_exscan(n, &total);
+        int wpos = s_carry + ex;                      // work tiles before i0
+#pragma unroll
+        for (int k = 0; k < COMPACT_PER_THREAD; ++k) {
+            const int i = i0 + k;
+            if (i >= num_tiles) break;
+            if (f[k]) work[wpos++] = i;
+            else bg[i - wpos] = i;                    // background tiles before i: i - (#work tiles before i)
         }
         __syncthreads();
-        if (threadIdx.x == 0) s_carry = carry + total;
+        if (threadIdx.x == 0) s_carry += total;
         __syncthreads();
     }
     if (threadIdx.x == 0) {
@@ -73,25 +92,40 @@ k_bg_compact(const int *__restrict__ tile_flag, int num_tiles, int *work_list, i
     }
 }
 
-}  // namespace
-
-extern "C" int b2s_rpn_bg_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, uint8_t *scratch,
-                               int *tile_flags, int *work_lists, int *bg_lists, int *counts, void *stream_)
+int bg_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, int tile, uint8_t *scratch,
+            int *tile_flags, int *work_lists, int *bg_lists, int *counts, cudaStream_t stream)
 {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    B2S_REQUIRE(batch >= 1 && H >= 1 && W >= 1 && num_layers >= 1 && num_layers <= 32, "b2s_rpn_bg_plan: bad sizes");
-    const int tiles_h = b2s_cdiv(H, TILE), tiles_w = b2s_cdiv(W, TILE);
+    B2S_REQUIRE(batch >= 1 && H >= 1 && W >= 1 && num_layers >= 1 && num_layers <= 32,
+                "b2s_rpn_block_plan / b2s_rpn_bg_plan: bad sizes");
+    const int regions_h = b2s_cdiv(H, REGION), regions_w = b2s_cdiv(W, REGION);
+    const int tiles_h = b2s_cdiv(H, tile), tiles_w = b2s_cdiv(W, tile);
     const int num_tiles = batch * tiles_h * tiles_w;
     const size_t map = (size_t)batch * H * W;
     const uint8_t *in = occupancy;
     for (int l = 0; l < num_layers; ++l) {
         uint8_t *out = scratch + (size_t)(l & 1) * map;
-        k_bg_layer<<<num_tiles, TILE * TILE, 0, stream>>>(in, H, W, tiles_h, tiles_w, out,
-                                                          tile_flags + (size_t)l * num_tiles);
+        k_bg_layer<<<batch * regions_h * regions_w, REGION * REGION, 0, stream>>>(
+            in, H, W, tile, regions_h, regions_w, tiles_h, tiles_w, out, tile_flags + (size_t)l * num_tiles);
         B2S_LAUNCH_OK();
         in = out;
     }
     k_bg_compact<<<num_layers, 1024, 0, stream>>>(tile_flags, num_tiles, work_lists, bg_lists, counts);
     B2S_LAUNCH_OK();
     return 0;
+}
+
+}  // namespace
+
+extern "C" int b2s_rpn_bg_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, uint8_t *scratch,
+                               int *tile_flags, int *work_lists, int *bg_lists, int *counts, void *stream)
+{
+    return bg_plan(occupancy, batch, H, W, num_layers, 16, scratch, tile_flags, work_lists, bg_lists, counts,
+                   (cudaStream_t)stream);
+}
+
+extern "C" int b2s_rpn_block_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, uint8_t *scratch,
+                                  int *block_flags, int *work_lists, int *bg_lists, int *counts, void *stream)
+{
+    return bg_plan(occupancy, batch, H, W, num_layers, 8, scratch, block_flags, work_lists, bg_lists, counts,
+                   (cudaStream_t)stream);
 }

@@ -79,6 +79,8 @@ SIGNATURES = {
                               c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2s_rpn_bg_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                 c_void_p]),
+    "b2s_rpn_block_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_void_p]),
     "b2s_conv2d_tc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                               c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "b2s_conv2d_tc_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
@@ -146,7 +148,7 @@ def load():
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
-    if lib.b2s_version() < 201:
+    if lib.b2s_version() < 202:
         raise ImportError("libb2second.so is too old")
     _lib = lib
     return lib
