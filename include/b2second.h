@@ -60,7 +60,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 202
+#define B2S_VERSION 203
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -320,6 +320,19 @@ int b2s_conv2d_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int batch, in
                                           [Hout+2, Wout+2, Cout] while its other warps compute the listed blocks*/,
                      const int *bg_count_dev, const b2s_half *bg_hi, const b2s_half *bg_lo, unsigned *status_dev,
                      void *stream);
+/* the same with strip lists: work_list / bg_list name output strips 8 pixels wide and list_rows high, list_rows 8
+ * (8x8 blocks, b2s_rpn_block_plan; what b2s_conv2d_tc_ex passes), 4 or 2 (b2s_rpn_strip_plan with rows = list_rows).
+ * Without a work list list_rows is ignored.  The results are the same bits for either strip height.
+ * bg_margin >= 0 promises that the field bg_hi/bg_lo equals its value at pixel (bg_margin, bg_margin) wherever it is at
+ * least bg_margin pixels from every border; background strips there are then stored from that value without reading
+ * the field.  < 0: every background strip is copied from the field. */
+int b2s_conv2d_tc_ex2(const b2s_half *in_hi, const b2s_half *in_lo, int batch, int Hin, int Win, int Cin,
+                      const b2s_half *w_hi, const b2s_half *w_lo, int kh, int kw, int stride, int pad, int Cout,
+                      int n_pad, const float *scale, const float *shift, int relu, int Hg, int Wg, void *out_hi,
+                      b2s_half *out_lo, int Hout, int Wout, int out_padded, int out_stride, int out_mul, int off_h,
+                      int off_w, const int *work_list, const int *work_count_dev, const int *bg_list,
+                      const int *bg_count_dev, const b2s_half *bg_hi, const b2s_half *bg_lo, int bg_margin,
+                      int list_rows, unsigned *status_dev, void *stream);
 
 /* ---- background tiles of the dense RPN ---------------------------------------------------------------
  * The output of layer l of a chain of 3x3 stride-1 pad-1 layers at pixel p depends on the BEV only inside the
@@ -333,10 +346,15 @@ int b2s_conv2d_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int batch, in
  *   bg_lists  [l*num_blocks ..]  background blocks,               counts[2l + 1] of them  -> bg_list
  * of b2s_conv2d_tc_ex, with num_blocks = batch * ceil(H/8) * ceil(W/8), block id = (b * blocks_h + bh) * blocks_w + bw.
  * scratch: 2*batch*H*W bytes; block_flags: num_layers*num_blocks ints (1 = the block is computed).
+ * b2s_rpn_strip_plan is the same plan over strips 8 pixels wide and `rows` (1, 2, 4 or 8) high: num_strips = batch *
+ * ceil(H/rows) * ceil(W/8), strip id = (b * strips_h + sh) * strips_w + sw; rows = 8 gives b2s_rpn_block_plan, and
+ * the lists of rows = 4 or 2 go to b2s_conv2d_tc_ex2 with list_rows = rows.
  * b2s_rpn_bg_plan is the same plan over 16x16 tiles (tile_flags / lists of num_tiles = batch * ceil(H/16) * ceil(W/16)
  * entries, tile id = (b * tiles_h + th) * tiles_w + tw); its lists are not accepted by b2s_conv2d_tc_ex. */
 int b2s_rpn_block_plan(const uint8_t *occupancy /*[B,H,W]*/, int batch, int H, int W, int num_layers, uint8_t *scratch,
                        int *block_flags, int *work_lists, int *bg_lists, int *counts, void *stream);
+int b2s_rpn_strip_plan(const uint8_t *occupancy /*[B,H,W]*/, int batch, int H, int W, int num_layers, int rows,
+                       uint8_t *scratch, int *strip_flags, int *work_lists, int *bg_lists, int *counts, void *stream);
 int b2s_rpn_bg_plan(const uint8_t *occupancy /*[B,H,W]*/, int batch, int H, int W, int num_layers, uint8_t *scratch,
                     int *tile_flags, int *work_lists, int *bg_lists, int *counts, void *stream);
 

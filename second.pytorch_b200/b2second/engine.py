@@ -39,6 +39,27 @@ from . import anchor_mask as _anchor_mask
 from . import spec as _spec
 from . import tc as _tc
 
+# height of the RPN background strips (8 pixels wide; csrc/rpn_bg.cu, csrc/conv_tc2.cu): two 8x4 strips make one
+# consumer warpgroup's 64-pixel tile.  k_conv3x3_tc2 is bound by the bytes it streams from L2 (weights 4.5 KB per
+# computed pixel, activation windows 1.9 / 2.25 / 3 KB at 8 / 4 / 2 rows), not by its MMAs: 8x4 moves the fewest
+# bytes per step, 8x2 computes 16 % fewer pixels than 8x8 but moves as many bytes and runs slower (DESIGN.md §7).
+# For the same reason background strips inside the field's constant interior (_field_margin) are stored from a value
+# the fill warps hold in registers instead of being copied from the field
+BG_ROWS = 4
+
+
+def _field_margin(hi, lo):
+    """the smallest m such that a layer's empty-frame response (halo-padded hi/lo planes [H+2, W+2, C]) holds, bit for
+    bit, its value at pixel (m, m) wherever it is at least m pixels from every border; -1 when no such interior exists.
+    The conv kernel stores that value into the background strips there instead of copying the field."""
+    H, W = hi.shape[0] - 2, hi.shape[1] - 2
+    f = torch.cat([hi[1:H + 1, 1:W + 1], lo[1:H + 1, 1:W + 1]], -1).view(torch.int16)    # bits: +0 and -0 differ
+    diff = (f != f[H // 2, W // 2]).any(-1)
+    ys, xs = torch.arange(H, device=f.device), torch.arange(W, device=f.device)
+    dist = torch.minimum(torch.minimum(ys, H - 1 - ys)[:, None], torch.minimum(xs, W - 1 - xs)[None, :])
+    m = int(dist[diff].max().item()) + 1 if bool(diff.any()) else 0
+    return m if 2 * m < H and 2 * m < W else -1
+
 
 def _pow2_at_least(n):
     c = 1024
@@ -304,12 +325,13 @@ class InferenceEngine:
             self.tc_heads = torch.zeros(B, hd["H"], hd["W"], self.tc_head_stride, dtype=torch.float32, device=dev)
             self.tc_bufs["heads"] = (self.tc_heads, None)
         self.tc_hw = (H, W)
-        # background blocks (csrc/rpn_bg.cu): through the leading chain of 3x3 stride-1 layers, 8x8 output blocks whose
-        # whole receptive field is empty BEV are not computed but copied from the layer's response to an empty frame
+        # background strips (csrc/rpn_bg.cu): through the leading chain of 3x3 stride-1 layers, output strips 8 pixels
+        # wide and BG_ROWS high whose whole receptive field is empty BEV are not computed but copied from the layer's
+        # response to an empty frame
         self.bg_idx = _tc.background_layers(plan)
         if self.bg_idx:
             nl = len(self.bg_idx)
-            self.bg_tiles = B * (-(-H // 8)) * (-(-W // 8))          # 8x8 blocks per layer
+            self.bg_tiles = B * (-(-H // BG_ROWS)) * (-(-W // 8))    # strips per layer
             self.bg_occ = torch.zeros(B, H, W, dtype=torch.uint8, device=dev)
             self.bg_scratch = torch.zeros(2, B, H, W, dtype=torch.uint8, device=dev)
             self.bg_flags = torch.zeros(nl, self.bg_tiles, dtype=torch.int32, device=dev)
@@ -317,6 +339,7 @@ class InferenceEngine:
             self.bg_list = torch.zeros(nl, self.bg_tiles, dtype=torch.int32, device=dev)
             self.bg_counts = torch.zeros(nl, 2, dtype=torch.int32, device=dev)
             self.bg_field = self._empty_frame_response()
+            self.bg_margin = [_field_margin(hi, lo) for hi, lo in self.bg_field]
 
     def _empty_frame_response(self):
         """per background-tracked layer: what the layer's own kernel produces for an empty frame, as one halo-padded
@@ -666,9 +689,9 @@ class InferenceEngine:
                                       L.ptr(self.bg_occ) if self.bg_idx else None, st), "b2s_to_bev_tc")
         self._mark("rpn")
         if self.bg_idx:
-            L.check(lib.b2s_rpn_block_plan(L.ptr(self.bg_occ), self.B, H, W, len(self.bg_idx), L.ptr(self.bg_scratch),
-                                           L.ptr(self.bg_flags), L.ptr(self.bg_work), L.ptr(self.bg_list),
-                                           L.ptr(self.bg_counts), st), "b2s_rpn_block_plan")
+            L.check(lib.b2s_rpn_strip_plan(L.ptr(self.bg_occ), self.B, H, W, len(self.bg_idx), BG_ROWS,
+                                           L.ptr(self.bg_scratch), L.ptr(self.bg_flags), L.ptr(self.bg_work),
+                                           L.ptr(self.bg_list), L.ptr(self.bg_counts), st), "b2s_rpn_strip_plan")
         marked_tail = False
         n_ops = len(self.tc_plan) - (2 if self.tc_tail_fused else 0)
         for oi, op in enumerate(self.tc_plan[:n_ops]):
@@ -685,19 +708,21 @@ class InferenceEngine:
             o_hi = ctypes_ptr(dst[0].data_ptr() + esz * op["dst_coff"])
             o_lo = ctypes_ptr(dst[1].data_ptr() + esz * op["dst_coff"]) if op["planes"] == 2 else None
             work = work_n = bgl = bgn = bhi = blo = None
+            margin = -1
             if oi in self.bg_idx:
                 bl = self.bg_idx.index(oi)
                 chi, clo = self.bg_field[bl]
                 work, work_n = L.ptr(self.bg_work[bl]), L.ptr(self.bg_counts[bl, 0:])
-                # the conv kernel's fill warps store the constant into the background blocks
+                # the conv kernel's fill warps store the constant into the background strips
                 bgl, bgn, bhi, blo = L.ptr(self.bg_list[bl]), L.ptr(self.bg_counts[bl, 1:]), L.ptr(chi), L.ptr(clo)
-            L.check(lib.b2s_conv2d_tc_ex(
+                margin = self.bg_margin[bl]
+            L.check(lib.b2s_conv2d_tc_ex2(
                 L.ptr(src[0]), L.ptr(src[1]), self.B, op["Hin"], op["Win"], op["cin"], L.ptr(op["w_hi"]),
                 L.ptr(op["w_lo"]), op["kh"], op["kw"], op["stride"], op["pad"], op["cout"], op["n_pad"],
                 L.ptr(op["scale"]), L.ptr(op["shift"]) if op["shift"] is not None else None,
                 1 if op["relu"] else 0, op["Hg"], op["Wg"], o_hi, o_lo, op["Hout"], op["Wout"],
                 1 if op["padded"] else 0, cdst, op["out_mul"], op["off_h"], op["off_w"], work, work_n, bgl, bgn, bhi, blo,
-                L.ptr(self.status), st), "b2s_conv2d_tc_ex(%s)" % op["kind"])
+                margin, BG_ROWS, L.ptr(self.status), st), "b2s_conv2d_tc_ex2(%s)" % op["kind"])
         if not marked_tail:
             self._mark("rpn_1x1")
         if self.tc_tail_fused:
@@ -870,7 +895,7 @@ class InferenceEngine:
             px = self.B * op["Hg"] * op["Wg"]
             px_in = self.B * op["Hin"] * op["Win"]
             out_b = 2 * 2 * px * cout if op["planes"] == 2 else 4 * px * cout
-            frac = 1.0                        # share of the 8x8 output blocks actually computed (the rest: background)
+            frac = 1.0                        # share of the 8 x BG_ROWS output strips actually computed (the rest: background)
             if getattr(self, "bg_idx", None) and i in self.bg_idx:
                 frac = float(self.bg_counts[self.bg_idx.index(i), 0].item()) / self.bg_tiles
             out.append({"index": i, "kind": op["kind"], "v2": op["v2"], "cin": cin, "cout": cout, "taps": taps,

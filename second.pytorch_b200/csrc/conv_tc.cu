@@ -210,8 +210,8 @@ int launch(const CUtensorMap &a_hi, const CUtensorMap &a_lo, const CUtensorMap &
 int b2s_conv3x3_tc2(const __half *in_hi, const __half *in_lo, int B, int H, int W, int Cin, const __half *w_hi,
                     const __half *w_lo, int Cout, const float *scale, const float *shift, int relu, __half *out_hi,
                     __half *out_lo, int out_stride, const int *work_list, const int *work_count, const int *bg_list,
-                    const int *bg_count, const __half *bg_hi, const __half *bg_lo, int *status, int num_sms,
-                    cudaStream_t stream);
+                    const int *bg_count, const __half *bg_hi, const __half *bg_lo, int bg_margin, int list_rows,
+                    int *status, int num_sms, cudaStream_t stream);
 
 // General form (include/b2second.h).  Input: halo-padded fp16 hi/lo planes [B, Hin+2, Win+2, Cin].  One GEMM pixel
 // (h, w) of the Hg x Wg grid reads input pixels (h*stride + dy - pad, w*stride + dx - pad), dy < kh, dx < kw, and is
@@ -219,13 +219,17 @@ int b2s_conv3x3_tc2(const __half *in_hi, const __half *in_lo, int B, int H, int 
 //   conv  k x k, stride s, pad p : Hg = Hout = conv output size, out_mul 1
 //   ConvTranspose2d k = s        : s*s launches with kh = kw = 1, Hg = Hin, out_mul = s, (off_h, off_w) = (a, c),
 //                                  weights W[:, :, a, c]
-extern "C" int b2s_conv2d_tc_ex(const b2s_half *in_hi_, const b2s_half *in_lo_, int B, int Hin, int Win, int Cin,
-                                const b2s_half *w_hi_, const b2s_half *w_lo_, int kh, int kw, int stride, int pad,
-                                int Cout, int n_pad, const float *scale, const float *shift, int relu, int Hg, int Wg,
-                                void *out_hi, b2s_half *out_lo_, int Hout, int Wout, int out_padded, int out_stride,
-                                int out_mul, int off_h, int off_w, const int *work_list, const int *work_count_dev,
-                                const int *bg_list, const int *bg_count_dev, const b2s_half *bg_hi,
-                                const b2s_half *bg_lo, unsigned *status_dev, void *stream_)
+// work_list / bg_list name output strips 8 wide and list_rows (8, 4 or 2) high (b2s_rpn_block_plan,
+// b2s_rpn_strip_plan).  bg_margin >= 0: the field bg_hi/bg_lo equals its value at pixel (bg_margin, bg_margin)
+// wherever it is at least bg_margin pixels from every border, and background strips there are stored from that value.
+extern "C" int b2s_conv2d_tc_ex2(const b2s_half *in_hi_, const b2s_half *in_lo_, int B, int Hin, int Win, int Cin,
+                                 const b2s_half *w_hi_, const b2s_half *w_lo_, int kh, int kw, int stride, int pad,
+                                 int Cout, int n_pad, const float *scale, const float *shift, int relu, int Hg, int Wg,
+                                 void *out_hi, b2s_half *out_lo_, int Hout, int Wout, int out_padded, int out_stride,
+                                 int out_mul, int off_h, int off_w, const int *work_list, const int *work_count_dev,
+                                 const int *bg_list, const int *bg_count_dev, const b2s_half *bg_hi,
+                                 const b2s_half *bg_lo, int bg_margin, int list_rows, unsigned *status_dev,
+                                 void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     const __half *in_hi = reinterpret_cast<const __half *>(in_hi_), *in_lo = reinterpret_cast<const __half *>(in_lo_);
@@ -250,14 +254,16 @@ extern "C" int b2s_conv2d_tc_ex(const b2s_half *in_hi_, const b2s_half *in_lo_, 
                     out_padded && out_mul == 1 && off_h == 0 && off_w == 0 && Hg == Hin && Wg == Win && Hout == Hin &&
                     Wout == Win;
     B2S_REQUIRE(work_list == nullptr || (v2 && work_count_dev != nullptr),
-                "b2s_conv2d_tc: a block work list is only taken by the 3x3 stride-1 128-channel kernel (8x8 blocks)");
+                "b2s_conv2d_tc: a strip work list is only taken by the 3x3 stride-1 128-channel kernel");
+    B2S_REQUIRE(work_list == nullptr || list_rows == 8 || list_rows == 4 || list_rows == 2,
+                "b2s_conv2d_tc: work-list strips are 8, 4 or 2 rows high");
     B2S_REQUIRE(bg_list == nullptr || (work_list != nullptr && bg_count_dev != nullptr && bg_hi != nullptr && bg_lo != nullptr),
                 "b2s_conv2d_tc: a background-block list needs the work list, its count and the constant's hi/lo planes");
     if (v2)
         return b2s_conv3x3_tc2(in_hi, in_lo, B, Hin, Win, Cin, w_hi, w_lo, Cout, scale, shift, relu,
                                reinterpret_cast<__half *>(out_hi), out_lo, out_stride, work_list, work_count_dev, bg_list,
                                bg_count_dev, reinterpret_cast<const __half *>(bg_hi), reinterpret_cast<const __half *>(bg_lo),
-                               (int *)status_dev, num_sms, stream);
+                               bg_margin, list_rows, (int *)status_dev, num_sms, stream);
     CUtensorMap a_hi, a_lo, b_hi, b_lo;
     {
         cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)(Win + 2), (cuuint64_t)(Hin + 2), (cuuint64_t)B};
@@ -292,6 +298,20 @@ extern "C" int b2s_conv2d_tc_ex(const b2s_half *in_hi_, const b2s_half *in_lo_, 
     }
     b2s_set_error("b2s_conv2d_tc: n_pad=%d not built (32, 64, 128)", n_pad);
     return -2;
+}
+
+// the same with the lists of b2s_rpn_block_plan (8x8 blocks)
+extern "C" int b2s_conv2d_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int B, int Hin, int Win, int Cin,
+                                const b2s_half *w_hi, const b2s_half *w_lo, int kh, int kw, int stride, int pad,
+                                int Cout, int n_pad, const float *scale, const float *shift, int relu, int Hg, int Wg,
+                                void *out_hi, b2s_half *out_lo, int Hout, int Wout, int out_padded, int out_stride,
+                                int out_mul, int off_h, int off_w, const int *work_list, const int *work_count_dev,
+                                const int *bg_list, const int *bg_count_dev, const b2s_half *bg_hi,
+                                const b2s_half *bg_lo, unsigned *status_dev, void *stream)
+{
+    return b2s_conv2d_tc_ex2(in_hi, in_lo, B, Hin, Win, Cin, w_hi, w_lo, kh, kw, stride, pad, Cout, n_pad, scale, shift,
+                             relu, Hg, Wg, out_hi, out_lo, Hout, Wout, out_padded, out_stride, out_mul, off_h, off_w,
+                             work_list, work_count_dev, bg_list, bg_count_dev, bg_hi, bg_lo, -1, 8, status_dev, stream);
 }
 
 // 3x3 pad 1 (taps = 9) or 1x1 (taps = 1), stride 1, output on the input grid

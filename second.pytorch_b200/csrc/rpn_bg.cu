@@ -1,4 +1,5 @@
-// rpn_bg.cu -- background planning for the dense RPN: b2s_rpn_block_plan (8 x 8 blocks), b2s_rpn_bg_plan (16 x 16).
+// rpn_bg.cu -- background planning for the dense RPN: b2s_rpn_strip_plan (8 x R strips), b2s_rpn_block_plan (8 x 8),
+// b2s_rpn_bg_plan (16 x 16).
 //
 // The BEV map that enters the RPN is mostly empty: 6-8 % of the 200 x 176 pixels of a synthetic KITTI cloud hold
 // data (real clouds: the camera-FOV wedge).  The output of layer l of a chain of 3x3 stride-1 pad-1 layers at pixel p
@@ -7,31 +8,34 @@
 // different within l pixels of the image border, where the zero padding is felt).  The engine computes that
 // empty-frame response once per layer with the very kernel that runs the layer (so the values are bit-identical to
 // what the kernel would have produced) and keeps it as one halo-padded frame [H+2, W+2, C] of hi/lo planes.
-// Per step, the data mask is dilated by one pixel per layer (one tiny kernel per layer); an 8 x 8 output block of
-// k_conv3x3_tc2 (the 64 pixels of one consumer warpgroup's accumulator tile) without a masked pixel is not computed --
-// the conv kernel's fill warps copy it from the empty-frame response -- and the conv kernel walks the compacted list
-// of the remaining blocks, so the work stays balanced over the SMs.
+// Per step, the data mask is dilated by one pixel per layer (one tiny kernel per layer); an output strip of
+// k_conv3x3_tc2 (8 pixels wide, R rows high; S = 8 / R strips make one consumer warpgroup's 64-pixel accumulator tile)
+// without a masked pixel is not computed -- the conv kernel's fill warps copy it from the empty-frame response -- and
+// the conv kernel walks the compacted list of the remaining strips, so the work stays balanced over the SMs.  The
+// engine plans 8 x 4 strips: the conv kernel's time follows the bytes it streams from L2, and 8 x 4 moves the fewest
+// (finer strips compute fewer pixels but load taller windows per output row).
 // Everything the reference computes is still produced; only the recomputation of a known field is skipped.
 #include "common.cuh"
 
 namespace {
 
 constexpr int REGION = 16;        // pixels per edge of the square handled by one CTA (one thread per pixel)
+constexpr int MAX_FLAGS = 32;     // granules per region: (16 / tile_h) x (16 / tile_w), tile_h >= 1, tile_w >= 8
 constexpr int COMPACT_PER_THREAD = 4;
 
 // one block per (frame, 16 x 16 region): out(p) = OR of `in` over the 3x3 window of p (outside the image: 0);
-// flag of each tile x tile block of the region (tile = 8 or 16) = OR of out over the block's in-image pixels
+// flag of each tile_h x tile_w granule of the region (both divide 16) = OR of out over the granule's in-image pixels
 __global__ void __launch_bounds__(REGION * REGION)
-k_bg_layer(const uint8_t *__restrict__ in, int H, int W, int tile, int regions_h, int regions_w, int tiles_h,
-           int tiles_w, uint8_t *__restrict__ out, int *__restrict__ tile_flag)
+k_bg_layer(const uint8_t *__restrict__ in, int H, int W, int tile_h, int tile_w, int regions_h, int regions_w,
+           int tiles_h, int tiles_w, uint8_t *__restrict__ out, int *__restrict__ tile_flag)
 {
     const int region = blockIdx.x;
     const int rw = region % regions_w, rh = (region / regions_w) % regions_h, b = region / (regions_w * regions_h);
     const int r = threadIdx.x >> 4, c = threadIdx.x & 15;
     const int h = rh * REGION + r, w = rw * REGION + c;
-    const int per_edge = REGION / tile;
-    __shared__ int s_any[4];
-    if (threadIdx.x < 4) s_any[threadIdx.x] = 0;
+    const int per_h = REGION / tile_h, per_w = REGION / tile_w;
+    __shared__ int s_any[MAX_FLAGS];
+    if (threadIdx.x < MAX_FLAGS) s_any[threadIdx.x] = 0;
     __syncthreads();
     if (h < H && w < W) {
         const uint8_t *f = in + (size_t)b * H * W;
@@ -44,11 +48,11 @@ k_bg_layer(const uint8_t *__restrict__ in, int H, int W, int tile, int regions_h
                 v |= (y < 0 || y >= H || x < 0 || x >= W) ? 0 : (int)f[(size_t)y * W + x];
             }
         out[((size_t)b * H + h) * W + w] = (uint8_t)(v != 0);
-        if (v) s_any[(r / tile) * per_edge + c / tile] = 1;
+        if (v) s_any[(r / tile_h) * per_w + c / tile_w] = 1;
     }
     __syncthreads();
-    if ((int)threadIdx.x < per_edge * per_edge) {
-        const int th = rh * per_edge + (int)threadIdx.x / per_edge, tw = rw * per_edge + (int)threadIdx.x % per_edge;
+    if ((int)threadIdx.x < per_h * per_w) {
+        const int th = rh * per_h + (int)threadIdx.x / per_w, tw = rw * per_w + (int)threadIdx.x % per_w;
         if (th < tiles_h && tw < tiles_w) tile_flag[((size_t)b * tiles_h + th) * tiles_w + tw] = s_any[threadIdx.x];
     }
 }
@@ -92,20 +96,20 @@ k_bg_compact(const int *__restrict__ tile_flag, int num_tiles, int *work_list, i
     }
 }
 
-int bg_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, int tile, uint8_t *scratch,
-            int *tile_flags, int *work_lists, int *bg_lists, int *counts, cudaStream_t stream)
+int bg_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, int tile_h, int tile_w,
+            uint8_t *scratch, int *tile_flags, int *work_lists, int *bg_lists, int *counts, cudaStream_t stream)
 {
     B2S_REQUIRE(batch >= 1 && H >= 1 && W >= 1 && num_layers >= 1 && num_layers <= 32,
-                "b2s_rpn_block_plan / b2s_rpn_bg_plan: bad sizes");
+                "b2s_rpn_strip_plan / b2s_rpn_block_plan / b2s_rpn_bg_plan: bad sizes");
     const int regions_h = b2s_cdiv(H, REGION), regions_w = b2s_cdiv(W, REGION);
-    const int tiles_h = b2s_cdiv(H, tile), tiles_w = b2s_cdiv(W, tile);
+    const int tiles_h = b2s_cdiv(H, tile_h), tiles_w = b2s_cdiv(W, tile_w);
     const int num_tiles = batch * tiles_h * tiles_w;
     const size_t map = (size_t)batch * H * W;
     const uint8_t *in = occupancy;
     for (int l = 0; l < num_layers; ++l) {
         uint8_t *out = scratch + (size_t)(l & 1) * map;
         k_bg_layer<<<batch * regions_h * regions_w, REGION * REGION, 0, stream>>>(
-            in, H, W, tile, regions_h, regions_w, tiles_h, tiles_w, out, tile_flags + (size_t)l * num_tiles);
+            in, H, W, tile_h, tile_w, regions_h, regions_w, tiles_h, tiles_w, out, tile_flags + (size_t)l * num_tiles);
         B2S_LAUNCH_OK();
         in = out;
     }
@@ -119,13 +123,22 @@ int bg_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, i
 extern "C" int b2s_rpn_bg_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, uint8_t *scratch,
                                int *tile_flags, int *work_lists, int *bg_lists, int *counts, void *stream)
 {
-    return bg_plan(occupancy, batch, H, W, num_layers, 16, scratch, tile_flags, work_lists, bg_lists, counts,
+    return bg_plan(occupancy, batch, H, W, num_layers, 16, 16, scratch, tile_flags, work_lists, bg_lists, counts,
                    (cudaStream_t)stream);
 }
 
 extern "C" int b2s_rpn_block_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, uint8_t *scratch,
                                   int *block_flags, int *work_lists, int *bg_lists, int *counts, void *stream)
 {
-    return bg_plan(occupancy, batch, H, W, num_layers, 8, scratch, block_flags, work_lists, bg_lists, counts,
+    return bg_plan(occupancy, batch, H, W, num_layers, 8, 8, scratch, block_flags, work_lists, bg_lists, counts,
+                   (cudaStream_t)stream);
+}
+
+extern "C" int b2s_rpn_strip_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, int rows,
+                                  uint8_t *scratch, int *strip_flags, int *work_lists, int *bg_lists, int *counts,
+                                  void *stream)
+{
+    B2S_REQUIRE(rows == 1 || rows == 2 || rows == 4 || rows == 8, "b2s_rpn_strip_plan: rows must be 1, 2, 4 or 8");
+    return bg_plan(occupancy, batch, H, W, num_layers, rows, 8, scratch, strip_flags, work_lists, bg_lists, counts,
                    (cudaStream_t)stream);
 }

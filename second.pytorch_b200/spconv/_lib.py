@@ -81,12 +81,18 @@ SIGNATURES = {
                                 c_void_p]),
     "b2s_rpn_block_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_void_p, c_void_p]),
+    "b2s_rpn_strip_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_void_p, c_void_p]),
     "b2s_conv2d_tc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                               c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "b2s_conv2d_tc_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                  c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                  c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                  c_void_p, c_void_p, c_void_p]),
+    "b2s_conv2d_tc_ex2": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
+                                  c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                  c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "b2s_rpn_tail_tc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                 c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "b2s_decode_filter_strided": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_longlong, ctypes.c_longlong,
@@ -148,7 +154,7 @@ def load():
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
-    if lib.b2s_version() < 202:
+    if lib.b2s_version() < 203:
         raise ImportError("libb2second.so is too old")
     _lib = lib
     return lib
