@@ -180,9 +180,10 @@ int b2s_sparse_conv(const float *feat_in, int cin, const float *weight, const in
                     const int *num_out_dev, int cap_out, const float *scale, const float *shift,
                     int relu, float *feat_out, int cout, void *stream);
 
-/* same contraction on the tensor pipe (wgmma f16, 3xF16 hi/lo split, fp32-grade): Cin in {8,16,32,64}, Cout in
- * {16,32,64}, K <= 27 (b2s_sparse_conv_tc_supported).  Every fp32 operand x travels as two fp16 planes hi = fp16(x),
- * lo = fp16(x - hi); per K step the kernel issues A_hi*W_hi + A_hi*W_lo + A_lo*W_hi with fp32 accumulation.
+/* same contraction on the tensor pipe (wgmma f16, 3xF16 hi/lo split; accuracy as for b2s_conv2d_tc): Cin in
+ * {8,16,32,64}, Cout in {16,32,64}, K <= 27 (b2s_sparse_conv_tc_supported).  Every fp32 operand x travels as two fp16
+ * planes hi = fp16(x), lo = fp16(x - hi); per K step the kernel issues A_hi*W_hi + A_hi*W_lo + A_lo*W_hi with fp32
+ * accumulation.
  *   feat_hi/lo  rows of in_stride halves (>= Cin, multiple of 8; e.g. interleaved [row][hi Cin | lo Cin] with
  *               feat_lo = feat_hi + Cin, in_stride = 2*Cin); a 3/4-feature input layer is zero-padded to Cin = 8;
  *   w_hi/lo     [K, Cout, 64] for Cin = 64; for Cin < 64 the 64/Cin consecutive kernel offsets that share one
@@ -286,8 +287,13 @@ int b2s_to_bev_tc(const float *feat, const b2s_half *feat_hi, const b2s_half *fe
 
 /* ---- dense RPN convolution on the tensor pipe (second/pytorch/models/rpn.py:467-497 blocks, :264-299 deblocks,
  *      :386-391 heads): 3x3 stride-1 pad-1 (taps=9) or 1x1 (taps=1) conv + per-channel scale/shift (+ReLU).
- * wgmma implicit GEMM (f16 operands), fp32-grade accuracy through the 3xF16 split (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi,
- * fp32 accumulation in registers, short chains drained with round-to-nearest adds).
+ * wgmma implicit GEMM (f16 operands) with the 3xF16 split (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi, fp32 accumulation in
+ * registers, short chains drained with round-to-nearest adds).  Accuracy contract (this kernel and b2s_sparse_conv_tc),
+ * per output element y of s * sum(a * w) + shift, with w pre-scaled by the power of two ws, against the exact value y*:
+ *     |y - y*| <= |s| * (8 * 2^-23 * S1 + 2^-25 * (Sw + Sa / ws)) + 2^-22 * |y*| + 2^-25,
+ *     S1 = sum|a * w|, Sa = sum|a|, Sw = sum|w| over the terms that feed y (before a ReLU, which only shrinks it).
+ * That is fp32-grade relative to S1 while |a| >= 2^-3 (and |w| * ws >= 2^-3): below, the fp16 lo plane is subnormal
+ * and an operand is good to 2^-25 absolute only (tests/test_gpu_tc_fp64.py pins the bound, tests/tc_ref.py states it).
  *   in_hi/in_lo  [B, H+2, W+2, Cin]   NHWC + zero halo, fp16 hi/lo planes (Cin multiple of 64)
  *   w_hi/w_lo    [taps, n_pad, Cin]   tap = ky*3+kx, w[tap][co][ci] = W_torch[co][ci][ky][kx] * 2^s (s folded into
  *                                     `scale`); rows >= Cout zero; n_pad in {32, 64, 128}

@@ -1,11 +1,15 @@
-"""GPU parity of the tensor-core RPN convolution (b2s_conv2d_tc, wgmma f16 + 3xF16 hi/lo split) against torch
-fp32 conv2d with TF32 disabled.  Bar: fp32-grade accuracy, |err| <= 2e-5 * max|ref| (plain fp16/TF32 would be ~1e-3)."""
+"""GPU parity of the tensor-core RPN convolution (b2s_conv2d_tc, wgmma f16 + 3xF16 hi/lo split) against float64 with
+the per-element 3xF16 bound of tests/tc_ref.py (single layers), and against torch fp32 conv2d with TF32 disabled (whole
+RPN programs, bar 1e-4 on the head outputs)."""
 import ctypes
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
+
+import tc_ref
+from tc_launch import assert_faults_rejected
 
 pytestmark = pytest.mark.gpu
 
@@ -53,13 +57,16 @@ def test_conv3x3_bn_relu(product, B, H, W, cin, cout):
     w = torch.randn(cout, cin, 3, 3, device="cuda", generator=g) * (2.0 / (9 * cin)) ** 0.5
     scale = torch.rand(cout, device="cuda", generator=g) + 0.5
     shift = torch.randn(cout, device="cuda", generator=g) * 0.1
-    ref = torch.relu(F.conv2d(x, w, padding=1) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
     wt = w.permute(2, 3, 0, 1).reshape(9, cout, cin).contiguous()
     n_pad = 128 if cout > 64 else (64 if cout > 32 else 32)
     o_hi, o_lo = run_tc(product, x, wt, 9, cout, n_pad, scale, shift, True, True, cout)
     got = (o_hi.float() + o_lo.float())[:, 1:-1, 1:-1, :].permute(0, 3, 1, 2)
-    err = (got - ref).abs().max().item()
-    assert err <= 2e-5 * ref.abs().max().item(), "max err %g (ref max %g)" % (err, ref.abs().max().item())
+    from b2second import tc
+    ws = tc.pow2_scale(tc._pad_rows(wt, n_pad))
+    r64 = tc_ref.dense_ref(x, w, scale, shift, True, padding=1)
+    tc_ref.assert_accurate(got.double(), r64, ws)
+    assert_faults_rejected(got.double(), o_lo[:, 1:-1, 1:-1, :].permute(0, 3, 1, 2).double(), x, w, ws, r64, True, "",
+                           padding=1)
     # halo untouched (stays zero); hi is the fp16 rounding of the value and lo the fp16 rounding of the rest
     assert float(o_hi[:, 0].float().abs().sum() + o_hi[:, -1].float().abs().sum() + o_hi[:, :, 0].float().abs().sum()
                  + o_hi[:, :, -1].float().abs().sum()) == 0.0
@@ -74,13 +81,15 @@ def test_conv1x1_heads_packed(product):
     x = torch.randn(B, cin, H, W, device="cuda", generator=g)
     w = torch.randn(cout, cin, 1, 1, device="cuda", generator=g) * 0.1
     bias = torch.randn(cout, device="cuda", generator=g)
-    ref = F.conv2d(x, w, bias)
     wt = w[:, :, 0, 0].unsqueeze(0).contiguous()
     o, _ = run_tc(product, x, wt, 1, cout, 32, None, bias, False, False, 32, want_lo=False)
     assert o.dtype == torch.float32
-    got = o[..., :cout].permute(0, 3, 1, 2)
-    err = (got - ref).abs().max().item()
-    assert err <= 2e-5 * ref.abs().max().item(), "max err %g" % err
+    got = o[..., :cout].permute(0, 3, 1, 2).double()
+    from b2second import tc
+    ws = tc.pow2_scale(tc._pad_rows(wt, 32))
+    r64 = tc_ref.dense_ref(x, w, None, bias)
+    tc_ref.assert_accurate(got, r64, ws)
+    assert_faults_rejected(got, None, x, w, ws, r64, False, "")
     assert float(o[..., cout:].abs().sum()) == 0.0
 
 
@@ -214,7 +223,14 @@ def test_fused_rpn_tail_is_bit_identical_to_two_launches(product, B, H, W):
     assert int(status.item()) == 0
     assert torch.equal(one[..., :cout], two[..., :cout]), "fused tail differs from the two-launch path"
     assert bool((one[..., cout:] == 7.0).all())                       # channels past Cout are not written
-    y = torch.relu(F.conv2d(x, w1.view(cmid, cin, 1, 1)) * scale1.view(1, -1, 1, 1) + shift1.view(1, -1, 1, 1))
-    ref = (F.conv2d(y, w2.view(cout, cmid, 1, 1)) + bias2.view(1, -1, 1, 1)).permute(0, 2, 3, 1)
-    err = (one[..., :cout] - ref).abs().max().item()
-    assert err <= 2e-5 * max(1.0, ref.abs().max().item()), "max err %g" % err
+    # against float64, stage by stage: the deblock output (the first launch's planes) from x, the heads from those planes
+    # (the values the fused kernel consumes, bit-identical to the first launch's)
+    r1 = tc_ref.dense_ref(x, w1.view(cmid, cin, 1, 1), scale1, shift1, True)
+    y = (y_hi.float() + y_lo.float())[:, 1:-1, 1:-1, :].permute(0, 3, 1, 2)
+    y_lo64 = y_lo[:, 1:-1, 1:-1, :].permute(0, 3, 1, 2).double()
+    tc_ref.assert_accurate(y.double(), r1, ws1, "deblock")
+    assert_faults_rejected(y.double(), y_lo64, x, w1.view(cmid, cin, 1, 1), ws1, r1, True, "deblock")
+    r2 = tc_ref.dense_ref(y, w2.view(cout, cmid, 1, 1), None, bias2)
+    got = one[..., :cout].permute(0, 3, 1, 2).double()
+    tc_ref.assert_accurate(got, r2, ws2, "heads")
+    assert_faults_rejected(got, None, y, w2.view(cout, cmid, 1, 1), ws2, r2, False, "heads")

@@ -4,6 +4,8 @@ import numpy as np
 import pytest
 import torch
 
+import tc_ref
+
 pytestmark = pytest.mark.gpu
 
 
@@ -87,6 +89,13 @@ def test_sparse_conv_tc_matches_oracle(product, oracle, cin, cout, subm, n):
     torch.cuda.synchronize()
     assert torch.equal(m, o_hi.float() + o_lo.float())          # merge is exact
     assert float((o32 - m).abs().max()) <= 2e-7 * max(1.0, float(o32.abs().max())) + 6e-8   # split drops < 2^-22 rel / 2^-25 abs
+    # fp32 rows against the float64 gather-GEMM of the same table, per element
+    r64 = tc_ref.sparse_ref(feats_d, w, rb.nbr[:rb.num_out], scale, shift, True)
+    tc_ref.assert_accurate(o32.double(), r64, ws, "fp32 rows")
+    tc_ref.assert_rejected(tc_ref.sparse_f1(o32.double(), feats_d, w, ws, rb.nbr[:rb.num_out], r64, True, cin_tc),
+                           r64, ws, "F1")
+    tc_ref.assert_rejected(tc_ref.sparse_f2(o32.double(), feats_d, w, ws, rb.nbr[:rb.num_out], r64, True), r64, ws, "F2")
+    tc_ref.assert_rejected(tc_ref.f3(o32.double(), None), r64, ws, "F3")
 
 
 @pytest.mark.timeout(180)
