@@ -49,6 +49,10 @@
  *   b2s_nms_aligned_host, b2s_nms_rotated_host
  *                       the numpy-facing spconv.utils.non_max_suppression /
  *                       rotate_non_max_suppression_cpu signatures (host arrays in, keep list out)
+ *   b2s_kitti_convert   KittiDataset.convert_detection_to_kitti_annos (second/data/kitti_dataset.py:37-106)
+ *   b2s_kitti_overlaps, b2s_kitti_eval
+ *                       calculate_iou_partly + eval_class_v3 behind get_official_eval_result /
+ *                       get_coco_eval_result (second/utils/eval.py:362-611,730-916)
  */
 #ifndef B2SECOND_H_
 #define B2SECOND_H_
@@ -518,6 +522,48 @@ int b2s_rotate_iou_eval(const float *boxes, int N, const float *query_boxes, int
  * standup_iou [N,K]; pairs with standup_iou <= standup_thresh give 0 (second/core/box_np_ops.py:10-34). */
 int b2s_rbbox_overlap_host(const float *corners, const float *qcorners, const float *standup_iou, int N, int K,
                            float standup_thresh, int criterion, float *out /*host [N,K]*/, int device_id);
+
+
+/* ---- KITTI detection formatting and evaluation (SURVEY.md §8(f)2) ------------------------------- */
+/* Annotations are float64 rows of B2S_KITTI_ROW values, packed frame after frame; frame f owns rows
+ * [off[f], off[f+1]) of an int32 offsets array [F+1]:
+ *   bbox x1 y1 x2 y2 (0-3), location xyz (4-6), dimensions l h w (7-9), rotation_y (10), alpha (11), score (12),
+ *   truncated (13), occluded (14), label (15: class index of a converted detection, unused otherwise).
+ * Names are int32 codes: the index of the lower-cased name in the evaluation's class vocabulary, -1 for any other name,
+ * B2S_KITTI_DONTCARE for exactly "DontCare". */
+#define B2S_KITTI_ROW 16
+#define B2S_KITTI_DONTCARE (-2)
+
+/* KittiDataset.convert_detection_to_kitti_annos (second/data/kitti_dataset.py:37-106): det rows of det_stride floats
+ * (box[code] as x y z w l h r..., score, label -- the engine's det_record layout), frame f owning [det_off[f],
+ * det_off[f+1]); calib [F, 3, 4, 4] float64 (R0_rect, Tr_velo_to_cam, P2 as extended 4x4 matrices); image_shape
+ * [F, 2] int32 (H, W).  Boxes whose projected bbox lies off the image are dropped; survivors are compacted per frame in
+ * detection order into out rows [det_off[f], det_off[f] + out_count_dev[f]) (truncated = occluded = 0). */
+int b2s_kitti_convert(const float *det, int det_stride, int code, const int *det_off, int num_frames,
+                      const double *calib, const int *image_shape, double *out, int *out_count_dev, void *stream);
+
+/* calculate_iou_partly's per-frame blocks (second/utils/eval.py:362-445): out[ov_off[f] + j*n_gt_f + i] is the overlap of
+ * detection j with ground truth i of frame f (ov_off int64 [F+1], the prefix sum of n_dt_f*n_gt_f).
+ * metric 0: image_box_overlap (eval.py:92-119), float64; 1: BEV rotate_iou_gpu_eval (eval.py:122-125), float32;
+ * 2: 3D box3d_overlap (eval.py:128-178), float32 rotated intersection times the float64 height overlap, stored through
+ * float32.  z_axis / z_center: 1 / 1.0 for camera boxes, 2 / 0.5 for lidar boxes. */
+int b2s_kitti_overlaps(int metric, const double *gt, const int *gt_off, const double *dt, const int *dt_off,
+                       int num_frames, const long long *ov_off, int z_axis, double z_center, double *out,
+                       void *stream);
+
+/* eval_class_v3 for one metric (second/utils/eval.py:479-611, with clean_data :33-89, get_thresholds :11-30,
+ * compute_statistics_jit :181-300 and fused_compute_statistics :312-359).  A task is one (class, difficulty,
+ * min_overlap): task_info int32 [T, 3] = (class vocabulary id, id that counts as "valid 0" for it -- Van for Car,
+ * Person_sitting for Pedestrian -- or -3, difficulty 0..2), task_min_overlap float64 [T].  overlaps / ov_off as
+ * b2s_kitti_overlaps writes them.  Outputs float64 [T, 41]: precision and orientation after the running max from the
+ * right, and the score thresholds (zero past the last).  Frames are reduced in frame order: bit-reproducible.
+ * max_dt_per_frame (host) <= 2048.  workspace: b2s_kitti_eval_workspace_bytes(num_frames, num_gt, num_dt, T). */
+size_t b2s_kitti_eval_workspace_bytes(int num_frames, int num_gt, int num_dt, int num_tasks);
+int b2s_kitti_eval(int metric, const double *gt, const int *gt_name, const int *gt_off, int num_gt, const double *dt,
+                   const int *dt_name, const int *dt_off, int num_dt, int num_frames, int max_dt_per_frame,
+                   const double *overlaps, const long long *ov_off, const int *task_info,
+                   const double *task_min_overlap, int num_tasks, int compute_aos, double *precision,
+                   double *orientation, double *thresholds, void *workspace, size_t workspace_bytes, void *stream);
 
 #ifdef __cplusplus
 }

@@ -120,6 +120,14 @@ SIGNATURES = {
     "b2s_rbbox_overlap_host": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_void_p, c_int]),
     "b2s_nms_aligned_host": (c_int, [c_void_p, c_int, c_float, c_float, c_int, c_void_p, c_int]),
     "b2s_nms_rotated_host": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p, c_int]),
+    "b2s_kitti_convert": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p]),
+    "b2s_kitti_overlaps": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int,
+                                   ctypes.c_double, c_void_p, c_void_p]),
+    "b2s_kitti_eval_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "b2s_kitti_eval": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                               c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                               c_void_p, c_size_t, c_void_p]),
 }
 
 
