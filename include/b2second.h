@@ -53,6 +53,8 @@
  *   b2s_kitti_overlaps, b2s_kitti_eval
  *                       calculate_iou_partly + eval_class_v3 behind get_official_eval_result /
  *                       get_coco_eval_result (second/utils/eval.py:362-611,730-916)
+ *   b2s_assign_targets  TargetAssigner.assign (second/core/target_assigner.py:38-167) through create_target_np
+ *                       (second/core/target_ops.py:29-229), positive_fraction None, for a batch of frames
  */
 #ifndef B2SECOND_H_
 #define B2SECOND_H_
@@ -64,7 +66,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 203
+#define B2S_VERSION 204
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -73,6 +75,8 @@ extern "C" {
 #define B2S_STATUS_CAND_OVERFLOW 8u    /* more score-threshold survivors than cand_cap (lowest dropped)  */
 #define B2S_STATUS_F16_RANGE 16u       /* an activation left the fp16 range (|x| > 65504) on the tensor-core path;
                                           it was clamped -- results are not fp32-grade for that frame batch      */
+#define B2S_STATUS_BAD_INPUT 32u       /* b2s_assign_targets: a frame's gt_offsets are decreasing or past num_gt; that
+                                          frame was assigned as if it had no ground truth                        */
 
 /* IEEE binary16 bit pattern (the tensor-core kernels' operand planes; torch.float16 storage) */
 typedef uint16_t b2s_half;
@@ -564,6 +568,36 @@ int b2s_kitti_eval(int metric, const double *gt, const int *gt_name, const int *
                    const double *overlaps, const long long *ov_off, const int *task_info,
                    const double *task_min_overlap, int num_tasks, int compute_aos, double *precision,
                    double *orientation, double *thresholds, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---- training targets (SURVEY.md §8(f)4) ------------------------------------------------------------ */
+/* TargetAssigner.assign (second/core/target_assigner.py:38-167) -> create_target_np (second/core/target_ops.py:29-229)
+ * with positive_fraction None, for `batch` frames at once.  The anchor side is fixed per anchor set (b2second.targets
+ * builds it once):
+ *   anchors [A, box_ndim] float32; anchor_sim [A, 4] float32: rbbox2d_to_near_bbox of the anchor for IoU segments,
+ *   (x, y, 0, 0) for distance segments; matched_thr / unmatched_thr [A] float32;
+ *   seg_info int32 [S, 4] (anchor_begin, anchor_end, kind 0 = NearestIouSimilarity / 1 = DistanceSimilarity without
+ *   rotation, 0) and seg_param float64 [S] (distance_norm) -- one segment per class in per-class mode, one over every
+ *   anchor in assign_all; blocks int32 [num_blocks, 4] (segment, anchor_begin, anchor_end, 0), at most 256 anchors each,
+ *   covering every segment.
+ * Ground truth: gt_boxes [num_gt, box_ndim] float32 (gt_double 0) or float64 (1), frame f owning rows
+ * [gt_offsets[f], gt_offsets[f+1]) (device int32 [batch+1]); gt_seg [num_gt] the segment of each GT (-1 or >= S: none);
+ * gt_class [num_gt] the label it gives; gt_importance [num_gt] float32 or NULL (ones), indexed with the GT's index
+ * within its segment (as assign_per_class passes the unmasked array).  anchors_mask uint8 [batch, A] or NULL.
+ * Outputs: labels int32 [batch, A], bbox_targets float32 [batch, A, code_size] (code_size = box_ndim, + 1 when
+ * coder_flags bit 1 = vec_encode; bit 0 = linear_dim), importance float32 [batch, A]; optional gt_id int32 [batch, A]
+ * (the segment-local GT index of each positive, -1 elsewhere) and overlap float32 [batch, A] (its similarity, 0
+ * elsewhere).  Per-GT maxima are integer atomics, everything else is written once: results are bit-reproducible.
+ * A segment whose anchors are all pruned gives -1 / 0 / 0 (the reference raises there).  Bad offsets raise
+ * B2S_STATUS_BAD_INPUT.  workspace: b2s_assign_targets_workspace_bytes(batch, num_gt, S) (host query) bytes. */
+size_t b2s_assign_targets_workspace_bytes(int batch, int num_gt, int num_segments);
+int b2s_assign_targets(const float *anchors, const float *anchor_sim, const float *matched_thr,
+                       const float *unmatched_thr, int num_anchors, int box_ndim, const int *seg_info,
+                       const double *seg_param, int num_segments, const int *blocks, int num_blocks,
+                       const void *gt_boxes, int gt_double, int num_gt, const int *gt_offsets, int batch,
+                       const int *gt_seg, const int *gt_class, const float *gt_importance,
+                       const uint8_t *anchors_mask, int code_size, int coder_flags, int *labels,
+                       float *bbox_targets, float *importance, int *gt_id, float *overlap, void *workspace,
+                       size_t workspace_bytes, unsigned *status_dev, void *stream);
 
 #ifdef __cplusplus
 }

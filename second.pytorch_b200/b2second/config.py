@@ -9,7 +9,10 @@ side needs neither protobuf nor the reference tree:
   (only the ``model.second`` and ``eval_input_reader`` blocks are interpreted);
 * ``BUILTIN`` holds the five BASELINE.json configurations, written out by hand from the values in
   SURVEY.md App. B (car.fhd, car.lite, all.fhd, pointpillars/car/xyres_16, nuscenes/all.pp.largea);
-  ``EXTRA`` the further ones ``get_config`` knows (nuscenes/all.pp.mhead, a ``MultiHeadModelConfig``).
+  ``EXTRA`` the further ones ``get_config`` knows (nuscenes/all.pp.mhead, a ``MultiHeadModelConfig``);
+* ``TargetAssignerSettings`` (what training target assignment reads: thresholds, similarity, box coder) rides along
+  as the ``target_assigner`` attribute of a config -- parsed from the file, or written out in ``TARGET_ASSIGNERS`` for
+  the builtins.  It is not a dataclass field, so the inference fields above keep their shape.
 """
 import re
 from dataclasses import dataclass, field
@@ -155,7 +158,7 @@ class ModelConfig:
         if _one(m.get("network_class_name", ["VoxelNet"])) == "VoxelNetNuscenesMultiHead":
             cls = MultiHeadModelConfig
             kw["class_feature_map_sizes"] = [[int(v) for v in c[1].get("feature_map_size", [])] for c in classes]
-        return cls(
+        cfg = cls(
             **kw,
             name=name,
             point_cloud_range=[float(v) for v in vg["point_cloud_range"]],
@@ -195,6 +198,8 @@ class ModelConfig:
             anchor_area_threshold=float(_one(prep.get("anchor_area_threshold", [-1]))),
             box_code_size=7 + len(classes[0][0].custom_values),
         )
+        cfg.target_assigner = _target_assigner_settings(m, ta)
+        return cfg
 
     @staticmethod
     def from_file(path, name=None):
@@ -210,6 +215,56 @@ class MultiHeadModelConfig(ModelConfig):
     large head come first in the config."""
     network_class: str = "VoxelNetNuscenesMultiHead"
     class_feature_map_sizes: List[List[int]] = field(default_factory=list)
+
+
+@dataclass
+class ClassTargetSettings:
+    """one ``class_settings`` entry's target-assignment part (second/protos/target.proto, similarity.proto).  Floats are
+    the float32 values protobuf stores, widened to Python floats as the reference's builders read them."""
+    matched_threshold: float
+    unmatched_threshold: float
+    similarity: str = "nearest_iou"            # nearest_iou | distance | rotate_iou
+    distance_norm: float = 0.0
+    with_rotation: bool = False
+
+
+@dataclass
+class TargetAssignerSettings:
+    """``target_assigner`` and ``box_coder`` settings behind TargetAssigner.assign (proto3 defaults where absent)."""
+    classes: List[ClassTargetSettings]
+    assign_per_class: bool = False
+    sample_positive_fraction: float = 0.0
+    box_coder: str = "ground_box3d"            # ground_box3d | bev
+    linear_dim: bool = False
+    encode_angle_vector: bool = False
+
+
+def _f32(v):
+    return float(np.float32(v))
+
+
+def _target_assigner_settings(m, ta):
+    classes = []
+    for cs in ta.get("class_settings", []):
+        sim = _one(cs.get("region_similarity_calculator", [{}]))
+        c = ClassTargetSettings(_f32(_one(cs.get("matched_threshold", [0.0]))),
+                                _f32(_one(cs.get("unmatched_threshold", [0.0]))))
+        if "distance_similarity" in sim:
+            d = _one(sim["distance_similarity"])
+            c.similarity = "distance"
+            c.distance_norm = _f32(_one(d.get("distance_norm", [0.0])))
+            c.with_rotation = bool(_one(d.get("with_rotation", [False])))
+        elif "rotate_iou_similarity" in sim:
+            c.similarity = "rotate_iou"
+        classes.append(c)
+    coder = _one(m.get("box_coder", [{"ground_box3d_coder": [{}]}]))
+    kind = "bev" if "bev_box_coder" in coder else "ground_box3d"
+    cc = _one(coder.get("bev_box_coder" if kind == "bev" else "ground_box3d_coder", [{}]))
+    return TargetAssignerSettings(
+        classes=classes, assign_per_class=bool(_one(ta.get("assign_per_class", [False]))),
+        sample_positive_fraction=_f32(_one(ta.get("sample_positive_fraction", [0.0]))), box_coder=kind,
+        linear_dim=bool(_one(cc.get("linear_dim", [False]))),
+        encode_angle_vector=bool(_one(cc.get("encode_angle_vector", [False]))))
 
 
 def _one(v):
@@ -457,9 +512,35 @@ EXTRA_REFERENCE_FILES = {
 }
 
 
+def _ta(per_class, *classes):
+    """classes: (matched, unmatched) or (matched, unmatched, distance_norm) for a DistanceSimilarity without rotation"""
+    return TargetAssignerSettings(
+        classes=[ClassTargetSettings(_f32(c[0]), _f32(c[1])) if len(c) == 2 else
+                 ClassTargetSettings(_f32(c[0]), _f32(c[1]), "distance", _f32(c[2])) for c in classes],
+        assign_per_class=per_class, sample_positive_fraction=-1.0)
+
+
+# target-assignment settings of the builtins (the target_assigner / box_coder blocks of the cited config files; every
+# one uses ground_box3d_coder with linear_dim and encode_angle_vector false)
+TARGET_ASSIGNERS = {
+    "car.fhd": lambda: _ta(True, (0.6, 0.45)),
+    "car.lite": lambda: _ta(True, (0.6, 0.45)),
+    "all.fhd": lambda: _ta(True, (0.6, 0.45), (0.35, 0.2), (0.35, 0.2), (0.6, 0.45)),
+    "pointpillars.car.xyres_16": lambda: _ta(True, (0.6, 0.45)),
+    "nuscenes.all.pp.largea": lambda: _ta(False, (0.4, 0.3), (0.5, 0.35), (0.5, 0.35), (0.5, 0.35), (0.5, 0.35),
+                                          (0.2, 0.15), (0.2, 0.15), (0.5, 0.35, 1.414), (0.5, 0.35, 1.414),
+                                          (0.3, 0.2)),
+    "nuscenes.all.pp.mhead": lambda: _ta(True, (0.5, 0.35), (0.4, 0.3), (0.4, 0.3), (0.5, 0.35), (0.5, 0.35),
+                                         (0.3, 0.2), (0.3, 0.2), (0.3, 0.2), (0.2, 0.1), (0.5, 0.35, 1.0)),
+}
+
+
 def get_config(name):
     if name in BUILTIN:
-        return BUILTIN[name]()
-    if name in EXTRA:
-        return EXTRA[name]()
-    raise KeyError("unknown config %r (have %s)" % (name, sorted(BUILTIN) + sorted(EXTRA)))
+        cfg = BUILTIN[name]()
+    elif name in EXTRA:
+        cfg = EXTRA[name]()
+    else:
+        raise KeyError("unknown config %r (have %s)" % (name, sorted(BUILTIN) + sorted(EXTRA)))
+    cfg.target_assigner = TARGET_ASSIGNERS[name]()
+    return cfg

@@ -386,22 +386,77 @@ class SmallObjectHead(DefaultHead):
 
 # ------------------------------------------------------------------------------ VoxelNet
 class _AnchorGeneratorInfo:
-    def __init__(self, ac):
+    def __init__(self, ac, ts):
         self.class_name = ac.class_name
         self.num_anchors_per_localization = ac.num_anchors_per_loc
+        self.match_threshold = ts.matched_threshold if ts is not None else None
+        self.unmatch_threshold = ts.unmatched_threshold if ts is not None else None
+        self.custom_ndim = len(ac.custom_values)
+        self.ndim = 7 + self.custom_ndim
+
+
+# the region similarity calculators and box coders of second/core/region_similarity.py and box_coders.py, by the
+# class names and attributes b2second.targets reads
+class NearestIouSimilarity:
+    pass
+
+
+class RotateIouSimilarity:
+    pass
+
+
+class DistanceSimilarity:
+    def __init__(self, distance_norm, with_rotation=False, rotation_alpha=0.5):
+        self._distance_norm = distance_norm
+        self._with_rotation = with_rotation
+        self._rotation_alpha = rotation_alpha
+
+
+class GroundBox3dCoder:
+    def __init__(self, linear_dim=False, vec_encode=False, custom_ndim=0):
+        self.linear_dim = linear_dim
+        self.vec_encode = vec_encode
+        self.custom_ndim = custom_ndim
+
+    @property
+    def code_size(self):
+        return self.custom_ndim + (8 if self.vec_encode else 7)
+
+
+class BevBoxCoder(GroundBox3dCoder):
+    pass
+
+
+def _similarity(ts):
+    if ts.similarity == "distance":
+        return DistanceSimilarity(ts.distance_norm, ts.with_rotation)
+    return RotateIouSimilarity() if ts.similarity == "rotate_iou" else NearestIouSimilarity()
 
 
 class MirrorTargetAssigner:
-    """the slice of second/core/target_assigner.py ``TargetAssigner`` that inference reads: anchors per location,
-    per-class anchor ranges (``anchors_range``, :269-278) and ``generate_anchors`` (:169-207)."""
+    """the slice of second/core/target_assigner.py ``TargetAssigner`` that inference and b2second.targets read: anchors
+    per location, per-class anchor ranges (``anchors_range``, :269-278), ``generate_anchors`` (:169-207) and the
+    assignment settings (thresholds, similarity calculators, box coder, positive fraction, per-class mode)."""
 
     def __init__(self, cfg):
         self._cfg = cfg
-        self._anchor_generators = [_AnchorGeneratorInfo(ac) for ac in cfg.classes]
+        ta = getattr(cfg, "target_assigner", None)
+        tcs = ta.classes if ta is not None else [None] * len(cfg.classes)
+        self._anchor_generators = [_AnchorGeneratorInfo(ac, ts) for ac, ts in zip(cfg.classes, tcs)]
         self._classes = [ac.class_name for ac in cfg.classes]
         # per-class anchor feature maps (class_settings.feature_map_size); None: every class on cfg.feature_map_size
         self._feature_map_sizes = [list(f) for f in cfg.class_feature_map_sizes] \
             if getattr(cfg, "class_feature_map_sizes", None) else None
+        if ta is not None:
+            self._sim_calcs = [_similarity(ts) for ts in ta.classes]
+            coder = BevBoxCoder if ta.box_coder == "bev" else GroundBox3dCoder
+            self._box_coder = coder(ta.linear_dim, ta.encode_angle_vector, self._anchor_generators[0].custom_ndim)
+            self._positive_fraction = ta.sample_positive_fraction if ta.sample_positive_fraction >= 0 else None
+            self._assign_per_class = ta.assign_per_class
+
+    @property
+    def classes(self):
+        return self._classes
 
     @property
     def num_anchors_per_location(self):

@@ -14,6 +14,10 @@ neighbour table (the tensor pipe where the widths allow, with the gradient split
 and the weight gradient with ``b2s_sparse_conv_wgrad``.  BatchNorm1d and ReLU run as the torch modules that follow the
 conv.  ``eval()`` keeps the fused BN/ReLU inference path, marked or not; an unmarked conv in training mode still raises
 ``NotImplementedError``.  Not covered: the fused engine, fp16/AMP, transposed / inverse sparse convs.
+
+The training targets ``VoxelNet.loss`` reads (labels, reg_targets, importance) come from ``b2second.targets`` on the GPU
+for a whole batch (``targets.plan(net.target_assigner, feature_map_size).assign_batch(...)``), after
+``b2second.inputs.anchor_area_mask``; see INTEGRATION.md, Training.
 """
 
 

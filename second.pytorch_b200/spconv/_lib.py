@@ -128,6 +128,11 @@ SIGNATURES = {
     "b2s_kitti_eval": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                c_void_p, c_size_t, c_void_p]),
+    "b2s_assign_targets_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "b2s_assign_targets": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int,
+                                   c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                   c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_size_t, c_void_p, c_void_p]),
 }
 
 
@@ -205,7 +210,8 @@ def require_cuda(t, name):
 STATUS_BITS = {1: "voxel overflow (more voxels than max_voxels; extra voxels dropped as upstream does)",
                2: "row overflow (strided conv produced more rows than the buffer capacity)",
                4: "hash table full", 8: "candidate overflow (more score survivors than cand_cap)",
-               16: "an activation left the fp16 range (|x| > 65504) on the tensor-core path"}
+               16: "an activation left the fp16 range (|x| > 65504) on the tensor-core path",
+               32: "bad ground-truth frame offsets (that frame was assigned as if it had no ground truth)"}
 
 
 def status_message(word):
