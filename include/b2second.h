@@ -55,6 +55,10 @@
  *                       get_coco_eval_result (second/utils/eval.py:362-611,730-916)
  *   b2s_assign_targets  TargetAssigner.assign (second/core/target_assigner.py:38-167) through create_target_np
  *                       (second/core/target_ops.py:29-229), positive_fraction None, for a batch of frames
+ *   b2s_augment         the augmentation of prep_pointcloud after database sampling (second/data/preprocess.py:255-294):
+ *                       noise_per_object_v3_, random_flip, global_rotation_v2 / scaling_v2 / translate_, the range
+ *                       filter, limit_period and the point shuffle (second/core/preprocess.py:153-164,244-273,450-476,
+ *                       582-678,749-800,803-899), for a batch of frames
  */
 #ifndef B2SECOND_H_
 #define B2SECOND_H_
@@ -66,7 +70,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 204
+#define B2S_VERSION 205
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -76,7 +80,10 @@ extern "C" {
 #define B2S_STATUS_F16_RANGE 16u       /* an activation left the fp16 range (|x| > 65504) on the tensor-core path;
                                           it was clamped -- results are not fp32-grade for that frame batch      */
 #define B2S_STATUS_BAD_INPUT 32u       /* b2s_assign_targets: a frame's gt_offsets are decreasing or past num_gt; that
-                                          frame was assigned as if it had no ground truth                        */
+                                          frame was assigned as if it had no ground truth.  b2s_augment: the same for
+                                          gt_offsets or point_offsets, or a perm entry outside its frame          */
+#define B2S_STATUS_AUG_BOX_CAP 64u     /* b2s_augment: a frame holds more than B2S_AUGMENT_MAX_BOXES ground truths; its
+                                          boxes and points got no per-object noise                               */
 
 /* IEEE binary16 bit pattern (the tensor-core kernels' operand planes; torch.float16 storage) */
 typedef uint16_t b2s_half;
@@ -598,6 +605,38 @@ int b2s_assign_targets(const float *anchors, const float *anchor_sim, const floa
                        const uint8_t *anchors_mask, int code_size, int coder_flags, int *labels,
                        float *bbox_targets, float *importance, int *gt_id, float *overlap, void *workspace,
                        size_t workspace_bytes, unsigned *status_dev, void *stream);
+
+/* ---- training augmentation (second/data/preprocess.py:255-294) ------------------------------------------------ */
+/* Per-object noise without per-object global rotation or groups, the flips, global rotation, scaling and translation, the
+ * range filter by centre, limit_period(0.5, 2 pi) and the point shuffle, for `batch` frames.  Random draws are inputs
+ * (b2second.augment.draw makes them from a numpy RandomState in the reference's order).
+ *   points [num_points, num_feat] float32, frame f owning rows [point_offsets[f], point_offsets[f+1]);
+ *   gt_boxes [num_gt, box_ndim] float32 (gt_double 0) or float64 (1), box_ndim 7 or 9 (x y z w l h r [vx vy]), frame f
+ *   owning rows [gt_offsets[f], gt_offsets[f+1]); gt_valid uint8 [num_gt] (the class mask: valid boxes get noise and
+ *   are kept, the others only block other boxes' tries and are dropped); gt_classes int32, gt_importance float32 (or
+ *   NULL: ones) [num_gt], carried to the kept boxes;
+ *   loc_noise [num_gt, num_try, 3] / rot_noise [num_gt, num_try] float64, read when object_noise = 1 (0: the
+ *   reference's early return when every noise setting is zero -- nothing moves);
+ *   frame_params [batch, 8] float64: flip_y, flip_x, translate (0/1, the applied flips and whether the translation
+ *   happens), rotation angle, scale, tx, ty, tz;
+ *   perm [num_points] int32 frame-local source rows (output row point_offsets[f] + m reads row point_offsets[f] +
+ *   perm[point_offsets[f] + m]) or NULL; range_host[4] float32: point_cloud_range[[0, 1, 3, 4]].
+ * Outputs: points_out [num_points, num_feat]; point_box int32 [num_points] (the input box row that moved each output
+ * point, -1: none) or NULL; boxes_out [num_gt, box_ndim] (input dtype), classes_out, importance_out, src_out (input
+ * row) [num_gt]: the kept boxes packed frame after frame in input order, zeros (source row -1) past them; gt_offsets_out int32 [batch + 1]; selected
+ * int32 [num_gt]: the chosen try of each box, -1 none, -2 the frame is over the cap.  Pose selection runs one CTA per
+ * frame with the frame's corners in shared memory: a frame of more than B2S_AUGMENT_MAX_BOXES boxes raises
+ * B2S_STATUS_AUG_BOX_CAP and gets no object noise.  Bad offsets raise B2S_STATUS_BAD_INPUT.  One memset and three
+ * kernels; deterministic.  workspace: b2s_augment_workspace_bytes(batch, num_gt, box_ndim) (host query) bytes. */
+#define B2S_AUGMENT_MAX_BOXES 1024
+size_t b2s_augment_workspace_bytes(int batch, int num_gt, int box_ndim);
+int b2s_augment(const float *points, int num_points, int num_feat, const int *point_offsets, int batch,
+                const void *gt_boxes, int gt_double, int box_ndim, int num_gt, const int *gt_offsets,
+                const uint8_t *gt_valid, const int *gt_classes, const float *gt_importance, const double *loc_noise,
+                const double *rot_noise, int num_try, int object_noise, const double *frame_params, const int *perm,
+                const float *range_host, float *points_out, int *point_box, void *boxes_out, int *gt_offsets_out,
+                int *classes_out, float *importance_out, int *src_out, int *selected, void *workspace,
+                size_t workspace_bytes, unsigned *status_dev, void *stream);
 
 #ifdef __cplusplus
 }

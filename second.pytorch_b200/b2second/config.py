@@ -13,6 +13,8 @@ side needs neither protobuf nor the reference tree:
 * ``TargetAssignerSettings`` (what training target assignment reads: thresholds, similarity, box coder) rides along
   as the ``target_assigner`` attribute of a config -- parsed from the file, or written out in ``TARGET_ASSIGNERS`` for
   the builtins.  It is not a dataclass field, so the inference fields above keep their shape.
+* ``AugmentSettings`` (``train_input_reader.preprocess``'s augmentation fields, what b2second.augment reads) rides
+  along the same way as the ``augment`` attribute, written out in ``AUGMENTS`` for the builtins.
 """
 import re
 from dataclasses import dataclass, field
@@ -199,6 +201,8 @@ class ModelConfig:
             box_code_size=7 + len(classes[0][0].custom_values),
         )
         cfg.target_assigner = _target_assigner_settings(m, ta)
+        tr = _one(tree["train_input_reader"]) if "train_input_reader" in tree else {}
+        cfg.augment = _augment_settings(_one(tr["preprocess"]) if "preprocess" in tr else {})
         return cfg
 
     @staticmethod
@@ -265,6 +269,41 @@ def _target_assigner_settings(m, ta):
         sample_positive_fraction=_f32(_one(ta.get("sample_positive_fraction", [0.0]))), box_coder=kind,
         linear_dim=bool(_one(cc.get("linear_dim", [False]))),
         encode_angle_vector=bool(_one(cc.get("encode_angle_vector", [False]))))
+
+
+@dataclass
+class AugmentSettings:
+    """``train_input_reader.preprocess``'s augmentation fields (second/protos/input_reader.proto), as
+    second/builder/dataset_builder.py:84-103 hands them to prep_pointcloud.  Floats are the float32 values protobuf
+    stores, widened to Python floats; absent fields take proto3's defaults (empty lists, false)."""
+    shuffle_points: bool = False
+    groundtruth_localization_noise_std: List[float] = field(default_factory=list)
+    groundtruth_rotation_uniform_noise: List[float] = field(default_factory=list)
+    global_rotation_uniform_noise: List[float] = field(default_factory=list)
+    global_scaling_uniform_noise: List[float] = field(default_factory=list)
+    global_random_rotation_range_per_object: List[float] = field(default_factory=list)
+    global_translate_noise_std: List[float] = field(default_factory=list)
+    random_flip_x: bool = False
+    random_flip_y: bool = False
+    use_group_id: bool = False
+
+
+def _augment_settings(prep):
+    def floats(key):
+        return [_f32(v) for v in prep.get(key, [])]
+
+    def flag(key):
+        return bool(_one(prep.get(key, [False])))
+
+    return AugmentSettings(
+        shuffle_points=flag("shuffle_points"),
+        groundtruth_localization_noise_std=floats("groundtruth_localization_noise_std"),
+        groundtruth_rotation_uniform_noise=floats("groundtruth_rotation_uniform_noise"),
+        global_rotation_uniform_noise=floats("global_rotation_uniform_noise"),
+        global_scaling_uniform_noise=floats("global_scaling_uniform_noise"),
+        global_random_rotation_range_per_object=floats("global_random_rotation_range_per_object"),
+        global_translate_noise_std=floats("global_translate_noise_std"),
+        random_flip_x=flag("random_flip_x"), random_flip_y=flag("random_flip_y"), use_group_id=flag("use_group_id"))
 
 
 def _one(v):
@@ -535,6 +574,29 @@ TARGET_ASSIGNERS = {
 }
 
 
+def _aug(loc, rot, grot, scale, translate, flip_x, shuffle):
+    return AugmentSettings(
+        shuffle_points=shuffle, groundtruth_localization_noise_std=[_f32(v) for v in loc],
+        groundtruth_rotation_uniform_noise=[_f32(v) for v in rot], global_rotation_uniform_noise=[_f32(v) for v in grot],
+        global_scaling_uniform_noise=[_f32(v) for v in scale], global_random_rotation_range_per_object=[0.0, 0.0],
+        global_translate_noise_std=[_f32(v) for v in translate], random_flip_x=flip_x, random_flip_y=True)
+
+
+_KITTI_AUG = ([1.0, 1.0, 0.5], [-0.78539816, 0.78539816], [-0.78539816, 0.78539816], [0.95, 1.05], [0, 0, 0])
+_NUSC_AUG = ([0, 0, 0], [0, 0], [0, 0], [1.0, 1.0], [0, 0, 0])
+# augmentation settings of the builtins (the train_input_reader.preprocess blocks of the cited config files)
+AUGMENTS = {
+    "car.fhd": lambda: _aug(*_KITTI_AUG, flip_x=False, shuffle=True),
+    "car.lite": lambda: _aug(*_KITTI_AUG, flip_x=False, shuffle=True),
+    "all.fhd": lambda: _aug(*_KITTI_AUG, flip_x=False, shuffle=True),
+    "pointpillars.car.xyres_16": lambda: _aug([0.25, 0.25, 0.25], [-0.15707963267, 0.15707963267],
+                                              [-0.78539816, 0.78539816], [0.95, 1.05], [0.2, 0.2, 0.2], flip_x=False,
+                                              shuffle=True),
+    "nuscenes.all.pp.largea": lambda: _aug(*_NUSC_AUG, flip_x=True, shuffle=False),
+    "nuscenes.all.pp.mhead": lambda: _aug(*_NUSC_AUG, flip_x=True, shuffle=False),
+}
+
+
 def get_config(name):
     if name in BUILTIN:
         cfg = BUILTIN[name]()
@@ -543,4 +605,5 @@ def get_config(name):
     else:
         raise KeyError("unknown config %r (have %s)" % (name, sorted(BUILTIN) + sorted(EXTRA)))
     cfg.target_assigner = TARGET_ASSIGNERS[name]()
+    cfg.augment = AUGMENTS[name]()
     return cfg
