@@ -32,11 +32,19 @@ __device__ __forceinline__ float poly_area(const float *p, int n)
 }
 
 // Sutherland-Hodgman clip of convex quad A by convex quad B; returns intersection area (>= 0).
+// All eight corners are first taken relative to A's first corner, so the shoelace and clip products stay of the
+// size of the pair, not of its position: on raw coordinates near (70, 40) the products are ~2800 against areas of a
+// few m^2, and the IoU error grew with the distance from the origin (DESIGN §2).  For a pair far from the origin
+// the subtraction is exact (Sterbenz).
 __device__ float quad_intersection(const float *a_in, const float *b_in, float *area_a, float *area_b)
 {
     float A[8], B[8];
+    const float ox = a_in[0], oy = a_in[1];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) { A[i] = a_in[i]; B[i] = b_in[i]; }
+    for (int i = 0; i < 8; i += 2) {
+        A[i] = __fsub_rn(a_in[i], ox); A[i + 1] = __fsub_rn(a_in[i + 1], oy);
+        B[i] = __fsub_rn(b_in[i], ox); B[i + 1] = __fsub_rn(b_in[i + 1], oy);
+    }
     float sa = poly_area(A, 4), sb = poly_area(B, 4);
     if (sa < 0.f) {
 #pragma unroll

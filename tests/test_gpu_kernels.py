@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 import torch
 
+import detect_ref as R
 import golden_util as gu
 from b2second import box_ops, config, models
 
@@ -258,21 +259,43 @@ def test_device_nms_matches_oracle(product, oracle, rotated, n, spread, thr, pre
     ws_bytes = lib.b2s_nms_workspace_bytes(B, cc, pre_max)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device="cuda")
     width = post_max * (code + 2) + 1
-    rec = torch.zeros(B, width, device="cuda")
-    det_count = torch.zeros(B, dtype=torch.int32, device="cuda")
-    L.check(lib.b2s_nms(L.ptr(d["box"]), L.ptr(d["score"]), L.ptr(d["label"]), L.ptr(d["dir"]), L.ptr(d["anchor"]),
-                        L.ptr(cnt), B, cc, code, 1 if rotated else 0, pre_max, post_max, thr, 1, 0.78, 0.5, 2,
-                        L.f6(rng6), L.ptr(rec), width, L.ptr(det_count), L.ptr(ws), ws_bytes, L.stream()), "b2s_nms")
-    torch.cuda.synchronize()
-    rec = rec.cpu()
-    assert rec[:, -1].tolist() == [float(c) for c in det_count.cpu().tolist()]      # the count rides in the record
+    recs = {}
+    for key, r6 in (("range", L.f6(rng6)), ("none", None)):
+        rec = torch.zeros(B, width, device="cuda")
+        det_count = torch.zeros(B, dtype=torch.int32, device="cuda")
+        L.check(lib.b2s_nms(L.ptr(d["box"]), L.ptr(d["score"]), L.ptr(d["label"]), L.ptr(d["dir"]), L.ptr(d["anchor"]),
+                            L.ptr(cnt), B, cc, code, 1 if rotated else 0, pre_max, post_max, thr, 1, 0.78, 0.5, 2, r6,
+                            L.ptr(rec), width, L.ptr(det_count), L.ptr(ws), ws_bytes, L.stream()), "b2s_nms")
+        torch.cuda.synchronize()
+        recs[key] = (rec.cpu(), det_count.cpu())
+    rec, det_count = recs["range"]
+    assert rec[:, -1].tolist() == [float(c) for c in det_count.tolist()]      # the count rides in the record
+    lo, hi = np.asarray(rng6[:3], np.float32), np.asarray(rng6[3:], np.float32)
     for b, m in enumerate(counts):
         rb, rs, rl, near = _nms_reference(oracle, cand_box[b, :m], cand_score[b, :m], cand_label[b, :m], cand_dir[b, :m],
                                           cand_anchor[b, :m], rotated, pre_max, post_max, thr, True, 0.78, 0.5, 2, rng6)
         k = int(det_count[b].item())
         got = rec[b, :-1].view(post_max, code + 2)[:k].numpy()
-        if near:                      # a pair within 1e-4 of the IoU threshold: only the size of the change is bounded
-            assert abs(k - len(rs)) <= 2 * near
+        # without the range test: the keep list must pass the fp64 certificate, and the range test filters its rows
+        k_all = int(recs["none"][1][b])
+        rows = recs["none"][0][b, :-1].view(post_max, code + 2)[:k_all].numpy()
+        inside = np.all(rows[:, :3] >= lo, 1) & np.all(rows[:, :3] <= hi, 1)
+        assert k == int(inside.sum()) and np.array_equal(got, rows[inside])
+        order = np.lexsort((cand_anchor[b, :m], -cand_score[b, :m].astype(np.float64)))[:pre_max]
+        slot = {cand_box[b, s, :6].tobytes() + cand_score[b, s].tobytes(): s for s in order}
+        kept = [slot[r[:6].tobytes() + r[7:8].tobytes()] for r in rows]
+        b5 = np.ascontiguousarray(cand_box[b, order][:, [0, 1, 3, 4, 6]])
+        c64 = R.bev_corners(b5)
+        if rotated:
+            ov = R.overlaps(c64, c64)
+            iou, bound = np.triu(ov[-1], 1), R.corner_bound(b5, b5, ov)
+        else:
+            st = R.standup(c64)
+            iou, bound = np.triu(R.aligned_iou(st, st, 1.0)[0], 1), R.aligned_bound(st, st, 1.0, R.corner_rounding(b5),
+                                                                                     R.corner_rounding(b5))
+        err = R.nms_certificate(order, kept, iou, bound, thr, post_max, inclusive=bool(rotated))
+        assert err is None, "frame %d: %s" % (b, err)
+        if near:                      # a pair within 1e-4 of the IoU threshold: the certificate above decides
             continue
         assert k == len(rs), "frame %d: %d kept, oracle %d" % (b, k, len(rs))
         np.testing.assert_array_equal(got[:, 7], rs)
