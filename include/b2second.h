@@ -59,6 +59,9 @@
  *                       noise_per_object_v3_, random_flip, global_rotation_v2 / scaling_v2 / translate_, the range
  *                       filter, limit_period and the point shuffle (second/core/preprocess.py:153-164,244-273,450-476,
  *                       582-678,749-800,803-899), for a batch of frames
+ *   b2s_db_sample       ground-truth database sampling of prep_pointcloud (second/data/preprocess.py:210-249):
+ *                       DataBaseSamplerV2.sample_all / sample_class_v2 collision rejection (second/core/sample_ops.py:
+ *                       95-285), points_in_rbbox point removal and the concatenation, for a batch of frames
  */
 #ifndef B2SECOND_H_
 #define B2SECOND_H_
@@ -70,7 +73,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 205
+#define B2S_VERSION 206
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -81,9 +84,14 @@ extern "C" {
                                           it was clamped -- results are not fp32-grade for that frame batch      */
 #define B2S_STATUS_BAD_INPUT 32u       /* b2s_assign_targets: a frame's gt_offsets are decreasing or past num_gt; that
                                           frame was assigned as if it had no ground truth.  b2s_augment: the same for
-                                          gt_offsets or point_offsets, or a perm entry outside its frame          */
+                                          gt_offsets or point_offsets, or a perm entry outside its frame.
+                                          b2s_db_sample: bad or overlapping point, box or candidate offsets (that
+                                          part of the frame is treated as empty), a candidate object id outside the
+                                          database or point offsets that disagree with it                        */
 #define B2S_STATUS_AUG_BOX_CAP 64u     /* b2s_augment: a frame holds more than B2S_AUGMENT_MAX_BOXES ground truths; its
                                           boxes and points got no per-object noise                               */
+#define B2S_STATUS_DB_BOX_CAP 128u     /* b2s_db_sample: a frame's ground truths plus candidates exceed
+                                          B2S_DBSAMPLE_MAX_BOXES; that frame got no samples                      */
 
 /* IEEE binary16 bit pattern (the tensor-core kernels' operand planes; torch.float16 storage) */
 typedef uint16_t b2s_half;
@@ -637,6 +645,47 @@ int b2s_augment(const float *points, int num_points, int num_feat, const int *po
                 const float *range_host, float *points_out, int *point_box, void *boxes_out, int *gt_offsets_out,
                 int *classes_out, float *importance_out, int *src_out, int *selected, void *workspace,
                 size_t workspace_bytes, unsigned *status_dev, void *stream);
+
+/* ---- training ground-truth database sampling (second/data/preprocess.py:210-249) ----------------------------- */
+/* The device half of DataBaseSamplerV2.sample_all without group sampling, per-object rotation or random crop, for
+ * `batch` frames.  The candidates are inputs (b2second.dbsample.draw makes them from a numpy RandomState in the
+ * reference's order); this call decides which are accepted and builds the frames prep_pointcloud holds at
+ * preprocess.py:249.
+ *   points / point_offsets / gt_boxes / gt_offsets / gt_valid / gt_classes / gt_importance: as b2s_augment's inputs
+ *   (gt_importance NULL: ones); every gt row of a frame blocks candidates, whatever its class mask;
+ *   cand_obj int32 [num_cand] database object ids, frame f owning rows [cand_offsets[f], cand_offsets[f+1]), class by
+ *   class in sample-group order; cand_group int32 [num_cand] the sample group of each (equal values: one class);
+ *   cand_point_offsets int32 [num_cand + 1] the prefix of the candidates' point counts (num_cand_points the total);
+ *   db_points [*, num_feat] float32, object o owning rows [db_point_offsets[o], db_point_offsets[o+1]) (int64, the
+ *   object's points relative to its box centre); db_boxes [num_objects, box_ndim] in the gt dtype; db_classes int32
+ *   [num_objects] 1-based class ids (class_names.index(name) + 1); sample_importance, remove_points 0/1
+ *   (remove_points_after_sample: a frame point inside an accepted box is dropped).
+ * A candidate is rejected when its BEV box collides with a gt box of its frame, an accepted candidate of an earlier
+ * class, an accepted earlier candidate of its own class, or any later candidate of its own class (dbsample.cu states
+ * why).  Outputs, packed frame after frame: points_out [num_points + num_cand_points, num_feat] (the accepted
+ * objects' points translated by their box centre in acceptance order, then the frame's kept points in order; zeros
+ * past point_offsets_out[batch]), point_offsets_out int32 [batch + 1]; boxes_out [num_gt + num_cand, box_ndim],
+ * valid_out uint8, classes_out int32, importance_out float32, src_object int32 (the database object, -1 for the
+ * frame's own rows) [num_gt + num_cand]: the frame's rows then its accepted ones (zeros past gt_offsets_out[batch]),
+ * gt_offsets_out int32 [batch + 1] -- b2s_augment's input layout; accepted uint8 [num_cand].  A frame whose gt rows
+ * plus candidates exceed B2S_DBSAMPLE_MAX_BOXES raises B2S_STATUS_DB_BOX_CAP and gets no samples.  A frame's range in
+ * an offsets array is used only when it is ordered, inside the array, and neither before an earlier entry nor after a
+ * later one (so the ranges in use never overlap); otherwise that part of the frame is empty.  Such ranges, object ids
+ * outside the database and cand_point_offsets steps that differ from the objects' point counts (those candidates are
+ * rejected) raise B2S_STATUS_BAD_INPUT; no output is written past its capacity.  Four memsets and five kernels; no
+ * sync, deterministic.  workspace:
+ * b2s_db_sample_workspace_bytes(batch, num_points, num_cand) (host query) bytes. */
+#define B2S_DBSAMPLE_MAX_BOXES 1024
+size_t b2s_db_sample_workspace_bytes(int batch, int num_points, int num_cand);
+int b2s_db_sample(const float *points, int num_points, int num_feat, const int *point_offsets, int batch,
+                  const void *gt_boxes, int gt_double, int box_ndim, int num_gt, const int *gt_offsets,
+                  const uint8_t *gt_valid, const int *gt_classes, const float *gt_importance, const int *cand_obj,
+                  const int *cand_group, const int *cand_offsets, const int *cand_point_offsets, int num_cand,
+                  int num_cand_points, const float *db_points, const long long *db_point_offsets,
+                  const void *db_boxes, const int *db_classes, int num_objects, float sample_importance,
+                  int remove_points, float *points_out, int *point_offsets_out, void *boxes_out, int *gt_offsets_out,
+                  uint8_t *valid_out, int *classes_out, float *importance_out, int *src_object, uint8_t *accepted,
+                  void *workspace, size_t workspace_bytes, unsigned *status_dev, void *stream);
 
 #ifdef __cplusplus
 }

@@ -15,6 +15,9 @@ side needs neither protobuf nor the reference tree:
   the builtins.  It is not a dataclass field, so the inference fields above keep their shape.
 * ``AugmentSettings`` (``train_input_reader.preprocess``'s augmentation fields, what b2second.augment reads) rides
   along the same way as the ``augment`` attribute, written out in ``AUGMENTS`` for the builtins.
+* ``DatabaseSamplerSettings`` (``train_input_reader.preprocess.database_sampler`` and the two preprocess fields that go
+  with it, what b2second.dbsample reads) rides along as the ``db_sampler`` attribute (None without a sampler), written
+  out in ``DB_SAMPLERS`` for the builtins.
 """
 import re
 from dataclasses import dataclass, field
@@ -203,6 +206,7 @@ class ModelConfig:
         cfg.target_assigner = _target_assigner_settings(m, ta)
         tr = _one(tree["train_input_reader"]) if "train_input_reader" in tree else {}
         cfg.augment = _augment_settings(_one(tr["preprocess"]) if "preprocess" in tr else {})
+        cfg.db_sampler = _db_sampler_settings(_one(tr["preprocess"]) if "preprocess" in tr else {})
         return cfg
 
     @staticmethod
@@ -304,6 +308,48 @@ def _augment_settings(prep):
         global_random_rotation_range_per_object=floats("global_random_rotation_range_per_object"),
         global_translate_noise_std=floats("global_translate_noise_std"),
         random_flip_x=flag("random_flip_x"), random_flip_y=flag("random_flip_y"), use_group_id=flag("use_group_id"))
+
+
+@dataclass
+class DatabaseSamplerSettings:
+    """``train_input_reader.preprocess.database_sampler`` (second/protos/sampler.proto) as
+    second/builder/dbsampler_builder.py hands it to DataBaseSamplerV2, with the two preprocess fields prep_pointcloud
+    uses with it (second/protos/input_reader.proto).  sample_groups: one ``{name: max_num}`` per group, in file order;
+    database_prep_steps: ``("filter_by_min_num_points", [(name, min_num), ...])`` or
+    ``("filter_by_difficulty", [difficulty, ...])``, in file order.  Floats are protobuf's float32 values widened;
+    absent fields take proto3's defaults."""
+    sample_groups: List[dict] = field(default_factory=list)
+    database_prep_steps: List[tuple] = field(default_factory=list)
+    rate: float = 0.0
+    global_random_rotation_range_per_object: List[float] = field(default_factory=list)
+    database_info_path: str = ""
+    remove_points_after_sample: bool = False
+    sample_importance: float = 0.0
+
+
+def _db_sampler_settings(prep):
+    """None when the block enables no sampler (second/builder/dataset_builder.py:61-64)"""
+    ds = _one(prep["database_sampler"]) if "database_sampler" in prep else {}
+    groups = [{_one(kv["key"]): int(_one(kv["value"])) for kv in g.get("name_to_max_num", [])}
+              for g in ds.get("sample_groups", [])]
+    path = _one(ds.get("database_info_path", [""]))
+    if not groups and path == "":
+        return None
+    steps = []
+    for st in ds.get("database_prep_steps", []):
+        if "filter_by_min_num_points" in st:
+            pairs = _one(st["filter_by_min_num_points"]).get("min_num_point_pairs", [])
+            steps.append(("filter_by_min_num_points", [(_one(kv["key"]), int(_one(kv["value"]))) for kv in pairs]))
+        elif "filter_by_difficulty" in st:
+            steps.append(("filter_by_difficulty",
+                          [int(v) for v in _one(st["filter_by_difficulty"]).get("removed_difficulties", [])]))
+        else:
+            raise ValueError("unknown database prep step %r" % (sorted(st),))
+    return DatabaseSamplerSettings(
+        sample_groups=groups, database_prep_steps=steps, rate=_f32(_one(ds.get("rate", [0.0]))),
+        global_random_rotation_range_per_object=[_f32(v) for v in ds.get("global_random_rotation_range_per_object", [])],
+        database_info_path=path, remove_points_after_sample=bool(_one(prep.get("remove_points_after_sample", [False]))),
+        sample_importance=_f32(_one(prep.get("sample_importance", [0.0]))))
 
 
 def _one(v):
@@ -597,6 +643,35 @@ AUGMENTS = {
 }
 
 
+_KITTI_DB = "/media/yy/960evo/datasets/kitti/kitti_dbinfos_train.pkl"
+_KITTI_DB_PASSPORT = "/media/yy/My Passport/datasets/kitti/kitti_dbinfos_train.pkl"
+_NUSC_DB = "/media/yy/960evo/datasets/nuscene/v1.0-trainval/kitti_dbinfos_train.pkl"
+
+
+def _dbs(groups, min_points, path, remove, importance=1.0, difficulties=(-1,)):
+    """groups: [(name, max_num)]; min_points: [(name, min_num)] or None (no prep steps at all)"""
+    steps = [] if min_points is None else [("filter_by_min_num_points", list(min_points)),
+                                           ("filter_by_difficulty", list(difficulties))]
+    return DatabaseSamplerSettings(
+        sample_groups=[{n: m} for n, m in groups], database_prep_steps=steps, rate=1.0,
+        global_random_rotation_range_per_object=[0.0, 0.0], database_info_path=path,
+        remove_points_after_sample=remove, sample_importance=_f32(importance))
+
+
+_NUSC_GROUPS = [("bus", 4), ("trailer", 4), ("truck", 4)]
+# database-sampler settings of the builtins (the train_input_reader.preprocess.database_sampler blocks of the cited
+# config files)
+DB_SAMPLERS = {
+    "car.fhd": lambda: _dbs([("Car", 15)], [("Car", 5)], _KITTI_DB, True),
+    "car.lite": lambda: _dbs([("Car", 15)], [("Car", 5)], _KITTI_DB_PASSPORT, False),
+    "all.fhd": lambda: _dbs([("Car", 11), ("Pedestrian", 6), ("Cyclist", 6), ("Van", 4)],
+                            [("Car", 5), ("Pedestrian", 10), ("Cyclist", 10), ("Van", 8)], _KITTI_DB, True),
+    "pointpillars.car.xyres_16": lambda: _dbs([("Car", 15)], [("Car", 5)], _KITTI_DB_PASSPORT, False),
+    "nuscenes.all.pp.largea": lambda: _dbs(_NUSC_GROUPS, None, _NUSC_DB, True),
+    "nuscenes.all.pp.mhead": lambda: _dbs(_NUSC_GROUPS, None, _NUSC_DB, True, importance=0.5),
+}
+
+
 def get_config(name):
     if name in BUILTIN:
         cfg = BUILTIN[name]()
@@ -606,4 +681,5 @@ def get_config(name):
         raise KeyError("unknown config %r (have %s)" % (name, sorted(BUILTIN) + sorted(EXTRA)))
     cfg.target_assigner = TARGET_ASSIGNERS[name]()
     cfg.augment = AUGMENTS[name]()
+    cfg.db_sampler = DB_SAMPLERS[name]()
     return cfg

@@ -138,6 +138,12 @@ SIGNATURES = {
                             c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
                             c_void_p, c_void_p]),
+    "b2s_db_sample_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "b2s_db_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
+                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                              c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p,
+                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                              c_void_p, c_void_p]),
 }
 
 
@@ -216,8 +222,11 @@ STATUS_BITS = {1: "voxel overflow (more voxels than max_voxels; extra voxels dro
                2: "row overflow (strided conv produced more rows than the buffer capacity)",
                4: "hash table full", 8: "candidate overflow (more score survivors than cand_cap)",
                16: "an activation left the fp16 range (|x| > 65504) on the tensor-core path",
-               32: "bad frame offsets (that frame was treated as having no ground truth) or a bad point permutation",
-               64: "a frame holds more ground truths than the augmentation's per-frame cap (no object noise there)"}
+               32: "bad frame offsets (that frame was treated as having no ground truth), a bad point permutation or a "
+                   "candidate outside the database",
+               64: "a frame holds more ground truths than the augmentation's per-frame cap (no object noise there)",
+               128: "a frame's ground truths plus database candidates exceed the sampler's per-frame cap (no samples "
+                    "there)"}
 
 
 def status_message(word):
