@@ -62,6 +62,9 @@
  *   b2s_db_sample       ground-truth database sampling of prep_pointcloud (second/data/preprocess.py:210-249):
  *                       DataBaseSamplerV2.sample_all / sample_class_v2 collision rejection (second/core/sample_ops.py:
  *                       95-285), points_in_rbbox point removal and the concatenation, for a batch of frames
+ *   b2s_detection_loss, b2s_detection_loss_backward
+ *                       VoxelNet.loss (second/pytorch/models/voxelnet.py:239-312, second/pytorch/core/losses.py:
+ *                       135-294) and the autograd backward of its four differentiable scalars
  */
 #ifndef B2SECOND_H_
 #define B2SECOND_H_
@@ -73,7 +76,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 206
+#define B2S_VERSION 207
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -87,7 +90,8 @@ extern "C" {
                                           gt_offsets or point_offsets, or a perm entry outside its frame.
                                           b2s_db_sample: bad or overlapping point, box or candidate offsets (that
                                           part of the frame is treated as empty), a candidate object id outside the
-                                          database or point offsets that disagree with it                        */
+                                          database or point offsets that disagree with it.  b2s_detection_loss: a
+                                          label outside [-1, num_class] (that anchor counts as not cared)        */
 #define B2S_STATUS_AUG_BOX_CAP 64u     /* b2s_augment: a frame holds more than B2S_AUGMENT_MAX_BOXES ground truths; its
                                           boxes and points got no per-object noise                               */
 #define B2S_STATUS_DB_BOX_CAP 128u     /* b2s_db_sample: a frame's ground truths plus candidates exceed
@@ -686,6 +690,49 @@ int b2s_db_sample(const float *points, int num_points, int num_feat, const int *
                   int remove_points, float *points_out, int *point_offsets_out, void *boxes_out, int *gt_offsets_out,
                   uint8_t *valid_out, int *classes_out, float *importance_out, int *src_object, uint8_t *accepted,
                   void *workspace, size_t workspace_bytes, unsigned *status_dev, void *stream);
+
+/* ---- training loss (second/pytorch/models/voxelnet.py:239-312) ------------------------------------------------- */
+/* VoxelNet.loss with the loss settings of every config: WeightedSmoothL1LocalizationLoss (second/pytorch/core/losses.py:
+ * 135-182) on the sin-encoded box (add_sin_difference, voxelnet.py:704-714), SigmoidFocalClassificationLoss
+ * (losses.py:184-192,236-294) on the one-hot target without background (voxelnet.py:255,737-741), NormByNumPositives
+ * weights times importance (prepare_loss_weights, voxelnet.py:756-795, :265-267), the reductions and _get_pos_neg_loss
+ * (voxelnet.py:20-34,275-282), and the softmax direction loss (get_direction_target, voxelnet.py:814-828, :284-297)
+ * weighted by positive importance over its per-frame sum.  Settings, read on the host: */
+typedef struct b2s_loss_params {
+    float alpha, gamma;            /* focal */
+    float sigma;                   /* smooth L1 */
+    float code_weight[7];
+    float pos_cls_weight, neg_cls_weight;
+    float loc_weight, cls_weight, dir_weight;   /* localization_weight, classification_weight, direction_loss_weight */
+    float sin_factor;              /* sin_error_factor */
+    float dir_offset;
+    int num_dir_bins;
+} b2s_loss_params;
+/* Inputs: box_preds [batch, A, 7], cls_preds [batch, A, num_class], dir_preds [batch, A, num_dir_bins] float32 (the
+ * heads' permuted outputs, contiguous); labels [batch, A] int32 (labels_int64 0) or int64 (1): -1 ignore, 0 background,
+ * c >= 1 class c; reg_targets [batch, A, 7], importance [batch, A], anchors [batch, A, 7] (only the yaw is read).
+ * Outputs: reduced float32 [4] = loss, cls_loss_reduced, loc_loss_reduced, dir_loss_reduced (unweighted; loss holds it
+ * times dir_weight); pos_neg [2] = cls_pos_loss, cls_neg_loss; optional (NULL: not written) cls_loss [batch, A,
+ * num_class], loc_loss [batch, A, 7], cared uint8 [batch, A]; norms [batch, 2] = max(positives, 1) and max(sum of
+ * positive importance, 1) per frame, which the backward reads.  A label outside [-1, num_class] counts as -1 and
+ * raises B2S_STATUS_BAD_INPUT.  Three kernels; sums in one fixed order (no float atomics), so results are
+ * bit-reproducible; no sync.  workspace: b2s_detection_loss_workspace_bytes(batch, A) (host query) bytes. */
+size_t b2s_detection_loss_workspace_bytes(int batch, int num_anchors);
+int b2s_detection_loss(const float *box_preds, const float *cls_preds, const float *dir_preds, int num_class,
+                       int num_dir_bins, const void *labels, int labels_int64, const float *reg_targets,
+                       const float *importance, const float *anchors, int batch, int num_anchors,
+                       const b2s_loss_params *params, float *reduced, float *pos_neg, float *cls_loss,
+                       float *loc_loss, uint8_t *cared, float *norms, void *workspace, size_t workspace_bytes,
+                       unsigned *status_dev, void *stream);
+/* The gradient of d_reduced[0] * loss + d_reduced[1] * cls_loss_reduced + d_reduced[2] * loc_loss_reduced +
+ * d_reduced[3] * dir_loss_reduced (d_reduced: device float32 [4], or NULL for zeros) in the preds, written to d_box,
+ * d_cls, d_dir in the preds' layout; the inputs and norms as the forward had them.  One kernel, one thread per anchor;
+ * an anchor of weight 0 gets exactly 0. */
+int b2s_detection_loss_backward(const float *box_preds, const float *cls_preds, const float *dir_preds, int num_class,
+                                int num_dir_bins, const void *labels, int labels_int64, const float *reg_targets,
+                                const float *importance, const float *anchors, int batch, int num_anchors,
+                                const b2s_loss_params *params, const float *norms, const float *d_reduced,
+                                float *d_box, float *d_cls, float *d_dir, void *stream);
 
 #ifdef __cplusplus
 }

@@ -18,6 +18,8 @@ side needs neither protobuf nor the reference tree:
 * ``DatabaseSamplerSettings`` (``train_input_reader.preprocess.database_sampler`` and the two preprocess fields that go
   with it, what b2second.dbsample reads) rides along as the ``db_sampler`` attribute (None without a sampler), written
   out in ``DB_SAMPLERS`` for the builtins.
+* ``LossSettings`` (``model.second.loss`` and the loss fields of ``model.second``, what VoxelNet.loss and
+  b2second.loss read) rides along as the ``loss`` attribute, written out in ``LOSSES`` for the builtins.
 """
 import re
 from dataclasses import dataclass, field
@@ -207,6 +209,7 @@ class ModelConfig:
         tr = _one(tree["train_input_reader"]) if "train_input_reader" in tree else {}
         cfg.augment = _augment_settings(_one(tr["preprocess"]) if "preprocess" in tr else {})
         cfg.db_sampler = _db_sampler_settings(_one(tr["preprocess"]) if "preprocess" in tr else {})
+        cfg.loss = _loss_settings(m)
         return cfg
 
     @staticmethod
@@ -350,6 +353,51 @@ def _db_sampler_settings(prep):
         global_random_rotation_range_per_object=[_f32(v) for v in ds.get("global_random_rotation_range_per_object", [])],
         database_info_path=path, remove_points_after_sample=bool(_one(prep.get("remove_points_after_sample", [False]))),
         sample_importance=_f32(_one(prep.get("sample_importance", [0.0]))))
+
+
+@dataclass
+class LossSettings:
+    """``model.second.loss`` (second/protos/losses.proto) and the loss fields of ``model.second`` (second.proto), as
+    second/pytorch/builder/second_builder.py:46-62 and losses_builder.py hand them to VoxelNet.  Floats are protobuf's
+    float32 values widened; absent fields take proto3's defaults, except sin_error_factor, where the builder turns 0
+    into 1.  code_weight empty: none (the loss applies no code weights)."""
+    classification_loss: str = ""                 # weighted_sigmoid_focal | weighted_sigmoid | weighted_softmax ...
+    alpha: float = 0.0
+    gamma: float = 0.0
+    localization_loss: str = ""                   # weighted_smooth_l1 | weighted_l2 ...
+    sigma: float = 0.0
+    code_weight: List[float] = field(default_factory=list)
+    classification_weight: float = 0.0
+    localization_weight: float = 0.0
+    loss_norm_type: str = "NormByNumExamples"
+    pos_class_weight: float = 0.0
+    neg_class_weight: float = 0.0
+    encode_rad_error_by_sin: bool = False
+    sin_error_factor: float = 1.0
+    direction_loss_weight: float = 0.0
+
+
+def _loss_settings(m):
+    loss = _one(m.get("loss", [{}]))
+    cl = _one(loss.get("classification_loss", [{}]))
+    ll = _one(loss.get("localization_loss", [{}]))
+    ckind = next(iter(cl), "")
+    lkind = next(iter(ll), "")
+    cc = _one(cl[ckind]) if ckind else {}
+    lc = _one(ll[lkind]) if lkind else {}
+    sin_factor = _f32(_one(m.get("sin_error_factor", [0.0])))
+    return LossSettings(
+        classification_loss=ckind, alpha=_f32(_one(cc.get("alpha", [0.0]))), gamma=_f32(_one(cc.get("gamma", [0.0]))),
+        localization_loss=lkind, sigma=_f32(_one(lc.get("sigma", [0.0]))),
+        code_weight=[_f32(v) for v in lc.get("code_weight", [])],
+        classification_weight=_f32(_one(loss.get("classification_weight", [0.0]))),
+        localization_weight=_f32(_one(loss.get("localization_weight", [0.0]))),
+        loss_norm_type=str(_one(m.get("loss_norm_type", ["NormByNumExamples"]))),
+        pos_class_weight=_f32(_one(m.get("pos_class_weight", [0.0]))),
+        neg_class_weight=_f32(_one(m.get("neg_class_weight", [0.0]))),
+        encode_rad_error_by_sin=bool(_one(m.get("encode_rad_error_by_sin", [False]))),
+        sin_error_factor=sin_factor if sin_factor != 0 else 1.0,
+        direction_loss_weight=_f32(_one(m.get("direction_loss_weight", [0.0]))))
 
 
 def _one(v):
@@ -672,6 +720,18 @@ DB_SAMPLERS = {
 }
 
 
+def _loss():
+    """the loss every builtin config sets (the loss blocks and fields of the cited config files agree)"""
+    return LossSettings(
+        classification_loss="weighted_sigmoid_focal", alpha=0.25, gamma=2.0, localization_loss="weighted_smooth_l1",
+        sigma=3.0, code_weight=[1.0] * 7, classification_weight=1.0, localization_weight=2.0,
+        loss_norm_type="NormByNumPositives", pos_class_weight=1.0, neg_class_weight=1.0, encode_rad_error_by_sin=True,
+        sin_error_factor=1.0, direction_loss_weight=_f32(0.2))
+
+
+LOSSES = {name: _loss for name in list(TARGET_ASSIGNERS)}
+
+
 def get_config(name):
     if name in BUILTIN:
         cfg = BUILTIN[name]()
@@ -682,4 +742,5 @@ def get_config(name):
     cfg.target_assigner = TARGET_ASSIGNERS[name]()
     cfg.augment = AUGMENTS[name]()
     cfg.db_sampler = DB_SAMPLERS[name]()
+    cfg.loss = LOSSES[name]()
     return cfg

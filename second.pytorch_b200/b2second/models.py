@@ -17,8 +17,10 @@ contract and *state-dict keys*, so reference checkpoints load unchanged:
 
 Every module takes the ``spconv`` *backend module* it should build on: the product backend is
 ``second.pytorch_b200/spconv`` (CUDA, fails loudly without the extension); tests and the CPU
-baseline pass the oracle package instead.  Only the inference path is mirrored (no losses).
+baseline pass the oracle package instead.  Only the inference path is mirrored; the training loss is b2second.loss.
 """
+from enum import Enum
+
 import numpy as np
 import torch
 from torch import nn
@@ -480,6 +482,38 @@ class MirrorTargetAssigner:
         return start, start + self._anchor_generators[class_idx].num_anchors_per_localization * self._class_hw(class_idx)
 
 
+class LossNormType(Enum):
+    """voxelnet.py:51-55"""
+    NormByNumPositives = "norm_by_num_positives"
+    NormByNumExamples = "norm_by_num_examples"
+    NormByNumPosNeg = "norm_by_num_pos_neg"
+    DontNorm = "dont_norm"
+
+
+class SigmoidFocalClassificationLoss:
+    """the settings of second/pytorch/core/losses.py:236-253 under the reference's attribute names"""
+
+    def __init__(self, gamma=2.0, alpha=0.25):
+        self._alpha = alpha
+        self._gamma = gamma
+
+
+class WeightedSmoothL1LocalizationLoss:
+    """the settings of losses.py:135-151 under the reference's attribute names"""
+
+    def __init__(self, sigma=3.0, code_weights=None):
+        self._sigma = sigma
+        self._code_weights = torch.from_numpy(np.array(code_weights, dtype=np.float32)) \
+            if code_weights is not None else None
+
+
+class _UnsupportedLoss:
+    """a loss block b2second.loss does not cover; ``kind`` is its protobuf name"""
+
+    def __init__(self, kind):
+        self.kind = kind
+
+
 class VoxelNet(nn.Module):
     """Inference network with the reference's ``forward(example)`` contract.
 
@@ -533,6 +567,23 @@ class VoxelNet(nn.Module):
         self._dir_offset = cfg.direction_offset
         self._dir_limit_offset = cfg.direction_limit_offset
         self.target_assigner = MirrorTargetAssigner(cfg)
+        self._box_coder = getattr(self.target_assigner, "_box_coder", None)
+        ls = getattr(cfg, "loss", None)
+        if ls is not None:
+            # the loss settings as second_builder.py:46-62 hands them to VoxelNet (voxelnet.py:110-141); what
+            # b2second.loss.plan reads.  ``loss`` itself exists only after b2second.loss.enable_gpu_loss(net).
+            self._cls_loss_ftor = SigmoidFocalClassificationLoss(ls.gamma, ls.alpha) \
+                if ls.classification_loss == "weighted_sigmoid_focal" else _UnsupportedLoss(ls.classification_loss)
+            self._loc_loss_ftor = WeightedSmoothL1LocalizationLoss(ls.sigma, ls.code_weight or None) \
+                if ls.localization_loss == "weighted_smooth_l1" else _UnsupportedLoss(ls.localization_loss)
+            self._loss_norm_type = LossNormType[ls.loss_norm_type]
+            self._pos_cls_weight = ls.pos_class_weight
+            self._neg_cls_weight = ls.neg_class_weight
+            self._loc_loss_weight = ls.localization_weight
+            self._cls_loss_weight = ls.classification_weight
+            self._direction_loss_weight = ls.direction_loss_weight
+            self._encode_rad_error_by_sin = ls.encode_rad_error_by_sin
+            self._sin_error_factor = ls.sin_error_factor
 
     # -- helpers --------------------------------------------------------------------------
     def anchors(self):
@@ -575,7 +626,10 @@ class VoxelNet(nn.Module):
         assert batch_anchors.shape[1] == box_preds.shape[1], \
             f"num_anchors={batch_anchors.shape[1]}, but num_output={box_preds.shape[1]}. please check size"
         if self.training:
-            raise NotImplementedError("only the inference path is mirrored (losses are out of scope)")
+            if getattr(self, "b2s_loss", None) is None:
+                raise NotImplementedError("only the inference path is mirrored (losses are out of scope)")
+            # b2second.loss.enable_gpu_loss(net) bound ``loss`` to the CUDA loss (voxelnet.py:367-368)
+            return self.loss(example, preds_dict)
         with torch.no_grad():
             return self.predict(example, preds_dict)
 

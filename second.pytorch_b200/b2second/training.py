@@ -5,8 +5,9 @@ Upstream ``spconv`` 1.x is mostly used to train: ``second/pytorch/train.py train
 same way ``fastpath.accelerate(net)`` is the opt-in for the fused inference engine::
 
     net = training.enable_sparse_backward(net)
+    net = loss.enable_gpu_loss(net)               # b2second.loss: VoxelNet.loss on the GPU
     net.train()
-    loss = criterion(net(example)); loss.backward()
+    loss = net(example)["loss"]; loss.backward()
 
 A marked sparse convolution in ``train()`` mode with grad enabled records autograd: its forward runs the inference
 kernels with fp32 output rows, its backward computes the input gradient on the same kernels over the transposed
@@ -17,7 +18,8 @@ conv.  ``eval()`` keeps the fused BN/ReLU inference path, marked or not; an unma
 
 The training targets ``VoxelNet.loss`` reads (labels, reg_targets, importance) come from ``b2second.targets`` on the GPU
 for a whole batch (``targets.plan(net.target_assigner, feature_map_size).assign_batch(...)``), after
-``b2second.inputs.anchor_area_mask``; see INTEGRATION.md, Training.
+``b2second.inputs.anchor_area_mask``, and the loss they feed runs in csrc/loss.cu through ``b2second.loss`` (the
+focal, smooth-L1 and direction terms and their gradient); see INTEGRATION.md, Training.
 """
 
 

@@ -144,7 +144,23 @@ SIGNATURES = {
                               c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p,
                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
                               c_void_p, c_void_p]),
+    "b2s_detection_loss_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "b2s_detection_loss": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                   c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "b2s_detection_loss_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p,
+                                            c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_void_p]),
 }
+
+
+class LossParams(ctypes.Structure):
+    """b2s_loss_params (include/b2second.h): the settings of b2s_detection_loss, passed by host pointer."""
+    _fields_ = [("alpha", ctypes.c_float), ("gamma", ctypes.c_float), ("sigma", ctypes.c_float),
+                ("code_weight", ctypes.c_float * 7), ("pos_cls_weight", ctypes.c_float),
+                ("neg_cls_weight", ctypes.c_float), ("loc_weight", ctypes.c_float), ("cls_weight", ctypes.c_float),
+                ("dir_weight", ctypes.c_float), ("sin_factor", ctypes.c_float), ("dir_offset", ctypes.c_float),
+                ("num_dir_bins", c_int)]
 
 
 class HeadSegment(ctypes.Structure):
@@ -222,8 +238,8 @@ STATUS_BITS = {1: "voxel overflow (more voxels than max_voxels; extra voxels dro
                2: "row overflow (strided conv produced more rows than the buffer capacity)",
                4: "hash table full", 8: "candidate overflow (more score survivors than cand_cap)",
                16: "an activation left the fp16 range (|x| > 65504) on the tensor-core path",
-               32: "bad frame offsets (that frame was treated as having no ground truth), a bad point permutation or a "
-                   "candidate outside the database",
+               32: "bad frame offsets (that frame was treated as having no ground truth), a bad point permutation, a "
+                   "candidate outside the database or a training label outside [-1, num_class]",
                64: "a frame holds more ground truths than the augmentation's per-frame cap (no object noise there)",
                128: "a frame's ground truths plus database candidates exceed the sampler's per-frame cap (no samples "
                     "there)"}

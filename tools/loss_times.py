@@ -1,0 +1,95 @@
+"""CUDA-event time of the training loss, forward + backward: python tools/loss_times.py [iters]
+
+Prints one JSON line.  Per config (car.fhd at batch 8, nuscenes.all.pp.mhead at batch 4, each with its config's real
+anchor count): milliseconds per forward + backward of
+  fused  b2second.loss (csrc/loss.cu: three forward kernels, one backward kernel, plus the few torch allocations)
+  torch  tests/loss_ref.py in float32 -- the reference's op chain (one-hot, cat, sigmoid, pow, log1p/exp, clamp, floor,
+         cross-entropy, sums) -- and its autograd backward
+on the same inputs (tests/loss_ref.make_case "a": mostly background, some ignored, a few positives), the kernels' HBM
+byte bound (DESIGN.md section 5) and the time that bound takes at the H100 SXM data-sheet 3.35 TB/s (arithmetic, not a
+measurement).  Also prints the card name, its power limit and the SM clock read during the run.
+"""
+import json
+import os
+import subprocess
+import sys
+
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
+sys.path.insert(0, os.path.join(REPO, "tests"))
+import torch  # noqa: E402
+
+import loss_ref  # noqa: E402
+from b2second import config, loader, loss, models  # noqa: E402
+
+ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 50
+HBM_BYTES_PER_S = 3.35e12
+
+
+def smi(query):
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=" + query, "--format=csv,noheader", "-i", "0"],
+                              capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        return "unknown"
+
+
+def byte_bound(B, A, C, nb, label_bytes):
+    """HBM bytes of one forward + backward: every input element read once per pass, every output written once"""
+    n = B * A
+    count = n * (label_bytes + 4)                                  # labels, importance
+    fwd_in = n * (4 * 7 + 4 * C + 4 * nb + label_bytes + 4 + 4 * 7 + 4 * 7)   # preds, labels, importance, targets,
+    fwd_out = n * (4 * C + 4 * 7 + 1)                              # anchors (the yaw's sectors); per-anchor outputs
+    bwd = fwd_in + n * (4 * 7 + 4 * C + 4 * nb)                    # the same reads, the three gradients
+    return count + fwd_in + fwd_out + bwd
+
+
+def time_ms(fn):
+    for _ in range(3):
+        fn()
+    torch.cuda.synchronize()
+    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    t0.record()
+    for _ in range(ITERS):
+        fn()
+    t1.record()
+    torch.cuda.synchronize()
+    return t0.elapsed_time(t1) / ITERS
+
+
+def main():
+    assert torch.cuda.is_available(), "this tool times CUDA kernels: it needs a GPU"
+    dev = "cuda:0"
+    rows, clocks = [], []
+    for name, B in (("car.fhd", 8), ("nuscenes.all.pp.mhead", 4)):
+        net = models.build_network(config.get_config(name), loader.oracle_spconv())
+        lp = loss.plan(net)
+        s = lp.settings
+        A = int(net.anchors().shape[0])
+        example, preds = loss_ref.make_case("a", B, A, s.num_class, s.num_dir_bins, s.dir_offset, seed=0)
+        ex = {k: v.to(dev) for k, v in example.items()}
+        ex["labels"] = ex["labels"].to(torch.int32)                # what b2second.targets.assign_batch gives
+        pr = {k: v.to(dev).requires_grad_() for k, v in preds.items()}
+
+        def fused():
+            lp.loss(ex, pr)["loss"].backward()
+
+        def chain():
+            loss_ref.loss(s, ex, pr)["loss"].backward()
+
+        row = {"config": name, "batch": B, "anchors": A, "num_class": s.num_class}
+        row["fused_ms"] = round(time_ms(fused), 4)
+        clocks.append(smi("clocks.sm"))
+        row["torch_ms"] = round(time_ms(chain), 4)
+        clocks.append(smi("clocks.sm"))
+        nbytes = byte_bound(B, A, s.num_class, s.num_dir_bins, 4)
+        row["byte_bound"] = nbytes
+        row["byte_bound_ms"] = round(nbytes / HBM_BYTES_PER_S * 1e3, 4)
+        rows.append(row)
+    print(json.dumps({"tool": "loss_times", "device": torch.cuda.get_device_name(0),
+                      "power_limit": smi("power.limit"), "sm_clock_during_run": clocks, "iters": ITERS,
+                      "results": rows}))
+
+
+if __name__ == "__main__":
+    main()
