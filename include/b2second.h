@@ -65,6 +65,10 @@
  *   b2s_detection_loss, b2s_detection_loss_backward
  *                       VoxelNet.loss (second/pytorch/models/voxelnet.py:239-312, second/pytorch/core/losses.py:
  *                       135-294) and the autograd backward of its four differentiable scalars
+ *   b2s_optim_step      everything after loss.backward() in the training step (second/pytorch/train.py:299,323-325):
+ *                       lr_scheduler.step (torchplus/train/learning_schedules_fastai.py:43-56),
+ *                       torch.nn.utils.clip_grad_norm_, OptimWrapper.step (torchplus/train/fastai_optim.py:154-167) over
+ *                       torch.optim.Adam (second/pytorch/builder/optimizer_builder.py:68-87) and zero_grad
  */
 #ifndef B2SECOND_H_
 #define B2SECOND_H_
@@ -76,7 +80,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 207
+#define B2S_VERSION 208
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -91,11 +95,15 @@ extern "C" {
                                           b2s_db_sample: bad or overlapping point, box or candidate offsets (that
                                           part of the frame is treated as empty), a candidate object id outside the
                                           database or point offsets that disagree with it.  b2s_detection_loss: a
-                                          label outside [-1, num_class] (that anchor counts as not cared)        */
+                                          label outside [-1, num_class] (that anchor counts as not cared).
+                                          b2s_optim_step: the step counter is outside the hyper-parameter table (the
+                                          nearest row was used) or a chunk row is malformed (skipped)            */
 #define B2S_STATUS_AUG_BOX_CAP 64u     /* b2s_augment: a frame holds more than B2S_AUGMENT_MAX_BOXES ground truths; its
                                           boxes and points got no per-object noise                               */
 #define B2S_STATUS_DB_BOX_CAP 128u     /* b2s_db_sample: a frame's ground truths plus candidates exceed
                                           B2S_DBSAMPLE_MAX_BOXES; that frame got no samples                      */
+#define B2S_STATUS_OPT_NONFINITE 256u  /* b2s_optim_step: the gradient norm was inf or NaN; the step was applied as
+                                          torch applies it (parameters become NaN)                               */
 
 /* IEEE binary16 bit pattern (the tensor-core kernels' operand planes; torch.float16 storage) */
 typedef uint16_t b2s_half;
@@ -733,6 +741,40 @@ int b2s_detection_loss_backward(const float *box_preds, const float *cls_preds, 
                                 const float *importance, const float *anchors, int batch, int num_anchors,
                                 const b2s_loss_params *params, const float *norms, const float *d_reduced,
                                 float *d_box, float *d_cls, float *d_dir, void *stream);
+
+/* ---- optimizer step (second/pytorch/train.py:299,323-325) -------------------------------------------------------- */
+/* One training step's work after loss.backward(), for all parameter tensors in two kernels: the L2 norm of all
+ * gradients and g *= min(1, max_norm / (norm + 1e-6)) (torch.nn.utils.clip_grad_norm_, train.py:323); weight decay,
+ * decoupled (fixed_weight_decay: p *= 1 - wd * lr before Adam, torchplus/train/fastai_optim.py:157-166) or L2 inside
+ * Adam (g += wd * p); torch.optim.Adam's update with amsgrad off (optimizer_builder.py:68-76, train.py:324); zero_grad
+ * (train.py:325); and the schedule's advance (lr_scheduler.step, train.py:299).  All tensors are float32.
+ * The hyper-parameters that change per step come from device memory: hyper [settings->total_step,
+ * B2S_OPTIM_HYPER_COLS] float64, row s for the step taken when *step_dev == s: lr, beta1, 1 - beta1^(s+1),
+ * sqrt(1 - beta2^(s+1)), 1 - wd * lr.  *step_dev (int64) is read by the first kernel and written back + 1 by the
+ * second, so a captured call advances the schedule by itself when replayed; past the table the last row is used and
+ * B2S_STATUS_BAD_INPUT raised.  Settings, read on the host: */
+#define B2S_OPTIM_CHUNK 4096       /* elements of one tensor one CTA handles */
+#define B2S_OPTIM_HYPER_COLS 5
+typedef struct b2s_optim_params {
+    double weight_decay, beta2, eps;
+    double max_norm;               /* clip_grad_norm_'s max_norm */
+    long long total_step;          /* rows of hyper */
+    int decoupled;                 /* 1: fixed_weight_decay (p *= hyper[4]); 0: L2 (g += weight_decay * p) */
+    int zero_grad;                 /* 1: write zeros into every gradient after it is used */
+} b2s_optim_params;
+/* params, grads, exp_avg, exp_avg_sq: device arrays of num_tensors device pointers; a NULL grads entry is a parameter
+ * without gradient (decayed in the decoupled form, otherwise untouched, as torch skips it).  chunks: device int32
+ * [num_chunks, 4], 16-byte aligned, rows (tensor, first element, elements <= B2S_OPTIM_CHUNK, 0) that tile every
+ * tensor once; tensors whose four pointers are 16-byte aligned at a chunk's start move as 16-byte words.  total_norm:
+ * device float32 [1], the norm before clipping.  A non-finite norm propagates as in torch (a NaN norm makes every
+ * parameter NaN) and raises B2S_STATUS_OPT_NONFINITE.  Sums run in one fixed order (float64 partials per chunk, no float
+ * atomics) and every float32 operation is a round-to-nearest intrinsic, so results are bit-reproducible; no sync.
+ * workspace: b2s_optim_workspace_bytes(num_chunks) (host query) bytes. */
+size_t b2s_optim_workspace_bytes(int num_chunks);
+int b2s_optim_step(float *const *params, float *const *grads, float *const *exp_avg, float *const *exp_avg_sq,
+                   int num_tensors, const int *chunks, int num_chunks, const double *hyper, long long *step_dev,
+                   const b2s_optim_params *settings, float *total_norm, void *workspace, size_t workspace_bytes,
+                   unsigned *status_dev, void *stream);
 
 #ifdef __cplusplus
 }

@@ -151,7 +151,13 @@ SIGNATURES = {
     "b2s_detection_loss_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p,
                                             c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_void_p, c_void_p]),
+    "b2s_optim_workspace_bytes": (c_size_t, [c_int]),
+    "b2s_optim_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                               c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
 }
+
+OPTIM_CHUNK = 4096       # B2S_OPTIM_CHUNK
+OPTIM_HYPER_COLS = 5     # B2S_OPTIM_HYPER_COLS
 
 
 class LossParams(ctypes.Structure):
@@ -161,6 +167,13 @@ class LossParams(ctypes.Structure):
                 ("neg_cls_weight", ctypes.c_float), ("loc_weight", ctypes.c_float), ("cls_weight", ctypes.c_float),
                 ("dir_weight", ctypes.c_float), ("sin_factor", ctypes.c_float), ("dir_offset", ctypes.c_float),
                 ("num_dir_bins", c_int)]
+
+
+class OptimParams(ctypes.Structure):
+    """b2s_optim_params (include/b2second.h): the settings of b2s_optim_step, passed by host pointer."""
+    _fields_ = [("weight_decay", ctypes.c_double), ("beta2", ctypes.c_double), ("eps", ctypes.c_double),
+                ("max_norm", ctypes.c_double), ("total_step", ctypes.c_longlong), ("decoupled", c_int),
+                ("zero_grad", c_int)]
 
 
 class HeadSegment(ctypes.Structure):
@@ -242,7 +255,8 @@ STATUS_BITS = {1: "voxel overflow (more voxels than max_voxels; extra voxels dro
                    "candidate outside the database or a training label outside [-1, num_class]",
                64: "a frame holds more ground truths than the augmentation's per-frame cap (no object noise there)",
                128: "a frame's ground truths plus database candidates exceed the sampler's per-frame cap (no samples "
-                    "there)"}
+                    "there)",
+               256: "the gradient norm of an optimizer step was inf or NaN (the step was applied, as torch applies it)"}
 
 
 def status_message(word):
