@@ -196,7 +196,8 @@ int b2s_rulebook_conv(const int *coors_in, const int *num_in_dev, int cap_in, in
 /* SubM rulebook of the level b2s_rulebook_conv has JUST produced, read off the occupancy structure that call left in
  * `workspace` (same batch / shape, nothing else run on the workspace in between): coordinate -> row is a bit test +
  * popcount rank, no hash table.  Pass hash_keys_out = hash_vals_out = NULL to b2s_rulebook_conv when every SubM of
- * the produced level is built this way.  nbr as b2s_rulebook_subm. */
+ * the produced level is built this way.  nbr as b2s_rulebook_subm, but only its live rows are written (each whole,
+ * no prefill of the rest).  At most 27 kernel offsets. */
 int b2s_rulebook_subm_ranked(const int *coors, const int *num_rows_dev, int cap_rows, int batch, const int *shape,
                              const int *ksize, const int *dilation, const void *workspace, size_t workspace_bytes,
                              int *nbr, unsigned *row_mask /*[cap_rows] or NULL*/, void *stream);

@@ -181,10 +181,10 @@ class InferenceEngine:
                     rulebooks[key] = {"nbr": torch.empty(level.cap, K, dtype=torch.int32, device=dev)}
                     lyr["build_rb"] = True
                     # the strided conv right before this layer produced `level`: its occupancy bitmap is still in the
-                    # rulebook workspace, so this SubM table is built by rank lookups (b2s_rulebook_subm_ranked) and
-                    # the level needs no hash table
+                    # rulebook workspace, so this SubM table is built by rank lookups (b2s_rulebook_subm_ranked, up
+                    # to 27 kernel offsets) and the level needs no hash table
                     prev = self.layers[-1] if self.layers else None
-                    lyr["ranked"] = bool(prev is not None and not prev["subm"] and prev["out_level"] is level)
+                    lyr["ranked"] = bool(prev is not None and not prev["subm"] and prev["out_level"] is level and K <= 27)
                 else:
                     lyr["build_rb"] = False
                 lyr["rb"] = rulebooks[key]

@@ -295,42 +295,78 @@ __global__ void k_conv_scatter_nbr(const int *__restrict__ coors_in, const int *
 }
 
 // SubM neighbour table of a level whose occupancy structure (bitmap + wrow0, from the strided conv that produced it)
-// is still in the workspace: coordinate -> row is a bit test + rank, no hash probing.  Symmetric like k_subm_nbr: one
-// thread per (row, k < K/2) writes both directions.
-__global__ void k_subm_ranked(const int *__restrict__ coors, const int *__restrict__ n_dev, int cap_rows, ConvGeom g,
-                              const unsigned *__restrict__ bitmap, const int *__restrict__ wrow0, int *nbr,
-                              unsigned *row_mask)
+// is still in the workspace: coordinate -> row is a bit test + rank, no hash probing.  Whole rows: a thread per row
+// looks up all K entries of its row (the x-neighbours of one (dz, dy) mostly share a bitmap word), kRowsBatch offsets
+// at a time so their loads are in flight together; the warp stages its 32 rows in shared memory and stores them as
+// one contiguous block, and the row's offset mask is stored once.  Every live row is written whole, so there is no -1
+// memset of the table, no mirrored scattered store and no atomic.
+constexpr int kRowsMaxK = 27;                                       // offsets per row staged in shared memory
+constexpr int kRowsBatch = 7;                                       // offsets whose lookups are in flight together
+
+__global__ void __launch_bounds__(kThreads)
+k_subm_rows(const int *__restrict__ coors, const int *__restrict__ n_dev, int cap_rows, ConvGeom g,
+            const unsigned *__restrict__ bitmap, const int *__restrict__ wrow0, int *nbr, unsigned *row_mask)
 {
+    __shared__ int s_off[kRowsMaxK][3];                               // (dz, dy, dx) of every kernel offset
+    __shared__ int s_stage[kThreads / 32][32 * kRowsMaxK];
+    if (threadIdx.x < g.K) {
+        const int k = threadIdx.x;
+        s_off[k][0] = (k / (g.k[2] * g.k[1]) - g.k[0] / 2) * g.d[0];
+        s_off[k][1] = ((k / g.k[2]) % g.k[1] - g.k[1] / 2) * g.d[1];
+        s_off[k][2] = (k % g.k[2] - g.k[2] / 2) * g.d[2];
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    int *s_rows = s_stage[threadIdx.x >> 5];
     const int n = min(*n_dev, cap_rows);
     const int half = g.K / 2;
-    const long long total = (long long)n * (half + 1);
-    for (long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x; gid < total;
-         gid += (long long)gridDim.x * blockDim.x) {
-        int row = (int)(gid / (half + 1)), k = (int)(gid % (half + 1));
-        if (k == half) {
-            nbr[(size_t)row * g.K + half] = row;
-            if (row_mask) atomicOr(&row_mask[row], 1u << half);
-            continue;
-        }
-        int kx = k % g.k[2], ky = (k / g.k[2]) % g.k[1], kz = k / (g.k[2] * g.k[1]);
-        int4 c = *reinterpret_cast<const int4 *>(coors + (size_t)row * 4);
-        int z = c.y + (kz - g.k[0] / 2) * g.d[0];
-        int y = c.z + (ky - g.k[1] / 2) * g.d[1];
-        int x = c.w + (kx - g.k[2] / 2) * g.d[2];
-        if (z < 0 || z >= g.in_shape[0] || y < 0 || y >= g.in_shape[1] || x < 0 || x >= g.in_shape[2]) continue;
-        const unsigned long long key = b2s_flat_key(c.x, z, y, x, g.in_shape[0], g.in_shape[1], g.in_shape[2]);
-        const unsigned bits = __ldg(&bitmap[key >> 5]);
-        const unsigned bit = (unsigned)(key & 31);
-        if (!((bits >> bit) & 1u)) continue;
-        const int j = __ldg(&wrow0[key >> 5]) + __popc(bits & ((1u << bit) - 1u));
-        if (j < n) {
-            nbr[(size_t)row * g.K + k] = j;
-            nbr[(size_t)j * g.K + (g.K - 1 - k)] = row;
-            if (row_mask) {
-                atomicOr(&row_mask[row], 1u << k);
-                atomicOr(&row_mask[j], 1u << (g.K - 1 - k));
+    for (long long row0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) - lane; row0 < n;
+         row0 += (long long)gridDim.x * blockDim.x) {
+        const long long row = row0 + lane;
+        if (row < n) {
+            const int4 c = *reinterpret_cast<const int4 *>(coors + (size_t)row * 4);
+            unsigned m = 0u;
+            for (int k0 = 0; k0 < g.K; k0 += kRowsBatch) {
+                int wi[kRowsBatch];                                   // bitmap word (< 2^31, checked on the host)
+                unsigned bits[kRowsBatch];                            // its bits up to and including the cell
+#pragma unroll
+                for (int t = 0; t < kRowsBatch; ++t) {
+                    const int k = k0 + t;
+                    wi[t] = -1;
+                    if (k < g.K && k != half) {
+                        const int z = c.y + s_off[k][0], y = c.z + s_off[k][1], x = c.w + s_off[k][2];
+                        if (z >= 0 && z < g.in_shape[0] && y >= 0 && y < g.in_shape[1] && x >= 0 && x < g.in_shape[2]) {
+                            const unsigned long long key =
+                                b2s_flat_key(c.x, z, y, x, g.in_shape[0], g.in_shape[1], g.in_shape[2]);
+                            const unsigned bit = (unsigned)(key & 31);
+                            wi[t] = (int)(key >> 5);
+                            bits[t] = __ldg(&bitmap[wi[t]]) & (0xffffffffu >> (31 - bit));
+                            if (!(bits[t] >> bit)) wi[t] = -1;
+                        }
+                    }
+                }
+#pragma unroll
+                for (int t = 0; t < kRowsBatch; ++t) {
+                    const int k = k0 + t;
+                    int j = -1;
+                    if (k == half) {
+                        j = (int)row;
+                    } else if (wi[t] >= 0) {
+                        const int r = __ldg(&wrow0[wi[t]]) + __popc(bits[t]) - 1;
+                        if (r < n) j = r;
+                    }
+                    if (k < g.K) {
+                        s_rows[lane * g.K + k] = j;
+                        if (j >= 0) m |= 1u << k;
+                    }
+                }
             }
+            if (row_mask) row_mask[row] = m;
         }
+        __syncwarp();
+        const int cnt = (int)min(32ll, (long long)n - row0) * g.K;
+        for (int f = lane; f < cnt; f += 32) nbr[(size_t)row0 * g.K + f] = s_rows[f];
+        __syncwarp();
     }
 }
 
@@ -530,11 +566,11 @@ extern "C" int b2s_rulebook_subm_ranked(const int *coors, const int *num_rows_de
     ConvWorkspace w;
     size_t need = carve(&w, (char *)workspace, batch, shape);
     B2S_REQUIRE(workspace_bytes >= need, "b2s_rulebook_subm_ranked: workspace too small (%zu < %zu)", workspace_bytes, need);
+    B2S_REQUIRE(g.K <= kRowsMaxK, "b2s_rulebook_subm_ranked: at most %d kernel offsets (got %d)", kRowsMaxK, g.K);
+    B2S_REQUIRE(w.nwords < (1ll << 31), "b2s_rulebook_subm_ranked: grid of %lld cells too large", w.nwords * 32);
     if (cap_rows > 0) {
-        B2S_CUDA_OK(cudaMemsetAsync(nbr, 0xFF, sizeof(int) * (size_t)cap_rows * g.K, stream));
-        if (row_mask) B2S_CUDA_OK(cudaMemsetAsync(row_mask, 0, sizeof(unsigned) * (size_t)cap_rows, stream));
-        k_subm_ranked<<<bounded_grid((long long)cap_rows * (g.K / 2 + 1), kThreads), kThreads, 0, stream>>>(
-            coors, num_rows_dev, cap_rows, g, w.bitmap, w.wrow0, nbr, row_mask);
+        k_subm_rows<<<bounded_grid(cap_rows, kThreads), kThreads, 0, stream>>>(coors, num_rows_dev, cap_rows, g, w.bitmap,
+                                                                               w.wrow0, nbr, row_mask);
         B2S_LAUNCH_OK();
     }
     return 0;
