@@ -69,6 +69,11 @@
  *                       lr_scheduler.step (torchplus/train/learning_schedules_fastai.py:43-56),
  *                       torch.nn.utils.clip_grad_norm_, OptimWrapper.step (torchplus/train/fastai_optim.py:154-167) over
  *                       torch.optim.Adam (second/pytorch/builder/optimizer_builder.py:68-87) and zero_grad
+ *   b2s_train_metrics   VoxelNet.update_metrics (second/pytorch/models/voxelnet.py:654-679, torchplus/metrics.py) and the
+ *                       log figures of train.py:335-373
+ *   b2s_pack_sparse_weights
+ *                       the tensor-core weight planes of a sparse conv in training (tc.pack_sparse_weights, pow2_scale,
+ *                       split_f16 in SparseConvolution._tc_weights / _dgrad_weights) on the device
  */
 #ifndef B2SECOND_H_
 #define B2SECOND_H_
@@ -80,7 +85,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 208
+#define B2S_VERSION 209
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -97,7 +102,8 @@ extern "C" {
                                           database or point offsets that disagree with it.  b2s_detection_loss: a
                                           label outside [-1, num_class] (that anchor counts as not cared).
                                           b2s_optim_step: the step counter is outside the hyper-parameter table (the
-                                          nearest row was used) or a chunk row is malformed (skipped)            */
+                                          nearest row was used) or a chunk row is malformed (skipped).
+                                          b2s_train_metrics: a label outside [-1, num_class]                      */
 #define B2S_STATUS_AUG_BOX_CAP 64u     /* b2s_augment: a frame holds more than B2S_AUGMENT_MAX_BOXES ground truths; its
                                           boxes and points got no per-object noise                               */
 #define B2S_STATUS_DB_BOX_CAP 128u     /* b2s_db_sample: a frame's ground truths plus candidates exceed
@@ -776,6 +782,67 @@ int b2s_optim_step(float *const *params, float *const *grads, float *const *exp_
                    int num_tensors, const int *chunks, int num_chunks, const double *hyper, long long *step_dev,
                    const b2s_optim_params *settings, float *total_norm, void *workspace, size_t workspace_bytes,
                    unsigned *status_dev, void *stream);
+
+/* ---- training metrics (second/pytorch/models/voxelnet.py:654-679, second/pytorch/train.py:327-373) -------------- */
+/* One step of VoxelNet.update_metrics through torchplus/metrics.py (Accuracy, PrecisionRecall, Scalar) with sigmoid
+ * scores and background encoded as zeros, plus the log figures train.py:335-373 computes.  Settings, read on the
+ * host: */
+#define B2S_METRICS_MAX_THRESHOLDS 16
+#define B2S_METRICS_MAX_CODE 8
+typedef struct b2s_metrics_params {
+    int num_thresholds;
+    float thresholds[B2S_METRICS_MAX_THRESHOLDS];   /* rpn_metrics.thresholds as float32 (score > threshold) */
+    float acc_threshold;                            /* rpn_acc._threshold (0.5) */
+} b2s_metrics_params;
+/* The reference's running buffers (device float32, updated in place): rpn_acc.total / count [1],
+ * rpn_metrics.prec_total / prec_count / rec_total / rec_count [num_thresholds], rpn_cls_loss.total / count and
+ * rpn_loc_loss.total / count [1].  Pointers read on the host. */
+typedef struct b2s_metrics_buffers {
+    float *acc_total, *acc_count;
+    float *prec_total, *prec_count, *rec_total, *rec_count;
+    float *cls_total, *cls_count, *loc_total, *loc_count;
+} b2s_metrics_buffers;
+/* record: float32 [B2S_METRICS_RECORD_HEAD + 2 * num_thresholds]; after the head, prec[T] then rec[T] */
+#define B2S_METRICS_REC_ACC 0           /* rpn_acc.total / count */
+#define B2S_METRICS_REC_CLS 1           /* rpn_cls_loss.total / count */
+#define B2S_METRICS_REC_CLS_RT 2        /* *cls_loss */
+#define B2S_METRICS_REC_LOC 3           /* rpn_loc_loss.total / count */
+#define B2S_METRICS_REC_LOC_RT 4        /* *loc_loss */
+#define B2S_METRICS_REC_CLS_POS_RT 5    /* *cls_pos_loss (0 when NULL) */
+#define B2S_METRICS_REC_CLS_NEG_RT 6    /* *cls_neg_loss (0 when NULL) */
+#define B2S_METRICS_REC_DIR_RT 7        /* *dir_loss (0 when NULL) */
+#define B2S_METRICS_REC_NUM_POS 8       /* labels > 0 in frame 0 */
+#define B2S_METRICS_REC_NUM_NEG 9       /* labels == 0 in frame 0 */
+#define B2S_METRICS_REC_NUM_ANCHORS 10  /* anchors_mask set in frame 0 (num_anchors when NULL) */
+#define B2S_METRICS_REC_LOC_ELEM 11     /* [B2S_METRICS_MAX_CODE]: loc_loss_elem[:, :, j] summed / batch (0 past code) */
+#define B2S_METRICS_RECORD_HEAD 19
+/* Inputs: cls_preds [batch, A, num_class] float32; labels [batch, A] int32 (labels_int64 0) or int64 (1); cared
+ * uint8 [batch, A] (the loss's `cared`, the metrics' weights); cls_loss, loc_loss: device float32 scalars
+ * (cls_loss_reduced, loc_loss_reduced).  Optional (NULL): loc_loss_elem [batch, A, code_size] (the loss's per-element
+ * loc_loss), anchors_mask uint8 [batch, A], and the device scalars cls_pos_loss, cls_neg_loss, dir_loss.  The score is
+ * max_c sigmoid(pred_c) with torch's float32 sigmoid; Accuracy counts pred == label over all anchors, unweighted, as
+ * Accuracy.forward does.  A label outside [-1, num_class] raises B2S_STATUS_BAD_INPUT (it is counted as the reference
+ * counts it).  Two kernels: one pass over cls_preds, labels and cared with per-CTA integer counts, then one CTA that adds
+ * them in a fixed order, updates the buffers and writes the record; bit-reproducible, no sync.  Per-step counts must
+ * stay below 2^24 (as the reference's float32 sums need).  workspace: b2s_train_metrics_workspace_bytes(batch, A) bytes. */
+size_t b2s_train_metrics_workspace_bytes(int batch, int num_anchors);
+int b2s_train_metrics(const float *cls_preds, int num_class, const void *labels, int labels_int64, const uint8_t *cared,
+                      int batch, int num_anchors, const b2s_metrics_params *params, const float *cls_loss,
+                      const float *loc_loss, const float *loc_loss_elem, int code_size, const uint8_t *anchors_mask,
+                      const float *cls_pos_loss, const float *cls_neg_loss, const float *dir_loss,
+                      const b2s_metrics_buffers *buffers, float *record, void *workspace, size_t workspace_bytes,
+                      unsigned *status_dev, void *stream);
+
+/* ---- sparse conv weights on the tensor pipe (b2second/tc.py: pack_sparse_weights, pow2_scale, split_f16) -------- */
+/* w [K, cin, cout] float32 (spconv's layout) -> the fp16 hi/lo planes b2s_sparse_conv_tc(_plan) takes as its B operand,
+ * bit-identical to tc.split_f16(tc.pack_sparse_weights(L), tc.pow2_scale(...)) with L[k] = w[k] (transpose 0) or
+ * L[k] = w[flip ? K-1-k : k]^T (transpose 1: the input gradient's weights).  With n_in x n_out the channels of L, the
+ * planes are [ceil(K / P), n_out, 64] halves, P = 64 / n_in' kernel offsets per 128-byte K block, n_in' = n_in padded to
+ * 8 (n_in in 1..8, 16, 32, 64).  scale_dev: device float32 [3]; [0] = s, the power of two with max|w| * s in
+ * (2^12, 2^13] (1 for zero or non-finite weights), [1] = 1/s, [2] scratch.  A memset and two kernels (max|w| as integer
+ * atomicMax on the bit patterns, then the pack and split); no sync. */
+int b2s_pack_sparse_weights(const float *w, int K, int cin, int cout, int transpose, int flip, b2s_half *hi,
+                            b2s_half *lo, float *scale_dev, void *stream);
 
 #ifdef __cplusplus
 }

@@ -591,8 +591,19 @@ class VoxelNet(nn.Module):
             self._anchors_np = generate_anchors(self.cfg)
         return self._anchors_np
 
+    def update_global_step(self):
+        """voxelnet.py:230-237"""
+        self.global_step += 1
+
+    def get_global_step(self):
+        return int(self.global_step.cpu().numpy()[0])
+
+    def clear_global_step(self):
+        self.global_step.zero_()
+
     def load_reference_state_dict(self, sd):
-        """load a reference checkpoint; training-metric buffers (rpn_acc.*, rpn_metrics.* ...) are skipped."""
+        """load a reference checkpoint; training-metric buffers (rpn_acc.*, rpn_metrics.* ...) load once
+        b2second.metrics.enable_gpu_metrics(net) has added them, and are skipped before."""
         own = self.state_dict()
         missing = [k for k in own if k not in sd]
         if missing:

@@ -1,7 +1,8 @@
 // sparse_grad.cu -- backward of the sparse convolution and of dense() (include/b2second.h, "sparse convolution
 // backward"): the weight gradient (b2s_sparse_conv_wgrad), the input-side neighbour table of a strided conv
 // (b2s_rulebook_transpose), the gather from a BEV gradient back into rows (b2s_from_bev) and the automatically scaled
-// 3xF16 split of a gradient (b2s_split_f16_autoscale).  The input gradient itself is the forward kernels on a
+// 3xF16 split of a gradient (b2s_split_f16_autoscale) and the packed, scaled weight planes of a layer in training
+// (b2s_pack_sparse_weights).  The input gradient itself is the forward kernels on a
 // transposed table (sparse_conv.cu, sparse_conv_tc.cu).
 //
 // Weight gradient in fp32 (b2s_sparse_conv_wgrad; the tensor-pipe version is further down): dW[k][ci][co] =
@@ -175,15 +176,62 @@ __global__ void k_absmax(const float *__restrict__ x, const int *__restrict__ n_
     if ((threadIdx.x & 31) == 0 && m) atomicMax(amax_bits, m);
 }
 
-// 2^e with max|x| * 2^e in (2^12, 2^13] (b2second/tc.py: pow2_scale), e clamped so that 2^e and 2^-e are normal floats
-__device__ __forceinline__ int autoscale_exponent(unsigned amax_bits)
+// e with max|x| * 2^e in (2^12, 2^13] (b2second/tc.py: pow2_scale), 0 for zero or non-finite max|x|
+__device__ __forceinline__ int pow2_exponent(unsigned amax_bits)
 {
     const float m = __uint_as_float(amax_bits);
     if (amax_bits == 0 || amax_bits >= 0x7F800000u) return 0;
     int ex;
     const float f = frexpf(m, &ex);                 // m = f * 2^ex, f in [0.5, 1)
     const int ceil_log2 = f == 0.5f ? ex - 1 : ex;
-    return min(max(13 - ceil_log2, -126), 126);
+    return 13 - ceil_log2;
+}
+
+// pow2_exponent clamped so that 2^e and 2^-e are normal floats
+__device__ __forceinline__ int autoscale_exponent(unsigned amax_bits)
+{
+    return min(max(pow2_exponent(amax_bits), -126), 126);
+}
+
+// one thread per 8 columns of a packed row: out[kb, o, p * n_in' + i] = L[kb * P + p, i, o] * s, zero past K and n_in
+// (tc.pack_sparse_weights), split into hi / lo.  s is the float32 the host path multiplies by: float(2.0 ** e).
+__global__ void k_pack_sparse_weights(const float *__restrict__ w, int K, int cin, int cout, int transpose, int flip,
+                                      int n_in, int n_in_pad, int n_out, int nkb, __half *__restrict__ hi,
+                                      __half *__restrict__ lo, float *__restrict__ scale_dev)
+{
+    const int e = pow2_exponent(*reinterpret_cast<const volatile unsigned *>(scale_dev + 2));
+    const float s = (float)ldexp(1.0, e);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        scale_dev[0] = s;
+        scale_dev[1] = (float)ldexp(1.0, -e);
+    }
+    const int pack = b2s_tc::BLOCK_K / n_in_pad;
+    const long long n = (long long)nkb * n_out * (b2s_tc::BLOCK_K / 8);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long row = i / (b2s_tc::BLOCK_K / 8);            // (kb, o)
+        const int c0 = (int)(i - row * (b2s_tc::BLOCK_K / 8)) * 8;
+        const int kb = (int)(row / n_out), o = (int)(row - (long long)kb * n_out);
+        float v[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int col = c0 + j, p = col / n_in_pad, ci = col - p * n_in_pad, k = kb * pack + p;
+            float x = 0.f;
+            if (k < K && ci < n_in) {
+                const int ks = flip ? K - 1 - k : k;
+                x = transpose ? __ldg(&w[((size_t)ks * cin + o) * cout + ci]) : __ldg(&w[((size_t)ks * cin + ci) * cout + o]);
+            }
+            v[j] = __fmul_rn(x, s);
+        }
+        uint32_t h[4], l[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const uint32_t pa = b2s_tc::split_f16(v[2 * j]), pb = b2s_tc::split_f16(v[2 * j + 1]);
+            h[j] = __byte_perm(pa, pb, 0x5410);
+            l[j] = __byte_perm(pa, pb, 0x7632);
+        }
+        *reinterpret_cast<uint4 *>(hi + row * b2s_tc::BLOCK_K + c0) = make_uint4(h[0], h[1], h[2], h[3]);
+        *reinterpret_cast<uint4 *>(lo + row * b2s_tc::BLOCK_K + c0) = make_uint4(l[0], l[1], l[2], l[3]);
+    }
 }
 
 __global__ void k_split_f16_scaled(const float *__restrict__ x, __half *__restrict__ hi, __half *__restrict__ lo,
@@ -242,7 +290,7 @@ k_wgrad_tc(const __half *__restrict__ x_hi, const __half *__restrict__ x_lo, int
 {
     using namespace b2s_tc;
     constexpr int N = COUT;
-    constexpr int PACK = BLOCK_K / CIN;
+    constexpr int PACK = b2s_tc::BLOCK_K / CIN;
     constexpr int A_BYTES = 64 * 128;
     constexpr int R = N;                                     // accumulator registers: 64 rows x 2N columns
     extern __shared__ uint8_t smem_raw[];
@@ -501,6 +549,32 @@ extern "C" int b2s_split_f16_autoscale(const float *x, b2s_half *hi, b2s_half *l
     k_split_f16_scaled<<<grid_for((long long)cap_rows * (out_channels / 8)), kThreads, 0, stream>>>(
         x, reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo), num_rows_dev, cap_rows, row_floats,
         out_channels, out_stride, scale_dev);
+    B2S_LAUNCH_OK();
+    return 0;
+}
+
+extern "C" int b2s_pack_sparse_weights(const float *w, int K, int cin, int cout, int transpose, int flip, b2s_half *hi,
+                                       b2s_half *lo, float *scale_dev, void *stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const int n_in = transpose ? cout : cin, n_out = transpose ? cin : cout;
+    const int n_in_pad = n_in <= 8 ? 8 : n_in;
+    B2S_REQUIRE(K >= 1 && cin >= 1 && cout >= 1 && n_in >= 1 && (n_in_pad == 8 || n_in_pad == 16 || n_in_pad == 32 ||
+                                                                  n_in_pad == 64),
+                "b2s_pack_sparse_weights: the packed input channels must be 1..8, 16, 32 or 64 (got %d)", n_in);
+    B2S_REQUIRE(transpose == 0 || transpose == 1, "b2s_pack_sparse_weights: transpose must be 0 or 1");
+    B2S_REQUIRE(w && hi && lo && scale_dev, "b2s_pack_sparse_weights: w, hi, lo and scale_dev required");
+    B2S_REQUIRE(((uintptr_t)hi & 15) == 0 && ((uintptr_t)lo & 15) == 0,
+                "b2s_pack_sparse_weights: planes must be 16-byte aligned");
+    const int pack = b2s_tc::BLOCK_K / n_in_pad, nkb = (K + pack - 1) / pack;
+    const long long n = (long long)K * cin * cout;
+    B2S_REQUIRE(n < (1ll << 31), "b2s_pack_sparse_weights: weight too large");
+    B2S_CUDA_OK(cudaMemsetAsync(scale_dev + 2, 0, sizeof(float), stream));
+    k_absmax<<<grid_for(n), kThreads, 0, stream>>>(w, nullptr, 1, (int)n, reinterpret_cast<unsigned *>(scale_dev + 2));
+    B2S_LAUNCH_OK();
+    k_pack_sparse_weights<<<grid_for((long long)nkb * n_out * (b2s_tc::BLOCK_K / 8)), kThreads, 0, stream>>>(
+        w, K, cin, cout, transpose, flip ? 1 : 0, n_in, n_in_pad, n_out, nkb, reinterpret_cast<__half *>(hi),
+        reinterpret_cast<__half *>(lo), scale_dev);
     B2S_LAUNCH_OK();
     return 0;
 }

@@ -299,6 +299,24 @@ class SparseSequential(SparseModule):
         return input
 
 
+def _pack_tc_weights(w, transpose=False, flip=False):
+    """fp32 weight [K, Cin, Cout] -> (hi, lo, s, 1/s): the fp16 planes of W[k] (transpose: W[k]^T, flip: W[K-1-k]^T) in
+    the tensor-core kernel's packed layout, pre-scaled by the power of two s of b2second.tc.pow2_scale, with s and 1/s as
+    [1] device tensors.  b2s_pack_sparse_weights reduces max|w| on the device, so nothing is read on the host; the
+    planes and the scale are bit for bit tc.split_f16(tc.pack_sparse_weights(...), tc.pow2_scale(...))."""
+    lib = _lib.load()
+    K, cin, cout = (int(v) for v in w.shape)
+    n_in, n_out = (cout, cin) if transpose else (cin, cout)
+    n_in_pad = 8 if n_in <= 8 else n_in
+    pack = 64 // n_in_pad
+    hi = torch.empty((K + pack - 1) // pack, n_out, 64, dtype=torch.float16, device=w.device)
+    lo = torch.empty_like(hi)
+    sc = torch.empty(3, dtype=torch.float32, device=w.device)
+    _lib.check(lib.b2s_pack_sparse_weights(_lib.ptr(w), K, cin, cout, int(transpose), int(flip), _lib.ptr(hi),
+                                           _lib.ptr(lo), _lib.ptr(sc), _lib.stream()), "b2s_pack_sparse_weights")
+    return hi, lo, sc[0:1], sc[1:2]
+
+
 def _triple(v):
     if isinstance(v, (list, tuple, np.ndarray)):
         assert len(v) == 3
@@ -342,20 +360,17 @@ class SparseConvolution(SparseModule):
             nn.init.uniform_(self.bias, -bound, bound)
 
     def _tc_weights(self, cin_tc):
-        """fp16 hi/lo planes of the (power-of-two scaled) weight in the tensor-core kernel's layout; cached until the
-        parameter changes."""
-        from b2second import tc as _tc
+        """fp16 hi/lo planes of the (power-of-two scaled) weight in the tensor-core kernel's layout, the scale as a [1]
+        device tensor and its inverse per output channel; cached until the parameter changes."""
         w = self.weight
         key = (w.data_ptr(), w._version, str(w.device))
         cached = getattr(self, "_b2s_tc_w", None)
         if cached is None or cached[0] != key:
             K = int(np.prod(self.kernel_size))
             with torch.no_grad():
-                wp = _tc.pack_sparse_weights(w.detach().float().contiguous().view(K, self.in_channels,
-                                                                                 self.out_channels))
-                ws = _tc.pow2_scale(wp)
-                hi, lo = _tc.split_f16(wp, ws)
-                inv = torch.full((self.out_channels,), 1.0 / ws, dtype=torch.float32, device=w.device)
+                hi, lo, ws, inv = _pack_tc_weights(w.detach().float().contiguous().view(K, self.in_channels,
+                                                                                        self.out_channels))
+                inv = inv.expand(self.out_channels).contiguous()
             cached = (key, hi, lo, ws, inv)
             self._b2s_tc_w = cached
         return cached[1:]
@@ -503,18 +518,15 @@ class SparseConvolution(SparseModule):
 
     def _dgrad_weights(self, w, flip):
         """packed fp16 hi/lo planes of W'[k] = W[k]^T (flip: W[K-1-k]^T) for the tensor-pipe input gradient, with their
-        power-of-two scale; cached until the weight changes (one scale measurement per weight version)."""
-        from b2second import tc as _tc
+        power-of-two scale as a [1] device tensor; cached until the weight changes (one scale measurement per weight
+        version)."""
         key = (w.data_ptr(), w._version, str(w.device), flip)
         cached = getattr(self, "_b2s_tc_wt", None)
         if cached is None or cached[0] != key:
             K = int(np.prod(self.kernel_size))
             with torch.no_grad():
-                wt = w.detach().float().reshape(K, self.in_channels, self.out_channels)
-                wt = (wt.flip(0) if flip else wt).transpose(1, 2).contiguous()
-                wp = _tc.pack_sparse_weights(wt)
-                ws = _tc.pow2_scale(wp)
-                hi, lo = _tc.split_f16(wp, ws)
+                wk = w.detach().float().contiguous().view(K, self.in_channels, self.out_channels)
+                hi, lo, ws, _ = _pack_tc_weights(wk, transpose=True, flip=flip)
             cached = (key, hi, lo, ws)
             self._b2s_tc_wt = cached
         return cached[1:]

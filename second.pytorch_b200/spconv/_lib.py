@@ -154,6 +154,12 @@ SIGNATURES = {
     "b2s_optim_workspace_bytes": (c_size_t, [c_int]),
     "b2s_optim_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "b2s_train_metrics_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "b2s_train_metrics": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                  c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_size_t, c_void_p, c_void_p]),
+    "b2s_pack_sparse_weights": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                        c_void_p]),
 }
 
 OPTIM_CHUNK = 4096       # B2S_OPTIM_CHUNK
@@ -174,6 +180,26 @@ class OptimParams(ctypes.Structure):
     _fields_ = [("weight_decay", ctypes.c_double), ("beta2", ctypes.c_double), ("eps", ctypes.c_double),
                 ("max_norm", ctypes.c_double), ("total_step", ctypes.c_longlong), ("decoupled", c_int),
                 ("zero_grad", c_int)]
+
+
+METRICS_MAX_THRESHOLDS = 16   # B2S_METRICS_MAX_THRESHOLDS
+METRICS_MAX_CODE = 8          # B2S_METRICS_MAX_CODE
+METRICS_RECORD_HEAD = 19      # B2S_METRICS_RECORD_HEAD; the B2S_METRICS_REC_* slots in order:
+METRICS_REC = ("rpn_acc", "cls_loss", "cls_loss_rt", "loc_loss", "loc_loss_rt", "cls_pos_rt", "cls_neg_rt", "dir_rt",
+               "num_pos", "num_neg", "num_anchors")
+METRICS_REC_LOC_ELEM = 11     # B2S_METRICS_REC_LOC_ELEM
+
+
+class MetricsParams(ctypes.Structure):
+    """b2s_metrics_params (include/b2second.h): the settings of b2s_train_metrics, passed by host pointer."""
+    _fields_ = [("num_thresholds", c_int), ("thresholds", ctypes.c_float * METRICS_MAX_THRESHOLDS),
+                ("acc_threshold", ctypes.c_float)]
+
+
+class MetricsBuffers(ctypes.Structure):
+    """b2s_metrics_buffers (include/b2second.h): device pointers of the reference's running metric buffers."""
+    _fields_ = [(n, c_void_p) for n in ("acc_total", "acc_count", "prec_total", "prec_count", "rec_total", "rec_count",
+                                        "cls_total", "cls_count", "loc_total", "loc_count")]
 
 
 class HeadSegment(ctypes.Structure):
