@@ -74,6 +74,9 @@
  *   b2s_pack_sparse_weights
  *                       the tensor-core weight planes of a sparse conv in training (tc.pack_sparse_weights, pow2_scale,
  *                       split_f16 in SparseConvolution._tc_weights / _dgrad_weights) on the device
+ *   b2s_split_halo_f16_autoscale, b2s_pack_conv2d_weights, b2s_conv2d_wgrad_tc
+ *                       forward and backward of the RPN's 3x3 stride-1 nn.Conv2d layers in training (rpn.py:486-495;
+ *                       cuDNN's convolution and its two backward convolutions), with b2s_conv2d_tc_ex
  */
 #ifndef B2SECOND_H_
 #define B2SECOND_H_
@@ -85,7 +88,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 209
+#define B2S_VERSION 210
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -843,6 +846,36 @@ int b2s_train_metrics(const float *cls_preds, int num_class, const void *labels,
  * atomicMax on the bit patterns, then the pack and split); no sync. */
 int b2s_pack_sparse_weights(const float *w, int K, int cin, int cout, int transpose, int flip, b2s_half *hi,
                             b2s_half *lo, float *scale_dev, void *stream);
+
+/* ---- dense RPN training: 3x3 stride-1 pad-1 convolutions on the tensor pipe (csrc/conv_train.cu) ------------------
+ * Forward y = conv(x, W) and input gradient dX = conv(dY, W') with W'[tap] = W[8 - tap]^T are b2s_conv2d_tc_ex
+ * launches (kh = kw = 3, stride 1, pad 1, fp32 output: out_lo NULL) on the planes below; the weight gradient is
+ * b2s_conv2d_wgrad_tc.  No entry point syncs, so a training step that uses them can be captured. */
+/* fp32 map x, [B, C, H, W] (layout B2S_LAYOUT_NCHW) or [B, H, W, C] (B2S_LAYOUT_NHWC, 16-byte aligned) -> x * 2^e as
+ * fp16 hi/lo planes [B, H+2, W+2, C] with a zero halo (the input b2s_conv2d_tc_ex and b2s_conv2d_wgrad_tc read), with e
+ * picked on the device from max|x| by the b2s_split_f16_autoscale rule.  C multiple of 8.  scale_dev [2] floats: [0] <-
+ * 2^-e, [1] workspace.  A non-finite x raises B2S_STATUS_F16_RANGE (status_dev may be NULL).  A memset, two kernels. */
+int b2s_split_halo_f16_autoscale(const float *x, int layout, int batch, int C, int H, int W, b2s_half *hi, b2s_half *lo,
+                                 float *scale_dev, unsigned *status_dev, void *stream);
+/* torch weight w [cout, cin, 3, 3] fp32 -> the b2s_conv2d_tc_ex weight planes, scaled by the power of two s with
+ * max|w| * s in (2^12, 2^13] (as b2s_pack_sparse_weights; scale_dev [3]: [0] = s, [1] = 1/s, [2] scratch).
+ * transpose 0: L[tap][o][i] = w[o][i][tap] (n_out = cout, n_in = cin, the forward); transpose 1: L[tap][o][i] =
+ * w[i][o][8 - tap] (n_out = cin, n_in = cout, the input gradient).  Planes [G][9][n_pad][n_in] halves with G =
+ * ceil(n_out / 128) launches of up to 128 output channels, n_pad = min(n_out, 128), zero rows past n_out.  cin, cout
+ * multiples of 64.  The epilogue scale of a launch is (the input planes' 2^-e) * (1/s). */
+int b2s_pack_conv2d_weights(const float *w, int cout, int cin, int transpose, b2s_half *hi, b2s_half *lo,
+                            float *scale_dev, void *stream);
+/* dW[co][ci][ky][kx] = sum_px dY[px][co] * X[px + (ky - 1, kx - 1)][ci] for a 3x3 stride-1 pad-1 conv, in torch's layout
+ * [Cout, Cin, 3, 3] fp32, from the halo planes of b2s_split_halo_f16_autoscale (x [B, H+2, W+2, Cin], dout
+ * [B, H+2, W+2, Cout], both halos zero), times both planes' 2^-e (x_scale_dev[0] * dout_scale_dev[0], applied as one
+ * exponent).  Cin multiple of 64, Cout 64, 128 or 256.  wgmma with MN-major operands fed by TMA from the planes, 3xF16
+ * (dY_hi*X_hi + dY_hi*X_lo + dY_lo*X_hi), fp32 chains of 12 MMAs drained with round-to-nearest adds.  Deterministic:
+ * per-slab partials of 2048 pixels (workspace) added in slab order by a second launch, no float atomics. */
+size_t b2s_conv2d_wgrad_tc_workspace_bytes(int batch, int H, int W, int Cin, int Cout);
+int b2s_conv2d_wgrad_tc(const b2s_half *x_hi, const b2s_half *x_lo, const b2s_half *dout_hi, const b2s_half *dout_lo,
+                        int batch, int H, int W, int Cin, int Cout, const float *x_scale_dev,
+                        const float *dout_scale_dev, float *dweight, void *workspace, size_t workspace_bytes,
+                        void *stream);
 
 #ifdef __cplusplus
 }

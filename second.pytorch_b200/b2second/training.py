@@ -6,6 +6,7 @@ same way ``fastpath.accelerate(net)`` is the opt-in for the fused inference engi
 
     net = training.enable_sparse_backward(net)
     net = loss.enable_gpu_loss(net)               # b2second.loss: VoxelNet.loss on the GPU
+    net = training.enable_rpn_training(net)       # the RPN's 3x3 stride-1 convs on the tensor pipe
     net.train()
     loss = net(example)["loss"]; loss.backward()
 
@@ -31,3 +32,12 @@ def enable_sparse_backward(module):
         if isinstance(m, sp.SparseConvolution):
             m._b2s_backward = True
     return module
+
+
+def enable_rpn_training(net):
+    """train the RPN's 3x3 stride-1 ``nn.Conv2d`` layers under ``net.rpn`` on the tensor pipe (b2second.rpn_train):
+    forward, input gradient and weight gradient in 3xF16 on wgmma, fp32-grade.  Layers it does not cover (stride-2
+    convs, deblocks, heads) stay torch; BatchNorm2d and ReLU run as the torch modules that follow the conv.  Module
+    classes, state-dict keys and ``eval()`` are unchanged; idempotent.  Returns ``net``."""
+    from . import rpn_train
+    return rpn_train.enable(net)

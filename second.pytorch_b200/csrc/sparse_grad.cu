@@ -2,7 +2,8 @@
 // backward"): the weight gradient (b2s_sparse_conv_wgrad), the input-side neighbour table of a strided conv
 // (b2s_rulebook_transpose), the gather from a BEV gradient back into rows (b2s_from_bev) and the automatically scaled
 // 3xF16 split of a gradient (b2s_split_f16_autoscale) and the packed, scaled weight planes of a layer in training
-// (b2s_pack_sparse_weights).  The input gradient itself is the forward kernels on a
+// (b2s_pack_sparse_weights), and with the same scale rule the weight planes of a dense 3x3 RPN layer in training
+// (b2s_pack_conv2d_weights, used with conv_train.cu).  The input gradient itself is the forward kernels on a
 // transposed table (sparse_conv.cu, sparse_conv_tc.cu).
 //
 // Weight gradient in fp32 (b2s_sparse_conv_wgrad; the tensor-pipe version is further down): dW[k][ci][co] =
@@ -14,6 +15,7 @@
 // on the table and the values, never on scheduling.
 #include <cuda_fp16.h>
 
+#include "autoscale.cuh"
 #include "tc_common.cuh"
 
 namespace {
@@ -162,37 +164,6 @@ __global__ void k_from_bev(const float *__restrict__ dmap, const int *__restrict
     }
 }
 
-// max |x| over the live rows as the bit pattern of a non-negative float (ordered like unsigned ints): integer atomicMax,
-// so the result does not depend on the order.  NaN compares above +inf and is treated as "not finite" below.
-__global__ void k_absmax(const float *__restrict__ x, const int *__restrict__ n_rows_dev, int cap_rows, int row_floats,
-                         unsigned *__restrict__ amax_bits)
-{
-    const long long n = (long long)(n_rows_dev ? min(*n_rows_dev, cap_rows) : cap_rows) * row_floats;
-    unsigned m = 0;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        m = max(m, __float_as_uint(__ldg(&x[i])) & 0x7FFFFFFFu);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0 && m) atomicMax(amax_bits, m);
-}
-
-// e with max|x| * 2^e in (2^12, 2^13] (b2second/tc.py: pow2_scale), 0 for zero or non-finite max|x|
-__device__ __forceinline__ int pow2_exponent(unsigned amax_bits)
-{
-    const float m = __uint_as_float(amax_bits);
-    if (amax_bits == 0 || amax_bits >= 0x7F800000u) return 0;
-    int ex;
-    const float f = frexpf(m, &ex);                 // m = f * 2^ex, f in [0.5, 1)
-    const int ceil_log2 = f == 0.5f ? ex - 1 : ex;
-    return 13 - ceil_log2;
-}
-
-// pow2_exponent clamped so that 2^e and 2^-e are normal floats
-__device__ __forceinline__ int autoscale_exponent(unsigned amax_bits)
-{
-    return min(max(pow2_exponent(amax_bits), -126), 126);
-}
-
 // one thread per 8 columns of a packed row: out[kb, o, p * n_in' + i] = L[kb * P + p, i, o] * s, zero past K and n_in
 // (tc.pack_sparse_weights), split into hi / lo.  s is the float32 the host path multiplies by: float(2.0 ** e).
 __global__ void k_pack_sparse_weights(const float *__restrict__ w, int K, int cin, int cout, int transpose, int flip,
@@ -231,6 +202,47 @@ __global__ void k_pack_sparse_weights(const float *__restrict__ w, int K, int ci
         }
         *reinterpret_cast<uint4 *>(hi + row * b2s_tc::BLOCK_K + c0) = make_uint4(h[0], h[1], h[2], h[3]);
         *reinterpret_cast<uint4 *>(lo + row * b2s_tc::BLOCK_K + c0) = make_uint4(l[0], l[1], l[2], l[3]);
+    }
+}
+
+// dense 3x3 weights, one thread per 8 columns of a packed row: out[g, tap, o, i] = L[tap][g * 128 + o][i] * s with
+// L[tap][o][i] = W[o][i][tap] (transpose 0: the forward) or W[i][o][8 - tap] (transpose 1: the input gradient), W the
+// torch weight [cout, cin, 3, 3]; rows past n_out of the last group are zero.  s as in k_pack_sparse_weights.
+__global__ void k_pack_conv2d_weights(const float *__restrict__ w, int cout, int cin, int transpose, int n_in,
+                                      int n_out, int n_pad, int groups, __half *__restrict__ hi, __half *__restrict__ lo,
+                                      float *__restrict__ scale_dev)
+{
+    const int e = pow2_exponent(*reinterpret_cast<const volatile unsigned *>(scale_dev + 2));
+    const float s = (float)ldexp(1.0, e);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        scale_dev[0] = s;
+        scale_dev[1] = (float)ldexp(1.0, -e);
+    }
+    const int cols = n_in / 8;
+    const long long n = (long long)groups * 9 * n_pad * cols;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long row = i / cols;                               // (g, tap, o)
+        const int c0 = (int)(i - row * cols) * 8;
+        const int o = (int)(row % n_pad), tap = (int)((row / n_pad) % 9), g = (int)(row / ((long long)n_pad * 9));
+        const int oo = g * 128 + o;
+        float v[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int ii = c0 + j;
+            float x = 0.f;
+            if (oo < n_out)
+                x = transpose ? __ldg(&w[((size_t)ii * cin + oo) * 9 + (8 - tap)]) : __ldg(&w[((size_t)oo * cin + ii) * 9 + tap]);
+            v[j] = __fmul_rn(x, s);
+        }
+        uint32_t h[4], l[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const uint32_t pa = b2s_tc::split_f16(v[2 * j]), pb = b2s_tc::split_f16(v[2 * j + 1]);
+            h[j] = __byte_perm(pa, pb, 0x5410);
+            l[j] = __byte_perm(pa, pb, 0x7632);
+        }
+        *reinterpret_cast<uint4 *>(hi + row * n_in + c0) = make_uint4(h[0], h[1], h[2], h[3]);
+        *reinterpret_cast<uint4 *>(lo + row * n_in + c0) = make_uint4(l[0], l[1], l[2], l[3]);
     }
 }
 
@@ -574,6 +586,30 @@ extern "C" int b2s_pack_sparse_weights(const float *w, int K, int cin, int cout,
     B2S_LAUNCH_OK();
     k_pack_sparse_weights<<<grid_for((long long)nkb * n_out * (b2s_tc::BLOCK_K / 8)), kThreads, 0, stream>>>(
         w, K, cin, cout, transpose, flip ? 1 : 0, n_in, n_in_pad, n_out, nkb, reinterpret_cast<__half *>(hi),
+        reinterpret_cast<__half *>(lo), scale_dev);
+    B2S_LAUNCH_OK();
+    return 0;
+}
+
+extern "C" int b2s_pack_conv2d_weights(const float *w, int cout, int cin, int transpose, b2s_half *hi, b2s_half *lo,
+                                       float *scale_dev, void *stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(cout >= 1 && cin >= 1 && cout % 64 == 0 && cin % 64 == 0,
+                "b2s_pack_conv2d_weights: cin and cout must be multiples of 64");
+    B2S_REQUIRE(transpose == 0 || transpose == 1, "b2s_pack_conv2d_weights: transpose must be 0 or 1");
+    B2S_REQUIRE(w && hi && lo && scale_dev, "b2s_pack_conv2d_weights: w, hi, lo and scale_dev required");
+    B2S_REQUIRE(((uintptr_t)hi & 15) == 0 && ((uintptr_t)lo & 15) == 0,
+                "b2s_pack_conv2d_weights: planes must be 16-byte aligned");
+    const long long n = 9ll * cin * cout;
+    B2S_REQUIRE(n < (1ll << 31), "b2s_pack_conv2d_weights: weight too large");
+    const int n_in = transpose ? cout : cin, n_out = transpose ? cin : cout;
+    const int n_pad = n_out < 128 ? n_out : 128, groups = (n_out + 127) / 128;
+    B2S_CUDA_OK(cudaMemsetAsync(scale_dev + 2, 0, sizeof(float), stream));
+    k_absmax<<<grid_for(n), kThreads, 0, stream>>>(w, nullptr, 1, (int)n, reinterpret_cast<unsigned *>(scale_dev + 2));
+    B2S_LAUNCH_OK();
+    k_pack_conv2d_weights<<<grid_for((long long)groups * 9 * n_pad * (n_in / 8)), kThreads, 0, stream>>>(
+        w, cout, cin, transpose, n_in, n_out, n_pad, groups, reinterpret_cast<__half *>(hi),
         reinterpret_cast<__half *>(lo), scale_dev);
     B2S_LAUNCH_OK();
     return 0;

@@ -160,6 +160,12 @@ SIGNATURES = {
                                   c_void_p, c_size_t, c_void_p, c_void_p]),
     "b2s_pack_sparse_weights": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                         c_void_p]),
+    "b2s_split_halo_f16_autoscale": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                             c_void_p, c_void_p]),
+    "b2s_pack_conv2d_weights": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2s_conv2d_wgrad_tc_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "b2s_conv2d_wgrad_tc": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
 
 OPTIM_CHUNK = 4096       # B2S_OPTIM_CHUNK
