@@ -88,7 +88,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 210
+#define B2S_VERSION 211
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -330,6 +330,14 @@ int b2s_to_bev_tc(const float *feat, const b2s_half *feat_hi, const b2s_half *fe
                   uint8_t *occupancy /*optional [B,H,W]: 1 where a pixel received data (input of b2s_rpn_block_plan)*/,
                   void *stream);
 
+/* the same scatter into planes kept between calls.  Precondition: the planes are zero except at the pixels flagged in
+ * `occupancy` (required), as after zero allocation.  The call zeroes those pixels and clears their flags, then scatters
+ * the rows and flags their pixels, so the planes end as b2s_to_bev_tc leaves them and the precondition holds for the
+ * next call.  Cost follows the flagged pixels, not the map.  C*D a multiple of 8, planes 16-byte aligned. */
+int b2s_to_bev_tc_ex(const float *feat, const b2s_half *feat_hi, const b2s_half *feat_lo, int feat_stride,
+                     const int *coors, const int *num_rows_dev, int cap_rows, int C, int batch, int D, int H, int W,
+                     b2s_half *out_hi, b2s_half *out_lo, uint8_t *occupancy, void *stream);
+
 /* ---- dense RPN convolution on the tensor pipe (second/pytorch/models/rpn.py:467-497 blocks, :264-299 deblocks,
  *      :386-391 heads): 3x3 stride-1 pad-1 (taps=9) or 1x1 (taps=1) conv + per-channel scale/shift (+ReLU).
  * wgmma implicit GEMM (f16 operands) with the 3xF16 split (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi, fp32 accumulation in
@@ -408,6 +416,20 @@ int b2s_rpn_strip_plan(const uint8_t *occupancy /*[B,H,W]*/, int batch, int H, i
                        uint8_t *scratch, int *strip_flags, int *work_lists, int *bg_lists, int *counts, void *stream);
 int b2s_rpn_bg_plan(const uint8_t *occupancy /*[B,H,W]*/, int batch, int H, int W, int num_layers, uint8_t *scratch,
                     int *tile_flags, int *work_lists, int *bg_lists, int *counts, void *stream);
+/* the background strips that must hold the empty-frame response, from the strip_flags of b2s_rpn_strip_plan (same
+ * batch, H, W, num_layers, rows), for a chain of layers that ends in the fused tail (b2s_rpn_tail_tc_ex).  Layer l + 1
+ * reads layer l only inside the windows of the strips it computes, which reach one pixel into each of the eight
+ * neighbouring strips; the tail reads the last layer in tiles of 8 rows x 16 columns (tiles_h = ceil(H/8),
+ * tiles_w = ceil(W/16), tile id = (b * tiles_h + th) * tiles_w + tw), and computes a tile iff the last layer computes
+ * one of its strips.  Per layer l, band_lists[l*num_strips ..] holds (ascending) the strips layer l does not compute
+ * that  - l < num_layers - 1: have a strip computed by layer l + 1 in their 3x3 strip neighbourhood of the same frame,
+ *         the strip itself included;
+ *       - l = num_layers - 1: lie in a computed tail tile;
+ * band_counts[l] of them.  tail_work / tail_bg [num_tiles] get the computed / other tail tiles (ascending),
+ * tail_counts[0] / [1] of them.  Passed as bg_list to b2s_conv2d_tc_ex2 and as the lists of b2s_rpn_tail_tc_ex, they
+ * leave every pixel a later launch reads, and every head record, as a full fill and a dense tail would. */
+int b2s_rpn_strip_bands(const int *strip_flags, int batch, int H, int W, int num_layers, int rows, int *band_lists,
+                        int *band_counts, int *tail_work, int *tail_bg, int *tail_counts, void *stream);
 
 
 /* the tail of a single-scale RPNV2 in one kernel (csrc/rpn_tail.cu): y = relu(bn(deblock_1x1(x))) (128 -> 128) never
@@ -419,6 +441,16 @@ int b2s_rpn_tail_tc(const b2s_half *in_hi, const b2s_half *in_lo, int B, int H, 
                     const b2s_half *w1_lo, int Cmid, const float *scale1, const float *shift1, const b2s_half *w2_hi,
                     const b2s_half *w2_lo, int cout2, int n_pad2, const float *scale2, const float *shift2, float *out,
                     int out_stride, unsigned *status_dev, void *stream);
+/* the same with tile lists (from b2s_rpn_strip_bands): only the tiles work_list[0 .. *work_count) are computed, and
+ * the records of the tiles bg_list[0 .. *bg_count) are written from `field` [H, W, out_stride], the records the tail
+ * gives for an empty frame (this kernel run on the last layer's empty-frame response).  margin >= 0 promises that
+ * field equals its record at pixel (margin, margin) wherever it is at least margin pixels from every border.  Other
+ * tiles are not written.  NULL lists: every tile is computed (b2s_rpn_tail_tc). */
+int b2s_rpn_tail_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int B, int H, int W, int Cin, const b2s_half *w1_hi,
+                       const b2s_half *w1_lo, int Cmid, const float *scale1, const float *shift1, const b2s_half *w2_hi,
+                       const b2s_half *w2_lo, int cout2, int n_pad2, const float *scale2, const float *shift2,
+                       float *out, int out_stride, const int *work_list, const int *work_count, const int *bg_list,
+                       const int *bg_count, const float *field, int margin, unsigned *status_dev, void *stream);
 
 /* ---- PointPillars feature net (single PFNLayer: Linear(F+5 -> Cout, no bias) + BN + ReLU + max) -- */
 int b2s_pfn(const float *points, int num_feat, const int *point_slots, const int *num_points_per_voxel,

@@ -14,7 +14,7 @@ buffers, so the whole frame batch is ONE CUDA graph:
   per sparse layer: b2s_rulebook_{subm,conv} (cached per indice_key) + b2s_sparse_conv_tc (wgmma, fp16 hi/lo
       planes flow from layer to layer) with BatchNorm1d/ReLU folded into the epilogue      middle.py:145-192
   b2s_pfn (PointPillars) / b2s_pfn_ex (PillarFeatureNetRadius) pointpillars.py:203-237,240-325
-  b2s_to_bev_tc (NHWC + halo, fp16 hi/lo)                      middle.py:206-209 / pointpillars.py:444-476
+  b2s_to_bev_tc_ex (NHWC + halo, fp16 hi/lo)                   middle.py:206-209 / pointpillars.py:444-476
   RPN as a program of b2s_conv2d_tc_ex launches (tc.plan_rpn)  rpn.py:314-331,393-420,467-497
       (rpn_impl="cudnn" keeps the torch modules as a cross-check: fp32, TF32 off)
   b2s_decode_filter_strided + b2s_nms (+ direction/range epilogue)   voxelnet.py:377-645
@@ -53,7 +53,17 @@ def _field_margin(hi, lo):
     bit, its value at pixel (m, m) wherever it is at least m pixels from every border; -1 when no such interior exists.
     The conv kernel stores that value into the background strips there instead of copying the field."""
     H, W = hi.shape[0] - 2, hi.shape[1] - 2
-    f = torch.cat([hi[1:H + 1, 1:W + 1], lo[1:H + 1, 1:W + 1]], -1).view(torch.int16)    # bits: +0 and -0 differ
+    return _bits_margin(torch.cat([hi[1:H + 1, 1:W + 1], lo[1:H + 1, 1:W + 1]], -1).view(torch.int16))
+
+
+def _record_margin(rec, n):
+    """_field_margin for the fused tail's empty-frame head records [H, W, stride] (fp32, the first n channels)."""
+    return _bits_margin(rec[:, :, :n].contiguous().view(torch.int32))
+
+
+def _bits_margin(f):
+    """f [H, W, K] integer bits (+0 and -0 differ) -> the margin of _field_margin."""
+    H, W = f.shape[0], f.shape[1]
     diff = (f != f[H // 2, W // 2]).any(-1)
     ys, xs = torch.arange(H, device=f.device), torch.arange(W, device=f.device)
     dist = torch.minimum(torch.minimum(ys, H - 1 - ys)[:, None], torch.minimum(xs, W - 1 - xs)[None, :])
@@ -308,7 +318,10 @@ class InferenceEngine:
         def plane(h, w, c):
             return (torch.zeros(B, h + 2, w + 2, c, dtype=torch.float16, device=dev),
                     torch.zeros(B, h + 2, w + 2, c, dtype=torch.float16, device=dev))
+        # the BEV planes are zero except at the pixels flagged in bev_occ (b2s_to_bev_tc_ex keeps that so from step
+        # to step); nothing else writes them
         self.tc_bev = plane(H, W, C)
+        self.bev_occ = torch.zeros(B, H, W, dtype=torch.uint8, device=dev)
         self.tc_bufs = {"in": self.tc_bev}
         for name, (h, w, c) in plan["buffers"].items():
             self.tc_bufs[name] = plane(h, w, c)
@@ -327,23 +340,36 @@ class InferenceEngine:
         self.tc_hw = (H, W)
         # background strips (csrc/rpn_bg.cu): through the leading chain of 3x3 stride-1 layers, output strips 8 pixels
         # wide and BG_ROWS high whose whole receptive field is empty BEV are not computed but copied from the layer's
-        # response to an empty frame
+        # response to an empty frame.  Only the strips a later launch reads need that response (b2s_rpn_strip_bands):
+        # the next layer's windows, and for the last layer the fused tail's computed 8 x 16 tiles; the tail writes the
+        # records of its other tiles from the records of an empty frame.  So the chain must end in the fused tail.
         self.bg_idx = _tc.background_layers(plan)
         if self.bg_idx:
+            assert (self.tc_tail_fused and len(plan["ops"]) == len(self.bg_idx) + 2
+                    and plan["ops"][-2]["src"] == plan["ops"][self.bg_idx[-1]]["dst"]), \
+                "background strips are tracked only through a 3x3 chain whose last layer feeds the fused tail"
             nl = len(self.bg_idx)
             self.bg_tiles = B * (-(-H // BG_ROWS)) * (-(-W // 8))    # strips per layer
-            self.bg_occ = torch.zeros(B, H, W, dtype=torch.uint8, device=dev)
             self.bg_scratch = torch.zeros(2, B, H, W, dtype=torch.uint8, device=dev)
             self.bg_flags = torch.zeros(nl, self.bg_tiles, dtype=torch.int32, device=dev)
             self.bg_work = torch.zeros(nl, self.bg_tiles, dtype=torch.int32, device=dev)
             self.bg_list = torch.zeros(nl, self.bg_tiles, dtype=torch.int32, device=dev)
             self.bg_counts = torch.zeros(nl, 2, dtype=torch.int32, device=dev)
-            self.bg_field = self._empty_frame_response()
+            self.bg_bands = torch.zeros(nl, self.bg_tiles, dtype=torch.int32, device=dev)
+            self.bg_band_counts = torch.zeros(nl, dtype=torch.int32, device=dev)
+            self.tail_tiles = B * (-(-H // 8)) * (-(-W // 16))         # fused-tail tiles of 8 x 16 pixels
+            self.tail_work = torch.zeros(self.tail_tiles, dtype=torch.int32, device=dev)
+            self.tail_bg = torch.zeros(self.tail_tiles, dtype=torch.int32, device=dev)
+            self.tail_counts = torch.zeros(2, dtype=torch.int32, device=dev)
+            self.bg_field, self.tail_field = self._empty_frame_response()
             self.bg_margin = [_field_margin(hi, lo) for hi, lo in self.bg_field]
+            self.tail_margin = _record_margin(self.tail_field, plan["ops"][-1]["cout"])
 
     def _empty_frame_response(self):
         """per background-tracked layer: what the layer's own kernel produces for an empty frame, as one halo-padded
-        frame [H+2, W+2, C] of fp16 hi/lo planes.  Run once at plan time on frame 0 of the (still all-zero) buffers."""
+        frame [H+2, W+2, C] of fp16 hi/lo planes; and the fused tail's head records [H, W, stride] for an empty frame,
+        from the tail kernel on the last layer's response.  Run once at plan time on frame 0 of the (still all-zero)
+        buffers."""
         L, lib = self._L, self.lib
         st = L.stream()
         fields = []
@@ -360,11 +386,24 @@ class InferenceEngine:
                 L.ptr(self.status), st), "b2s_conv2d_tc_ex(empty frame)")
             fields.append((dst[0][0, :, :, :op["cout"]].clone().contiguous(),
                            dst[1][0, :, :, :op["cout"]].clone().contiguous()))
+        d, h = self.tc_plan[-2], self.tc_plan[-1]
+        src = self.tc_bufs[d["src"]]
+        records = torch.zeros(1, d["Hin"], d["Win"], self.tc_head_stride, dtype=torch.float32, device=self.dev)
+        self._launch_fused_tail(src, records, 1, None, None, None, None, None, -1, st)
         torch.cuda.synchronize(self.dev)
         for oi in self.bg_idx:                    # leave the activation buffers as they were (all zero)
             for t in self.tc_bufs[self.tc_plan[oi]["dst"]]:
                 t[0].zero_()
-        return fields
+        return fields, records[0]
+
+    def _launch_fused_tail(self, src, out, batch, work, work_n, bgl, bgn, field, margin, st):
+        L, lib = self._L, self.lib
+        d, h = self.tc_plan[-2], self.tc_plan[-1]
+        L.check(lib.b2s_rpn_tail_tc_ex(
+            L.ptr(src[0]), L.ptr(src[1]), batch, d["Hin"], d["Win"], d["cin"], L.ptr(d["w_hi"]), L.ptr(d["w_lo"]),
+            d["cout"], L.ptr(d["scale"]), L.ptr(d["shift"]), L.ptr(h["w_hi"]), L.ptr(h["w_lo"]), h["cout"], h["n_pad"],
+            L.ptr(h["scale"]), L.ptr(h["shift"]), L.ptr(out), self.tc_head_stride, work, work_n, bgl, bgn,
+            L.ptr(field), margin, L.ptr(self.status), st), "b2s_rpn_tail_tc_ex")
 
     def _feature_hw(self):
         if self.rpn_impl == "tc":
@@ -679,19 +718,23 @@ class InferenceEngine:
         D, H, W = fl.shape
         self._mark("to_bev")
         if hilo is not None:
-            L.check(lib.b2s_to_bev_tc(None, L.ptr(hilo[0]), L.ptr(hilo[1]), hilo[2], L.ptr(fl.coors), L.ptr(fl.n_dev),
-                                      fl.cap, self.feat_final_c, self.B, D, H, W, L.ptr(self.tc_bev[0]),
-                                      L.ptr(self.tc_bev[1]), L.ptr(self.bg_occ) if self.bg_idx else None, st),
-                    "b2s_to_bev_tc")
+            L.check(lib.b2s_to_bev_tc_ex(None, L.ptr(hilo[0]), L.ptr(hilo[1]), hilo[2], L.ptr(fl.coors),
+                                         L.ptr(fl.n_dev), fl.cap, self.feat_final_c, self.B, D, H, W,
+                                         L.ptr(self.tc_bev[0]), L.ptr(self.tc_bev[1]), L.ptr(self.bev_occ), st),
+                    "b2s_to_bev_tc_ex")
         else:
-            L.check(lib.b2s_to_bev_tc(L.ptr(feats), None, None, 0, L.ptr(fl.coors), L.ptr(fl.n_dev), fl.cap,
-                                      self.feat_final_c, self.B, D, H, W, L.ptr(self.tc_bev[0]), L.ptr(self.tc_bev[1]),
-                                      L.ptr(self.bg_occ) if self.bg_idx else None, st), "b2s_to_bev_tc")
+            L.check(lib.b2s_to_bev_tc_ex(L.ptr(feats), None, None, 0, L.ptr(fl.coors), L.ptr(fl.n_dev), fl.cap,
+                                         self.feat_final_c, self.B, D, H, W, L.ptr(self.tc_bev[0]),
+                                         L.ptr(self.tc_bev[1]), L.ptr(self.bev_occ), st), "b2s_to_bev_tc_ex")
         self._mark("rpn")
-        if self.bg_idx:
-            L.check(lib.b2s_rpn_strip_plan(L.ptr(self.bg_occ), self.B, H, W, len(self.bg_idx), BG_ROWS,
+        nl = len(self.bg_idx)
+        if nl:
+            L.check(lib.b2s_rpn_strip_plan(L.ptr(self.bev_occ), self.B, H, W, nl, BG_ROWS,
                                            L.ptr(self.bg_scratch), L.ptr(self.bg_flags), L.ptr(self.bg_work),
                                            L.ptr(self.bg_list), L.ptr(self.bg_counts), st), "b2s_rpn_strip_plan")
+            L.check(lib.b2s_rpn_strip_bands(L.ptr(self.bg_flags), self.B, H, W, nl, BG_ROWS, L.ptr(self.bg_bands),
+                                            L.ptr(self.bg_band_counts), L.ptr(self.tail_work), L.ptr(self.tail_bg),
+                                            L.ptr(self.tail_counts), st), "b2s_rpn_strip_bands")
         marked_tail = False
         n_ops = len(self.tc_plan) - (2 if self.tc_tail_fused else 0)
         for oi, op in enumerate(self.tc_plan[:n_ops]):
@@ -713,8 +756,10 @@ class InferenceEngine:
                 bl = self.bg_idx.index(oi)
                 chi, clo = self.bg_field[bl]
                 work, work_n = L.ptr(self.bg_work[bl]), L.ptr(self.bg_counts[bl, 0:])
-                # the conv kernel's fill warps store the constant into the background strips
-                bgl, bgn, bhi, blo = L.ptr(self.bg_list[bl]), L.ptr(self.bg_counts[bl, 1:]), L.ptr(chi), L.ptr(clo)
+                # the conv kernel's fill warps store the empty-frame response into the background strips a later
+                # launch reads
+                bgl, bgn = L.ptr(self.bg_bands[bl]), L.ptr(self.bg_band_counts[bl:])
+                bhi, blo = L.ptr(chi), L.ptr(clo)
                 margin = self.bg_margin[bl]
             L.check(lib.b2s_conv2d_tc_ex2(
                 L.ptr(src[0]), L.ptr(src[1]), self.B, op["Hin"], op["Win"], op["cin"], L.ptr(op["w_hi"]),
@@ -726,13 +771,13 @@ class InferenceEngine:
         if not marked_tail:
             self._mark("rpn_1x1")
         if self.tc_tail_fused:
-            d, h = self.tc_plan[-2], self.tc_plan[-1]
-            src = self.tc_bufs[d["src"]]
-            L.check(lib.b2s_rpn_tail_tc(
-                L.ptr(src[0]), L.ptr(src[1]), self.B, d["Hin"], d["Win"], d["cin"], L.ptr(d["w_hi"]), L.ptr(d["w_lo"]),
-                d["cout"], L.ptr(d["scale"]), L.ptr(d["shift"]), L.ptr(h["w_hi"]), L.ptr(h["w_lo"]), h["cout"], h["n_pad"],
-                L.ptr(h["scale"]), L.ptr(h["shift"]), L.ptr(self.tc_heads), self.tc_head_stride, L.ptr(self.status), st),
-                "b2s_rpn_tail_tc")
+            src = self.tc_bufs[self.tc_plan[-2]["src"]]
+            if nl:          # computed tiles only; background tiles' records from the empty frame's records
+                self._launch_fused_tail(src, self.tc_heads, self.B, L.ptr(self.tail_work), L.ptr(self.tail_counts[0:]),
+                                        L.ptr(self.tail_bg), L.ptr(self.tail_counts[1:]), self.tail_field,
+                                        self.tail_margin, st)
+            else:
+                self._launch_fused_tail(src, self.tc_heads, self.B, None, None, None, None, None, -1, st)
         if self.segments is not None:
             self._mark("decode_filter")
             segs = []
@@ -861,8 +906,9 @@ class InferenceEngine:
         if self.rpn_impl == "tc":
             # one tensor-core kernel per RPN layer (fused tail: 1 for 2); the multi-head crop op is one b2s_crop_nhwc kernel
             n += len(self.tc_plan) - (1 if self.tc_tail_fused else 0)
+            n += 1                               # k_bev_clear (b2s_to_bev_tc_ex)
             if self.bg_idx:
-                n += len(self.bg_idx) + 1        # k_bg_layer per layer, k_bg_compact
+                n += len(self.bg_idx) + 2        # k_bg_layer per layer, k_bg_compact, k_strip_bands
         elif getattr(self, "any_sparse_tc", False):
             n += 1                               # b2s_merge_f16
         if self.mc:

@@ -1,6 +1,7 @@
 // bev.cu -- sparse rows -> dense BEV map (b2s_to_bev), the PointPillars feature net (b2s_pfn / b2s_pfn_ex) and the
 // crop of a halo-padded map into a zero-halo map (b2s_crop_nhwc).  See include/b2second.h.  Pure HBM-bound data movement: zero-fill the dense map once, then one
-// scattered write per (row, channel).
+// scattered write per (row, channel).  b2s_to_bev_tc_ex keeps the map between calls and zeroes only the pixels the
+// previous call wrote (7 % of the map for a KITTI cloud), which its occupancy map still flags.
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -66,6 +67,30 @@ __global__ void k_to_bev_tc(const float *__restrict__ feat, const __half *__rest
         } else {
             out_hi[idx] = feat_hi[(size_t)row * feat_stride + c];
             out_lo[idx] = feat_lo[(size_t)row * feat_stride + c];
+        }
+    }
+}
+
+// the pixels the previous step flagged in `occ` back to zero in both planes (CV 16-byte vectors per pixel), and their
+// flags cleared: each warp reads the flags of 32 pixels and zeroes the flagged ones one pixel at a time
+__global__ void k_bev_clear(uint8_t *__restrict__ occ, int batch, int H, int W, int CV, uint4 *__restrict__ out_hi,
+                            uint4 *__restrict__ out_lo)
+{
+    const long long n = (long long)batch * H * W;
+    const int lane = threadIdx.x & 31;
+    const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+    for (long long base = (((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 32; base < n; base += nwarps * 32) {
+        const long long i = base + lane;
+        const bool flagged = i < n && occ[i];
+        if (flagged) occ[i] = 0;
+        for (unsigned m = __ballot_sync(0xffffffffu, flagged); m; m &= m - 1) {
+            const long long px = base + __ffs(m) - 1;
+            const long long row = px / W;                                    // b * H + y
+            const size_t o = ((size_t)(row + row / H * 2 + 1) * (W + 2) + (px % W) + 1) * CV;
+            for (int v = lane; v < CV; v += 32) {
+                out_hi[o + v] = make_uint4(0u, 0u, 0u, 0u);
+                out_lo[o + v] = make_uint4(0u, 0u, 0u, 0u);
+            }
         }
     }
 }
@@ -226,6 +251,29 @@ extern "C" int b2s_to_bev_tc(const float *feat, const b2s_half *feat_hi, const b
     B2S_CUDA_OK(cudaMemsetAsync(out_hi, 0, sizeof(__half) * total, stream));
     B2S_CUDA_OK(cudaMemsetAsync(out_lo, 0, sizeof(__half) * total, stream));
     if (occupancy) B2S_CUDA_OK(cudaMemsetAsync(occupancy, 0, (size_t)batch * H * W, stream));
+    if (cap_rows > 0) {
+        k_to_bev_tc<<<bounded_grid((long long)cap_rows * C), kThreads, 0, stream>>>(
+            feat, reinterpret_cast<const __half *>(feat_hi), reinterpret_cast<const __half *>(feat_lo), feat_stride, coors,
+            num_rows_dev, cap_rows, C, batch, D, H, W, reinterpret_cast<__half *>(out_hi),
+            reinterpret_cast<__half *>(out_lo), occupancy);
+        B2S_LAUNCH_OK();
+    }
+    return 0;
+}
+
+extern "C" int b2s_to_bev_tc_ex(const float *feat, const b2s_half *feat_hi, const b2s_half *feat_lo, int feat_stride,
+                                const int *coors, const int *num_rows_dev, int cap_rows, int C, int batch, int D, int H,
+                                int W, b2s_half *out_hi, b2s_half *out_lo, uint8_t *occupancy, void *stream_)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(C >= 1 && batch >= 1 && D >= 1 && H >= 1 && W >= 1, "b2s_to_bev_tc_ex: bad sizes");
+    B2S_REQUIRE((feat != nullptr) != (feat_hi != nullptr && feat_lo != nullptr),
+                "b2s_to_bev_tc_ex: pass either fp32 rows or hi/lo fp16 rows");
+    B2S_REQUIRE(occupancy != nullptr && (C * D) % 8 == 0 && ((uintptr_t)out_hi & 15) == 0 && ((uintptr_t)out_lo & 15) == 0,
+                "b2s_to_bev_tc_ex: needs the occupancy map, C*D a multiple of 8 and 16-byte aligned planes");
+    k_bev_clear<<<bounded_grid((long long)batch * H * W), kThreads, 0, stream>>>(
+        occupancy, batch, H, W, C * D / 8, reinterpret_cast<uint4 *>(out_hi), reinterpret_cast<uint4 *>(out_lo));
+    B2S_LAUNCH_OK();
     if (cap_rows > 0) {
         k_to_bev_tc<<<bounded_grid((long long)cap_rows * C), kThreads, 0, stream>>>(
             feat, reinterpret_cast<const __half *>(feat_hi), reinterpret_cast<const __half *>(feat_lo), feat_stride, coors,

@@ -15,6 +15,11 @@
 // engine plans 8 x 4 strips: the conv kernel's time follows the bytes it streams from L2, and 8 x 4 moves the fewest
 // (finer strips compute fewer pixels but load taller windows per output row).
 // Everything the reference computes is still produced; only the recomputation of a known field is skipped.
+// Nor does every background strip need the field: layer l + 1 reads layer l only inside the windows of the strips it
+// computes, which reach one pixel into each neighbouring strip.  b2s_rpn_strip_bands lists, per layer, the background
+// strips next to a strip of the following layer (the "band"); the others are read by nothing and are left stale.  The
+// last layer's band is the part of its background inside the fused tail's computed tiles, and the tail writes the
+// records of its background tiles from the empty frame's records (rpn_tail.cu).
 #include "common.cuh"
 
 namespace {
@@ -57,43 +62,94 @@ k_bg_layer(const uint8_t *__restrict__ in, int H, int W, int tile_h, int tile_w,
     }
 }
 
-// one block per layer: stable compaction of the tile ids into work (flag 1) and background (flag 0) lists; each
-// thread takes COMPACT_PER_THREAD consecutive ids per pass
-__global__ void __launch_bounds__(1024)
-k_bg_compact(const int *__restrict__ tile_flag, int num_tiles, int *work_list, int *bg_list, int *counts)
+// stable compaction of the ids 0 .. n-1 by flag_of(i) into list (flag 1, ascending) and, when rest is not NULL, rest
+// (flag 0); each of the 1024 threads takes COMPACT_PER_THREAD consecutive ids per pass.  Returns the listed count.
+template <class Flag>
+__device__ int compact_ids(Flag flag_of, int n, int *list, int *rest)
 {
-    const int layer = blockIdx.x;
-    const int *flag = tile_flag + (size_t)layer * num_tiles;
-    int *work = work_list + (size_t)layer * num_tiles, *bg = bg_list + (size_t)layer * num_tiles;
     __shared__ int s_carry;
     if (threadIdx.x == 0) s_carry = 0;
     __syncthreads();
-    for (int base = 0; base < num_tiles; base += 1024 * COMPACT_PER_THREAD) {
+    for (int base = 0; base < n; base += 1024 * COMPACT_PER_THREAD) {
         const int i0 = base + (int)threadIdx.x * COMPACT_PER_THREAD;
-        int f[COMPACT_PER_THREAD], n = 0;
+        int f[COMPACT_PER_THREAD], k1 = 0;
 #pragma unroll
         for (int k = 0; k < COMPACT_PER_THREAD; ++k) {
-            f[k] = i0 + k < num_tiles ? flag[i0 + k] : 0;
-            n += f[k];
+            f[k] = i0 + k < n ? flag_of(i0 + k) : 0;
+            k1 += f[k];
         }
         int total;
-        const int ex = b2s_block_exscan(n, &total);
-        int wpos = s_carry + ex;                      // work tiles before i0
+        const int ex = b2s_block_exscan(k1, &total);
+        int wpos = s_carry + ex;                      // listed ids before i0
 #pragma unroll
         for (int k = 0; k < COMPACT_PER_THREAD; ++k) {
             const int i = i0 + k;
-            if (i >= num_tiles) break;
-            if (f[k]) work[wpos++] = i;
-            else bg[i - wpos] = i;                    // background tiles before i: i - (#work tiles before i)
+            if (i >= n) break;
+            if (f[k]) list[wpos++] = i;
+            else if (rest) rest[i - wpos] = i;        // unlisted ids before i: i - (#listed ids before i)
         }
         __syncthreads();
         if (threadIdx.x == 0) s_carry += total;
         __syncthreads();
     }
+    return s_carry;
+}
+
+// one block per layer: the tile ids into work (flag 1) and background (flag 0) lists
+__global__ void __launch_bounds__(1024)
+k_bg_compact(const int *__restrict__ tile_flag, int num_tiles, int *work_list, int *bg_list, int *counts)
+{
+    const int layer = blockIdx.x;
+    const int *flag = tile_flag + (size_t)layer * num_tiles;
+    const int n_work = compact_ids([&](int i) { return flag[i]; }, num_tiles, work_list + (size_t)layer * num_tiles,
+                                   bg_list + (size_t)layer * num_tiles);
     if (threadIdx.x == 0) {
-        counts[2 * layer] = s_carry;
-        counts[2 * layer + 1] = num_tiles - s_carry;
+        counts[2 * layer] = n_work;
+        counts[2 * layer + 1] = num_tiles - n_work;
     }
+}
+
+// blocks 0 .. num_layers - 2: the band of layer l = the strips layer l does not compute whose 3 x 3 strip
+// neighbourhood in the same frame (the strip itself included) holds a strip layer l + 1 computes.
+// Block num_layers - 1: the band of the last layer, read by the fused RPN tail in tiles of 8 rows x 16 columns
+// (per = 8 / rows strip rows x 2 strip columns): the strips the last layer does not compute inside a computed tail tile,
+// i.e. one with a computed strip.  Block num_layers: the tail's work (computed) and background tile lists.
+__global__ void __launch_bounds__(1024)
+k_strip_bands(const int *__restrict__ strip_flags, int num_layers, int strips_h, int strips_w, int num_strips,
+              int per, int tiles_h, int tiles_w, int *band_lists, int *band_counts, int *tail_work, int *tail_bg,
+              int *tail_counts)
+{
+    const int layer = blockIdx.x;
+    const int *last = strip_flags + (size_t)(num_layers - 1) * num_strips;
+    const auto tile_computed = [&](int b, int th, int tw) {
+        int any = 0;
+        for (int y = th * per; y < min(th * per + per, strips_h); ++y)
+            for (int x = 2 * tw; x < min(2 * tw + 2, strips_w); ++x) any |= last[((size_t)b * strips_h + y) * strips_w + x];
+        return any;
+    };
+    if (layer == num_layers) {
+        const int num_tiles = num_strips / (strips_h * strips_w) * tiles_h * tiles_w;
+        const int n = compact_ids([&](int i) { return tile_computed(i / (tiles_h * tiles_w), (i / tiles_w) % tiles_h,
+                                                                    i % tiles_w); },
+                                  num_tiles, tail_work, tail_bg);
+        if (threadIdx.x == 0) {
+            tail_counts[0] = n;
+            tail_counts[1] = num_tiles - n;
+        }
+        return;
+    }
+    const int *cur = strip_flags + (size_t)layer * num_strips, *next = cur + num_strips;
+    const auto in_band = [&](int i) {
+        if (cur[i]) return 0;
+        const int sw = i % strips_w, sh = (i / strips_w) % strips_h, f0 = i - sh * strips_w - sw;
+        if (layer == num_layers - 1) return tile_computed(i / (strips_h * strips_w), sh / per, sw / 2);
+        int any = 0;
+        for (int y = max(sh - 1, 0); y <= min(sh + 1, strips_h - 1); ++y)
+            for (int x = max(sw - 1, 0); x <= min(sw + 1, strips_w - 1); ++x) any |= next[f0 + y * strips_w + x];
+        return any;
+    };
+    const int n = compact_ids(in_band, num_strips, band_lists + (size_t)layer * num_strips, nullptr);
+    if (threadIdx.x == 0) band_counts[layer] = n;
 }
 
 int bg_plan(const uint8_t *occupancy, int batch, int H, int W, int num_layers, int tile_h, int tile_w,
@@ -141,4 +197,19 @@ extern "C" int b2s_rpn_strip_plan(const uint8_t *occupancy, int batch, int H, in
     B2S_REQUIRE(rows == 1 || rows == 2 || rows == 4 || rows == 8, "b2s_rpn_strip_plan: rows must be 1, 2, 4 or 8");
     return bg_plan(occupancy, batch, H, W, num_layers, rows, 8, scratch, strip_flags, work_lists, bg_lists, counts,
                    (cudaStream_t)stream);
+}
+
+extern "C" int b2s_rpn_strip_bands(const int *strip_flags, int batch, int H, int W, int num_layers, int rows,
+                                   int *band_lists, int *band_counts, int *tail_work, int *tail_bg, int *tail_counts,
+                                   void *stream)
+{
+    B2S_REQUIRE(batch >= 1 && H >= 1 && W >= 1 && num_layers >= 1 && num_layers <= 32,
+                "b2s_rpn_strip_bands: bad sizes (num_layers 1..32)");
+    B2S_REQUIRE(rows == 1 || rows == 2 || rows == 4 || rows == 8, "b2s_rpn_strip_bands: rows must be 1, 2, 4 or 8");
+    const int strips_h = b2s_cdiv(H, rows), strips_w = b2s_cdiv(W, 8);
+    k_strip_bands<<<num_layers + 1, 1024, 0, (cudaStream_t)stream>>>(
+        strip_flags, num_layers, strips_h, strips_w, batch * strips_h * strips_w, 8 / rows, b2s_cdiv(H, 8),
+        b2s_cdiv(W, 16), band_lists, band_counts, tail_work, tail_bg, tail_counts);
+    B2S_LAUNCH_OK();
+    return 0;
 }

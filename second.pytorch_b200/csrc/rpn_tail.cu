@@ -14,8 +14,13 @@
 //
 // CTA = 3 warpgroups, persistent over 8 x 16-pixel tiles:
 //   warp 0            TMA: weights once, then per tile the two 64-channel K blocks of x (hi + lo) into the ring
+//   warps 1-3         background tiles (b2s_rpn_tail_tc_ex with a background list): their records are the records of
+//                     an empty frame (the tail run once on the last layer's empty-frame response), stored from a
+//                     record each thread holds in registers where the tile lies >= margin pixels from every border,
+//                     copied from that one-frame record field nearer to it.  Nothing in the launch reads the records.
 //   warpgroups 1, 2   consumers: warpgroup g owns tile pixels 64g .. 64g+63 through GEMM 1, the y epilogue, GEMM 2
 //                     and the record stores
+// With a work list, TMA and consumers walk the listed tiles only (a tile id = (b * tiles_h + th) * tiles_w + tw).
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -44,6 +49,11 @@ struct TailParams {
     const float *scale1, *shift1, *scale2, *shift2;
     float *out;
     int *status;
+    const int *work_list, *work_count;   // optional (device): the tiles to compute; NULL: every tile
+    const int *bg_list, *bg_count;       // optional (device): tiles whose records come from `field`
+    const float *field;                  // [H, W, out_stride]: the records of an empty frame
+    int margin;                          // >= 0: field equals its record at (margin, margin) wherever it is >= margin
+                                         // pixels from every border; < 0: no such promise
 };
 
 __global__ void __launch_bounds__(kThreads, 1)
@@ -73,11 +83,13 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    const int my_tiles = (int)blockIdx.x < p.num_tiles ? (p.num_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+    const int n_work = p.work_list ? min(*p.work_count, p.num_tiles) : p.num_tiles;
+    const auto tile_at = [&](int i) { return p.work_list ? __ldg(&p.work_list[i]) : i; };
+    const bool has_work = (int)blockIdx.x < n_work;
 
     if (warp == 0) {
         // ===================== TMA producer =====================
-        if (lane == 0 && my_tiles > 0) {
+        if (lane == 0 && has_work) {
             mbar_arrive_expect_tx(&bar_w, KB * (W1_KB_BYTES + W2_KB_BYTES));
             for (int kb = 0; kb < KB; ++kb) {
                 tma_load_3d(smem + OFF_W1 + kb * W1_KB_BYTES, &map_w1_hi, &bar_w, kb * BLOCK_K, 0, 0);
@@ -86,7 +98,8 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
                 tma_load_3d(smem + OFF_W2 + kb * W2_KB_BYTES + W2_KB_BYTES / 2, &map_w2_lo, &bar_w, kb * BLOCK_K, 0, 0);
             }
             int u = 0;                                                 // K blocks of x loaded so far: slot u % XS, its (u / XS)-th use
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+            for (int i = blockIdx.x; i < n_work; i += gridDim.x) {
+                const int tile = tile_at(i);
                 const int tw = tile % p.tiles_w, th = (tile / p.tiles_w) % p.tiles_h, b = tile / (p.tiles_w * p.tiles_h);
                 const int h0 = th * TILE_H + 1, w0 = tw * TILE_W + 1;          // + 1: the one-pixel halo of the input planes
                 for (int kb = 0; kb < KB; ++kb, ++u) {
@@ -99,16 +112,42 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
                 }
             }
         }
-    } else if (warp >= 4) {
+    } else if (warp <= 3) {
+        // ===================== background tiles: thread t stores the 16-byte record chunk q = t % nq of pixels
+        // t / nq, t / nq + per, ... of each tile (per = 96 / nq pixels per pass)
+        const int nq = p.cout2 / 4, per = 96 / nq;
+        const int t = (warp - 1) * 32 + lane, q = t % nq;
+        const size_t s4 = (size_t)p.out_stride / 4;
+        if (p.bg_list && t < per * nq) {
+            const int n_bg = min(*p.bg_count, p.num_tiles);
+            const int m = p.margin;
+            const float4 *field = reinterpret_cast<const float4 *>(p.field);
+            float4 *out = reinterpret_cast<float4 *>(p.out);
+            const float4 c = m >= 0 ? __ldg(field + ((size_t)m * p.W + m) * s4 + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int i = blockIdx.x; i < n_bg; i += gridDim.x) {
+                const int tile = __ldg(&p.bg_list[i]);
+                const int tw = tile % p.tiles_w, th = (tile / p.tiles_w) % p.tiles_h, b = tile / (p.tiles_w * p.tiles_h);
+                const int h0 = th * TILE_H, w0 = tw * TILE_W;
+                const bool inner = m >= 0 && h0 >= m && h0 + TILE_H <= p.H - m && w0 >= m && w0 + TILE_W <= p.W - m;
+                for (int px = t / nq; px < TILE_H * TILE_W; px += per) {
+                    const int h = h0 + px / TILE_W, w = w0 + px % TILE_W;
+                    if (h >= p.H || w >= p.W) continue;
+                    const size_t f = (size_t)h * p.W + w;
+                    out[((size_t)b * p.H * p.W + f) * s4 + q] = inner ? c : __ldg(field + f * s4 + q);
+                }
+            }
+        }
+    } else {
         // ===================== consumers =====================
         const int cg = (warp >> 2) - 1;                          // tile pixels 64 cg .. 64 cg + 63
         const int wl = warp & 3;
         const uint32_t smem0 = smem_u32(smem);
         const uint32_t a_off = (uint32_t)cg * 64u * 128u;
         bool range_bad = false;
-        mbar_wait(&bar_w, 0);
+        if (has_work) mbar_wait(&bar_w, 0);
         int u = 0;
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        for (int i = blockIdx.x; i < n_work; i += gridDim.x) {
+            const int tile = tile_at(i);
             const int tw = tile % p.tiles_w, th = (tile / p.tiles_w) % p.tiles_h, b = tile / (p.tiles_w * p.tiles_h);
             // ---- GEMM 1: D1 = x * W1^T; per K step the three products of the 3xF16 split in k_conv_tc's order
             float d1[N1 / 2];
@@ -192,17 +231,21 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
 
 // in: halo-padded hi/lo planes [B, H+2, W+2, 128]; w1: [128][128] (y channel, x channel), w2: [n_pad][128] (rows >= cout2
 // zero), both K-major hi/lo planes pre-scaled by a power of two folded into scale1 / scale2; out: fp32 [B, H, W, out_stride].
-extern "C" int b2s_rpn_tail_tc(const b2s_half *in_hi, const b2s_half *in_lo, int B, int H, int W, int Cin,
-                               const b2s_half *w1_hi, const b2s_half *w1_lo, int Cmid, const float *scale1,
-                               const float *shift1, const b2s_half *w2_hi, const b2s_half *w2_lo, int cout2, int n_pad2,
-                               const float *scale2, const float *shift2, float *out, int out_stride, unsigned *status_dev,
-                               void *stream_)
+extern "C" int b2s_rpn_tail_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int B, int H, int W, int Cin,
+                                  const b2s_half *w1_hi, const b2s_half *w1_lo, int Cmid, const float *scale1,
+                                  const float *shift1, const b2s_half *w2_hi, const b2s_half *w2_lo, int cout2,
+                                  int n_pad2, const float *scale2, const float *shift2, float *out, int out_stride,
+                                  const int *work_list, const int *work_count, const int *bg_list, const int *bg_count,
+                                  const float *field, int margin, unsigned *status_dev, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     B2S_REQUIRE(Cin == C && Cmid == N1, "b2s_rpn_tail_tc: built for a 128 -> 128 deblock (got %d -> %d)", Cin, Cmid);
     B2S_REQUIRE(n_pad2 == N2 && cout2 >= 4 && cout2 <= n_pad2 && cout2 % 4 == 0 && out_stride >= cout2 && out_stride % 4 == 0,
                 "b2s_rpn_tail_tc: up to 32 packed head channels (multiple of 4), out_stride a multiple of 4");
     B2S_REQUIRE(B >= 1 && H >= 1 && W >= 1 && ((uintptr_t)out & 15) == 0, "b2s_rpn_tail_tc: bad sizes / unaligned output");
+    B2S_REQUIRE((work_list == nullptr) == (work_count == nullptr) && (bg_list == nullptr) == (bg_count == nullptr) &&
+                    (bg_list == nullptr || (field != nullptr && ((uintptr_t)field & 15) == 0)),
+                "b2s_rpn_tail_tc_ex: a list needs its count, a background list a 16-byte aligned record field");
     CUtensorMap x_hi, x_lo, m1_hi, m1_lo, m2_hi, m2_lo;
     {
         cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)(W + 2), (cuuint64_t)(H + 2), (cuuint64_t)B};
@@ -231,10 +274,23 @@ extern "C" int b2s_rpn_tail_tc(const b2s_half *in_hi, const b2s_half *in_lo, int
     p.cout2 = cout2; p.out_stride = out_stride;
     p.scale1 = scale1; p.shift1 = shift1; p.scale2 = scale2; p.shift2 = shift2;
     p.out = out; p.status = (int *)status_dev;
+    p.work_list = work_list; p.work_count = work_count; p.bg_list = bg_list; p.bg_count = bg_count; p.field = field;
+    p.margin = (bg_list && margin >= 0 && 2 * margin < H && 2 * margin < W) ? margin : -1;
     const int num_sms = num_sms_current();
     const int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
     B2S_SMEM_OPT_IN(k_rpn_tail, SMEM_BYTES);
     k_rpn_tail<<<grid, kThreads, SMEM_BYTES, stream>>>(x_hi, x_lo, m1_hi, m1_lo, m2_hi, m2_lo, p);
     B2S_LAUNCH_OK();
     return 0;
+}
+
+extern "C" int b2s_rpn_tail_tc(const b2s_half *in_hi, const b2s_half *in_lo, int B, int H, int W, int Cin,
+                               const b2s_half *w1_hi, const b2s_half *w1_lo, int Cmid, const float *scale1,
+                               const float *shift1, const b2s_half *w2_hi, const b2s_half *w2_lo, int cout2, int n_pad2,
+                               const float *scale2, const float *shift2, float *out, int out_stride, unsigned *status_dev,
+                               void *stream)
+{
+    return b2s_rpn_tail_tc_ex(in_hi, in_lo, B, H, W, Cin, w1_hi, w1_lo, Cmid, scale1, shift1, w2_hi, w2_lo, cout2, n_pad2,
+                              scale2, shift2, out, out_stride, nullptr, nullptr, nullptr, nullptr, nullptr, -1,
+                              status_dev, stream);
 }

@@ -77,6 +77,10 @@ SIGNATURES = {
                              c_void_p]),
     "b2s_to_bev_tc": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                               c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2s_to_bev_tc_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                 c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2s_rpn_strip_bands": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p, c_void_p]),
     "b2s_rpn_bg_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                 c_void_p]),
     "b2s_rpn_block_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -95,6 +99,9 @@ SIGNATURES = {
                                   c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "b2s_rpn_tail_tc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                 c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "b2s_rpn_tail_tc_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                   c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "b2s_decode_filter_strided": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_longlong, ctypes.c_longlong,
                                           ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                           c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
