@@ -271,9 +271,11 @@ int b2s_split_f16(const float *x, b2s_half *hi, b2s_half *lo, const int *num_row
 int b2s_merge_f16(const b2s_half *hi, const b2s_half *lo, float *x, const int *num_rows_dev, int cap_rows,
                   int row_floats, int in_stride, void *stream);
 /* b2s_split_f16 of x * 2^e with 2^e chosen on the device from max|x| over the live rows (the b2second.tc.pow2_scale
- * rule: max|x| * 2^e in (2^12, 2^13]; 2^e = 1 when x is all zero or not finite) -- for gradients, which are often far
- * below the fp16 normal range.  scale_dev [2] floats: [0] <- 2^-e (multiply the tensor-core result by it), [1] is
- * workspace.  Two launches, no host sync. */
+ * rule: max|x| over the finite elements, max|x| * 2^e in (2^12, 2^13], e clamped to [-126, 126]; 2^e = 1 when no
+ * finite element is non-zero) -- for gradients, which are often far below the fp16 normal range.  Unlike b2s_split_f16
+ * nothing saturates: +-inf and NaN go through as hi = x, lo = +0, so they reach the result as in fp32 arithmetic.
+ * scale_dev [2] floats: [0] <- 2^-e (multiply the tensor-core result by it), [1] is workspace.  Two launches, no host
+ * sync. */
 int b2s_split_f16_autoscale(const float *x, b2s_half *hi, b2s_half *lo, const int *num_rows_dev, int cap_rows,
                             int row_floats, int out_channels, int out_stride, float *scale_dev, void *stream);
 
@@ -874,8 +876,10 @@ int b2s_train_metrics(const float *cls_preds, int num_class, const void *labels,
  * L[k] = w[flip ? K-1-k : k]^T (transpose 1: the input gradient's weights).  With n_in x n_out the channels of L, the
  * planes are [ceil(K / P), n_out, 64] halves, P = 64 / n_in' kernel offsets per 128-byte K block, n_in' = n_in padded to
  * 8 (n_in in 1..8, 16, 32, 64).  scale_dev: device float32 [3]; [0] = s, the power of two with max|w| * s in
- * (2^12, 2^13] (1 for zero or non-finite weights), [1] = 1/s, [2] scratch.  A memset and two kernels (max|w| as integer
- * atomicMax on the bit patterns, then the pack and split); no sync. */
+ * (2^12, 2^13] over the finite weights, clamped to [2^-126, 2^126] (1 when no finite weight is non-zero), [1] = 1/s,
+ * [2] scratch.  A non-finite weight is packed as itself (hi = w, lo = +0; tc.split_f16 would saturate it), so the planes
+ * equal the host path's for finite weights.  A memset and two kernels (max|w| as integer atomicMax on the bit patterns,
+ * then the pack and split); no sync. */
 int b2s_pack_sparse_weights(const float *w, int K, int cin, int cout, int transpose, int flip, b2s_half *hi,
                             b2s_half *lo, float *scale_dev, void *stream);
 
@@ -886,11 +890,13 @@ int b2s_pack_sparse_weights(const float *w, int K, int cin, int cout, int transp
 /* fp32 map x, [B, C, H, W] (layout B2S_LAYOUT_NCHW) or [B, H, W, C] (B2S_LAYOUT_NHWC, 16-byte aligned) -> x * 2^e as
  * fp16 hi/lo planes [B, H+2, W+2, C] with a zero halo (the input b2s_conv2d_tc_ex and b2s_conv2d_wgrad_tc read), with e
  * picked on the device from max|x| by the b2s_split_f16_autoscale rule.  C multiple of 8.  scale_dev [2] floats: [0] <-
- * 2^-e, [1] workspace.  A non-finite x raises B2S_STATUS_F16_RANGE (status_dev may be NULL).  A memset, two kernels. */
+ * 2^-e, [1] workspace.  A non-finite element goes through as hi = x, lo = +0 (as in b2s_split_f16_autoscale) and raises
+ * B2S_STATUS_F16_RANGE (status_dev may be NULL).  A memset, two kernels. */
 int b2s_split_halo_f16_autoscale(const float *x, int layout, int batch, int C, int H, int W, b2s_half *hi, b2s_half *lo,
                                  float *scale_dev, unsigned *status_dev, void *stream);
 /* torch weight w [cout, cin, 3, 3] fp32 -> the b2s_conv2d_tc_ex weight planes, scaled by the power of two s with
- * max|w| * s in (2^12, 2^13] (as b2s_pack_sparse_weights; scale_dev [3]: [0] = s, [1] = 1/s, [2] scratch).
+ * max|w| * s in (2^12, 2^13] (as b2s_pack_sparse_weights, non-finite weights and the clamp included; scale_dev [3]:
+ * [0] = s, [1] = 1/s, [2] scratch).
  * transpose 0: L[tap][o][i] = w[o][i][tap] (n_out = cout, n_in = cin, the forward); transpose 1: L[tap][o][i] =
  * w[i][o][8 - tap] (n_out = cin, n_in = cout, the input gradient).  Planes [G][9][n_pad][n_in] halves with G =
  * ceil(n_out / 128) launches of up to 128 output channels, n_pad = min(n_out, 128), zero rows past n_out.  cin, cout

@@ -14,11 +14,15 @@ from torch import nn
 def pow2_scale(w):
     """power of two s with max|w| * s in (2^12, 2^13]: fp16 keeps 11 significant bits down to 2^-14, so after this
     scaling the lo plane of every weight above 2^-17 of the largest one is a NORMAL fp16 (full 22-bit split);
-    2^13 leaves three binades of head-room below the fp16 maximum.  The kernels multiply by 1/s in the epilogue."""
-    m = float(w.detach().abs().max()) if w.numel() else 0.0
-    if not np.isfinite(m) or m <= 0.0:
+    2^13 leaves three binades of head-room below the fp16 maximum.  The kernels multiply by 1/s in the epilogue.
+    max|w| is taken over the finite elements (1 when none is non-zero), and the exponent is clamped to [-126, 126] so
+    that s and 1/s are normal floats -- the rule of the device-side packs and splits (csrc/autoscale.cuh)."""
+    a = w.detach().abs()
+    a = a[torch.isfinite(a)]
+    m = float(a.max()) if a.numel() else 0.0
+    if m <= 0.0:
         return 1.0
-    return float(2.0 ** (13 - int(np.ceil(np.log2(m)))))
+    return float(2.0 ** min(max(13 - int(np.ceil(np.log2(m))), -126), 126))
 
 
 def split_f16(t, scale=1.0):

@@ -47,17 +47,15 @@ inline int num_slabs(int B, int H, int W) { return (num_strips(B, H, W) + WS_SLA
 
 // fp32 map [B, C, H, W] (layout NCHW) or [B, H, W, C] (NHWC) -> x * 2^e as fp16 hi/lo planes [B, H+2, W+2, C] with a zero
 // halo.  One thread per (padded pixel, 8 channels); for NCHW consecutive threads take consecutive pixels of one channel
-// group, so the reads of each channel row are coalesced.
+// group, so the reads of each channel row are coalesced.  A non-finite element goes through as itself
+// (split_f16_keep_nonfinite) and raises B2S_STATUS_F16_RANGE.
 __global__ void k_split_halo(const float *__restrict__ x, int layout, int B, int C, int H, int W, __half *__restrict__ hi,
                              __half *__restrict__ lo, float *__restrict__ scale_dev, unsigned *__restrict__ status)
 {
-    const unsigned amax = *reinterpret_cast<const volatile unsigned *>(scale_dev + 1);
-    const int e = autoscale_exponent(amax);
+    const int e = autoscale_exponent(*reinterpret_cast<const volatile unsigned *>(scale_dev + 1));
     const float s = ldexpf(1.f, e);
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        scale_dev[0] = ldexpf(1.f, -e);
-        if (amax >= 0x7F800000u && status) atomicOr(status, B2S_STATUS_F16_RANGE);
-    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) scale_dev[0] = ldexpf(1.f, -e);
+    bool nonfinite = false;
     const int G = C / 8, Hp = H + 2, Wp = W + 2;
     const long long n = (long long)B * Hp * Wp * G;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -90,7 +88,8 @@ __global__ void k_split_halo(const float *__restrict__ x, int layout, int B, int
             uint32_t h[4], l[4];
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                const uint32_t pa = split_f16(v[2 * j]), pb = split_f16(v[2 * j + 1]);
+                nonfinite |= !isfinite(v[2 * j]) || !isfinite(v[2 * j + 1]);
+                const uint32_t pa = split_f16_keep_nonfinite(v[2 * j]), pb = split_f16_keep_nonfinite(v[2 * j + 1]);
                 h[j] = __byte_perm(pa, pb, 0x5410);
                 l[j] = __byte_perm(pa, pb, 0x7632);
             }
@@ -100,6 +99,7 @@ __global__ void k_split_halo(const float *__restrict__ x, int layout, int B, int
         *reinterpret_cast<uint4 *>(hi + pix * C + g * 8) = h4;
         *reinterpret_cast<uint4 *>(lo + pix * C + g * 8) = l4;
     }
+    if (nonfinite && status) atomicOr(status, B2S_STATUS_F16_RANGE);
 }
 
 // MN-major SWIZZLE_128B descriptor: the 8-row (pixel) groups along K are 1024 B apart.  An operand here is one 64-wide

@@ -170,7 +170,7 @@ __global__ void k_pack_sparse_weights(const float *__restrict__ w, int K, int ci
                                       int n_in, int n_in_pad, int n_out, int nkb, __half *__restrict__ hi,
                                       __half *__restrict__ lo, float *__restrict__ scale_dev)
 {
-    const int e = pow2_exponent(*reinterpret_cast<const volatile unsigned *>(scale_dev + 2));
+    const int e = autoscale_exponent(*reinterpret_cast<const volatile unsigned *>(scale_dev + 2));
     const float s = (float)ldexp(1.0, e);
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         scale_dev[0] = s;
@@ -196,7 +196,8 @@ __global__ void k_pack_sparse_weights(const float *__restrict__ w, int K, int ci
         uint32_t h[4], l[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            const uint32_t pa = b2s_tc::split_f16(v[2 * j]), pb = b2s_tc::split_f16(v[2 * j + 1]);
+            const uint32_t pa = b2s_tc::split_f16_keep_nonfinite(v[2 * j]),
+                           pb = b2s_tc::split_f16_keep_nonfinite(v[2 * j + 1]);
             h[j] = __byte_perm(pa, pb, 0x5410);
             l[j] = __byte_perm(pa, pb, 0x7632);
         }
@@ -212,7 +213,7 @@ __global__ void k_pack_conv2d_weights(const float *__restrict__ w, int cout, int
                                       int n_out, int n_pad, int groups, __half *__restrict__ hi, __half *__restrict__ lo,
                                       float *__restrict__ scale_dev)
 {
-    const int e = pow2_exponent(*reinterpret_cast<const volatile unsigned *>(scale_dev + 2));
+    const int e = autoscale_exponent(*reinterpret_cast<const volatile unsigned *>(scale_dev + 2));
     const float s = (float)ldexp(1.0, e);
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         scale_dev[0] = s;
@@ -237,7 +238,8 @@ __global__ void k_pack_conv2d_weights(const float *__restrict__ w, int cout, int
         uint32_t h[4], l[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            const uint32_t pa = b2s_tc::split_f16(v[2 * j]), pb = b2s_tc::split_f16(v[2 * j + 1]);
+            const uint32_t pa = b2s_tc::split_f16_keep_nonfinite(v[2 * j]),
+                           pb = b2s_tc::split_f16_keep_nonfinite(v[2 * j + 1]);
             h[j] = __byte_perm(pa, pb, 0x5410);
             l[j] = __byte_perm(pa, pb, 0x7632);
         }
@@ -264,7 +266,7 @@ __global__ void k_split_f16_scaled(const float *__restrict__ x, __half *__restri
             const int c = c0 + 2 * j;
             const float a = c < row_floats ? __ldg(&x[row * row_floats + c]) * s : 0.f;    // power of two: exact
             const float b = c + 1 < row_floats ? __ldg(&x[row * row_floats + c + 1]) * s : 0.f;
-            const uint32_t pa = b2s_tc::split_f16(a), pb = b2s_tc::split_f16(b);
+            const uint32_t pa = b2s_tc::split_f16_keep_nonfinite(a), pb = b2s_tc::split_f16_keep_nonfinite(b);
             h[j] = __byte_perm(pa, pb, 0x5410);
             l[j] = __byte_perm(pa, pb, 0x7632);
         }

@@ -153,6 +153,18 @@ __device__ __forceinline__ uint32_t split_f16(float v)
     asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(l) : "f"(v - hf));
     return (uint32_t)h | ((uint32_t)l << 16);
 }
+// the split of the automatically scaled paths (training inputs, gradients, weight packs): v is x * 2^e with
+// max|x_finite| * 2^e <= 2^13, so a finite v never needs the saturation.  A non-finite v stays itself in hi (+-inf, NaN)
+// with lo = +0, so it reaches the result as torch's fp32 arithmetic would carry it.
+__device__ __forceinline__ uint32_t split_f16_keep_nonfinite(float v)
+{
+    uint16_t h, l;
+    float hf;
+    asm("cvt.rn.f16.f32 %0, %1;" : "=h"(h) : "f"(v));
+    asm("cvt.f32.f16 %0, %1;" : "=f"(hf) : "h"(h));
+    asm("cvt.rn.f16.f32 %0, %1;" : "=h"(l) : "f"(isfinite(v) ? v - hf : 0.f));
+    return (uint32_t)h | ((uint32_t)l << 16);
+}
 __device__ __forceinline__ float f16_bits_to_float(uint16_t h)
 {
     float f;

@@ -171,7 +171,8 @@ class _SparseConvFunction(torch.autograd.Function):
     def forward(ctx, feats, weight, bias, conv, rb):
         ctx.conv, ctx.rb = conv, rb
         ctx.save_for_backward(feats, weight)
-        return conv._forward_rows(feats, rb)
+        out, ctx.x_split = conv._forward_rows(feats, rb)
+        return out
 
     @staticmethod
     def backward(ctx, dy):
@@ -183,7 +184,7 @@ class _SparseConvFunction(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             dx = conv._dgrad(dy, weight, rb, feats.shape[0], split)
         if ctx.needs_input_grad[1]:
-            dw = conv._wgrad(feats, dy, rb, split).view_as(weight)
+            dw = conv._wgrad(feats, dy, rb, split, ctx.x_split).view_as(weight)
         if ctx.needs_input_grad[2]:
             db = dy.sum(0)
         return dx, dw, db, None, None
@@ -303,7 +304,8 @@ def _pack_tc_weights(w, transpose=False, flip=False):
     """fp32 weight [K, Cin, Cout] -> (hi, lo, s, 1/s): the fp16 planes of W[k] (transpose: W[k]^T, flip: W[K-1-k]^T) in
     the tensor-core kernel's packed layout, pre-scaled by the power of two s of b2second.tc.pow2_scale, with s and 1/s as
     [1] device tensors.  b2s_pack_sparse_weights reduces max|w| on the device, so nothing is read on the host; the
-    planes and the scale are bit for bit tc.split_f16(tc.pack_sparse_weights(...), tc.pow2_scale(...))."""
+    planes and the scale are bit for bit tc.split_f16(tc.pack_sparse_weights(...), tc.pow2_scale(...)) for finite weights
+    (a non-finite weight is packed as itself, not saturated)."""
     lib = _lib.load()
     K, cin, cout = (int(v) for v in w.shape)
     n_in, n_out = (cout, cin) if transpose else (cin, cout)
@@ -469,33 +471,36 @@ class SparseConvolution(SparseModule):
     _b2s_backward = False
 
     def _forward_rows(self, feats, rb):
-        """fp32 output rows [n_out, Cout] (+ bias) from fp32 input rows, on the kernel the inference path would pick
-        (tensor pipe with fp32 output, or b2s_sparse_conv)."""
+        """(fp32 output rows [n_out, Cout] (+ bias) from fp32 input rows, the _GradSplit of X or None) on the kernel the
+        inference path would pick (tensor pipe with fp32 output, or b2s_sparse_conv).  On the tensor pipe X is split
+        under its own power-of-two scale, as in the backward: unscaled, an activation above 65504 would saturate and one
+        below 2^-3 keep only 2^-25 absolute precision.  The split is kept for the weight gradient."""
         lib = _lib.load()
-        K, n_in, n_out = rb.K, feats.shape[0], rb.num_out
+        K, n_out = rb.K, rb.num_out
         dev = feats.device
         shift = self.bias.detach().float().contiguous() if self.bias is not None else None
         out = torch.empty(n_out, self.out_channels, dtype=torch.float32, device=dev)
         if n_out == 0:
-            return out
+            return out, None
         cin_tc = self._wgrad_tc_cin(lib, K)
         if cin_tc is not None:
-            buf = self._split_rows(feats, cin_tc)
-            hi, lo = buf[:, 0], buf[:, 1]
+            split = _GradSplit(feats, cin_tc)
+            hi, lo, stride, inv_x = split.planes()
             w_hi, w_lo, ws, inv = self._tc_weights(cin_tc)
+            scale = inv * inv_x                                        # powers of two: exact, no host sync
             status = torch.zeros(1, dtype=torch.int32, device=dev)
             perm, tmask = ops.tile_plan(rb)
             _lib.check(lib.b2s_sparse_conv_tc_plan(
-                _lib.ptr(hi), _lib.ptr(lo), 2 * cin_tc, buf.shape[0], cin_tc, _lib.ptr(w_hi), _lib.ptr(w_lo),
-                _lib.ptr(rb.nbr), K, _lib.ptr(rb.num_out_dev), n_out, _lib.ptr(perm), _lib.ptr(tmask), _lib.ptr(inv),
+                _lib.ptr(hi), _lib.ptr(lo), stride, hi.shape[0], cin_tc, _lib.ptr(w_hi), _lib.ptr(w_lo),
+                _lib.ptr(rb.nbr), K, _lib.ptr(rb.num_out_dev), n_out, _lib.ptr(perm), _lib.ptr(tmask), _lib.ptr(scale),
                 _lib.ptr(shift), 0, _lib.ptr(out), None, self.out_channels, self.out_channels, _lib.ptr(status),
                 _lib.stream()), "b2s_sparse_conv_tc_plan")
-            return out
+            return out, split
         w = self.weight.detach().float().contiguous().view(K, self.in_channels, self.out_channels)
         _lib.check(lib.b2s_sparse_conv(_lib.ptr(feats), self.in_channels, _lib.ptr(w), _lib.ptr(rb.nbr), K,
                                        _lib.ptr(rb.num_out_dev), n_out, None, _lib.ptr(shift), 0, _lib.ptr(out),
                                        self.out_channels, _lib.stream()), "b2s_sparse_conv")
-        return out
+        return out, None
 
     def _wgrad_tc_cin(self, lib, K):
         """channel count of the tensor-pipe forward / weight gradient (the input padded to 8), or None: fp32 kernels"""
@@ -505,16 +510,6 @@ class SparseConvolution(SparseModule):
                 and bool(lib.b2s_sparse_conv_tc_supported(cin_tc, self.out_channels))):
             return cin_tc
         return None
-
-    def _split_rows(self, feats, cin_tc):
-        """fp32 rows -> interleaved fp16 hi/lo planes [max(n, 1), 2, cin_tc] (b2s_split_f16, zero padded)"""
-        lib = _lib.load()
-        n = feats.shape[0]
-        buf = torch.empty(max(n, 1), 2, cin_tc, dtype=torch.float16, device=feats.device)
-        if n > 0:
-            _lib.check(lib.b2s_split_f16(_lib.ptr(feats), _lib.ptr(buf[:, 0]), _lib.ptr(buf[:, 1]), None, n,
-                                         self.in_channels, cin_tc, 2 * cin_tc, _lib.stream()), "b2s_split_f16")
-        return buf
 
     def _dgrad_weights(self, w, flip):
         """packed fp16 hi/lo planes of W'[k] = W[k]^T (flip: W[K-1-k]^T) for the tensor-pipe input gradient, with their
@@ -567,18 +562,18 @@ class SparseConvolution(SparseModule):
                                        None, 0, _lib.ptr(dx), cin, _lib.stream()), "b2s_sparse_conv")
         return dx
 
-    def _wgrad(self, feats, dy, rb, split=None):
+    def _wgrad(self, feats, dy, rb, split=None, x_split=None):
         """weight gradient [K, Cin, Cout] = sum over output rows of X[nbr[o,k]]^T dY[o]: b2s_sparse_conv_wgrad_tc on the
         tensor pipe, b2s_sparse_conv_wgrad (fp32 FMA) otherwise.  On the tensor pipe both operands are split under their
-        own power-of-two scale (b2s_split_f16_autoscale): the forward's unscaled planes of X carry a small activation
-        with only 2^-25 absolute precision, which a weight gradient of few pairs would see; rows are reduced in the
-        forward's tile-plan order."""
+        own power-of-two scale (b2s_split_f16_autoscale; X's split is the forward's when given): unscaled, a small
+        activation would keep only 2^-25 absolute precision, which a weight gradient of few pairs would see; rows are
+        reduced in the forward's tile-plan order."""
         lib = _lib.load()
         K, cin, cout, n_out = rb.K, self.in_channels, self.out_channels, rb.num_out
         dev = dy.device
         cin_tc = self._wgrad_tc_cin(lib, K)
         if cin_tc is not None and n_out > 0 and feats.shape[0] > 0:
-            x_hi, x_lo, x_stride, inv_x = _GradSplit(feats, cin_tc).planes()
+            x_hi, x_lo, x_stride, inv_x = (x_split or _GradSplit(feats, cin_tc)).planes()
             g_hi, g_lo, g_stride, inv_g = (split or _GradSplit(dy)).planes()
             scale = inv_x * inv_g                                      # powers of two: exact
             perm, tmask = ops.tile_plan(rb)

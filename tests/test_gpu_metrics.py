@@ -233,7 +233,7 @@ def _pairs():
     return out
 
 
-@pytest.mark.parametrize("kind", ["random", "zero", "pow2"])
+@pytest.mark.parametrize("kind", ["random", "zero", "pow2", "tiny", "subnormal"])
 def test_device_pack_equals_host_pack(kind):
     sp = loader.product_spconv()
     pairs = _pairs()
@@ -247,6 +247,10 @@ def test_device_pack_equals_host_pack(kind):
             elif kind == "pow2":
                 w[K // 2, 0, cout - 1] = -0.125          # max |w| is exactly 2^-3
                 w.clamp_(-0.125, 0.125)
+            elif kind == "tiny":                          # max |w| = 2^-120: the scale clamps at 2^126
+                w.mul_(2.0 ** -118).clamp_(-2.0 ** -120, 2.0 ** -120)[K // 2, 0, cout - 1] = 2.0 ** -120
+            elif kind == "subnormal":                     # every weight an fp32 subnormal
+                w.mul_(2.0 ** -128).clamp_(-2.0 ** -127, 2.0 ** -127)
             for transpose, flip in ((False, False), (True, False), (True, True)):
                 if transpose and tc.sparse_tc_cin(cout) != cout:
                     continue
@@ -262,6 +266,8 @@ def test_device_pack_equals_host_pack(kind):
                 assert float(sp._pack_tc_weights(w)[2]) == 2.0 ** 16          # 2^-3 * 2^16 = 2^13
             if kind == "zero":
                 assert float(sp._pack_tc_weights(w)[2]) == 1.0
+            if kind in ("tiny", "subnormal"):
+                assert float(sp._pack_tc_weights(w)[2]) == 2.0 ** 126
 
 
 def _train_step(net, ex):
