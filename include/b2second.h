@@ -88,7 +88,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 211
+#define B2S_VERSION 212
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -632,10 +632,15 @@ int b2s_kitti_overlaps(int metric, const double *gt, const int *gt_off, const do
  * Person_sitting for Pedestrian -- or -3, difficulty 0..2), task_min_overlap float64 [T].  overlaps / ov_off as
  * b2s_kitti_overlaps writes them.  Outputs float64 [T, 41]: precision and orientation after the running max from the
  * right, and the score thresholds (zero past the last).  Frames are reduced in frame order: bit-reproducible.
- * max_dt_per_frame (host) <= 2048.  workspace: b2s_kitti_eval_workspace_bytes(num_frames, num_gt, num_dt, T). */
+ * max_dt_per_frame (host) <= 2048.  workspace: b2s_kitti_eval_workspace_bytes(num_frames, num_gt, num_dt, T).
+ * gt_limits / dt_limits uint8 [num_gt] / [num_dt], required when there are boxes: bit d (0..2) set when clean_data
+ * puts the box outside difficulty d -- ground truth: occluded > (0, 1, 2)[d] or truncated > (0.15, 0.3, 0.5)[d] or y2 - y1 <= (40, 25, 25)[d];
+ * detections: |y2 - y1| < (40, 25, 25)[d] -- compared in the annotation's own dtype, as the reference does (so a
+ * float32 height is a float32 difference); the rows' float64 copies of those fields are not read. */
 size_t b2s_kitti_eval_workspace_bytes(int num_frames, int num_gt, int num_dt, int num_tasks);
-int b2s_kitti_eval(int metric, const double *gt, const int *gt_name, const int *gt_off, int num_gt, const double *dt,
-                   const int *dt_name, const int *dt_off, int num_dt, int num_frames, int max_dt_per_frame,
+int b2s_kitti_eval(int metric, const double *gt, const int *gt_name, const uint8_t *gt_limits, const int *gt_off,
+                   int num_gt, const double *dt, const int *dt_name, const uint8_t *dt_limits, const int *dt_off,
+                   int num_dt, int num_frames, int max_dt_per_frame,
                    const double *overlaps, const long long *ov_off, const int *task_info,
                    const double *task_min_overlap, int num_tasks, int compute_aos, double *precision,
                    double *orientation, double *thresholds, void *workspace, size_t workspace_bytes, void *stream);

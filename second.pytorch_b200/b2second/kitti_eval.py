@@ -9,6 +9,14 @@ Python packs the annotations into flat float64 rows plus int32 frame offsets (in
 encodes the names once into a small vocabulary, and formats the result strings.  The overlaps, ignore flags, matching,
 thresholds and precision run in libb2second.so.  Unlike the reference (whose 50-part split needs at least 50 frames),
 any number of frames >= 1 is accepted, with or without ground truth or detections in each.
+
+clean_data compares each box's height, truncation and occlusion with the difficulty limits in the annotation's own
+dtype: for float32 boxes the height y2 - y1 is a float32 difference, which can be exactly 40 where the float64 one is
+not.  So pack_limits takes those comparisons on the original arrays, with numpy scalar promotion as clean_data's
+scalar code gets it, and hands the kernel one limit bit per (box, difficulty) instead of the widened values.  Under
+numpy 1.x a float32 truncation was compared with the Python float in float64 (np.float32(0.15) > 0.15 is True there,
+False under numpy 2), so float32 truncation results depend on the numpy version, exactly as they do for the
+reference.
 """
 import io
 
@@ -20,6 +28,10 @@ ROW = 16                     # B2S_KITTI_ROW
 DONTCARE = -2                # B2S_KITTI_DONTCARE
 NO_ALT = -3
 MAX_DT_PER_FRAME = 2048
+# clean_data's difficulty tables (eval.py:38-40), Python numbers as there
+MIN_HEIGHT = [40, 25, 25]
+MAX_OCCLUSION = [0, 1, 2]
+MAX_TRUNCATION = [0.15, 0.3, 0.5]
 
 # clean_data's class table (eval.py:34-37) and get_*_eval_result's class_to_name
 CLASS_NAMES = ["car", "pedestrian", "cyclist", "van", "person_sitting", "car", "tractor", "trailer"]
@@ -49,6 +61,43 @@ def encode_names(names):
     uniq, inv = np.unique(np.asarray(names, dtype=str), return_inverse=True)
     codes = np.array([DONTCARE if u == "DontCare" else vocab_id(u.lower()) for u in uniq], dtype=np.int32)
     return codes[inv.reshape(-1)] if len(uniq) else np.zeros(0, np.int32)
+
+
+def _scalar_dtype(a, value):
+    """a's values as clean_data's scalar `a[i] <op> value` compares them: in the dtype numpy's scalar promotion gives a
+    scalar of a's dtype and the Python number value (float32 under numpy 2, float64 under numpy 1.x for a float)."""
+    t = (a.dtype.type(0) + value).dtype
+    return a.astype(t, copy=False), t.type(value)
+
+
+def _exceeds(a, limit):
+    a, v = _scalar_dtype(a, limit)
+    return a > v
+
+
+def difficulty_limits(anno, is_gt):
+    """uint8 [n]: bit d set when clean_data puts the box outside difficulty d -- for ground truth occluded >
+    MAX_OCCLUSION[d] or truncated > MAX_TRUNCATION[d] or height <= MIN_HEIGHT[d], for detections |height| <
+    MIN_HEIGHT[d] -- computed from the anno's own arrays, the height in the bbox's dtype."""
+    bbox = np.asarray(anno["bbox"]).reshape(-1, 4)
+    height = bbox[:, 3] - bbox[:, 1]
+    out = np.zeros(height.shape[0], dtype=np.uint8)
+    for d in range(3):
+        if is_gt:
+            h, v = _scalar_dtype(height, MIN_HEIGHT[d])
+            out_d = (_exceeds(np.asarray(anno["occluded"]), MAX_OCCLUSION[d]) |
+                     _exceeds(np.asarray(anno["truncated"]), MAX_TRUNCATION[d]) | (h <= v))
+        else:
+            h, v = _scalar_dtype(np.abs(height), MIN_HEIGHT[d])
+            out_d = h < v
+        out |= out_d.astype(np.uint8) << d
+    return out
+
+
+def pack_limits(annos, is_gt):
+    """list of anno dicts -> difficulty_limits of every box, frame after frame: uint8 [N], in pack_annos' row order."""
+    parts = [difficulty_limits(a, is_gt) for a in annos if len(a["name"])]
+    return np.concatenate(parts) if parts else np.zeros(0, np.uint8)
 
 
 def pack_annos(annos, with_score):
@@ -120,6 +169,7 @@ class _Packed:
         self.z_axis, self.z_center = int(z_axis), float(z_center)
         gt, gn, go = pack_annos(gt_annos, with_score=False)
         dt, dn, do = pack_annos(dt_annos, with_score=True)
+        gl, dl = pack_limits(gt_annos, is_gt=True), pack_limits(dt_annos, is_gt=False)
         self.F, self.G, self.D = len(gt_annos), gt.shape[0], dt.shape[0]
         ng, nd = np.diff(go).astype(np.int64), np.diff(do).astype(np.int64)
         self.max_dt = int(nd.max(initial=0))
@@ -128,8 +178,8 @@ class _Packed:
         ov_off = np.zeros(self.F + 1, dtype=np.int64)
         np.cumsum(ng * nd, out=ov_off[1:])
         to = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(self.dev)
-        self.gt, self.gn, self.go = to(gt), to(gn), to(go)
-        self.dt, self.dn, self.do = to(dt), to(dn), to(do)
+        self.gt, self.gn, self.go, self.gl = to(gt), to(gn), to(go), to(gl)
+        self.dt, self.dn, self.do, self.dl = to(dt), to(dn), to(do), to(dl)
         self.ov_off, self.n_ov = to(ov_off), int(ov_off[-1])
         self._ov = {}
 
@@ -144,7 +194,7 @@ class _Packed:
             self._ov[metric] = out
         return self._ov[metric]
 
-    def eval(self, metric, current_classes, difficultys, min_overlaps, compute_aos):
+    def eval(self, metric, current_classes, difficultys, min_overlaps, compute_aos, ignored=False):
         L, lib = _lib()
         info, mo = task_table(current_classes, difficultys, min_overlaps, metric)
         T = info.shape[0]
@@ -156,15 +206,25 @@ class _Packed:
             ws = torch.empty(lib.b2s_kitti_eval_workspace_bytes(self.F, self.G, self.D, T), dtype=torch.uint8,
                              device=self.dev)
             with torch.cuda.device(self.dev):
-                L.check(lib.b2s_kitti_eval(int(metric), L.ptr(self.gt), L.ptr(self.gn), L.ptr(self.go), self.G,
-                                           L.ptr(self.dt), L.ptr(self.dn), L.ptr(self.do), self.D, self.F, self.max_dt,
+                L.check(lib.b2s_kitti_eval(int(metric), L.ptr(self.gt), L.ptr(self.gn), L.ptr(self.gl), L.ptr(self.go),
+                                           self.G, L.ptr(self.dt), L.ptr(self.dn), L.ptr(self.dl), L.ptr(self.do),
+                                           self.D, self.F, self.max_dt,
                                            L.ptr(ov), L.ptr(self.ov_off), L.ptr(ti), L.ptr(tm), T, int(bool(compute_aos)),
                                            L.ptr(prec), L.ptr(aos), L.ptr(thr), L.ptr(ws), ws.numel(), L.stream()),
                         "b2s_kitti_eval")
         shape = (len(current_classes), len(difficultys), min_overlaps.shape[0], N_SAMPLE_PTS)
-        return {"recall": np.zeros(shape), "precision": prec.cpu().numpy().reshape(shape),
-                "orientation": aos.cpu().numpy().reshape(shape), "thresholds": thr.cpu().numpy().reshape(shape),
-                "min_overlaps": min_overlaps}
+        out = {"recall": np.zeros(shape), "precision": prec.cpu().numpy().reshape(shape),
+               "orientation": aos.cpu().numpy().reshape(shape), "thresholds": thr.cpu().numpy().reshape(shape),
+               "min_overlaps": min_overlaps}
+        if ignored:
+            # clean_data's flags as the kernel left them in the workspace: after three int32 [T] counters, int8
+            # ignored_gt [T, G] then ignored_dt [T, D], each block 256-byte aligned (carve in kitti_eval.cu)
+            align = lambda n: (n + 255) // 256 * 256
+            w = ws.cpu().numpy().view(np.int8) if T else np.zeros(0, np.int8)
+            o = align(12 * T)
+            flags = lambda lo, n: w[lo:lo + T * n].reshape(shape[:3] + (n,))
+            out["ignored_gt"], out["ignored_dt"] = flags(o, self.G), flags(o + align(T * self.G), self.D)
+        return out
 
 
 def _device(device):
@@ -176,12 +236,14 @@ def _device(device):
 
 
 def eval_class(gt_annos, dt_annos, current_classes, difficultys, metric, min_overlaps, compute_aos=False, z_axis=1,
-               z_center=1.0, device=None):
+               z_center=1.0, device=None, ignored=False):
     """eval_class_v3: {"recall" (zeros, as the reference), "precision", "orientation", "thresholds"} each
-    [num_class, num_difficulty, num_minoverlap, 41], and "min_overlaps" [num_minoverlap, 3, num_class]."""
+    [num_class, num_difficulty, num_minoverlap, 41], and "min_overlaps" [num_minoverlap, 3, num_class].  ignored:
+    also clean_data's "ignored_gt" [num_class, num_difficulty, num_minoverlap, num_gt] and "ignored_dt" [..., num_dt]
+    (int8, -1 / 0 / 1, all frames' boxes in order) as the kernel computed them."""
     p = _Packed(gt_annos, dt_annos, z_axis, z_center, _device(device))
     return p.eval(metric, list(current_classes), list(difficultys), np.asarray(min_overlaps, dtype=np.float64),
-                  compute_aos)
+                  compute_aos, ignored)
 
 
 # ------------------------------------------------------------------------------------------------ host: results

@@ -18,11 +18,6 @@ constexpr int kSamplePts = 41;                 // N_SAMPLE_PTS of eval_class_v3
 constexpr int kMaxDtPerFrame = 2048;           // assigned_detection bitmask held per thread
 constexpr double kNoDetection = -10000000.0;   // NO_DETECTION of compute_statistics_jit
 
-// clean_data's difficulty tables (eval.py:38-40)
-__constant__ double c_min_height[3] = {40.0, 25.0, 25.0};
-__constant__ double c_max_occlusion[3] = {0.0, 1.0, 2.0};
-__constant__ double c_max_truncation[3] = {0.15, 0.3, 0.5};
-
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
@@ -203,9 +198,11 @@ __device__ __forceinline__ Task load_task(const int *task_info, const double *ta
     return Task{task_info[3 * t], task_info[3 * t + 1], task_info[3 * t + 2], task_min_overlap[t]};
 }
 
-// clean_data (eval.py:33-89) for every (task, box): ignored_gt / ignored_dt in {-1, 0, 1}; num_valid_gt per task
-__global__ void k_kitti_clean(const double *__restrict__ gt, const int *__restrict__ gt_name, int G,
-                              const double *__restrict__ dt, const int *__restrict__ dt_name, int D,
+// clean_data (eval.py:33-89) for every (task, box): ignored_gt / ignored_dt in {-1, 0, 1}; num_valid_gt per task.
+// Whether a box lies outside the task's difficulty (height, truncation, occlusion) is bit `difficulty` of its limits
+// byte: the host takes those comparisons in the annotation's own dtype, as the reference does.
+__global__ void k_kitti_clean(const int *__restrict__ gt_name, const uint8_t *__restrict__ gt_limits, int G,
+                              const int *__restrict__ dt_name, const uint8_t *__restrict__ dt_limits, int D,
                               const int *__restrict__ task_info, const double *__restrict__ task_min_overlap, int T,
                               int8_t *__restrict__ ign_gt, int8_t *__restrict__ ign_dt, int *__restrict__ num_valid)
 {
@@ -216,12 +213,9 @@ __global__ void k_kitti_clean(const double *__restrict__ gt, const int *__restri
         const Task task = load_task(task_info, task_min_overlap, t);
         const int diff = task.difficulty;
         if (k < G) {
-            const double *b = gt + (size_t)k * B2S_KITTI_ROW;
             const int name = gt_name[k];
             const int valid = (name == task.cls) ? 1 : (name == task.alt) ? 0 : -1;
-            const double height = dsub(b[3], b[1]);
-            const bool ignore = b[14] > c_max_occlusion[diff] || b[13] > c_max_truncation[diff] ||
-                                height <= c_min_height[diff];
+            const bool ignore = (gt_limits[k] >> diff) & 1;
             int8_t v;
             if (valid == 1 && !ignore) {
                 v = 0;
@@ -234,9 +228,7 @@ __global__ void k_kitti_clean(const double *__restrict__ gt, const int *__restri
             ign_gt[(size_t)t * G + k] = v;
         } else {
             const int j = k - G;
-            const double *b = dt + (size_t)j * B2S_KITTI_ROW;
-            const double height = fabs(dsub(b[3], b[1]));
-            ign_dt[(size_t)t * D + j] = (height < c_min_height[diff]) ? 1 : (dt_name[j] == task.cls) ? 0 : -1;
+            ign_dt[(size_t)t * D + j] = ((dt_limits[j] >> diff) & 1) ? 1 : (dt_name[j] == task.cls) ? 0 : -1;
         }
     }
 }
@@ -524,8 +516,9 @@ extern "C" size_t b2s_kitti_eval_workspace_bytes(int num_frames, int num_gt, int
     return carve(nullptr, num_frames, num_gt, num_dt, num_tasks).bytes;
 }
 
-extern "C" int b2s_kitti_eval(int metric, const double *gt, const int *gt_name, const int *gt_off, int num_gt,
-                              const double *dt, const int *dt_name, const int *dt_off, int num_dt, int num_frames,
+extern "C" int b2s_kitti_eval(int metric, const double *gt, const int *gt_name, const uint8_t *gt_limits,
+                              const int *gt_off, int num_gt, const double *dt, const int *dt_name,
+                              const uint8_t *dt_limits, const int *dt_off, int num_dt, int num_frames,
                               int max_dt_per_frame, const double *overlaps, const long long *ov_off,
                               const int *task_info, const double *task_min_overlap, int num_tasks, int compute_aos,
                               double *precision, double *orientation, double *thresholds, void *workspace,
@@ -536,6 +529,8 @@ extern "C" int b2s_kitti_eval(int metric, const double *gt, const int *gt_name, 
                 "b2s_kitti_eval: bad arguments");
     B2S_REQUIRE(max_dt_per_frame <= kMaxDtPerFrame, "b2s_kitti_eval: %d detections in one frame (at most %d)",
                 max_dt_per_frame, kMaxDtPerFrame);
+    B2S_REQUIRE((num_gt == 0 || gt_limits != nullptr) && (num_dt == 0 || dt_limits != nullptr),
+                "b2s_kitti_eval: gt_limits / dt_limits (difficulty limit bits) are required");
     if (num_tasks == 0) return 0;
     const int F = num_frames, G = num_gt, D = num_dt, T = num_tasks, Gp = next_pow2(G > 0 ? G : 1);
     EvalWorkspace w = carve((char *)workspace, F, G, D, T);
@@ -545,8 +540,8 @@ extern "C" int b2s_kitti_eval(int metric, const double *gt, const int *gt_name, 
         long long total = (long long)T * (G + D);
         int blocks = b2s_cdiv(total, 256);
         if (blocks > 132 * 16) blocks = 132 * 16;
-        k_kitti_clean<<<blocks, 256, 0, stream>>>(gt, gt_name, G, dt, dt_name, D, task_info, task_min_overlap, T,
-                                                  w.ign_gt, w.ign_dt, w.num_valid);
+        k_kitti_clean<<<blocks, 256, 0, stream>>>(gt_name, gt_limits, G, dt_name, dt_limits, D, task_info,
+                                                  task_min_overlap, T, w.ign_gt, w.ign_dt, w.num_valid);
         B2S_LAUNCH_OK();
     }
     k_kitti_pass1<<<b2s_cdiv((long long)T * F, 128), 128, 0, stream>>>(

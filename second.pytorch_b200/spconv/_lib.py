@@ -132,9 +132,9 @@ SIGNATURES = {
     "b2s_kitti_overlaps": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int,
                                    ctypes.c_double, c_void_p, c_void_p]),
     "b2s_kitti_eval_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
-    "b2s_kitti_eval": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                               c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
-                               c_void_p, c_size_t, c_void_p]),
+    "b2s_kitti_eval": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                               c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                               c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "b2s_assign_targets_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b2s_assign_targets": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int,
                                    c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p,
@@ -246,7 +246,7 @@ def load():
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
-    if lib.b2s_version() < 203:
+    if lib.b2s_version() < 212:
         raise ImportError("libb2second.so is too old")
     _lib = lib
     return lib
