@@ -36,6 +36,23 @@ def make_cloud(name, seed, n):
     return synth.kitti_cloud(seed, n, cfg.point_cloud_range)
 
 
+def border_cloud(cfg, F, seed, n=2000):
+    """points on the first and last row and column of the voxel grid (hence of the BEV map), z mid-range"""
+    rng = np.random.default_rng(seed)
+    r, vs = np.asarray(cfg.point_cloud_range, np.float64), np.asarray(cfg.voxel_size, np.float64)
+    pts = np.zeros((n, F), np.float32)
+    side = np.arange(n) % 4
+    t = rng.random(n)
+    x = r[0] + t * (r[3] - r[0])
+    y = r[1] + t * (r[4] - r[1])
+    x = np.where(side == 0, r[0] + 0.25 * vs[0], np.where(side == 1, r[3] - 0.25 * vs[0], x))
+    y = np.where(side == 2, r[1] + 0.25 * vs[1], np.where(side == 3, r[4] - 0.25 * vs[1], y))
+    pts[:, 0], pts[:, 1] = x, y
+    pts[:, 2] = 0.5 * (r[2] + r[5]) + 0.25 * (r[5] - r[2]) * (rng.random(n) - 0.5)
+    pts[:, 3:] = rng.random((n, F - 3))
+    return pts
+
+
 def assert_detections_close(got, fix, box_tol=1e-4, score_tol=1e-5):
     gb = np.asarray(got["box3d_lidar"], dtype=np.float32)
     gs = np.asarray(got["scores"], dtype=np.float32)

@@ -22,6 +22,10 @@ import torch
 CASES = "abcde"
 CONFIGS = ["car.fhd", "all.fhd", "pointpillars.car.xyres_16", "nuscenes.all.pp.largea", "nuscenes.all.pp.mhead"]
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "loss")
+# the bounds of the loss checks (tests/test_gpu_loss.py docstring): scalars within 1e-5 relative, every element of
+# the per-anchor outputs and gradients within C_REL eps32 |v64| + C_MAX eps32 max|v64|
+EPS32 = float(np.finfo(np.float32).eps)
+C_REL, C_MAX = 8.0, 1.0
 SCALARS = ["loss", "cls_loss_reduced", "loc_loss_reduced", "dir_loss_reduced", "cls_pos_loss", "cls_neg_loss"]
 
 
@@ -212,3 +216,13 @@ def reference_run(s, example, preds, dtype):
     out = {k: r[k].detach().numpy() for k in SCALARS + ["cls_loss", "loc_loss", "cared", "dir_bins"]}
     grads = {k: pr[k].grad.numpy() for k in pr}
     return out, grads
+
+
+def check_scalars(got, want64, what):
+    """the six scalars (SCALARS order) within 1e-5 relative of float64, within 1e-7 absolute where that is 0"""
+    got = np.asarray(got, np.float64)
+    for k, g, w in zip(SCALARS, got, want64):
+        if w == 0:
+            assert abs(g) <= 1e-7, (what, k, g)
+        else:
+            assert abs(g - w) <= 1e-5 * abs(w), (what, k, g, w)

@@ -171,3 +171,14 @@ def assert_targets_match(got, want, log_ulp=4):
     if len(want):
         d = ulp_diff(got[:, list(LOG_COLUMNS)], want[:, list(LOG_COLUMNS)])
         assert d.max() <= log_ulp, "log components differ by %d ulp" % d.max()
+
+
+def check_frame(labels, tg, imp, fr):
+    """one frame's CUDA labels, box targets and importance against the expected ones of `fr` (labels,
+    importance_out, pos, targets): equal, the log components of the targets within assert_targets_match's ulp"""
+    labels, tg, imp = (x.cpu().numpy() for x in (labels, tg, imp))
+    np.testing.assert_array_equal(labels, fr["labels"])
+    np.testing.assert_array_equal(imp, fr["importance_out"])
+    np.testing.assert_array_equal(np.flatnonzero(labels > 0), fr["pos"])
+    assert_targets_match(tg[fr["pos"]], fr["targets"])
+    assert not tg[labels <= 0].any()

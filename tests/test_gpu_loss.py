@@ -20,8 +20,7 @@ from b2second import config, loader, loss, models, targets, training
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-EPS32 = float(np.finfo(np.float32).eps)
-C_REL, C_MAX = 8.0, 1.0
+EPS32, C_REL, C_MAX = lr.EPS32, lr.C_REL, lr.C_MAX
 
 
 def _plan(name):
@@ -47,13 +46,7 @@ def _check_elem(got, want, what):
         what, int(bad.sum()), float(err[bad].max()), float(bound[bad][np.argmax(err[bad])]))
 
 
-def _check_scalars(got, want64, what):
-    got = np.asarray(got, np.float64)
-    for k, g, w in zip(lr.SCALARS, got, want64):
-        if w == 0:
-            assert abs(g) <= 1e-7, (what, k, g)
-        else:
-            assert abs(g - w) <= 1e-5 * abs(w), (what, k, g, w)
+_check_scalars = lr.check_scalars
 
 
 def _scalars(r):

@@ -90,6 +90,23 @@ def test_layer_against_float64(case):
     assert torch.equal(dx2.view(torch.int32), dx.view(torch.int32))
 
 
+@pytest.mark.timeout(600)
+def test_layer_one_sign_against_float64():
+    """car.fhd's 200 x 176 map at its training batch B = 8, 128 -> 128, X post-ReLU (every term of one sign) and dY of
+    mostly one sign: the accumulator cuts toward zero add up instead of cancelling.  Forward and dX (k_conv_tc) meet
+    the tc_ref bound plus engine_ref's accumulation-chain term, dW (b2s_conv2d_wgrad_tc) the bound plus the chain term
+    in its strip and slab order (train_ref.wgrad_chain_term): the terms tc_ref's ALPHA, calibrated on random-sign data,
+    leaves out"""
+    import train_ref
+    conv, g = _layer(128, 128, 3)
+    B, H, W = 8, 200, 176
+    x = torch.relu(torch.randn(B, 128, H, W, generator=g) + 0.5).to(DEV)
+    dy = ((torch.randn(B, 128, H, W, generator=g) * 0.5 + 1.0) * 2.0 ** -20).to(DEV)
+    y, dx, dw = _run_layer(conv, x, dy)
+    ws = 1.0 / float(rpn_train.pack_weights(conv, False)[2])
+    train_ref.check_conv3x3_train(x, dy, y, dx, dw, conv.weight.detach(), ws, "one-sign 128 -> 128")
+
+
 def test_layer_scale_follows_the_input():
     """the same layer at input scales 2^-30 and 2^20: results scale exactly (the split picks a new 2^e each call)"""
     conv, g = _layer(128, 128, 2)

@@ -16,13 +16,7 @@ def _anchors_dict(plan):
     return {plan.classes[i]: {"anchors": plan.anchors[s.begin:s.end]} for i, s in enumerate(plan.segments)}
 
 
-def _check(labels, tg, imp, fr):
-    labels, tg, imp = (x.cpu().numpy() for x in (labels, tg, imp))
-    np.testing.assert_array_equal(labels, fr["labels"])
-    np.testing.assert_array_equal(imp, fr["importance_out"])
-    np.testing.assert_array_equal(np.flatnonzero(labels > 0), fr["pos"])
-    tr.assert_targets_match(tg[fr["pos"]], fr["targets"])
-    assert not tg[labels <= 0].any()
+_check = tr.check_frame
 
 
 def _pack(plan, frames, device=DEV):
