@@ -32,6 +32,9 @@
  *                       second/pytorch/train.py through SubMConv3d / SparseConv3d)
  *   b2s_pfn             PillarFeatureNet.forward (pointpillars.py:203-237, single PFNLayer :51-65)
  *   b2s_pfn_ex          the same, or PillarFeatureNetRadius.forward (pointpillars.py:240-325)
+ *   b2s_pfn_train_forward, b2s_pfn_train_backward
+ *                       PillarFeatureNet / PillarFeatureNetRadius.forward in train() mode and its autograd backward
+ *                       (pointpillars.py:51-65,203-237,290-325): train-mode BatchNorm1d with its running-buffer update
  *   b2s_crop_nhwc       stage0[:, :, c:-c, c:-c] in VoxelNetNuscenesMultiHead.network_forward
  *                       (second/pytorch/models/net_multi_head.py:155-160)
  *   b2s_decode_filter   box_coder.decode_torch + sigmoid + score threshold
@@ -88,7 +91,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 212
+#define B2S_VERSION 213
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -471,6 +474,41 @@ int b2s_pfn_ex(const float *points, int num_feat, const int *point_slots, const 
                const float *weight /*[Cout, F+5] or [Cout, F+4]*/, const float *scale, const float *shift, int cout,
                float vx, float vy, float x_offset, float y_offset, int decoration, float *out /*[cap_rows,Cout]*/,
                void *stream);
+
+/* ---- PointPillars feature net in training (csrc/pfn_train.cu) ----------------------------------------------------
+ * One PFNLayer of PillarFeatureNet (B2S_PFN_PLAIN) or PillarFeatureNetRadius (B2S_PFN_RADIUS) in train() mode
+ * (pointpillars.py:51-65,203-237,290-325): Linear(D -> 64, no bias), BatchNorm1d over all N * T slots with batch
+ * statistics, ReLU, max over the T slots; D = num_feat + 5 (plain) or + 4 (radius).  The padded [N, T, 64] map is never
+ * built: the BN statistics come from the float64 mean mu and covariance C of the decorated inputs d (padded slots are
+ * zero rows and count in M = N * T), mean_c = w_c . mu, var_c = w_c^T C w_c, and the weight gradient is the closed form
+ *   dW_c = gamma_c s_c (G - A mu - B s_c C w_c),  s_c = 1 / sqrt(var_c + eps),
+ * with A = sum delta (= dbeta), B = sum delta xhat (= dgamma), G = sum delta d over the argmax slot of each (n, c),
+ * delta = dout[n, c] * [out[n, c] > 0].  No input gradient (the voxels are data).  Sums run in one fixed order in
+ * float64 (no float atomics: two runs give the same bits); no entry point syncs, so both can be captured.
+ *   voxels      [num_rows, max_points, num_feat] fp32 (the training example's `voxels`); only the first
+ *               num_points[n] slots of a row are read, the others are taken as the zero rows upstream masks them to;
+ *   num_points  [num_rows] int32; a count outside [1, max_points] raises B2S_STATUS_BAD_INPUT (it is clamped);
+ *   coors       [num_rows, 4] int32 (b, z, y, x), 16-byte aligned;  max_points <= 254 (the argmax is one byte);
+ *   weight      [64, D] fp32;  gamma, beta [64];  cout must be 64;
+ *   running_mean, running_var [64] fp32, num_batches_tracked int64 [1]: updated in place as BatchNorm1d does
+ *               (rm = momentum * mean + (1 - momentum) * rm, the variance unbiased by M / (M - 1); nbt += 1);
+ *   out         [num_rows, 64] fp32;  argmax [num_rows, 64] uint8: the slot of the maximum, 255 = the padded slot;
+ *   workspace   b2s_pfn_train_workspace_bytes(num_rows) (host query) bytes, 16-byte aligned; it carries mu, C and the
+ *               per-channel statistics from the forward to the backward, so pass the same workspace to both.
+ * Forward: three kernels (moments, statistics and running buffers, output); backward: two (partials, reduce). */
+size_t b2s_pfn_train_workspace_bytes(int num_rows);
+int b2s_pfn_train_forward(const float *voxels, int num_rows, int max_points, int num_feat, const int *num_points,
+                          const int *coors, const float *weight, const float *gamma, const float *beta, int cout,
+                          float *running_mean, float *running_var, int64_t *num_batches_tracked, float momentum,
+                          float eps, float vx, float vy, float x_offset, float y_offset, int decoration, float *out,
+                          uint8_t *argmax, void *workspace, size_t workspace_bytes, unsigned *status_dev,
+                          void *stream);
+/* dweight [64, D], dgamma, dbeta [64] fp32 from the forward's out, argmax and workspace and dout [num_rows, 64] */
+int b2s_pfn_train_backward(const float *voxels, int num_rows, int max_points, int num_feat, const int *num_points,
+                           const int *coors, const float *weight, const float *gamma, int cout, float vx, float vy,
+                           float x_offset, float y_offset, int decoration, const float *out, const uint8_t *argmax,
+                           const float *dout, void *workspace, size_t workspace_bytes, float *dweight, float *dgamma,
+                           float *dbeta, void *stream);
 
 /* ---- crop of a halo-padded NHWC map ----------------------------------------------------------------
  * src [B, H+2, W+2, C] (fp16 hi/lo planes, one-pixel halo) -> dst [B, H-2*crop+2, W-2*crop+2, C]: the interior window

@@ -7,6 +7,7 @@ same way ``fastpath.accelerate(net)`` is the opt-in for the fused inference engi
     net = training.enable_sparse_backward(net)
     net = loss.enable_gpu_loss(net)               # b2second.loss: VoxelNet.loss on the GPU
     net = training.enable_rpn_training(net)       # the RPN's 3x3 stride-1 convs on the tensor pipe
+    net = training.enable_pfn_training(net)       # PointPillars' pillar feature net and scatter
     net.train()
     loss = net(example)["loss"]; loss.backward()
 
@@ -41,3 +42,13 @@ def enable_rpn_training(net):
     classes, state-dict keys and ``eval()`` are unchanged; idempotent.  Returns ``net``."""
     from . import rpn_train
     return rpn_train.enable(net)
+
+
+def enable_pfn_training(net):
+    """train PointPillars' pillar feature net and scatter on the GPU (b2second.pfn_train): ``PillarFeatureNet`` /
+    ``PillarFeatureNetRadius`` with one PFNLayer run the Linear, train-mode BatchNorm1d (batch statistics from the float64
+    moments of the decorated inputs, running buffers updated as torch does), ReLU and max without the padded per-point
+    map, and their weight gradient in closed form; ``PointPillarsScatter`` runs on b2s_to_bev / b2s_from_bev.  Other
+    VFEs stay torch; module classes, state-dict keys and ``eval()`` are unchanged; idempotent.  Returns ``net``."""
+    from . import pfn_train
+    return pfn_train.enable(net)

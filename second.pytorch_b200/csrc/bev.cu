@@ -4,6 +4,7 @@
 // previous call wrote (7 % of the map for a KITTI cloud), which its occupancy map still flags.
 #include <cuda_fp16.h>
 
+#include "pfn_deco.cuh"
 #include "tc_common.cuh"
 
 namespace {
@@ -123,19 +124,9 @@ k_pfn(const float *__restrict__ points, int F, const int *__restrict__ slots, co
     const int row = warp;
     const int np = num[row];
     const int *sl = slots + (size_t)row * T;
-    // mean of xyz over the valid points, summed in slot order (sequential fp32 like the oracle)
-    float sx = 0.f, sy = 0.f, sz = 0.f;
-    for (int t = 0; t < np; ++t) {
-        const float *p = points + (size_t)__ldg(&sl[t]) * F;
-        sx = __fadd_rn(sx, __ldg(&p[0]));
-        sy = __fadd_rn(sy, __ldg(&p[1]));
-        sz = __fadd_rn(sz, __ldg(&p[2]));
-    }
-    const float fn = (float)np;
-    const float mx = __fdiv_rn(sx, fn), my = __fdiv_rn(sy, fn), mz = __fdiv_rn(sz, fn);
-    int4 q = __ldg(reinterpret_cast<const int4 *>(coors + (size_t)row * 4));
-    const float cx = __fadd_rn(__fmul_rn((float)q.w, vx), xoff);
-    const float cy = __fadd_rn(__fmul_rn((float)q.z, vy), yoff);
+    const auto point = [&](int t) { return points + (size_t)__ldg(&sl[t]) * F; };
+    const B2sPfnPillar g = b2s_pfn_pillar(point, np, __ldg(reinterpret_cast<const int4 *>(coors + (size_t)row * 4)),
+                                          vx, vy, xoff, yoff);
     float sc[NCH], sh[NCH], best[NCH];
 #pragma unroll
     for (int j = 0; j < NCH; ++j) {
@@ -145,28 +136,14 @@ k_pfn(const float *__restrict__ points, int F, const int *__restrict__ slots, co
         best[j] = (np < T) ? fmaxf(sh[j], 0.f) : -INFINITY;
     }
     for (int t = 0; t < np; ++t) {
-        const float *p = points + (size_t)__ldg(&sl[t]) * F;
-        float feat[16];
-#pragma unroll
-        for (int f = 0; f < 9; ++f) feat[f] = (f < F) ? __ldg(&p[f]) : 0.f;
-        float raw[8];
-        if (DECO == B2S_PFN_RADIUS) {
-            // torch.norm(xy, p=2) with the multiply and add rounded separately, like the mean above
-            raw[0] = __fsqrt_rn(__fadd_rn(__fmul_rn(feat[0], feat[0]), __fmul_rn(feat[1], feat[1])));
-#pragma unroll
-            for (int f = 1; f < 8; ++f) raw[f] = feat[f + 1];
-        } else {
-#pragma unroll
-            for (int f = 0; f < 8; ++f) raw[f] = feat[f];
-        }
+        float raw[8], dec[5];
+        b2s_pfn_decorate<DECO>(point(t), F, g, raw, dec);
         float acc[NCH];
 #pragma unroll
         for (int j = 0; j < NCH; ++j) acc[j] = 0.f;
         for (int f = 0; f < NRAW; ++f)
 #pragma unroll
             for (int j = 0; j < NCH; ++j) acc[j] = fmaf(raw[f], s_w[f * COUT + lane + 32 * j], acc[j]);
-        float dec[5] = {__fsub_rn(feat[0], mx), __fsub_rn(feat[1], my), __fsub_rn(feat[2], mz),
-                        __fsub_rn(feat[0], cx), __fsub_rn(feat[1], cy)};
 #pragma unroll
         for (int f = 0; f < 5; ++f)
 #pragma unroll
