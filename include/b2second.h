@@ -80,6 +80,10 @@
  *   b2s_split_halo_f16_autoscale, b2s_pack_conv2d_weights, b2s_conv2d_wgrad_tc
  *                       forward and backward of the RPN's 3x3 stride-1 nn.Conv2d layers in training (rpn.py:486-495;
  *                       cuDNN's convolution and its two backward convolutions), with b2s_conv2d_tc_ex
+ *   b2s_bn_relu_train_forward, b2s_bn_relu_train_backward
+ *                       a train-mode BatchNorm1d / BatchNorm2d followed by ReLU in a Sequential (the RPN's blocks and
+ *                       deblocks, rpn.py; the middle encoder's SparseSequential, middle.py:146-191) and their autograd
+ *                       backward
  */
 #ifndef B2SECOND_H_
 #define B2SECOND_H_
@@ -91,7 +95,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 213
+#define B2S_VERSION 214
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -957,6 +961,34 @@ int b2s_conv2d_wgrad_tc(const b2s_half *x_hi, const b2s_half *x_lo, const b2s_ha
                         int batch, int H, int W, int Cin, int Cout, const float *x_scale_dev,
                         const float *dout_scale_dev, float *dweight, void *workspace, size_t workspace_bytes,
                         void *stream);
+
+/* ---- BatchNorm + ReLU in training (csrc/bn_train.cu) --------------------------------------------------------------
+ * y = relu(BatchNorm(x)) as torch.nn.BatchNorm1d / BatchNorm2d.forward in train() (affine, track_running_stats, a
+ * numeric momentum) followed by nn.ReLU, and its backward.  x is fp32 with `channels` channels and M = batch * spatial
+ * values per channel, in one of two layouts:
+ *   B2S_LAYOUT_NHWC  rows [batch * spatial, channels] (a BatchNorm1d input, or a channels_last map with spatial = H * W),
+ *                    x, y, dy, dx 16-byte aligned;
+ *   B2S_LAYOUT_NCHW  [batch, channels, spatial] contiguous.
+ * channels a multiple of 4 in 4..1024, M >= 2, eps > 0, 0 <= momentum <= 1.
+ * Forward, three kernels: float64 per-CTA sums of x - K and (x - K)^2 with K the channel's first value; one CTA adds
+ * them in a fixed order into mean, the biased variance var and s = 1 / sqrt(var + eps), updates running_mean,
+ * running_var (fp32, as torch's CUDA kernel: rm = momentum * mean + (1 - momentum) * rm, the variance unbiased by
+ * M / (M - 1)) and num_batches_tracked (+1), and stores mu32 = fp32(mean), fp32(gamma s) and beta in the workspace; then
+ * y = relu(fmaf(x - mu32, fp32(gamma s), beta)) in x's layout (y may not alias x).
+ * Backward, three kernels: g = dy where that same expression is not <= 0 (torch's ReLU backward), else 0;
+ * dbeta = sum g and dgamma = sum g xhat (xhat = (x - mean) s) from float64 per-CTA partials added in a fixed order;
+ * dx = gamma s (g - dbeta / M - xhat dgamma / M) in float64, stored fp32 (dx NULL: only dgamma and dbeta).
+ * No float atomics (two runs give the same bits), no sync (both can be captured).  workspace:
+ * b2s_bn_relu_train_workspace_bytes(layout, batch, channels, spatial) (host query; 0 for a shape that is not accepted)
+ * bytes, 16-byte aligned; it carries the statistics from the forward to the backward, so pass the same one to both. */
+size_t b2s_bn_relu_train_workspace_bytes(int layout, int batch, int channels, int spatial);
+int b2s_bn_relu_train_forward(const float *x, int layout, int batch, int channels, int spatial, const float *gamma,
+                              const float *beta, float *running_mean, float *running_var, int64_t *num_batches_tracked,
+                              float momentum, float eps, float *y, void *workspace, size_t workspace_bytes,
+                              void *stream);
+int b2s_bn_relu_train_backward(const float *x, const float *dy, int layout, int batch, int channels, int spatial,
+                               const float *gamma, void *workspace, size_t workspace_bytes, float *dx, float *dgamma,
+                               float *dbeta, void *stream);
 
 #ifdef __cplusplus
 }

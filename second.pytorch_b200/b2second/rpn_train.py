@@ -1,11 +1,14 @@
 """Training of the RPN's 3x3 stride-1 convolutions on the tensor pipe (csrc/conv_train.cu).
 
-``training.enable_rpn_training(net)`` rebinds the ``forward`` of every covered ``nn.Conv2d`` under ``net.rpn`` to
-``Conv3x3TC`` and the ``forward`` of a ``nn.ZeroPad2d(1)`` directly in front of a covered ``padding=0`` conv to the
-identity (the pair is one pad-1 conv; the halo of the split input is the pad, so the padded copy is never built).
+``training.enable_rpn_training(net)`` rebinds the ``forward`` of every covered ``nn.Conv2d`` in a sequential container
+under ``net.rpn`` to ``Conv3x3TC`` and the ``forward`` of a ``nn.ZeroPad2d(1)`` directly in front of a covered
+``padding=0`` conv to the identity (the pair is one pad-1 conv; the halo of the split input is the pad, so the padded
+copy is never built).  A subclass that does not override ``forward`` counts (see ``sequences`` and ``plain``), so the
+reference's own ``change_default_args`` convs inside torchplus' ``Sequential`` are covered as well as the mirror's.
 Covered: 3x3 kernel, stride 1, no dilation, no groups, no bias, zero padding 1 (or 0 after the pad), ``C_in`` a
 multiple of 64, ``C_out`` in {64, 128, 256} -- every 3x3 layer of car.fhd and car.lite and every stride-1 3x3 layer of
-all.fhd, xyres_16 and all.pp.largea.  Stride-2 convs, deblocks, heads, BatchNorm2d and ReLU stay the torch modules.
+all.fhd, xyres_16 and all.pp.largea.  Stride-2 convs, deblocks and heads stay the torch modules; BatchNorm2d + ReLU
+pairs are ``enable_bn_relu_training``'s (b2second.bn_train).
 
 The rebound forward takes the kernels only in ``train()`` mode with grad enabled on float32 CUDA input; otherwise it is
 ``nn.Conv2d.forward`` (and the pad pads), so ``eval()`` and the state dict are unchanged.
@@ -32,27 +35,38 @@ def _lib():
     return sp._lib, sp._lib.load()
 
 
+def plain(m, cls):
+    """True when ``m`` is a ``cls`` whose class does not override ``forward`` (``cls`` itself, or a subclass such as the
+    reference's ``change_default_args`` layers, which only change constructor defaults)."""
+    return isinstance(m, cls) and type(m).forward is cls.forward
+
+
+def sequences(root):
+    """-> [list of children] of every sequential container under ``root`` (``root`` included), in module order:
+    ``nn.Sequential``, torchplus' ``Sequential`` (a plain ``nn.Module``) and the ``spconv`` drop-in's
+    ``SparseSequential``, each of which runs its children in ``_modules`` order."""
+    return [list(m._modules.values()) for m in root.modules()
+            if isinstance(m, nn.Sequential) or type(m).__name__ in ("Sequential", "SparseSequential")]
+
+
 def qualifies(conv, padding):
     """True when ``conv`` (an nn.Conv2d) is covered once its input is padded by ``padding`` - conv.padding."""
-    return (type(conv) is nn.Conv2d and tuple(conv.kernel_size) == (3, 3) and tuple(conv.stride) == (1, 1)
+    return (plain(conv, nn.Conv2d) and tuple(conv.kernel_size) == (3, 3) and tuple(conv.stride) == (1, 1)
             and tuple(conv.dilation) == (1, 1) and conv.groups == 1 and conv.bias is None
             and conv.padding_mode == "zeros" and tuple(conv.padding) == (padding, padding)
             and conv.in_channels % 64 == 0 and conv.out_channels in COUT_BUILT)
 
 
 def _is_pad1(m):
-    return type(m) is nn.ZeroPad2d and tuple(m.padding) == (1, 1, 1, 1)
+    return plain(m, nn.ZeroPad2d) and tuple(m.padding) == (1, 1, 1, 1)
 
 
 def select(rpn):
     """-> [(conv, pad or None)] of the covered layers under ``rpn``, in module order."""
     out = []
-    for seq in rpn.modules():
-        if not isinstance(seq, nn.Sequential):
-            continue
-        mods = list(seq)
+    for mods in sequences(rpn):
         for i, m in enumerate(mods):
-            if type(m) is not nn.Conv2d:
+            if not plain(m, nn.Conv2d):
                 continue
             if qualifies(m, 1):
                 out.append((m, None))

@@ -8,14 +8,16 @@ same way ``fastpath.accelerate(net)`` is the opt-in for the fused inference engi
     net = loss.enable_gpu_loss(net)               # b2second.loss: VoxelNet.loss on the GPU
     net = training.enable_rpn_training(net)       # the RPN's 3x3 stride-1 convs on the tensor pipe
     net = training.enable_pfn_training(net)       # PointPillars' pillar feature net and scatter
+    net = training.enable_bn_relu_training(net)   # every BatchNorm + ReLU pair of a Sequential
     net.train()
     loss = net(example)["loss"]; loss.backward()
 
 A marked sparse convolution in ``train()`` mode with grad enabled records autograd: its forward runs the inference
 kernels with fp32 output rows, its backward computes the input gradient on the same kernels over the transposed
 neighbour table (the tensor pipe where the widths allow, with the gradient split under an automatic power-of-two scale)
-and the weight gradient with ``b2s_sparse_conv_wgrad``.  BatchNorm1d and ReLU run as the torch modules that follow the
-conv.  ``eval()`` keeps the fused BN/ReLU inference path, marked or not; an unmarked conv in training mode still raises
+and the weight gradient with ``b2s_sparse_conv_wgrad``.  The BatchNorm1d and ReLU that follow the conv run as torch
+modules, or as one fused train-mode pair after ``enable_bn_relu_training``.  ``eval()`` keeps the fused BN/ReLU
+inference path, marked or not; an unmarked conv in training mode still raises
 ``NotImplementedError``.  Not covered: the fused engine, fp16/AMP, transposed / inverse sparse convs.
 
 The training targets ``VoxelNet.loss`` reads (labels, reg_targets, importance) come from ``b2second.targets`` on the GPU
@@ -38,8 +40,8 @@ def enable_sparse_backward(module):
 def enable_rpn_training(net):
     """train the RPN's 3x3 stride-1 ``nn.Conv2d`` layers under ``net.rpn`` on the tensor pipe (b2second.rpn_train):
     forward, input gradient and weight gradient in 3xF16 on wgmma, fp32-grade.  Layers it does not cover (stride-2
-    convs, deblocks, heads) stay torch; BatchNorm2d and ReLU run as the torch modules that follow the conv.  Module
-    classes, state-dict keys and ``eval()`` are unchanged; idempotent.  Returns ``net``."""
+    convs, deblocks, heads) stay torch; the BatchNorm2d and ReLU that follow the conv are
+    ``enable_bn_relu_training``'s.  Module classes, state-dict keys and ``eval()`` are unchanged; idempotent.  Returns ``net``."""
     from . import rpn_train
     return rpn_train.enable(net)
 
@@ -52,3 +54,14 @@ def enable_pfn_training(net):
     VFEs stay torch; module classes, state-dict keys and ``eval()`` are unchanged; idempotent.  Returns ``net``."""
     from . import pfn_train
     return pfn_train.enable(net)
+
+
+def enable_bn_relu_training(net):
+    """train every (BatchNorm1d or BatchNorm2d, ReLU) pair of consecutive children of a ``Sequential`` /
+    ``SparseSequential`` under ``net`` as one fused pair on the GPU (b2second.bn_train): batch statistics in float64
+    with the running buffers updated as torch does, y = relu(BN(x)) in x's layout (rows [M, C] or NCHW), and a backward
+    that recomputes the ReLU mask from x, so only x is kept; deterministic, no host sync.  BatchNorms without affine
+    parameters, running statistics or a numeric momentum, in-place ReLUs and other norms stay torch; module classes,
+    state-dict keys and ``eval()`` are unchanged; idempotent.  Returns ``net``."""
+    from . import bn_train
+    return bn_train.enable(net)

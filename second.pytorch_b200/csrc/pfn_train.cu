@@ -16,6 +16,7 @@
 // pillar's mean, then pillar into warp, warp into CTA, CTA partials in order), so nothing cancels when |mu| >> std.
 // Every sum runs in one fixed order (fixed grid, fixed pillar-to-warp map, no float atomics): two runs give the same
 // bits.  No host sync: the entry points can be captured in a CUDA graph.
+#include "bn_common.cuh"
 #include "pfn_deco.cuh"
 
 namespace {
@@ -283,16 +284,13 @@ k_pfn_stats(const double *__restrict__ part, int nparts, int N, int T, int D, co
             v += (double)w[k] * cw;
         }
         v = fmax(v, 0.0);
-        const double s = 1.0 / sqrt(v + (double)eps);
+        const double s = b2s_bn_inv_std(v, eps);
         const double gs = (double)gamma[c] * s;
         mean_c[c] = m;
         s_c[c] = s;
         scale[c] = (float)gs;
         shift[c] = (float)((double)beta[c] - m * gs);
-        const float m32 = (float)m, uv32 = (float)(v * (M / (M - 1.0)));
-        const float keep = __fsub_rn(1.f, momentum);
-        rmean[c] = __fadd_rn(__fmul_rn(momentum, m32), __fmul_rn(keep, rmean[c]));
-        rvar[c] = __fadd_rn(__fmul_rn(momentum, uv32), __fmul_rn(keep, rvar[c]));
+        b2s_bn_update_running(rmean, rvar, c, m, v, M, momentum);
         if (c == 0) *nbt += 1;
     }
 }

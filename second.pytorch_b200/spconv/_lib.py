@@ -80,6 +80,11 @@ SIGNATURES = {
     "b2s_pfn_train_backward": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                        c_float, c_float, c_float, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                        c_size_t, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2s_bn_relu_train_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "b2s_bn_relu_train_forward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_float, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "b2s_bn_relu_train_backward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t,
+                                           c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2s_from_bev":(c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
                              c_void_p]),
     "b2s_to_bev_tc": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
@@ -253,7 +258,7 @@ def load():
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
-    if lib.b2s_version() < 213:
+    if lib.b2s_version() < 214:
         raise ImportError("libb2second.so is too old")
     _lib = lib
     return lib
