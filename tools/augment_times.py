@@ -5,31 +5,16 @@ copies, one memset and the three kernels), the bytes the call must move (points 
 read) and their floor at the H100 SXM data-sheet 3.35 TB/s (arithmetic, not a measurement), and separately the host time
 of ``draw`` for the same batch.  Frames hold 20 k to 30 k points, half of them in and around the boxes.
 """
-import json
-import os
-import subprocess
 import sys
 import time
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
+import _measure
+import numpy as np
+import torch
 
-from b2second import augment, config  # noqa: E402
+from b2second import augment, config
 
-ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 20
 HBM_BYTES_PER_S = 3.35e12
-
-
-def card():
-    name = torch.cuda.get_device_name(0)
-    try:
-        limit = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                               capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        limit = "unknown"
-    return name, limit
 
 
 def batch(cfg, B, G, rng):
@@ -62,41 +47,32 @@ def batch(cfg, B, G, rng):
 
 
 def main():
-    assert torch.cuda.is_available(), "this tool times CUDA kernels: it needs a GPU"
+    ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 20
+    _measure.require_gpu("augment_times")
     rng = np.random.default_rng(0)
     rows = []
-    for name in ("car.fhd", "nuscenes.all.pp.largea"):
-        cfg = config.get_config(name)
-        plan = augment.plan(cfg.augment, cfg.point_cloud_range, [c.class_name for c in cfg.classes])
-        for B in (8, 32):
-            for G in (30, 200):
-                args, npts, pbytes, bbytes = batch(cfg, B, G, rng)
-                rs = np.random.RandomState(0)
-                h0 = time.perf_counter()
-                draws = [augment.draw(rs, cfg.augment, [G] * B, npts) for _ in range(3)]
-                draw_ms = (time.perf_counter() - h0) * 1e3 / 3
-                d = draws[0]
-                for _ in range(3):
-                    plan.augment_batch(*args, None, d)
-                torch.cuda.synchronize()
-                assert int(plan.last_status.item()) == 0
-                t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                t0.record()
-                for _ in range(ITERS):
-                    plan.augment_batch(*args, None, d)
-                t1.record()
-                torch.cuda.synchronize()
-                ms = t0.elapsed_time(t1) / ITERS
-                draw_bytes = (B * G * 100 * 32 if plan.object_noise else 0) + B * 64 + \
-                    (4 * sum(npts) if cfg.augment.shuffle_points else 0)
-                moved = 2 * pbytes + 2 * bbytes + draw_bytes
-                rows.append({"config": name, "batch": B, "gt_per_frame": G, "points": int(sum(npts)),
-                             "box_dtype": "float64" if name.startswith("nuscenes") else "float32",
-                             "object_noise": plan.object_noise, "ms": round(ms, 4), "draw_host_ms": round(draw_ms, 3),
-                             "bytes_moved": moved, "hbm_floor_ms": round(moved / HBM_BYTES_PER_S * 1e3, 4)})
-    name, limit = card()
-    print(json.dumps({"tool": "augment_times", "device": name, "power_limit": limit, "iters": ITERS,
-                      "results": rows}))
+    with _measure.clocks() as clk:
+        for name in ("car.fhd", "nuscenes.all.pp.largea"):
+            cfg = config.get_config(name)
+            plan = augment.plan(cfg.augment, cfg.point_cloud_range, [c.class_name for c in cfg.classes])
+            for B in (8, 32):
+                for G in (30, 200):
+                    args, npts, pbytes, bbytes = batch(cfg, B, G, rng)
+                    rs = np.random.RandomState(0)
+                    h0 = time.perf_counter()
+                    draws = [augment.draw(rs, cfg.augment, [G] * B, npts) for _ in range(3)]
+                    draw_ms = (time.perf_counter() - h0) * 1e3 / 3
+                    ms = _measure.timed(lambda: plan.augment_batch(*args, None, draws[0]), ITERS)
+                    assert int(plan.last_status.item()) == 0
+                    draw_bytes = (B * G * 100 * 32 if plan.object_noise else 0) + B * 64 + \
+                        (4 * sum(npts) if cfg.augment.shuffle_points else 0)
+                    moved = 2 * pbytes + 2 * bbytes + draw_bytes
+                    rows.append({"config": name, "batch": B, "gt_per_frame": G, "points": int(sum(npts)),
+                                 "box_dtype": "float64" if name.startswith("nuscenes") else "float32",
+                                 "object_noise": plan.object_noise, "ms": round(ms, 4),
+                                 "draw_host_ms": round(draw_ms, 3),
+                                 "bytes_moved": moved, "hbm_floor_ms": round(moved / HBM_BYTES_PER_S * 1e3, 4)})
+    _measure.report("augment_times", rows, clk, iters=ITERS)
 
 
 if __name__ == "__main__":

@@ -9,45 +9,29 @@ each pair's input; then, per pair, relu(bn(x)) forward + backward (loss = sum(y 
 torch.cuda.max_memory_allocated over one pass, and the least time the pair's map traffic can take at 3.35 TB/s (3 map
 passes forward, 5 backward).  For the two RPNs the whole rpn forward + backward is timed the same way with and without
 the opt-in.  Prints the card name and power limit of the run."""
-import json
-import os
-import subprocess
-import sys
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, REPO)
-sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
 import copy
+import sys
 
+import _measure
 import numpy as np
 import torch
-import bench
-from b2second import bn_train, config, loader, models, training
 
-ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 20
+from b2second import bn_train, training
+
 CASES = [("car.fhd", 8, "rpn"), ("pointpillars.car.xyres_16", 2, "rpn"), ("car.fhd", 8, "middle")]
 HBM = 3.35e12                       # H100 SXM data-sheet HBM3 bandwidth, bytes/s
-torch.backends.cudnn.allow_tf32 = False
-torch.backends.cuda.matmul.allow_tf32 = False
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
 
 
 def network(name, B):
     """the drop-in network in train() with sparse backward and RPN training, and the inputs of its three stages"""
-    cfg = config.get_config(name)
-    net = models.build_network(cfg, loader.product_spconv())
-    models.synthetic_weights_(net, name, seed=0)
-    net = training.enable_rpn_training(training.enable_sparse_backward(net.cuda())).train()
+    net, clouds = _measure.mirror(name, B)
+    net = training.enable_rpn_training(training.enable_sparse_backward(net)).train()
 
     def t(a):
         return a if torch.is_tensor(a) else torch.from_numpy(np.asarray(a))
     vox, num, coors = [], [], []
-    for b, c in enumerate(bench.make_clouds(name, B, 29000)):
-        res = net.voxel_generator.generate(c, cfg.max_voxels)
+    for b, c in enumerate(clouds):
+        res = net.voxel_generator.generate(c, net.cfg.max_voxels)
         n = int(res["voxel_num"])
         vox.append(t(res["voxels"])[:n].cuda())
         num.append(t(res["num_points_per_voxel"])[:n].cuda())
@@ -55,25 +39,7 @@ def network(name, B):
     return net, torch.cat(vox).float().contiguous(), torch.cat(num).int(), torch.cat(coors).int().contiguous()
 
 
-def timed(step):
-    for _ in range(3):
-        step()
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats()
-    base = torch.cuda.memory_allocated()
-    step()
-    torch.cuda.synchronize()
-    peak = torch.cuda.max_memory_allocated() - base
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(ITERS):
-        step()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / ITERS, peak
-
-
-def pair_times(bn, relu, x):
+def pair_times(bn, relu, x, iters):
     """(ms, peak bytes) of relu(bn(x)) forward + backward, fused and torch, on copies of the modules"""
     G = torch.randn(x.shape, device=x.device, generator=torch.Generator(x.device).manual_seed(0))
     G = G.contiguous(memory_format=torch.channels_last) if x.dim() == 4 and not x.is_contiguous() else G
@@ -90,59 +56,62 @@ def pair_times(bn, relu, x):
         def step():
             y = seq(xi)
             (y * G).sum().backward()
-        out[fused] = timed(step)
+        out[fused] = _measure.timed(step, iters), _measure.peak_bytes(step)
     return out
 
 
 def main():
-    assert torch.cuda.is_available(), "bn_train_times.py measures on a CUDA device"
-    for name, B, part in CASES:
-        net, vox, num, coors = network(name, B)
-        stage = net.rpn if part == "rpn" else net.middle_feature_extractor
-        pairs = bn_train.select(stage)
-        seen = {}
-        hooks = [bn.register_forward_pre_hook(lambda m, i: seen.setdefault(id(m), i[0].detach().clone()))
-                 for bn, _ in pairs]
-        rpn_in = {}
-        hooks.append(net.rpn.register_forward_pre_hook(lambda m, i: rpn_in.setdefault("x", i[0].detach().clone())))
-        feats = net.voxel_feature_extractor(vox, num, coors)       # grad on: the layers take their training path
-        net.rpn(net.middle_feature_extractor(feats, coors, B))
-        for h in hooks:
-            h.remove()
-        tot = {"ours": 0.0, "torch": 0.0, "floor": 0.0}
-        for i, (bn, relu) in enumerate(pairs):
-            x = seen[id(bn)]
-            t = pair_times(bn, relu, x)
-            floor = 8 * x.numel() * 4 / HBM * 1e3
-            layout = "rows" if x.dim() == 2 or not x.is_contiguous() else "nchw"
-            row = {"config": name, "batch": B, "stage": part, "pair": i, "shape": list(x.shape), "layout": layout,
-                   "ms_ours": round(t[True][0], 4), "ms_torch": round(t[False][0], 4), "ms_floor": round(floor, 4),
-                   "peak_MB_ours": round(t[True][1] / 2 ** 20, 1), "peak_MB_torch": round(t[False][1] / 2 ** 20, 1)}
-            tot["ours"] += t[True][0]
-            tot["torch"] += t[False][0]
-            tot["floor"] += floor
-            print(json.dumps(row), flush=True)
-        summary = {"config": name, "batch": B, "stage": part, "pairs": len(pairs),
-                   "ms_ours_sum": round(tot["ours"], 3), "ms_torch_sum": round(tot["torch"], 3),
-                   "ms_floor_sum": round(tot["floor"], 3)}
-        if part == "rpn":
-            x = rpn_in["x"]
-            for fused in (False, True):
-                if fused:
-                    training.enable_bn_relu_training(net)
-                xi = x.clone().requires_grad_(True)
+    ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 20
+    _measure.require_gpu("bn_train_times")
+    rows = []
+    with _measure.clocks() as clk:
+        for name, B, part in CASES:
+            net, vox, num, coors = network(name, B)
+            stage = net.rpn if part == "rpn" else net.middle_feature_extractor
+            pairs = bn_train.select(stage)
+            seen = {}
+            hooks = [bn.register_forward_pre_hook(lambda m, i: seen.setdefault(id(m), i[0].detach().clone()))
+                     for bn, _ in pairs]
+            rpn_in = {}
+            hooks.append(net.rpn.register_forward_pre_hook(lambda m, i: rpn_in.setdefault("x", i[0].detach().clone())))
+            feats = net.voxel_feature_extractor(vox, num, coors)       # grad on: the layers take their training path
+            net.rpn(net.middle_feature_extractor(feats, coors, B))
+            for h in hooks:
+                h.remove()
+            tot = {"ours": 0.0, "torch": 0.0, "floor": 0.0}
+            for i, (bn, relu) in enumerate(pairs):
+                x = seen[id(bn)]
+                t = pair_times(bn, relu, x, ITERS)
+                floor = 8 * x.numel() * 4 / HBM * 1e3
+                layout = "rows" if x.dim() == 2 or not x.is_contiguous() else "nchw"
+                row = {"config": name, "batch": B, "stage": part, "pair": i, "shape": list(x.shape), "layout": layout,
+                       "ms_ours": round(t[True][0], 4), "ms_torch": round(t[False][0], 4), "ms_floor": round(floor, 4),
+                       "peak_MB_ours": round(t[True][1] / 2 ** 20, 1), "peak_MB_torch": round(t[False][1] / 2 ** 20, 1)}
+                tot["ours"] += t[True][0]
+                tot["torch"] += t[False][0]
+                tot["floor"] += floor
+                rows.append(row)
+            summary = {"config": name, "batch": B, "stage": part, "pairs": len(pairs),
+                       "ms_ours_sum": round(tot["ours"], 3), "ms_torch_sum": round(tot["torch"], 3),
+                       "ms_floor_sum": round(tot["floor"], 3)}
+            if part == "rpn":
+                x = rpn_in["x"]
+                for fused in (False, True):
+                    if fused:
+                        training.enable_bn_relu_training(net)
+                    xi = x.clone().requires_grad_(True)
 
-                def step():
-                    r = net.rpn(xi)
-                    sum(v.float().sum() for v in r.values() if torch.is_tensor(v) and v.requires_grad).backward()
-                ms, peak = timed(step)
-                key = "ours" if fused else "torch"
-                summary["rpn_ms_" + key] = round(ms, 3)
-                summary["rpn_peak_MB_" + key] = round(peak / 2 ** 20, 1)
-        print(json.dumps(summary), flush=True)
-        del net
-        torch.cuda.empty_cache()
-    print(json.dumps({"card": card(), "iters": ITERS}))
+                    def step():
+                        r = net.rpn(xi)
+                        sum(v.float().sum() for v in r.values() if torch.is_tensor(v) and v.requires_grad).backward()
+                    ms, peak = _measure.timed(step, ITERS), _measure.peak_bytes(step)
+                    key = "ours" if fused else "torch"
+                    summary["rpn_ms_" + key] = round(ms, 3)
+                    summary["rpn_peak_MB_" + key] = round(peak / 2 ** 20, 1)
+            rows.append(summary)
+            del net
+            torch.cuda.empty_cache()
+    _measure.report("bn_train_times", rows, clk, iters=ITERS)
 
 
 if __name__ == "__main__":

@@ -3,39 +3,23 @@
 Prints one JSON line.  Per config (car.fhd, nuscenes.all.pp.mhead) at batch 8 with a synthetic object database (400
 objects per sampled class, 20 to 400 points each, written to a temporary directory): milliseconds per call on the
 device (the candidates' host-to-device copy, four memsets and the kernels), the host time of ``draw`` for the batch,
-and the database's device footprint; with the card, its power limit and the SM clock read right after each timing
-loop.  Frames hold 20 k to 30 k points and 10 ground truths.  Where the reference tree is importable (refcompat),
-the same frames also go through the reference's DataBaseSamplerV2.sample_all plus preprocess.py:224-249
-(points_in_rbbox removal, concatenation) on the host, one frame after another on one core.
+and the database's device footprint; with the card, its power limit and the SM clock sampled during the run.  Frames
+hold 20 k to 30 k points and 10 ground truths.  Where the reference tree is importable (refcompat), the same frames
+also go through the reference's DataBaseSamplerV2.sample_all plus preprocess.py:224-249 (points_in_rbbox removal,
+concatenation) on the host, one frame after another on one core.
 """
-import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
+import _measure
+import numpy as np
+import torch
 
-from b2second import config, dbsample, refcompat  # noqa: E402
+from b2second import config, dbsample, refcompat
 
-ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 20
 B = 8
-
-
-def card():
-    """device name, power limit and the SM clock / its maximum as read now (read-only nvidia-smi queries)"""
-    name = torch.cuda.get_device_name(0)
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
-                            "-i", "0"], capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
-        limit, sm, sm_max = (q + ["unknown"] * 3)[:3]
-    except (OSError, subprocess.SubprocessError):
-        limit = sm = sm_max = "unknown"
-    return name, limit, sm, sm_max
 
 
 def database(cfg, root, rng):
@@ -78,7 +62,7 @@ def frames(cfg, rng):
 
 
 def reference_ms(cfg, infos, root, fr):
-    refcompat.install(os.path.join(REPO, "oracle"))
+    refcompat.install(os.path.join(_measure.REPO, "oracle"))
     from second.core import box_np_ops
     from second.core.sample_ops import DataBaseSamplerV2
     np.random.seed(0)
@@ -96,52 +80,44 @@ def reference_ms(cfg, infos, root, fr):
 
 
 def main():
-    assert torch.cuda.is_available(), "this tool times CUDA kernels: it needs a GPU"
+    ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 20
+    _measure.require_gpu("db_sample_times")
     rng = np.random.default_rng(0)
     rows = []
     dev = "cuda:0"
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)   # noqa: E731
-    for name in ("car.fhd", "nuscenes.all.pp.mhead"):
-        cfg = config.get_config(name)
-        classes = [c.class_name for c in cfg.classes]
-        with tempfile.TemporaryDirectory() as root:
-            infos = database(cfg, root, rng)
-            fr = frames(cfg, rng)
-            ds = dbsample.sampler(cfg.db_sampler, infos, root, cfg.num_point_features, classes, dev,
-                                  np.random.RandomState(0))
-            names = [f[2] for f in fr]
-            h0 = time.perf_counter()
-            cand = dbsample.draw(np.random.RandomState(1), ds.state, names)
-            draw_ms = (time.perf_counter() - h0) * 1e3
-            P = np.concatenate([f[0] for f in fr])
-            G = np.concatenate([f[1] for f in fr])
-            args = (t(P), t(np.cumsum([0] + [len(f[0]) for f in fr]).astype(np.int32)), t(G),
-                    t(np.arange(0, 10 * B + 1, 10, dtype=np.int32)), t(np.ones(10 * B, bool)),
-                    t(np.ones(10 * B, np.int32)), None, cand)
-            for _ in range(3):
+    with _measure.clocks() as clk:
+        for name in ("car.fhd", "nuscenes.all.pp.mhead"):
+            cfg = config.get_config(name)
+            classes = [c.class_name for c in cfg.classes]
+            with tempfile.TemporaryDirectory() as root:
+                infos = database(cfg, root, rng)
+                fr = frames(cfg, rng)
+                ds = dbsample.sampler(cfg.db_sampler, infos, root, cfg.num_point_features, classes, dev,
+                                      np.random.RandomState(0))
+                names = [f[2] for f in fr]
+                h0 = time.perf_counter()
+                cand = dbsample.draw(np.random.RandomState(1), ds.state, names)
+                draw_ms = (time.perf_counter() - h0) * 1e3
+                P = np.concatenate([f[0] for f in fr])
+                G = np.concatenate([f[1] for f in fr])
+                args = (t(P), t(np.cumsum([0] + [len(f[0]) for f in fr]).astype(np.int32)), t(G),
+                        t(np.arange(0, 10 * B + 1, 10, dtype=np.int32)), t(np.ones(10 * B, bool)),
+                        t(np.ones(10 * B, np.int32)), None, cand)
                 res = ds.sample_batch(*args)
-            torch.cuda.synchronize()
-            assert int(ds.last_status.item()) == 0
-            nb, npts = res.counts()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(ITERS):
-                ds.sample_batch(*args)
-            e1.record()
-            torch.cuda.synchronize()
-            _, _, sm, _ = card()
-            row = {"config": name, "batch": B, "points_in": int(len(P)), "candidates": int(len(cand.objects)),
-                   "accepted": int(res["accepted"].sum().item()), "points_out": int(sum(npts)),
-                   "ms": round(e0.elapsed_time(e1) / ITERS, 4), "draw_host_ms": round(draw_ms, 3),
-                   "db_nbytes": ds.db.nbytes, "sm_clock_after": sm}
-            if refcompat.reference_available():
-                row["reference_host_ms"] = round(reference_ms(cfg, infos, root, fr), 2)
-            else:
-                row["reference_host_ms"] = "not measured (reference tree not importable here)"
-            rows.append(row)
-    name, limit, _, sm_max = card()
-    print(json.dumps({"tool": "db_sample_times", "device": name, "power_limit": limit, "sm_clock_max": sm_max,
-                      "iters": ITERS, "results": rows}))
+                torch.cuda.synchronize()
+                assert int(ds.last_status.item()) == 0
+                nb, npts = res.counts()
+                ms = _measure.timed(lambda: ds.sample_batch(*args), ITERS, warmup=2)
+                row = {"config": name, "batch": B, "points_in": int(len(P)), "candidates": int(len(cand.objects)),
+                       "accepted": int(res["accepted"].sum().item()), "points_out": int(sum(npts)),
+                       "ms": round(ms, 4), "draw_host_ms": round(draw_ms, 3), "db_nbytes": ds.db.nbytes}
+                if refcompat.reference_available():
+                    row["reference_host_ms"] = round(reference_ms(cfg, infos, root, fr), 2)
+                else:
+                    row["reference_host_ms"] = "not measured (reference tree not importable here)"
+                rows.append(row)
+    _measure.report("db_sample_times", rows, clk, iters=ITERS)
 
 
 if __name__ == "__main__":

@@ -5,25 +5,14 @@ synthetic set the size of KITTI val: 3769 frames, 8 ground truths and 50 detecti
 
 Reports conversion (detections -> annos, including the device-to-host copy), the three overlap passes, and the
 official and COCO evaluations (each end to end: packing, copies, kernels, formatting), with the card's name and power
-limit read in the same run.  Needs a CUDA device.
+limit read in the same run and the SM clock sampled during it.  Needs a CUDA device.
 """
 import argparse
-import json
 import os
-import subprocess
-import sys
 
+import _measure
 import numpy as np
 import torch
-
-REPO = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
-sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
 
 
 def synthetic(frames, n_gt, n_dt, seed=0):
@@ -55,18 +44,9 @@ def synthetic(frames, n_gt, n_dt, seed=0):
 
 
 def timed(fn, repeats):
-    """median of CUDA-event times of fn() (ms), after one warm-up call."""
+    """median of CUDA-event times of single calls of fn() (ms), after one warm-up call."""
     fn()
-    ts = []
-    for _ in range(repeats):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b))
-    return float(np.median(ts))
+    return float(np.median([_measure.timed(fn, 1, warmup=0) for _ in range(repeats)]))
 
 
 def main():
@@ -77,8 +57,7 @@ def main():
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("kitti_eval_times needs a CUDA device")
+    _measure.require_gpu("kitti_eval_times")
     from b2second import kitti_eval as ke, loader
     loader.product_spconv()
     gts, dts, dets = synthetic(args.frames, args.gt, args.dt)
@@ -89,19 +68,20 @@ def main():
     infos = [{"calib": {"R0_rect": np.eye(4), "Tr_velo_to_cam": Tr, "P2": P2},
               "image": {"image_idx": i, "image_shape": np.array([375, 1242])}} for i in range(args.frames)]
     classes = [0, 1, 2]
-    res = {"card": card(), "frames": args.frames, "gt_per_frame": args.gt, "dt_per_frame": args.dt}
-    res["convert_ms"] = timed(lambda: ke.convert_detection_to_kitti_annos(dets, infos, ["Car", "Pedestrian", "Cyclist"]),
-                              args.repeats)
-    packed = ke._Packed(gts, dts, 1, 1.0, "cuda")
-    for metric in range(3):
-        def ov(metric=metric):
-            packed._ov.pop(metric, None)
-            packed.overlaps(metric)
-        res["overlaps_m%d_ms" % metric] = timed(ov, args.repeats)
-    res["official_ms"] = timed(lambda: ke.get_official_eval_result(gts, dts, classes), args.repeats)
-    res["coco_ms"] = timed(lambda: ke.get_coco_eval_result(gts, dts, classes), args.repeats)
-    line = json.dumps(res)
-    print(line)
+    res = {}
+    with _measure.clocks() as clk:
+        res["convert_ms"] = timed(lambda: ke.convert_detection_to_kitti_annos(dets, infos, ["Car", "Pedestrian",
+                                                                                           "Cyclist"]), args.repeats)
+        packed = ke._Packed(gts, dts, 1, 1.0, "cuda")
+        for metric in range(3):
+            def ov(metric=metric):
+                packed._ov.pop(metric, None)
+                packed.overlaps(metric)
+            res["overlaps_m%d_ms" % metric] = timed(ov, args.repeats)
+        res["official_ms"] = timed(lambda: ke.get_official_eval_result(gts, dts, classes), args.repeats)
+        res["coco_ms"] = timed(lambda: ke.get_coco_eval_result(gts, dts, classes), args.repeats)
+    line = _measure.report("kitti_eval_times", res, clk, frames=args.frames, gt_per_frame=args.gt,
+                           dt_per_frame=args.dt, repeats=args.repeats)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:

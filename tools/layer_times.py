@@ -10,14 +10,12 @@ device from the engine's own tables (nbr, perm, tile_mask) after the timed runs:
             H100 SXM data-sheet dense FP16 rate, 989 TFLOP/s
   l2_us     gath_MB at the L2-resident copy bandwidth this script measures on the same card
 """
-import os
+import json
 import sys
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, REPO)
-sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
+
+import _measure
 import torch
-import bench
-from b2second import config, loader, models
+
 from b2second.engine import InferenceEngine
 
 TILE, BLOCK_K = 128, 64
@@ -28,15 +26,7 @@ def l2_copy_bandwidth(nbytes=16 << 20, iters=200):
     """bytes/s of a device copy whose source and destination (2 x 16 MB) stay resident in the 50 MB L2"""
     a = torch.empty(nbytes // 4, dtype=torch.float32, device="cuda").uniform_()
     b = torch.empty_like(a)
-    for _ in range(10):
-        b.copy_(a)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        b.copy_(a)
-    e1.record()
-    torch.cuda.synchronize()
-    return 2.0 * nbytes * iters / (e0.elapsed_time(e1) * 1e-3)
+    return 2.0 * nbytes / (_measure.timed(lambda: b.copy_(a), iters, warmup=10) * 1e-3)
 
 
 def gather_counts(lyr, n_out):
@@ -63,19 +53,16 @@ def gather_counts(lyr, n_out):
 
 def main():
     B = int(sys.argv[1]) if len(sys.argv) > 1 else 16
-    sp = loader.product_spconv()
-    cfg = config.get_config("car.fhd")
-    net = models.build_network(cfg, sp).eval()
-    models.synthetic_weights_(net, "car.fhd", seed=0)
-    net = net.cuda()
-    eng = InferenceEngine(net, batch_size=B, max_points=30000, use_cuda_graph=False)
-    clouds = [torch.from_numpy(c).cuda() for c in bench.make_clouds("car.fhd", B, 29000)]
-    eng.load_points(clouds)
-    st = eng.run_timed(iters=5)
+    _measure.require_gpu("layer_times")
+    print(json.dumps(_measure.card()))
+    net, clouds = _measure.mirror("car.fhd", B)
+    eng = InferenceEngine(net.eval(), batch_size=B, max_points=30000, use_cuda_graph=False)
+    eng.load_points([torch.from_numpy(c).cuda() for c in clouds])
+    with _measure.clocks() as clk:
+        st = eng.run_timed(iters=5)
+        l2_bw = l2_copy_bandwidth()
     stats = {s["index"]: s for s in eng.sparse_layer_stats()}
-    l2_bw = l2_copy_bandwidth()
-    props = torch.cuda.get_device_properties(0)
-    print("device %s, batch %d, L2-resident copy bandwidth %.0f GB/s (read + write)" % (props.name, B, l2_bw / 1e9))
+    print("batch %d, L2-resident copy bandwidth %.0f GB/s (read + write)" % (B, l2_bw / 1e9))
     tot = {"us": 0.0, "gath": 0, "halo": 0}
     for k, v in st.items():
         extra = ""
@@ -98,6 +85,7 @@ def main():
         print("%-16s %8.1f us%s" % (k, v * 1e3, extra))
     print("tensor-pipe sparse layers: %.1f us, gathered %.1f MB, per-tile halo %.1f MB"
           % (tot["us"], tot["gath"] / 1e6, tot["halo"] / 1e6))
+    print(json.dumps({"sm_clock": clk}))
 
 
 if __name__ == "__main__":

@@ -7,31 +7,17 @@ anchor count): milliseconds per forward + backward of
          cross-entropy, sums) -- and its autograd backward
 on the same inputs (tests/loss_ref.make_case "a": mostly background, some ignored, a few positives), the kernels' HBM
 byte bound (DESIGN.md section 5) and the time that bound takes at the H100 SXM data-sheet 3.35 TB/s (arithmetic, not a
-measurement).  Also prints the card name, its power limit and the SM clock read during the run.
+measurement).  Also prints the card name, its power limit and the SM clock sampled during the run.
 """
-import json
-import os
-import subprocess
 import sys
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
-sys.path.insert(0, os.path.join(REPO, "tests"))
-import torch  # noqa: E402
+import _measure
+import loss_ref
+import torch
 
-import loss_ref  # noqa: E402
-from b2second import config, loader, loss, models  # noqa: E402
+from b2second import loss
 
-ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 50
 HBM_BYTES_PER_S = 3.35e12
-
-
-def smi(query):
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=" + query, "--format=csv,noheader", "-i", "0"],
-                              capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def byte_bound(B, A, C, nb, label_bytes):
@@ -44,51 +30,36 @@ def byte_bound(B, A, C, nb, label_bytes):
     return count + fwd_in + fwd_out + bwd
 
 
-def time_ms(fn):
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0.record()
-    for _ in range(ITERS):
-        fn()
-    t1.record()
-    torch.cuda.synchronize()
-    return t0.elapsed_time(t1) / ITERS
-
-
 def main():
-    assert torch.cuda.is_available(), "this tool times CUDA kernels: it needs a GPU"
+    ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 50
+    _measure.require_gpu("loss_times")
     dev = "cuda:0"
-    rows, clocks = [], []
-    for name, B in (("car.fhd", 8), ("nuscenes.all.pp.mhead", 4)):
-        net = models.build_network(config.get_config(name), loader.oracle_spconv())
-        lp = loss.plan(net)
-        s = lp.settings
-        A = int(net.anchors().shape[0])
-        example, preds = loss_ref.make_case("a", B, A, s.num_class, s.num_dir_bins, s.dir_offset, seed=0)
-        ex = {k: v.to(dev) for k, v in example.items()}
-        ex["labels"] = ex["labels"].to(torch.int32)                # what b2second.targets.assign_batch gives
-        pr = {k: v.to(dev).requires_grad_() for k, v in preds.items()}
+    rows = []
+    with _measure.clocks() as clk:
+        for name, B in (("car.fhd", 8), ("nuscenes.all.pp.mhead", 4)):
+            net = _measure.mirror(name, spconv="oracle")
+            lp = loss.plan(net)
+            s = lp.settings
+            A = int(net.anchors().shape[0])
+            example, preds = loss_ref.make_case("a", B, A, s.num_class, s.num_dir_bins, s.dir_offset, seed=0)
+            ex = {k: v.to(dev) for k, v in example.items()}
+            ex["labels"] = ex["labels"].to(torch.int32)                # what b2second.targets.assign_batch gives
+            pr = {k: v.to(dev).requires_grad_() for k, v in preds.items()}
 
-        def fused():
-            lp.loss(ex, pr)["loss"].backward()
+            def fused():
+                lp.loss(ex, pr)["loss"].backward()
 
-        def chain():
-            loss_ref.loss(s, ex, pr)["loss"].backward()
+            def chain():
+                loss_ref.loss(s, ex, pr)["loss"].backward()
 
-        row = {"config": name, "batch": B, "anchors": A, "num_class": s.num_class}
-        row["fused_ms"] = round(time_ms(fused), 4)
-        clocks.append(smi("clocks.sm"))
-        row["torch_ms"] = round(time_ms(chain), 4)
-        clocks.append(smi("clocks.sm"))
-        nbytes = byte_bound(B, A, s.num_class, s.num_dir_bins, 4)
-        row["byte_bound"] = nbytes
-        row["byte_bound_ms"] = round(nbytes / HBM_BYTES_PER_S * 1e3, 4)
-        rows.append(row)
-    print(json.dumps({"tool": "loss_times", "device": torch.cuda.get_device_name(0),
-                      "power_limit": smi("power.limit"), "sm_clock_during_run": clocks, "iters": ITERS,
-                      "results": rows}))
+            row = {"config": name, "batch": B, "anchors": A, "num_class": s.num_class}
+            row["fused_ms"] = round(_measure.timed(fused, ITERS), 4)
+            row["torch_ms"] = round(_measure.timed(chain, ITERS), 4)
+            nbytes = byte_bound(B, A, s.num_class, s.num_dir_bins, 4)
+            row["byte_bound"] = nbytes
+            row["byte_bound_ms"] = round(nbytes / HBM_BYTES_PER_S * 1e3, 4)
+            rows.append(row)
+    _measure.report("loss_times", rows, clk, iters=ITERS)
 
 
 if __name__ == "__main__":

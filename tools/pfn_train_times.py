@@ -6,36 +6,23 @@ nuscenes.all.pp.mhead at B = 3 (T = 60, at most 25 000 per frame, NuScenes-sized
 VoxelGeneratorV2 on the GPU.  Each case times the VFE's forward + backward (loss = sum(out * G)) with
 enable_pfn_training (b2s_pfn_train_forward / _backward) against the torch modules (TF32 off), after a warm-up, and
 reports torch.cuda.max_memory_allocated of each path over the pass.  Prints the card name and power limit of the run."""
-import json
-import os
-import subprocess
 import sys
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, REPO)
-sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
+
+import _measure
 import numpy as np
 import torch
-import bench
-from b2second import config, loader, models, training
 
-ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 20
+from b2second import training
+
 CASES = [("pointpillars.car.xyres_16", 2, 29000), ("nuscenes.all.pp.mhead", 3, 300000)]
-torch.backends.cudnn.allow_tf32 = False
-torch.backends.cuda.matmul.allow_tf32 = False
 
 
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
-
-
-def batch(net, cfg, name, B, points):
+def batch(net, clouds):
     def t(a):
         return a if torch.is_tensor(a) else torch.from_numpy(np.asarray(a))
     vox, num, coors = [], [], []
-    for b, c in enumerate(bench.make_clouds(name, B, points)):
-        res = net.voxel_generator.generate(c, cfg.max_voxels)
+    for b, c in enumerate(clouds):
+        res = net.voxel_generator.generate(c, net.cfg.max_voxels)
         n = int(res["voxel_num"])
         vox.append(t(res["voxels"])[:n].cuda())
         num.append(t(res["num_points_per_voxel"])[:n].cuda())
@@ -43,51 +30,34 @@ def batch(net, cfg, name, B, points):
     return torch.cat(vox).float().contiguous(), torch.cat(num).int(), torch.cat(coors).int().contiguous()
 
 
-def measure(vfe, vox, num, coors, G):
+def measure(vfe, vox, num, coors, G, iters):
     def step():
         out = vfe(vox, num, coors)
         (out * G).sum().backward()
-    for _ in range(3):
-        step()
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats()
-    base = torch.cuda.memory_allocated()
-    step()
-    torch.cuda.synchronize()
-    peak = torch.cuda.max_memory_allocated() - base
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(ITERS):
-        step()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / ITERS, peak
+    return _measure.timed(step, iters), _measure.peak_bytes(step)
 
 
 def main():
-    assert torch.cuda.is_available(), "pfn_train_times.py measures on a CUDA device"
-    sp = loader.product_spconv()
+    ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 20
+    _measure.require_gpu("pfn_train_times")
     rows = []
-    for name, B, points in CASES:
-        cfg = config.get_config(name)
-        res = {}
-        for ours in (False, True):
-            net = models.build_network(cfg, sp)
-            models.synthetic_weights_(net, name, seed=0)
-            net = net.cuda().train()
-            if ours:
-                training.enable_pfn_training(net)
-            vox, num, coors = batch(net, cfg, name, B, points)
-            G = torch.randn(vox.shape[0], 64, device="cuda", generator=torch.Generator("cuda").manual_seed(0))
-            res["ours" if ours else "torch"] = measure(net.voxel_feature_extractor, vox, num, coors, G)
-        N, T, F = vox.shape
-        row = {"config": name, "batch": B, "pillars": N, "T": T, "real_points": int(num.sum()),
-               "ms_ours": round(res["ours"][0], 3), "ms_torch": round(res["torch"][0], 3),
-               "peak_MB_ours": round(res["ours"][1] / 2 ** 20, 1), "peak_MB_torch": round(res["torch"][1] / 2 ** 20, 1)}
-        rows.append(row)
-        print(json.dumps(row), flush=True)
-    print(json.dumps({"card": card(), "iters": ITERS}))
-
+    with _measure.clocks() as clk:
+        for name, B, points in CASES:
+            res = {}
+            for ours in (False, True):
+                net, clouds = _measure.mirror(name, B, points=points)
+                net.train()
+                if ours:
+                    training.enable_pfn_training(net)
+                vox, num, coors = batch(net, clouds)
+                G = torch.randn(vox.shape[0], 64, device="cuda", generator=torch.Generator("cuda").manual_seed(0))
+                res["ours" if ours else "torch"] = measure(net.voxel_feature_extractor, vox, num, coors, G, ITERS)
+            N, T, F = vox.shape
+            rows.append({"config": name, "batch": B, "pillars": N, "T": T, "real_points": int(num.sum()),
+                         "ms_ours": round(res["ours"][0], 3), "ms_torch": round(res["torch"][0], 3),
+                         "peak_MB_ours": round(res["ours"][1] / 2 ** 20, 1),
+                         "peak_MB_torch": round(res["torch"][1] / 2 ** 20, 1)})
+    _measure.report("pfn_train_times", rows, clk, iters=ITERS)
 
 if __name__ == "__main__":
     main()

@@ -10,17 +10,13 @@ Printed per step:
   - the fill stores of the six k_conv3x3_tc2 launches: every background strip, against the bands;
   - the fused tail's reads of layer 6: every tile, against the computed tiles.
 A map is B x 200 x 176 pixels of 2 planes x 128 channels x 2 bytes."""
-import os
 import sys
 
+import _measure  # noqa: F401  (the path set-up)
 import numpy as np
+from rpn_bands_ref import strip_bands, strip_flags, tail_tiles
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
-sys.path.insert(0, os.path.join(REPO, "tests"))
-
-from b2second import config, synth  # noqa: E402
-from rpn_bands_ref import strip_bands, strip_flags, tail_tiles  # noqa: E402
+from b2second import config, synth
 
 ROWS, LAYERS, PIXEL_BYTES = 4, 6, 2 * 128 * 2
 

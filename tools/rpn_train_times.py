@@ -5,47 +5,25 @@ layer shape: forward, input gradient (dgrad) and weight gradient (wgrad) of b2se
 included in forward and dgrad), of cuDNN fp32 (allow_tf32 False) and, for information, of cuDNN TF32, with the
 algorithmic rate 2 * B * H * W * 9 * Cin * Cout / t and each kernel's bound: f16 MMA work (3 products) at the data-sheet
 989 TFLOP/s, or its L2 -> SM operand bytes.  Then the whole RPN forward + backward in train() mode, and the error of
-each path's forward against float64 (max |y - y64| / max |y64|).  Prints the card and its power limit."""
-import os
-import subprocess
-import sys
-
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, REPO)
-sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
+each path's forward against float64 (max |y - y64| / max |y64|).  Prints the card, its power limit and the SM clock
+sampled during the run."""
 import copy
+import json
 
+import _measure
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from b2second import config, loader, models, rpn_train
+from b2second import rpn_train
 
 ITERS = 20
 DEV = "cuda:0"
 MMA_PEAK = 989e12          # dense f16 wgmma, H100 SXM data sheet
 
 
-def card():
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                            capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception as e:                       # noqa: BLE001 - report, do not fail the timing
-        pl = "nvidia-smi unavailable (%s)" % e
-    return "%s | %s" % (torch.cuda.get_device_name(0), pl)
-
-
 def timed(fn, iters=ITERS):
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters * 1e3     # us
+    return _measure.timed(fn, iters) * 1e3     # us
 
 
 def tf32(on):
@@ -91,12 +69,10 @@ def layer_row(B, cin, cout, H, W):
 
 
 def rpn_step(name, B):
-    cfg = config.get_config(name)
-    net = models.build_network(cfg, loader.product_spconv())
-    models.synthetic_weights_(net, name, seed=0)
+    net = _measure.mirror(name)
     rpn = net.rpn
     first = rpn.blocks[0][1]
-    H, W = (int(v) * first.stride[0] for v in cfg.feature_map_size[1:])
+    H, W = (int(v) * first.stride[0] for v in net.cfg.feature_map_size[1:])
     x = (torch.relu(torch.randn(B, first.in_channels, H, W, device=DEV)) *
          (torch.rand(B, 1, H, W, device=DEV) < 0.15)).requires_grad_(True)
     torch_rpn = copy.deepcopy(rpn).to(DEV).train()
@@ -113,36 +89,42 @@ def rpn_step(name, B):
     t_tf32 = timed(lambda: step(torch_rpn), 5)
     tf32(False)
     layers = [(c.in_channels, c.out_channels) for c, _ in rpn_train.select(rpn)]
-    return H, W, layers, t_ours, t_fp32, t_tf32
+    return rpn, H, W, layers, t_ours, t_fp32, t_tf32
+
+
+def config_rows(name, B):
+    """the whole-RPN line and the per-layer table of one config"""
+    rpn, H, W, layers, t_ours, t_fp32, t_tf32 = rpn_step(name, B)
+    print("\n%s, batch %d, RPN input %d x %d, %d covered layers" % (name, B, H, W, len(layers)))
+    print("whole RPN forward + backward (train mode): b2second %.2f ms, cuDNN fp32 %.2f ms (x%.2f), cuDNN TF32 "
+          "%.2f ms" % (t_ours / 1e3, t_fp32 / 1e3, t_fp32 / t_ours, t_tf32 / 1e3))
+    shapes = []
+    h, w = H, W
+    for blk in rpn.blocks:
+        st = blk[1].stride[0]
+        h, w = (h + 2 - 3) // st + 1, (w + 2 - 3) // st + 1
+        for m in blk:
+            if type(m) is nn.Conv2d and m.stride == (1, 1) and rpn_train.qualifies(m, m.padding[0]):
+                key = (m.in_channels, m.out_channels, h, w)
+                if key not in shapes:
+                    shapes.append(key)
+    print("%9s %9s | %8s %8s %8s | %8s %8s %8s | %8s %8s %8s | %6s %6s %6s | %7s %7s | %8s %8s %8s" % (
+        "cin>cout", "H x W", "fwd us", "dgrad", "wgrad", "fp32 fwd", "dgrad", "wgrad", "tf32 fwd", "dgrad",
+        "wgrad", "TF/s f", "d", "w", "MMA us", "L2 GB", "err ours", "fp32", "tf32"))
+    for cin, cout, h, w in shapes:
+        flop, o, f, t, e, mma_us, l2 = layer_row(B, cin, cout, h, w)
+        print("%4d>%-4d %4dx%-4d | %8.1f %8.1f %8.1f | %8.1f %8.1f %8.1f | %8.1f %8.1f %8.1f | %6.1f %6.1f %6.1f |"
+              " %7.1f %7.2f | %8.1e %8.1e %8.1e" % (cin, cout, h, w, *o, *f, *t, *(flop / x / 1e6 for x in o),
+                                                   mma_us, l2 / 1e9, *e))
 
 
 def main():
-    print("card:", card())
-    for name, B in (("car.fhd", 8), ("pointpillars.car.xyres_16", 2)):
-        H, W, layers, t_ours, t_fp32, t_tf32 = rpn_step(name, B)
-        print("\n%s, batch %d, RPN input %d x %d, %d covered layers" % (name, B, H, W, len(layers)))
-        print("whole RPN forward + backward (train mode): b2second %.2f ms, cuDNN fp32 %.2f ms (x%.2f), cuDNN TF32 "
-              "%.2f ms" % (t_ours / 1e3, t_fp32 / 1e3, t_fp32 / t_ours, t_tf32 / 1e3))
-        shapes = []
-        cfg = config.get_config(name)
-        net = models.build_network(cfg, loader.product_spconv())
-        h, w = H, W
-        for blk in net.rpn.blocks:
-            st = blk[1].stride[0]
-            h, w = (h + 2 - 3) // st + 1, (w + 2 - 3) // st + 1
-            for m in blk:
-                if type(m) is nn.Conv2d and m.stride == (1, 1) and rpn_train.qualifies(m, m.padding[0]):
-                    key = (m.in_channels, m.out_channels, h, w)
-                    if key not in shapes:
-                        shapes.append(key)
-        print("%9s %9s | %8s %8s %8s | %8s %8s %8s | %8s %8s %8s | %6s %6s %6s | %7s %7s | %8s %8s %8s" % (
-            "cin>cout", "H x W", "fwd us", "dgrad", "wgrad", "fp32 fwd", "dgrad", "wgrad", "tf32 fwd", "dgrad",
-            "wgrad", "TF/s f", "d", "w", "MMA us", "L2 GB", "err ours", "fp32", "tf32"))
-        for cin, cout, h, w in shapes:
-            flop, o, f, t, e, mma_us, l2 = layer_row(B, cin, cout, h, w)
-            print("%4d>%-4d %4dx%-4d | %8.1f %8.1f %8.1f | %8.1f %8.1f %8.1f | %8.1f %8.1f %8.1f | %6.1f %6.1f %6.1f |"
-                  " %7.1f %7.2f | %8.1e %8.1e %8.1e" % (cin, cout, h, w, *o, *f, *t, *(flop / x / 1e6 for x in o),
-                                                       mma_us, l2 / 1e9, *e))
+    _measure.require_gpu("rpn_train_times")
+    print(json.dumps(_measure.card()))
+    with _measure.clocks() as clk:
+        for name, B in (("car.fhd", 8), ("pointpillars.car.xyres_16", 2)):
+            config_rows(name, B)
+    print(json.dumps({"sm_clock": clk}))
 
 
 if __name__ == "__main__":

@@ -6,21 +6,19 @@ For the bench workload (synthetic 29 k-point KITTI clouds, batch 32 and batch 1)
     (launches are attributed to the stage whose window the host launched them in); the chrome traces go to OUT_DIR
     (default: rulebook_times under the system's temporary directory);
   * live rows per level and the bytes of the tables built for them (nbr, row_mask; capacity-sized for comparison).
-Prints one table per batch and writes OUT_DIR/rulebook_times.json."""
+Prints the card first, one table per batch, and the SM clock sampled during the run; writes the same with the results
+to OUT_DIR/rulebook_times.json."""
 import json
 import os
 import re
 import sys
 import tempfile
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, REPO)
-sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
+
+import _measure
 import torch
-import bench
-from b2second import config, loader, models
+
 from b2second.engine import InferenceEngine
 
-OUT = sys.argv[1] if len(sys.argv) > 1 else os.path.join(tempfile.gettempdir(), "rulebook_times")
 ITERS = 10
 
 
@@ -30,7 +28,7 @@ def short(name):
     return re.sub(r"^.*::", "", name) or name        # and the namespace
 
 
-def profile_stage(eng, prefix="rulebook"):
+def profile_stage(eng, out, prefix="rulebook"):
     """{kernel or memset name: (launches per step, us per step)} of the stages named prefix*"""
     from torch.profiler import record_function
     cur = [None]
@@ -51,8 +49,8 @@ def profile_stage(eng, prefix="rulebook"):
             cur[0] = None
         torch.cuda.synchronize()
     del eng._mark
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "trace_b%d.json" % eng.B)
+    os.makedirs(out, exist_ok=True)
+    path = os.path.join(out, "trace_b%d.json" % eng.B)
     prof.export_chrome_trace(path)
     return stage_split(path, prefix)
 
@@ -95,18 +93,14 @@ def level_stats(eng):
     return out
 
 
-def run(B):
-    sp = loader.product_spconv()
-    cfg = config.get_config("car.fhd")
-    net = models.build_network(cfg, sp).eval()
-    models.synthetic_weights_(net, "car.fhd", seed=0)
-    eng = InferenceEngine(net.cuda(), batch_size=B, max_points=30000, use_cuda_graph=False)
-    clouds = [torch.from_numpy(c).cuda() for c in bench.make_clouds("car.fhd", B, 29000)]
-    eng.load_points(clouds)
+def run(B, out):
+    net, clouds = _measure.mirror("car.fhd", B)
+    eng = InferenceEngine(net.eval(), batch_size=B, max_points=30000, use_cuda_graph=False)
+    eng.load_points([torch.from_numpy(c).cuda() for c in clouds])
     stages = eng.run_timed(iters=20)
     rb_ms = sum(v for k, v in stages.items() if k.startswith("rulebook"))
     step_ms = sum(stages.values())
-    kernels = profile_stage(eng)
+    kernels = profile_stage(eng, out)
     levels = level_stats(eng)
     eng.check_status()
     print("car.fhd B=%d: rulebook stage %.3f ms of %.3f ms (run_timed, eager)  launches/step %d" % (
@@ -128,10 +122,18 @@ def run(B):
     return res
 
 
+def main():
+    out = sys.argv[1] if len(sys.argv) > 1 else os.path.join(tempfile.gettempdir(), "rulebook_times")
+    _measure.require_gpu("rulebook_times")
+    card = _measure.card()
+    print(json.dumps(card))
+    with _measure.clocks() as clk:
+        results = [run(B, out) for B in (32, 1)]
+    print(json.dumps({"sm_clock": clk}))
+    os.makedirs(out, exist_ok=True)
+    with open(os.path.join(out, "rulebook_times.json"), "w") as f:
+        json.dump({**card, "sm_clock": clk, "results": results}, f, indent=1)
+
+
 if __name__ == "__main__":
-    props = torch.cuda.get_device_properties(0)
-    print("device: %s" % props.name)
-    results = [run(B) for B in (32, 1)]
-    os.makedirs(OUT, exist_ok=True)
-    with open(os.path.join(OUT, "rulebook_times.json"), "w") as f:
-        json.dump({"device": props.name, "results": results}, f, indent=1)
+    main()

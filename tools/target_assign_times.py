@@ -6,30 +6,15 @@ row; thresholds and the box encode only touch positives' neighbours), (8 + 4 * c
 (label, importance, box target) -- the write floor at the H100 SXM data-sheet 3.35 TB/s (arithmetic, not a
 measurement), and the anchor-GT pair evaluations (two per pair: one per pass).  GTs are drawn around random anchors.
 """
-import json
-import os
-import subprocess
 import sys
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(REPO, "second.pytorch_b200"))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
+import _measure
+import numpy as np
+import torch
 
-from b2second import config, models, targets  # noqa: E402
+from b2second import config, models, targets
 
-ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 50
 HBM_BYTES_PER_S = 3.35e12
-
-
-def card():
-    name = torch.cuda.get_device_name(0)
-    try:
-        limit = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                               capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        limit = "unknown"
-    return name, limit
 
 
 def frames(plan, B, G, dtype, rng):
@@ -44,40 +29,32 @@ def frames(plan, B, G, dtype, rng):
 
 
 def main():
-    assert torch.cuda.is_available(), "this tool times CUDA kernels: it needs a GPU"
+    ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 50
+    _measure.require_gpu("target_assign_times")
     rng = np.random.default_rng(0)
     rows = []
-    for name, dtype in (("car.fhd", np.float32), ("all.fhd", np.float32), ("nuscenes.all.pp.largea", np.float64)):
-        cfg = config.get_config(name)
-        plan = targets.plan(models.MirrorTargetAssigner(cfg), cfg.feature_map_size)
-        A = plan.num_anchors
-        for B in (8, 32):
-            for G in (30, 200):
-                gt, offs, cls = frames(plan, B, G, dtype, rng)
-                for _ in range(3):
-                    plan.assign_batch(gt, offs, cls)
-                torch.cuda.synchronize()
-                t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                t0.record()
-                for _ in range(ITERS):
-                    plan.assign_batch(gt, offs, cls)
-                t1.record()
-                torch.cuda.synchronize()
-                ms = t0.elapsed_time(t1) / ITERS
-                written = B * A * (8 + 4 * plan.code_size)
-                # pairs: each anchor against its segment's GTs of the frame (per class in per-class mode)
-                seg_of = (cls - 1).cpu().numpy() if plan.assign_per_class else np.zeros(B * G, np.int64)
-                pairs = 0
-                for b in range(B):
-                    counts = np.bincount(seg_of[b * G:(b + 1) * G], minlength=len(plan.segments))
-                    pairs += sum(int(counts[i]) * (s.end - s.begin) for i, s in enumerate(plan.segments))
-                rows.append({"config": name, "batch": B, "gt_per_frame": G, "anchors": A, "gt_dtype": np.dtype(dtype).name,
-                             "ms": round(ms, 4), "bytes_read": 16 * A, "bytes_written": written,
-                             "write_floor_ms": round(written / HBM_BYTES_PER_S * 1e3, 4),
-                             "pair_evaluations": 2 * pairs})
-    name, limit = card()
-    print(json.dumps({"tool": "target_assign_times", "device": name, "power_limit": limit, "iters": ITERS,
-                      "results": rows}))
+    with _measure.clocks() as clk:
+        for name, dtype in (("car.fhd", np.float32), ("all.fhd", np.float32), ("nuscenes.all.pp.largea", np.float64)):
+            cfg = config.get_config(name)
+            plan = targets.plan(models.MirrorTargetAssigner(cfg), cfg.feature_map_size)
+            A = plan.num_anchors
+            for B in (8, 32):
+                for G in (30, 200):
+                    gt, offs, cls = frames(plan, B, G, dtype, rng)
+                    ms = _measure.timed(lambda: plan.assign_batch(gt, offs, cls), ITERS)
+                    written = B * A * (8 + 4 * plan.code_size)
+                    # pairs: each anchor against its segment's GTs of the frame (per class in per-class mode)
+                    seg_of = (cls - 1).cpu().numpy() if plan.assign_per_class else np.zeros(B * G, np.int64)
+                    pairs = 0
+                    for b in range(B):
+                        counts = np.bincount(seg_of[b * G:(b + 1) * G], minlength=len(plan.segments))
+                        pairs += sum(int(counts[i]) * (s.end - s.begin) for i, s in enumerate(plan.segments))
+                    rows.append({"config": name, "batch": B, "gt_per_frame": G, "anchors": A,
+                                 "gt_dtype": np.dtype(dtype).name, "ms": round(ms, 4), "bytes_read": 16 * A,
+                                 "bytes_written": written,
+                                 "write_floor_ms": round(written / HBM_BYTES_PER_S * 1e3, 4),
+                                 "pair_evaluations": 2 * pairs})
+    _measure.report("target_assign_times", rows, clk, iters=ITERS)
 
 
 if __name__ == "__main__":
