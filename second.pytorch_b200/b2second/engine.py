@@ -87,6 +87,23 @@ class _Level:
     __slots__ = ("coors", "n_dev", "keys", "vals", "hcap", "cap", "shape")
 
 
+class _Streamed:
+    """what streamed batches add to an engine, allocated on the first streamed call: slot 1's input buffers (slot 0's
+    are the engine's own ``points`` / ``offsets``), the copy stream, and per slot the free / ready / done events and
+    the pinned read-back buffers."""
+
+    def __init__(self, eng):
+        self.points = torch.zeros_like(eng.points)
+        self.offsets = torch.zeros_like(eng.offsets)
+        self.copy = torch.cuda.Stream(eng.dev)
+        self.free = [torch.cuda.Event(), torch.cuda.Event()]
+        self.ready = [torch.cuda.Event(), torch.cuda.Event()]
+        self.done = [torch.cuda.Event(), torch.cuda.Event()]
+        self.rec_host = [torch.empty(eng.B, eng.rec_width, dtype=torch.float32).pin_memory() for _ in range(2)]
+        self.status_host = [torch.zeros(1, dtype=torch.int32).pin_memory() for _ in range(2)]
+        self.next_slot = 0
+
+
 class InferenceEngine:
     def __init__(self, net, batch_size=1, max_points=None, max_voxels=None, row_cap_factor=2.0,
                  cand_cap=None, use_cuda_graph=True, rpn_impl="auto", sparse_impl="tc", device=None,
@@ -576,20 +593,21 @@ class InferenceEngine:
         return self.det_record[:, :self.rec_width - 1].view(self.B, self.post_max, self.code + 2)
 
     # ---------------------------------------------------------------- the launch sequence
-    def _launch(self, mode="points"):
+    def _launch(self, mode="points", slot=0):
         L, lib, s = self._L, self.lib, self.spec
         st = L.stream()
         self.status.zero_()
         if mode == "points":
+            points, offsets = self._inputs(slot)
             self._mark("voxelize")
             L.check(lib.b2s_voxelize(
-                L.ptr(self.points), L.ptr(self.offsets), self.P_cap, self.F, self.B,
+                L.ptr(points), L.ptr(offsets), self.P_cap, self.F, self.B,
                 L.f3(s.point_cloud_range[:3]), L.f3(s.voxel_size), L.i3(self.grid), self.T, self.max_voxels,
                 L.ptr(self.vox_coors), L.ptr(self.vox_num), L.ptr(self.vox_slots), None, self.vfe_mode, self.vfe_nf,
                 L.ptr(self.vfe_out), L.ptr(self.num_voxels), L.ptr(self.vox_keys), L.ptr(self.vox_vals), self.vox_hcap,
                 int(self.level0.shape[0]),       # hash keys in the middle encoder's shape (grid_z + 1, middle.py:139)
                 L.ptr(self.vox_ws), self.vox_ws_bytes, L.ptr(self.status), st), "b2s_voxelize")
-            pfn_points, pfn_slots = self.points, self.vox_slots
+            pfn_points, pfn_slots = points, self.vox_slots
         else:
             # the caller's voxels / num_points / coordinates are already in in_voxels / vox_num / vox_coors and
             # num_voxels[0] holds their count: build level 0's locator and the voxel features from them
@@ -979,12 +997,14 @@ class InferenceEngine:
         self._mask_src, self.use_mask = "given", True
         self.anchors_mask.copy_(mask.reshape(self.B, self.A).to(torch.uint8), non_blocking=True)
 
-    def load_points(self, frames):
-        """frames: list of B CUDA (or pinned/CPU) float32 [P_i, F] tensors -> static input buffers."""
+    def load_points(self, frames, slot=0):
+        """frames: list of B CUDA (or pinned/CPU) float32 [P_i, F] tensors -> static input buffers (of input slot
+        `slot`; slot 1 is streamed batches' second pair, see stream_load).  The copies go on the current stream."""
         assert len(frames) == self.B
         sizes = [int(f.shape[0]) for f in frames]
         total = sum(sizes)
         assert total <= self.P_cap, "more points (%d) than the engine's capacity (%d)" % (total, self.P_cap)
+        points, offsets = self._inputs(slot)
         # frames that lie back to back in memory (views of one pinned slab, or of one device tensor) go over in ONE copy:
         # a serving loop that reads clouds into a pinned ring buffer pays one cudaMemcpyAsync per batch instead of B.
         # The run structure only depends on where the frames lie: a serving loop cycles through a few slabs, so it is
@@ -1006,10 +1026,10 @@ class InferenceEngine:
             for i, off, run_rows, whole in runs:
                 if whole:
                     src = torch.as_strided(frames[i], (run_rows, self.F), (self.F, 1))
-                    self.points[off:off + run_rows].copy_(src, non_blocking=True)
+                    points[off:off + run_rows].copy_(src, non_blocking=True)
                 else:
-                    self.points[off:off + run_rows].copy_(frames[i], non_blocking=True)
-            return self._load_offsets(sizes, total)
+                    points[off:off + run_rows].copy_(frames[i], non_blocking=True)
+            return self._load_offsets(sizes, total, offsets)
         runs = []
         off, i = 0, 0
         while i < len(frames):
@@ -1029,17 +1049,17 @@ class InferenceEngine:
             if run_rows:
                 if j - i > 1:
                     src = torch.as_strided(f, (run_rows, self.F), (self.F, 1))      # the whole run through frame i's storage
-                    self.points[off:off + run_rows].copy_(src, non_blocking=True)
+                    points[off:off + run_rows].copy_(src, non_blocking=True)
                 else:
-                    self.points[off:off + run_rows].copy_(f, non_blocking=True)
+                    points[off:off + run_rows].copy_(f, non_blocking=True)
                 runs.append((i, off, run_rows, j - i > 1))
             off += run_rows
             i = j
         if len(cache) < 16 and all(f.dtype == torch.float32 for f in frames):
             cache[key] = runs
-        return self._load_offsets(sizes, total)
+        return self._load_offsets(sizes, total, offsets)
 
-    def _load_offsets(self, sizes, total):
+    def _load_offsets(self, sizes, total, offsets):
         # frame offsets through a pinned staging buffer that is allocated once (a fresh pin_memory() per call is a
         # cudaHostAlloc on the serving path); two slots, so the copy of the previous call is never overwritten in flight
         if getattr(self, "_offs_host", None) is None:
@@ -1050,7 +1070,7 @@ class InferenceEngine:
         self._offs_slot ^= 1
         self._offs_evt[slot].synchronize()                 # (no-op unless two calls ago is still copying)
         self._offs_host[slot].copy_(torch.from_numpy(np.cumsum([0] + sizes).astype(np.int32)))
-        self.offsets.copy_(self._offs_host[slot], non_blocking=True)
+        offsets.copy_(self._offs_host[slot], non_blocking=True)
         self._offs_evt[slot].record()
         return total
 
@@ -1112,15 +1132,17 @@ class InferenceEngine:
         self.num_voxels.copy_(self._nvox_host, non_blocking=True)
         return n
 
-    def run(self, mode="points"):
-        """launch the pipeline on the data currently in the static buffers (async)."""
+    def run(self, mode="points", slot=0):
+        """launch the pipeline on the data currently in the static buffers (of input slot `slot`) (async)."""
         # the grid sizes of the per-point kernels are fixed at capacity so one graph serves any frame mix
         with torch.cuda.device(self.dev):
             if not self.use_graph:
                 with torch.no_grad():
-                    self._launch(mode)
+                    self._launch(mode, slot)
                 return self.det, self.det_count
-            key = (mode, self._mask_src)
+            # a slot's graph reads that slot's input buffers; every other buffer is shared by the slots' graphs, which
+            # replay in order on one stream
+            key = (mode, self._mask_src) if slot == 0 else (mode, self._mask_src, slot)
             g = self._graphs.get(key)
             if g is None:
                 with torch.no_grad():
@@ -1128,12 +1150,12 @@ class InferenceEngine:
                     side.wait_stream(torch.cuda.current_stream())
                     with torch.cuda.stream(side):
                         for _ in range(3):          # warm-up: cuDNN autotune, lazy module init, func attributes
-                            self._launch(mode)
+                            self._launch(mode, slot)
                     torch.cuda.current_stream().wait_stream(side)
                     torch.cuda.synchronize()
                     g = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(g):
-                        self._launch(mode)
+                        self._launch(mode, slot)
                     self._graphs[key] = g
             g.replay()
         return self.det, self.det_count
@@ -1145,6 +1167,77 @@ class InferenceEngine:
     def infer_voxels(self, voxels, num_points, coordinates):
         self.load_voxels(voxels, num_points, coordinates)
         return self.run("voxels")
+
+    # ---------------------------------------------------------------- streamed batches (FastPath.stream)
+    # Two input slots: while the graph of one slot's batch runs on the compute stream (the current stream), the next
+    # batch's clouds go over the copy stream into the other slot.  Per slot k: the copy stream waits on free[k]
+    # (recorded after the last replay that read slot k) before writing the slot and records ready[k]; the compute
+    # stream waits on ready[k] before replaying slot k's graph; done[k] follows slot k's read-back into its own pinned
+    # buffers.  Every buffer after the inputs is shared: the graphs replay in order on the compute stream.
+    _streamed = None
+
+    def _inputs(self, slot):
+        """(points, offsets) of input slot `slot`: slot 0 is the pair every entry point loads, slot 1 the second pair
+        streamed batches alternate with"""
+        if slot == 0:
+            return self.points, self.offsets
+        return self._streamed.points, self._streamed.offsets
+
+    def _stream_state(self):
+        s = self._streamed
+        if s is None:
+            with torch.cuda.device(self.dev):
+                s = self._streamed = _Streamed(self)
+        return s
+
+    def stream_load(self, frames):
+        """enqueue frames (a list of B float32 [P_i, F] clouds: pinned, pageable or CUDA) on the engine's copy stream
+        into the input slot the previous streamed batch did not use; returns that slot.  Raises before any copy is
+        enqueued when the batch exceeds the point capacity.  The copies overlap the current (compute) stream's work
+        only from pinned memory; device clouds are copied once the compute stream has reached this call (they may
+        still be being written there)."""
+        s = self._stream_state()
+        slot = s.next_slot
+        compute = torch.cuda.current_stream(self.dev)
+        with torch.cuda.device(self.dev), torch.cuda.stream(s.copy):
+            s.copy.wait_event(s.free[slot])
+            if any(f.is_cuda for f in frames):
+                s.copy.wait_stream(compute)
+            self.load_points(frames, slot)
+            s.ready[slot].record(s.copy)
+        s.next_slot ^= 1
+        return slot
+
+    def stream_run(self, slot, mode="points"):
+        """replay slot `slot`'s graph on the current stream once stream_load's copies have landed"""
+        s = self._streamed
+        compute = torch.cuda.current_stream(self.dev)
+        compute.wait_event(s.ready[slot])
+        self.run(mode, slot)
+        s.free[slot].record(compute)
+
+    def stream_read_back(self, slot, output):
+        """enqueue on the current stream the read-back of the batch just run from slot `slot` into the slot's pinned
+        buffers (and, for output="device", the snapshot clone); returns what stream_results needs besides the slot"""
+        s = self._streamed
+        with torch.cuda.device(self.dev):
+            snap = self._read_back(s.rec_host[slot], s.status_host[slot], output)
+            s.done[slot].record(torch.cuda.current_stream(self.dev))
+        return snap
+
+    def stream_results(self, slot, snap, metadata, output):
+        """wait for slot `slot`'s read-back and build its list of dicts, as detections() does"""
+        s = self._streamed
+        s.done[slot].synchronize()
+        return self._results(s.rec_host[slot], s.status_host[slot], snap, metadata, output)
+
+    def stream_wait(self):
+        """wait for every streamed copy and read-back enqueued so far"""
+        s = self._streamed
+        if s is not None:
+            s.copy.synchronize()
+            for ev in s.done:
+                ev.synchronize()
 
     def check_status(self):
         """sync + raise on data-dependent overflow (call when results are read back)."""
@@ -1162,24 +1255,35 @@ class InferenceEngine:
         output="host": ONE pinned D2H copy of the detection records (counts ride in the records' last element) +
         one stream sync, sliced on the host into CPU tensors.  output="device": the tensors stay on the GPU like the
         reference's (one snapshot clone, per-frame views)."""
-        code, B = self.code, self.B
-        meta = metadata if metadata is not None and len(metadata) > 0 else [None] * B
         if getattr(self, "_rec_host", None) is None:
-            self._rec_host = torch.empty(B, self.rec_width, dtype=torch.float32).pin_memory()
+            self._rec_host = torch.empty(self.B, self.rec_width, dtype=torch.float32).pin_memory()
             self._status_host = torch.zeros(1, dtype=torch.int32).pin_memory()
         with torch.cuda.device(self.dev):
-            self._rec_host.copy_(self.det_record, non_blocking=True)
-            self._status_host.copy_(self.status, non_blocking=True)
-            if output == "device":
-                snap = self.det.clone()
-                labels = snap[..., code + 1].long()
+            snap = self._read_back(self._rec_host, self._status_host, output)
             torch.cuda.current_stream().synchronize()          # the one sync of the step
-        st = int(self._status_host[0])
+        return self._results(self._rec_host, self._status_host, snap, metadata, output)
+
+    def _read_back(self, rec_host, status_host, output):
+        """enqueue on the current stream the D2H of the detection records and the status word into the given pinned
+        buffers, and for output="device" the snapshot clone; returns (snapshot, labels) or None"""
+        rec_host.copy_(self.det_record, non_blocking=True)
+        status_host.copy_(self.status, non_blocking=True)
+        if output == "device":
+            snap = self.det.clone()
+            return snap, snap[..., self.code + 1].long()
+        return None
+
+    def _results(self, rec_host, status_host, snap, metadata, output):
+        """the list of dicts from a read-back that has landed; raises on a status bit other than voxel overflow"""
+        code, B = self.code, self.B
+        meta = metadata if metadata is not None and len(metadata) > 0 else [None] * B
+        st = int(status_host[0])
         if st & ~1:   # bit 1 (voxel overflow) is the reference's own drop-extra-voxels behaviour
             raise RuntimeError("b2second engine: " + self._L.status_message(st))
-        cnt = self._rec_host[:, -1].round().to(torch.int64).tolist()
+        cnt = rec_host[:, -1].round().to(torch.int64).tolist()
         out = []
         if output == "device":
+            snap, labels = snap
             for b in range(B):
                 n = cnt[b]
                 out.append({"box3d_lidar": snap[b, :n, :code], "scores": snap[b, :n, code],
@@ -1187,7 +1291,7 @@ class InferenceEngine:
             return out
         # per-frame views through numpy: 3 B tensor views cost ~0.1 ms this way and ~0.8 ms as torch indexing ops (the
         # Python between two steps is GPU idle time on the serving path)
-        host = self._rec_host.numpy()[:, :-1].reshape(B, self.post_max, code + 2).copy()
+        host = rec_host.numpy()[:, :-1].reshape(B, self.post_max, code + 2).copy()
         labels = host[..., code + 1].astype(np.int64)
         fn = torch.from_numpy
         for b in range(B):

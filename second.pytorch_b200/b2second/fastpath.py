@@ -27,10 +27,15 @@ The list of result dicts holds GPU tensors like the reference's (``output="devic
 output="host")`` returns CPU tensors through ONE pinned device-to-host copy of the detection records instead of one
 small copy per frame and field.
 
+``net.b2s_fastpath.stream(examples)`` (``FastPath.stream``) serves an iterable of ``points`` examples: it yields what
+``net(example)`` would return for each, while the next batch's clouds go over to the GPU during the current batch's
+graph (two input slots per engine, ``InferenceEngine.stream_load``).
+
 Anything the engine does not cover (training mode, the DataParallel padded layout, a layer pattern
 ``spec_from_module`` rejects) falls through to the module's original ``forward`` -- which still computes on the CUDA
 ``spconv`` drop-in; there is no CPU path anywhere.
 """
+import collections
 import types
 
 import torch
@@ -77,12 +82,7 @@ class FastPath:
         else:
             B = int(example["anchors"].shape[0])
         eng = self.engine(B)
-        if "anchors" in example and example["anchors"] is not None:
-            anchors = example["anchors"]
-            eng.set_anchors(anchors.reshape(anchors.shape[0], -1, anchors.shape[-1]))   # asserts the anchor count
-        elif eng._anchors_key is None:
-            raise KeyError("example has no 'anchors' and the network cannot generate them")
-        eng.set_anchors_mask(example.get("anchors_mask"))
+        self._set_anchors(eng, example)
         if "sweeps" in example:
             eng.load_sweeps(list(frames))             # NuScenes: key frame + sweeps merged on the GPU
             eng.run("points")
@@ -96,6 +96,82 @@ class FastPath:
         if self.post_run is not None:
             self.post_run(eng)
         return eng.detections(metadata=example.get("metadata"), output=self.output)
+
+    @staticmethod
+    def _set_anchors(eng, example):
+        if "anchors" in example and example["anchors"] is not None:
+            anchors = example["anchors"]
+            eng.set_anchors(anchors.reshape(anchors.shape[0], -1, anchors.shape[-1]))   # asserts the anchor count
+        elif eng._anchors_key is None:
+            raise KeyError("example has no 'anchors' and the network cannot generate them")
+        eng.set_anchors_mask(example.get("anchors_mask"))
+
+    def _stream_frames(self, example):
+        """the clouds of a streamed example; raises for what stream() does not take"""
+        if self.net.training:
+            raise RuntimeError("stream() runs the fused engine, which serves eval() networks only")
+        carried = [k for k in ("voxels", "sweeps", "crop_planes") if example.get(k) is not None]
+        if carried or "points" not in example:
+            raise ValueError("stream() takes examples of raw clouds under 'points' (without %s); other examples go "
+                             "through net(example)" % "/".join(carried or ["voxels", "sweeps", "crop_planes"]))
+        return list(example["points"])
+
+    def stream(self, examples):
+        """yield, in input order, what ``net(example)`` returns for each example of the iterable ``examples``, with the
+        host-to-device copies of each batch overlapping the previous batch's graph.
+
+        An example is a ``points`` dict as ``net(example)`` takes it: B float32 ``[P_i, F]`` clouds (pinned, pageable
+        or CUDA), ``anchors`` unless the network generates them, optional ``anchors_mask`` and ``metadata``.  The
+        batch size may change from example to example.  Only pinned clouds are copied while the previous batch
+        computes; pageable and CUDA clouds give the same results with less overlap.  ``voxels``, ``sweeps`` and
+        ``crop_planes`` examples raise ValueError (they go through ``net(example)``); a network in ``train()`` mode
+        raises RuntimeError.  Neither enqueues anything.
+
+        At most two batches are in flight: example k+1 is taken from the iterable and enqueued before the result of
+        example k is built and yielded, so the host builds that result while batch k+1 computes.  The caller may
+        reuse or overwrite an example's memory once that example's result has been yielded, and not before.
+
+        Errors are raised at the failing batch's turn, after every earlier result has been yielded: a status error
+        (anything but voxel overflow) raises the RuntimeError ``detections()`` raises; a batch over the point
+        capacity raises load_points' AssertionError before its copy is enqueued; a refused example raises as above.
+        Closing the generator early (``break``, ``close()``, an exception in the caller) waits for the work in flight;
+        the engines are then ready for ``net(example)`` or a new stream.  ``post_run`` is called once per batch, on
+        the stream that runs the graphs, after the batch's graph and before its read-back."""
+        # (engine, slot, snapshot, example) of the batches in flight, in input order: holding the example keeps its
+        # clouds alive until their copies are known to be done
+        pending = collections.deque()
+        compute = None
+        try:
+            for example in examples:
+                try:
+                    frames = self._stream_frames(example)
+                    eng = self.engine(len(frames))
+                    if compute is None:     # every engine's graphs replay on this one stream, so batches stay in order
+                        compute = torch.cuda.current_stream(eng.dev)
+                    with torch.no_grad(), torch.cuda.stream(compute):
+                        slot = eng.stream_load(frames)
+                        self._set_anchors(eng, example)
+                        eng.stream_run(slot)
+                        if self.post_run is not None:
+                            self.post_run(eng)
+                        snap = eng.stream_read_back(slot, self.output)
+                except Exception:
+                    while pending:
+                        yield self._stream_result(pending.popleft())
+                    raise
+                pending.append((eng, slot, snap, example))
+                if len(pending) == 2:
+                    yield self._stream_result(pending.popleft())
+            while pending:
+                yield self._stream_result(pending.popleft())
+        finally:
+            pending.clear()
+            for eng in self.engines.values():
+                eng.stream_wait()
+
+    def _stream_result(self, item):
+        eng, slot, snap, example = item
+        return eng.stream_results(slot, snap, example.get("metadata"), self.output)
 
 
 def accelerate(net, **kw):
