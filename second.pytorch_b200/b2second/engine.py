@@ -143,15 +143,118 @@ class InferenceEngine:
         self.sparse_impl = sparse_impl
         # anchor-area mask of the reference's eval preprocessing (preprocess.py:345-357): None / negative = off
         self.area_threshold = float(anchor_area_threshold) if _anchor_mask.enabled(anchor_area_threshold) else None
+        # every operand derived from the weights is allocated by its first fill (_fill) while the engine is built;
+        # refresh() runs the same fills again into the same tensors
+        self._allocating = True
         with torch.cuda.device(dev):
             self.status = torch.zeros(1, dtype=torch.int32, device=dev)
             self._plan_middle(row_cap_factor)
             self._alloc_voxel_buffers()
             if rpn_impl == "tc":
                 self._alloc_tc_rpn()
+            else:
+                self._module_ptrs = self._rpn_module_ptrs()
             self._alloc_detect_buffers(cand_cap)
             if self.area_threshold is not None:
                 self._alloc_area_mask()
+        self._allocating = False
+
+    # ---------------------------------------------------------------- weight-derived operands
+    def _fill(self, dst, key, value):
+        """store the weight-derived operand ``value`` as ``dst[key]``: allocated while the engine is built, written in
+        place by a refresh, so the addresses the captured graphs hold stay valid"""
+        if value is None:
+            assert dst.get(key) is None, "operand %s appeared or vanished" % key
+            dst[key] = None
+            return
+        if self._allocating:
+            dst[key] = torch.empty(value.shape, dtype=value.dtype, device=self.dev)
+        t = dst[key]
+        if t is None or t.shape != value.shape or t.dtype != value.dtype:
+            raise _spec.UnsupportedNetwork("operand %s changed shape or type since the engine was built" % key)
+        t.copy_(value)
+
+    def _fill_middle(self):
+        """the PFN's weight and folded BatchNorm, or every sparse layer's weight, folded BatchNorm and, on the tensor
+        pipe, its packed fp16 hi/lo weight planes and epilogue scale -- from the spec"""
+        s = self.spec
+        if self.is_pillars:
+            p = s.pfn
+            for key, v in (("pfn_w", p["w"]), ("pfn_scale", p["scale"]), ("pfn_shift", p["shift"])):
+                self._fill(vars(self), key, v)
+            return
+        for lyr, ls in zip(self.layers, s.layers):
+            for key in ("w", "scale", "shift"):
+                self._fill(lyr, key, ls[key])
+            if lyr["tc"]:
+                wp = _tc.pack_sparse_weights(lyr["w"])
+                ws = _tc.pow2_scale(wp)
+                hi, lo = _tc.split_f16(wp, ws)
+                base = lyr["scale"] if lyr["scale"] is not None else torch.ones(lyr["cout"], device=self.dev)
+                self._fill(lyr, "w_hi", hi)
+                self._fill(lyr, "w_lo", lo)
+                self._fill(lyr, "scale_tc", (base.float() / ws).contiguous())
+
+    def _rpn_plan(self):
+        D, H, W = self.final_level.shape
+        rpn, heads = self.spec.rpn, getattr(self.spec, "heads", None)
+        return _tc.plan_rpn(rpn, H, W) if heads is None else _tc.plan_rpn_multihead(rpn, dict(heads), H, W)
+
+    def _fill_tc_rpn(self):
+        """every tensor-core RPN op's weight planes, epilogue scale and shift -- blocks, deblock sub-grids, packed head
+        records, the multi-head network's crop-branch convs -- from the live modules through tc.plan_rpn*"""
+        plan = self._rpn_plan()
+        if self._allocating:
+            self.tc_prog, self.tc_plan = plan, plan["ops"]
+        elif _tc.plan_layout(plan) != _tc.plan_layout(self.tc_prog):
+            raise _spec.UnsupportedNetwork("the RPN's layer plan changed since the engine was built")
+        for op, new in zip(self.tc_plan, plan["ops"]):
+            for key in _tc.OP_OPERANDS:
+                self._fill(op, key, new.get(key))
+            if "w_scale" in new:
+                op["w_scale"] = new["w_scale"]
+
+    def _fill_background(self):
+        """the background-tracked layers' empty-frame responses, the fused tail's empty-frame records and their margins;
+        -> whether a margin (a host-side launch argument of the captured graphs) changed"""
+        fields, records = self._empty_frame_response()
+        if self._allocating:
+            self.bg_field, self.tail_field = fields, records
+        else:
+            for old, new in zip(self.bg_field, fields):
+                for o, n in zip(old, new):
+                    o.copy_(n)
+            self.tail_field.copy_(records)
+        margins = ([_field_margin(hi, lo) for hi, lo in self.bg_field],
+                   _record_margin(self.tail_field, self.tc_plan[-1]["cout"]))
+        changed = margins != (getattr(self, "bg_margin", None), getattr(self, "tail_margin", None))
+        self.bg_margin, self.tail_margin = margins
+        return changed
+
+    def _rpn_module_ptrs(self):
+        """addresses of the RPN / head modules' tensors, which the rpn_impl="cudnn" graphs read directly"""
+        mods = [self.spec.rpn] + [m for _, m in (getattr(self.spec, "heads", None) or [])]
+        return [t.data_ptr() for m in mods for t in list(m.parameters()) + list(m.buffers())]
+
+    def refresh(self):
+        """re-derive every weight-derived operand from the spec (``b2second.spec.refresh`` re-reads the network into
+        it) by the fills that built them, into the same tensors; bit for bit what a newly built engine holds.  The
+        work is enqueued on the current stream, after whatever is already there, so batches enqueued before finish with
+        the weights they were enqueued with.  The captured graphs stay valid unless a host-side launch argument changed
+        (a background margin; for rpn_impl="cudnn" the address of a module tensor): then they are dropped and
+        re-captured on the next run.  -> whether they were dropped."""
+        with torch.cuda.device(self.dev), torch.no_grad():
+            self._fill_middle()
+            if self.rpn_impl == "tc":
+                self._fill_tc_rpn()
+                drop = bool(self.bg_idx) and self._fill_background()
+            else:
+                ptrs = self._rpn_module_ptrs()
+                drop, self._module_ptrs = ptrs != self._module_ptrs, ptrs
+            if drop and self._graphs:
+                torch.cuda.synchronize(self.dev)        # no replay of a graph in flight when it is destroyed
+                self._graphs = {}
+        return drop
 
     # ---------------------------------------------------------------- planning / allocation
     def _new_level(self, cap, shape, with_storage=True):
@@ -180,11 +283,10 @@ class InferenceEngine:
         if self.is_pillars:
             self.level0 = self._new_level(cap0, s.sparse_shape, with_storage=False)
             p = s.pfn
-            self.pfn_w = p["w"].to(dev)
-            self.pfn_scale, self.pfn_shift = p["scale"].to(dev), p["shift"].to(dev)
             self.pfn_cout = p["cout"]
             if p["with_distance"]:
                 raise _spec.UnsupportedNetwork("PillarFeatureNet with_distance (off in every BASELINE config)")
+            self._fill_middle()                                          # pfn_w, pfn_scale, pfn_shift
             self.pfn_geom = (p["vx"], p["vy"], p["x_offset"], p["y_offset"])
             self.pfn_deco = int(getattr(s, "pfn_decoration", 0))      # B2S_PFN_PLAIN / B2S_PFN_RADIUS
             self.feat_final_c = self.pfn_cout
@@ -197,11 +299,8 @@ class InferenceEngine:
         max_ws = 0
         for j, ls in enumerate(s.layers):
             K = ls["K"]
-            lyr = dict(ls)
+            lyr = {k: v for k, v in ls.items() if not isinstance(v, torch.Tensor)}    # operands: _fill_middle
             lyr["index"] = j
-            lyr["w"] = ls["w"].to(dev)
-            lyr["scale"] = None if ls["scale"] is None else ls["scale"].to(dev)
-            lyr["shift"] = None if ls["shift"] is None else ls["shift"].to(dev)
             if ls["subm"]:
                 key = ("subm", ls["indice_key"], id(level)) if ls["indice_key"] is not None else ("subm", j)
                 if key not in rulebooks:
@@ -259,17 +358,13 @@ class InferenceEngine:
         for j, lyr in enumerate(self.layers):
             cap = lyr["out_level"].cap
             if lyr["tc"]:
-                wp = _tc.pack_sparse_weights(lyr["w"])
-                ws = _tc.pow2_scale(wp)
-                lyr["w_hi"], lyr["w_lo"] = _tc.split_f16(wp, ws)
-                base = lyr["scale"] if lyr["scale"] is not None else torch.ones(lyr["cout"], device=dev)
-                lyr["scale_tc"] = (base.float() / ws).contiguous()
                 lyr["out_buf"], lyr["out_hi"], lyr["out_lo"], lyr["out_stride"] = self._hilo_rows(cap, lyr["cout"])
                 if j == 0 or not self.layers[j - 1]["tc"]:
                     # first tensor-pipe layer: its fp32 input rows are split into fp16 hi/lo planes first
                     lyr["in_split"] = self._hilo_rows(lyr["in_level"].cap, lyr["cin_tc"])
             else:
                 lyr["out"] = torch.zeros(cap, lyr["cout"], dtype=torch.float32, device=dev)
+        self._fill_middle()
         self.any_sparse_tc = any(l["tc"] for l in self.layers)
         self.rb_ws = torch.empty(max(max_ws, 1), dtype=torch.uint8, device=dev)
         self.rb_ws_bytes = max_ws
@@ -324,9 +419,8 @@ class InferenceEngine:
         if next(rpn.parameters()).device != dev:
             raise ValueError("the RPN's parameters must live on the engine's device")
         heads = getattr(self.spec, "heads", None)
-        plan = _tc.plan_rpn(rpn, H, W) if heads is None else _tc.plan_rpn_multihead(rpn, dict(heads), H, W)
-        self.tc_prog = plan
-        self.tc_plan = plan["ops"]
+        self._fill_tc_rpn()                                 # tc_prog, tc_plan and the ops' operands
+        plan = self.tc_prog
         # single-scale tail (one k = s = 1 deblock 128 -> 128 feeding the heads): one fused kernel, the deblock output
         # never goes to HBM (csrc/rpn_tail.cu; bit-identical to the two launches)
         self.tc_tail_fused = _tc.fusable_tail(plan)
@@ -378,21 +472,29 @@ class InferenceEngine:
             self.tail_work = torch.zeros(self.tail_tiles, dtype=torch.int32, device=dev)
             self.tail_bg = torch.zeros(self.tail_tiles, dtype=torch.int32, device=dev)
             self.tail_counts = torch.zeros(2, dtype=torch.int32, device=dev)
-            self.bg_field, self.tail_field = self._empty_frame_response()
-            self.bg_margin = [_field_margin(hi, lo) for hi, lo in self.bg_field]
-            self.tail_margin = _record_margin(self.tail_field, plan["ops"][-1]["cout"])
+            self._fill_background()                         # bg_field, tail_field, bg_margin, tail_margin
 
     def _empty_frame_response(self):
         """per background-tracked layer: what the layer's own kernel produces for an empty frame, as one halo-padded
         frame [H+2, W+2, C] of fp16 hi/lo planes; and the fused tail's head records [H, W, stride] for an empty frame,
-        from the tail kernel on the last layer's response.  Run once at plan time on frame 0 of the (still all-zero)
-        buffers."""
+        from the tail kernel on the last layer's response.  Computed in one-frame zero planes of its own, so the
+        engine's activation buffers, BEV planes, bev_occ and strip state -- which the next batch reads -- are not
+        touched."""
         L, lib = self._L, self.lib
         st = L.stream()
+        shapes = dict(self.tc_prog["buffers"], **{"in": self.tc_hw + (self.tc_bev[0].shape[-1],)})
+        planes = {}
+
+        def plane(name):
+            if name not in planes:
+                h, w, c = shapes[name]
+                planes[name] = tuple(torch.zeros(1, h + 2, w + 2, c, dtype=torch.float16, device=self.dev)
+                                     for _ in range(2))
+            return planes[name]
         fields = []
         for oi in self.bg_idx:
             op = self.tc_plan[oi]
-            src, dst = self.tc_bufs[op["src"]], self.tc_bufs[op["dst"]]
+            src, dst = plane(op["src"]), plane(op["dst"])
             cdst = dst[0].shape[-1]
             L.check(lib.b2s_conv2d_tc_ex(
                 L.ptr(src[0]), L.ptr(src[1]), 1, op["Hin"], op["Win"], op["cin"], L.ptr(op["w_hi"]),
@@ -403,14 +505,9 @@ class InferenceEngine:
                 L.ptr(self.status), st), "b2s_conv2d_tc_ex(empty frame)")
             fields.append((dst[0][0, :, :, :op["cout"]].clone().contiguous(),
                            dst[1][0, :, :, :op["cout"]].clone().contiguous()))
-        d, h = self.tc_plan[-2], self.tc_plan[-1]
-        src = self.tc_bufs[d["src"]]
+        d = self.tc_plan[-2]
         records = torch.zeros(1, d["Hin"], d["Win"], self.tc_head_stride, dtype=torch.float32, device=self.dev)
-        self._launch_fused_tail(src, records, 1, None, None, None, None, None, -1, st)
-        torch.cuda.synchronize(self.dev)
-        for oi in self.bg_idx:                    # leave the activation buffers as they were (all zero)
-            for t in self.tc_bufs[self.tc_plan[oi]["dst"]]:
-                t[0].zero_()
+        self._launch_fused_tail(plane(d["src"]), records, 1, None, None, None, None, None, -1, st)
         return fields, records[0]
 
     def _launch_fused_tail(self, src, out, batch, work, work_n, bgl, bgn, field, margin, st):

@@ -31,6 +31,11 @@ small copy per frame and field.
 ``net(example)`` would return for each, while the next batch's clouds go over to the GPU during the current batch's
 graph (two input slots per engine, ``InferenceEngine.stream_load``).
 
+The engine holds copies of the weights in its own layouts (folded BatchNorm, packed fp16 planes, background fields).
+``eval()`` / ``train(False)`` and ``load_state_dict`` on the accelerated network mark them stale, and the next call
+re-derives them from the network's current parameters and buffers (``FastPath.refresh``), so a training loop can
+evaluate on the engine between steps and a restored checkpoint is served as loaded.
+
 Anything the engine does not cover (training mode, the DataParallel padded layout, a layer pattern
 ``spec_from_module`` rejects) falls through to the module's original ``forward`` -- which still computes on the CUDA
 ``spconv`` drop-in; there is no CPU path anywhere.
@@ -56,8 +61,37 @@ class FastPath:
         self.engine_kw = engine_kw
         self.spec = _spec.spec_from_module(net, max_voxels)      # raises UnsupportedNetwork for foreign layer patterns
         self.engines = {}
+        self.stale = False           # the network's weights may have changed since the engines' operands were derived
+        self.refreshes = 0           # refresh() calls that completed
+
+    def mark_stale(self):
+        """note that the network's weights may have changed: the next call, streamed batch or engine build refreshes
+        first (accelerate marks on every train(False) / eval() and after load_state_dict)"""
+        self.stale = True
+
+    def refresh(self):
+        """re-derive every engine operand from the network's current parameters and buffers: the folded BatchNorm, the
+        packed weight planes of the sparse layers, the PFN and every RPN op, and the background fields the RPN's
+        empty strips are filled from.  Each operand then equals, bit for bit, what a newly built engine would hold.
+        Every engine built so far is refreshed in place (same addresses: captured graphs stay valid, unless a
+        background margin changed, when they are re-captured on their next run); engines built later read the refreshed
+        spec.  The work is enqueued on the current stream after everything already enqueued there, so batches in
+        flight finish with the weights they were enqueued with.  Idempotent.
+
+        Raises ``b2second.spec.UnsupportedNetwork`` when the network's structure (layer list, shapes, head layout)
+        changed since ``accelerate`` or a parameter moved to another device; the fast path then stays stale, so every
+        later call raises too, rather than serving a different network.  Non-weight attributes (NMS thresholds, the
+        anchor configuration, the voxel generator) are read once, at ``accelerate``, and not re-read here."""
+        with torch.no_grad():
+            _spec.refresh(self.spec, self.net)
+            for eng in self.engines.values():
+                eng.refresh()
+        self.stale = False
+        self.refreshes += 1
 
     def engine(self, batch_size):
+        if self.stale:
+            self.refresh()
         eng = self.engines.get(batch_size)
         if eng is None:
             from .engine import InferenceEngine
@@ -145,6 +179,9 @@ class FastPath:
             for example in examples:
                 try:
                     frames = self._stream_frames(example)
+                    if self.stale and compute is not None:
+                        with torch.cuda.stream(compute):       # after the replays of the batches in flight
+                            self.refresh()
                     eng = self.engine(len(frames))
                     if compute is None:     # every engine's graphs replay on this one stream, so batches stay in order
                         compute = torch.cuda.current_stream(eng.dev)
@@ -176,11 +213,24 @@ class FastPath:
 
 def accelerate(net, **kw):
     """re-bind ``net.forward`` to the fused engine (see module docstring); returns ``net``.
-    ``net.b2s_fastpath`` is the FastPath object, ``net.b2s_reference_forward`` the original bound method."""
+    ``net.b2s_fastpath`` is the FastPath object, ``net.b2s_reference_forward`` the original bound method.
+
+    ``net.train`` is wrapped as well: ``train(False)`` / ``eval()`` set the modes exactly as before and then mark the
+    fast path stale, and so does a ``load_state_dict`` on ``net`` (a post-hook).  A stale fast path refreshes
+    (``FastPath.refresh``) at its next call, streamed batch or engine build; a call that is not stale does no refresh
+    work.  So a training loop can evaluate on the engine between steps, and a restored checkpoint is served as
+    loaded."""
     if getattr(net, "b2s_fastpath", None) is not None:
         return net
     fast = FastPath(net, **kw)
     original = net.forward
+    original_train = net.train
+
+    def train(self, mode=True):
+        out = original_train(mode)
+        if not mode:
+            fast.mark_stale()
+        return out
 
     def forward(self, example):
         if fast.applicable(example):
@@ -191,4 +241,6 @@ def accelerate(net, **kw):
     net.b2s_fastpath = fast
     net.b2s_reference_forward = original
     net.forward = types.MethodType(forward, net)
+    net.train = types.MethodType(train, net)
+    net.register_load_state_dict_post_hook(lambda module, incompatible_keys: fast.mark_stale())
     return net

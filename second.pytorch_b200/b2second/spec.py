@@ -224,7 +224,51 @@ def spec_from_module(net, max_voxels=None):
             raise UnsupportedNetwork("the per-class NMS branch on the multi-head network")
         _check_head_feature_maps(net, s)
     s.anchor_source = net
+    s.layout = structure(s)          # as read now: the RPN and head modules are live, so refresh compares to this
     return s
+
+
+STRUCTURE_KEYS = ("device", "vfe_kind", "vfe_num_features", "num_point_features", "is_pillars", "sparse_shape",
+                  "pfn_decoration", "num_class", "box_code_size", "num_anchors_per_loc", "use_direction_classifier",
+                  "num_direction_bins", "head_feature_map_sizes")
+
+
+def structure(s):
+    """what an engine's layout depends on: the spec with every weight tensor replaced by its shape (the predict()
+    parameters and the voxel generator are left out: refresh does not re-read them)"""
+    def layout(d):
+        return None if d is None else {k: tuple(v.shape) if isinstance(v, torch.Tensor) else v for k, v in d.items()}
+
+    def shapes(m):
+        return {k: tuple(v.shape) for k, v in m.state_dict().items()}
+
+    st = {k: getattr(s, k) for k in STRUCTURE_KEYS}
+    st["layers"] = [layout(lyr) for lyr in s.layers]
+    st["pfn"] = layout(s.pfn)
+    st["rpn"] = shapes(s.rpn)
+    st["heads"] = None if s.heads is None else [(name, shapes(m)) for name, m in s.heads]
+    return st
+
+
+def refresh(s, net):
+    """re-read the weights of ``net`` (the module ``s`` was read from) into the spec ``s``: the sparse layers' weights
+    and folded BatchNorm, the PFN's, and the RPN / head modules the engine plans from.  Raises UnsupportedNetwork, and
+    leaves ``s`` as it was, when the network no longer has the structure of ``s`` (layers, shapes, head layout) or a
+    parameter or BatchNorm buffer has left the spec's device."""
+    new = spec_from_module(net, s.max_voxels)
+    old_st, new_st = s.layout, new.layout
+    if old_st != new_st:
+        changed = sorted(k for k in old_st if old_st[k] != new_st[k])
+        raise UnsupportedNetwork("the network's structure changed since it was accelerated (%s); accelerate a newly "
+                                 "built network instead" % ", ".join(changed))
+    tensors = list(net.parameters())
+    for m in net.modules():
+        if isinstance(m, nn.modules.batchnorm._BatchNorm):
+            tensors += [t for t in (m.running_mean, m.running_var) if t is not None]
+    if any(t.device != s.device for t in tensors):
+        raise UnsupportedNetwork("a parameter or BatchNorm buffer is no longer on %s, the device the network was "
+                                 "accelerated on" % s.device)
+    s.layers, s.pfn, s.rpn, s.heads = new.layers, new.pfn, new.rpn, new.heads
 
 
 def _head_module(m, what, with_net):

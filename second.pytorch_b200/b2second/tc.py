@@ -294,6 +294,18 @@ def _plan_backbone(rpn, H, W, dry):
     return bufs, ops, emit, (cur, h, w), stage0
 
 
+# the fields of an op that plan_rpn* derives from the weights: the device operands and the host power of two behind
+# "scale"
+OP_OPERANDS = ("w_hi", "w_lo", "scale", "shift")
+
+
+def plan_layout(plan):
+    """a plan of plan_rpn* without its weight-derived fields: what the engine's buffers and launches depend on"""
+    out = {k: v for k, v in plan.items() if k != "ops"}
+    out["ops"] = [{k: v for k, v in op.items() if k not in OP_OPERANDS + ("w_scale",)} for op in plan["ops"]]
+    return out
+
+
 def fusable_tail(plan):
     """True when the program ends with ONE k = s = 1 deblock 128 -> 128 (+BN+ReLU) whose output only feeds the packed heads
     (<= 32 channels): the shape b2s_rpn_tail_tc runs as a single kernel (car.fhd, car.lite; all.fhd packs 104 head
