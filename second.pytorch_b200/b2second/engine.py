@@ -13,9 +13,9 @@ buffers, so the whole frame batch is ONE CUDA graph:
   b2s_anchor_area_mask (only with anchor_area_threshold >= 0 and no example mask)   preprocess.py:345-357
   per sparse layer: b2s_rulebook_{subm,conv} (cached per indice_key) + b2s_sparse_conv_tc (wgmma, fp16 hi/lo
       planes flow from layer to layer) with BatchNorm1d/ReLU folded into the epilogue      middle.py:145-192
-  b2s_pfn (PointPillars) / b2s_pfn_ex (PillarFeatureNetRadius) pointpillars.py:203-237,240-325
+  b2s_pfn_ex (PointPillars: plain decoration, PillarFeatureNetRadius: radius)   pointpillars.py:203-237,240-325
   b2s_to_bev_tc_ex (NHWC + halo, fp16 hi/lo)                   middle.py:206-209 / pointpillars.py:444-476
-  RPN as a program of b2s_conv2d_tc_ex launches (tc.plan_rpn)  rpn.py:314-331,393-420,467-497
+  RPN as a program of b2s_conv2d_tc_ex2 launches (tc.plan_rpn) rpn.py:314-331,393-420,467-497
       (rpn_impl="cudnn" keeps the torch modules as a cross-check: fp32, TF32 off)
   b2s_decode_filter_strided + b2s_nms (+ direction/range epilogue)   voxelnet.py:377-645
 
@@ -46,6 +46,11 @@ from . import tc as _tc
 # For the same reason background strips inside the field's constant interior (_field_margin) are stored from a value
 # the fill warps hold in registers instead of being copied from the field
 BG_ROWS = 4
+
+# one head map as the decode kernels read it: b2s_decode_filter_strided's leading arguments, in order, and the leading
+# fields of b2s_head_segment
+_HEAD_VIEW = ("box", "cls", "dir", "box_batch_stride", "cls_batch_stride", "dir_batch_stride", "ch_stride",
+              "pix_stride")
 
 
 def _field_margin(hi, lo):
@@ -137,7 +142,8 @@ class InferenceEngine:
             rpn_impl = "tc" if _tc.supported(s.rpn, s.heads) else "cudnn"
         assert rpn_impl in ("tc", "cudnn")
         if rpn_impl == "tc" and not _tc.supported(s.rpn, s.heads):
-            raise ValueError("rpn_impl='tc': this RPN has a layer b2s_conv2d_tc_ex does not cover (channels % 64, kernel > 4)")
+            raise ValueError("rpn_impl='tc': this RPN has a layer b2s_conv2d_tc_ex2 does not cover (channels % 64, "
+                             "kernel > 4)")
         self.rpn_impl = rpn_impl
         assert sparse_impl in ("tc", "fma")       # sparse-conv inner product: wgmma 3xF16 | fp32 FMA tiles
         self.sparse_impl = sparse_impl
@@ -480,8 +486,7 @@ class InferenceEngine:
         from the tail kernel on the last layer's response.  Computed in one-frame zero planes of its own, so the
         engine's activation buffers, BEV planes, bev_occ and strip state -- which the next batch reads -- are not
         touched."""
-        L, lib = self._L, self.lib
-        st = L.stream()
+        st = self._L.stream()
         shapes = dict(self.tc_prog["buffers"], **{"in": self.tc_hw + (self.tc_bev[0].shape[-1],)})
         planes = {}
 
@@ -495,20 +500,32 @@ class InferenceEngine:
         for oi in self.bg_idx:
             op = self.tc_plan[oi]
             src, dst = plane(op["src"]), plane(op["dst"])
-            cdst = dst[0].shape[-1]
-            L.check(lib.b2s_conv2d_tc_ex(
-                L.ptr(src[0]), L.ptr(src[1]), 1, op["Hin"], op["Win"], op["cin"], L.ptr(op["w_hi"]),
-                L.ptr(op["w_lo"]), op["kh"], op["kw"], op["stride"], op["pad"], op["cout"], op["n_pad"],
-                L.ptr(op["scale"]), L.ptr(op["shift"]) if op["shift"] is not None else None,
-                1 if op["relu"] else 0, op["Hg"], op["Wg"], L.ptr(dst[0]), L.ptr(dst[1]), op["Hout"], op["Wout"],
-                1, cdst, op["out_mul"], op["off_h"], op["off_w"], None, None, None, None, None, None,
-                L.ptr(self.status), st), "b2s_conv2d_tc_ex(empty frame)")
+            self._launch_conv(op, src, dst, 1, None, None, -1, st)
             fields.append((dst[0][0, :, :, :op["cout"]].clone().contiguous(),
                            dst[1][0, :, :, :op["cout"]].clone().contiguous()))
         d = self.tc_plan[-2]
         records = torch.zeros(1, d["Hin"], d["Win"], self.tc_head_stride, dtype=torch.float32, device=self.dev)
         self._launch_fused_tail(plane(d["src"]), records, 1, None, None, None, None, None, -1, st)
         return fields, records[0]
+
+    def _launch_conv(self, op, src, dst, batch, lists, field, margin, st):
+        """one b2s_conv2d_tc_ex2 launch of the tc_plan op ``op``: hi/lo planes ``src`` -> planes ``dst`` from the op's
+        channel offset on.  ``lists``: (strip work list, its count, background strip list, its count), or None for a
+        dense launch; ``field``: the (hi, lo) empty-frame response the background strips are stored from, or None."""
+        L = self._L
+        cdst = dst[0].shape[-1]                                   # channels per pixel of the destination map
+        esz = dst[0].element_size()
+        o_hi = ctypes_ptr(dst[0].data_ptr() + esz * op["dst_coff"])
+        o_lo = ctypes_ptr(dst[1].data_ptr() + esz * op["dst_coff"]) if op["planes"] == 2 else None
+        work, work_n, bgl, bgn = lists or (None,) * 4
+        bhi, blo = (L.ptr(field[0]), L.ptr(field[1])) if field is not None else (None, None)
+        L.check(self.lib.b2s_conv2d_tc_ex2(
+            L.ptr(src[0]), L.ptr(src[1]), batch, op["Hin"], op["Win"], op["cin"], L.ptr(op["w_hi"]),
+            L.ptr(op["w_lo"]), op["kh"], op["kw"], op["stride"], op["pad"], op["cout"], op["n_pad"],
+            L.ptr(op["scale"]), L.ptr(op["shift"]), 1 if op["relu"] else 0, op["Hg"], op["Wg"], o_hi, o_lo,
+            op["Hout"], op["Wout"], 1 if op["padded"] else 0, cdst, op["out_mul"], op["off_h"], op["off_w"],
+            work, work_n, bgl, bgn, bhi, blo, margin, BG_ROWS, L.ptr(self.status), st),
+            "b2s_conv2d_tc_ex2(%s)" % op["kind"])
 
     def _launch_fused_tail(self, src, out, batch, work, work_n, bgl, bgn, field, margin, st):
         L, lib = self._L, self.lib
@@ -524,7 +541,7 @@ class InferenceEngine:
             return self.tc_prog["heads"]["H"], self.tc_prog["heads"]["W"]
         D, H, W = self.final_level.shape
         with torch.no_grad():
-            y = self.spec.rpn.conv_box(self._rpn_backbone(torch.zeros(1, self.bev_cd, H, W, device=self.dev)))
+            y = self.spec.rpn.conv_box(self._rpn_backbone(torch.zeros(1, self.bev_cd, H, W, device=self.dev))[0])
         return int(y.shape[2]), int(y.shape[3])
 
     def _head_segments(self):
@@ -550,6 +567,15 @@ class InferenceEngine:
     def _rpn_multihead(self, x):
         """VoxelNetNuscenesMultiHead.network_forward after the scatter (net_multi_head.py:155-161) on the torch modules:
         cuDNN cross-check path.  -> [(box, cls, dir) NCHW conv outputs] per head, large first."""
+        x, stage0 = self._rpn_backbone(x)
+        c = int(np.round(stage0.shape[2] * 0.1))
+        hd = dict(self.spec.heads)
+        small = hd["small"].net(stage0[:, :, c:-c, c:-c])
+        return [self._conv_heads(hd["large"], x), self._conv_heads(hd["small"], small)]
+
+    def _rpn_backbone(self, x):
+        """RPNNoHeadBase.forward (rpn.py:314-331) on the torch modules: cuDNN cross-check path only.  -> (the
+        concatenated map, stage 0's output)"""
         rpn = self.spec.rpn
         ups, stage0 = [], None
         for i in range(len(rpn.blocks)):
@@ -560,26 +586,12 @@ class InferenceEngine:
                 ups.append(rpn.deblocks[i - rpn._upsample_start_idx](x))
         if len(ups) > 0:
             x = torch.cat(ups, dim=1)
-        c = int(np.round(stage0.shape[2] * 0.1))
-        hd = dict(self.spec.heads)
-        small = hd["small"].net(stage0[:, :, c:-c, c:-c])
-        out = []
-        for m, feat in ((hd["large"], x), (hd["small"], small)):
-            out.append((m.conv_box(feat).contiguous(), m.conv_cls(feat).contiguous(),
-                        m.conv_dir_cls(feat).contiguous() if self.spec.use_direction_classifier else None))
-        return out
+        return x, stage0
 
-    def _rpn_backbone(self, x):
-        """RPNNoHeadBase.forward (rpn.py:314-331) on the torch modules: cuDNN cross-check path only."""
-        rpn = self.spec.rpn
-        ups = []
-        for i in range(len(rpn.blocks)):
-            x = rpn.blocks[i](x)
-            if i - rpn._upsample_start_idx >= 0:
-                ups.append(rpn.deblocks[i - rpn._upsample_start_idx](x))
-        if len(ups) > 0:
-            x = torch.cat(ups, dim=1)
-        return x
+    def _conv_heads(self, m, x):
+        """a head module's box / cls / dir 1x1 convs on the torch modules -> (box, cls, dir or None), NCHW"""
+        return (m.conv_box(x).contiguous(), m.conv_cls(x).contiguous(),
+                m.conv_dir_cls(x).contiguous() if self.spec.use_direction_classifier else None)
 
     def _alloc_detect_buffers(self, cand_cap):
         s, dev = self.spec, self.dev
@@ -721,16 +733,10 @@ class InferenceEngine:
         if self.is_pillars:
             vx, vy, xo, yo = self.pfn_geom
             self._mark("pfn")
-            if self.pfn_deco == 0:
-                L.check(lib.b2s_pfn(L.ptr(pfn_points), self.F, L.ptr(pfn_slots), L.ptr(self.vox_num),
-                                    L.ptr(self.vox_coors), L.ptr(self.num_voxels), self.level0.cap, self.T,
-                                    L.ptr(self.pfn_w), L.ptr(self.pfn_scale), L.ptr(self.pfn_shift), self.pfn_cout,
-                                    vx, vy, xo, yo, L.ptr(self.pfn_out), st), "b2s_pfn")
-            else:
-                L.check(lib.b2s_pfn_ex(L.ptr(pfn_points), self.F, L.ptr(pfn_slots), L.ptr(self.vox_num),
-                                       L.ptr(self.vox_coors), L.ptr(self.num_voxels), self.level0.cap, self.T,
-                                       L.ptr(self.pfn_w), L.ptr(self.pfn_scale), L.ptr(self.pfn_shift), self.pfn_cout,
-                                       vx, vy, xo, yo, self.pfn_deco, L.ptr(self.pfn_out), st), "b2s_pfn_ex")
+            L.check(lib.b2s_pfn_ex(L.ptr(pfn_points), self.F, L.ptr(pfn_slots), L.ptr(self.vox_num),
+                                   L.ptr(self.vox_coors), L.ptr(self.num_voxels), self.level0.cap, self.T,
+                                   L.ptr(self.pfn_w), L.ptr(self.pfn_scale), L.ptr(self.pfn_shift), self.pfn_cout,
+                                   vx, vy, xo, yo, self.pfn_deco, L.ptr(self.pfn_out), st), "b2s_pfn_ex")
             feats, hilo = self.pfn_out, None
         else:
             feats, hilo = self.vfe_out, None          # hilo = (hi, lo, stride) once on the tensor pipe
@@ -785,8 +791,14 @@ class InferenceEngine:
                                                 lyr["cout"], st), "b2s_sparse_conv")
                     feats, hilo = lyr["out"], None
         if self.rpn_impl == "tc":
-            self._launch_tc_tail(feats, hilo)
-            return
+            heads = self._launch_tc_rpn(feats, hilo, st)
+        else:
+            heads = self._launch_cudnn_rpn(feats, hilo, st)
+        self._launch_detect(heads, st)
+
+    def _launch_cudnn_rpn(self, feats, hilo, st):
+        """sparse rows -> NCHW BEV -> the torch RPN modules (cuDNN cross-check) -> one _head_view per head."""
+        L, lib = self._L, self.lib
         fl = self.final_level
         D, H, W = fl.shape
         if hilo is not None:          # back to plain fp32 rows for the NCHW scatter (hi + lo is exact)
@@ -800,47 +812,23 @@ class InferenceEngine:
                                D, H, W, L.ptr(self.bev), 0, st), "b2s_to_bev")
         self._mark("rpn")
         if self.segments is not None:
-            outs = self._rpn_multihead(self.bev)
-            self._keep = outs
-            self._mark("decode_filter")
-            segs = []
-            for g, (box, cls, dirp) in zip(self.segments, outs):
-                HW = g["H"] * g["W"]
-                segs.append({"box": box.data_ptr(), "cls": cls.data_ptr(), "dir": dirp.data_ptr() if dirp is not None else None,
-                             "box_batch_stride": g["a_loc"] * self.code * HW, "cls_batch_stride": g["a_loc"] * s.num_class * HW,
-                             "dir_batch_stride": g["a_loc"] * s.num_direction_bins * HW, "ch_stride": HW, "pix_stride": 1,
-                             "a_loc": g["a_loc"], "H": g["H"], "W": g["W"], "anchor_base": g["base"]})
-            self._launch_decode_segments(segs, st)                                   # NCHW conv outputs
-            self._launch_nms(st)
-            return
-        rpn = s.rpn
-        x = self._rpn_backbone(self.bev)
-        box = rpn.conv_box(x).contiguous()
-        cls = rpn.conv_cls(x).contiguous()
-        dirp = rpn.conv_dir_cls(x).contiguous() if s.use_direction_classifier else None
-        self._keep = (x, box, cls, dirp)
-        self._mark("decode_filter")
-        HW = self.fH * self.fW
-        self._launch_decode(L.ptr(box), L.ptr(cls), L.ptr(dirp), self.a_loc * self.code * HW, self.a_loc * s.num_class * HW,
-                            self.a_loc * s.num_direction_bins * HW, HW, 1, st)      # NCHW conv outputs
-        self._launch_nms(st)
+            self._keep = self._rpn_multihead(self.bev)
+            return [self._head_view(o, g["H"], g["W"], g["a_loc"]) for g, o in zip(self.segments, self._keep)]
+        x, _ = self._rpn_backbone(self.bev)
+        self._keep = (x,) + self._conv_heads(self.spec.rpn, x)
+        return [self._head_view(self._keep[1:], self.fH, self.fW, self.a_loc)]
 
-    def _launch_tc_tail(self, feats, hilo):
-        """BEV (NHWC, halo, fp16 hi/lo) -> wgmma RPN layers -> packed heads -> decode/filter -> NMS."""
-        L, lib, s = self._L, self.lib, self.spec
-        st = L.stream()
+    def _launch_tc_rpn(self, feats, hilo, st):
+        """sparse rows -> BEV (NHWC, halo, fp16 hi/lo) -> wgmma RPN layers -> packed head records -> one _head_view
+        per head."""
+        L, lib = self._L, self.lib
         fl = self.final_level
         D, H, W = fl.shape
         self._mark("to_bev")
-        if hilo is not None:
-            L.check(lib.b2s_to_bev_tc_ex(None, L.ptr(hilo[0]), L.ptr(hilo[1]), hilo[2], L.ptr(fl.coors),
-                                         L.ptr(fl.n_dev), fl.cap, self.feat_final_c, self.B, D, H, W,
-                                         L.ptr(self.tc_bev[0]), L.ptr(self.tc_bev[1]), L.ptr(self.bev_occ), st),
-                    "b2s_to_bev_tc_ex")
-        else:
-            L.check(lib.b2s_to_bev_tc_ex(L.ptr(feats), None, None, 0, L.ptr(fl.coors), L.ptr(fl.n_dev), fl.cap,
-                                         self.feat_final_c, self.B, D, H, W, L.ptr(self.tc_bev[0]),
-                                         L.ptr(self.tc_bev[1]), L.ptr(self.bev_occ), st), "b2s_to_bev_tc_ex")
+        feat, f_hi, f_lo, f_stride = (feats, None, None, 0) if hilo is None else (None,) + hilo
+        L.check(lib.b2s_to_bev_tc_ex(L.ptr(feat), L.ptr(f_hi), L.ptr(f_lo), f_stride, L.ptr(fl.coors), L.ptr(fl.n_dev),
+                                     fl.cap, self.feat_final_c, self.B, D, H, W, L.ptr(self.tc_bev[0]),
+                                     L.ptr(self.tc_bev[1]), L.ptr(self.bev_occ), st), "b2s_to_bev_tc_ex")
         self._mark("rpn")
         nl = len(self.bg_idx)
         if nl:
@@ -861,28 +849,15 @@ class InferenceEngine:
                 L.check(lib.b2s_crop_nhwc(L.ptr(src[0]), L.ptr(src[1]), self.B, op["Hin"], op["Win"], op["cin"],
                                           op["crop"], L.ptr(dst[0]), L.ptr(dst[1]), st), "b2s_crop_nhwc")
                 continue
-            cdst = dst[0].shape[-1]                                   # channels per pixel of the destination map
-            esz = dst[0].element_size()
-            o_hi = ctypes_ptr(dst[0].data_ptr() + esz * op["dst_coff"])
-            o_lo = ctypes_ptr(dst[1].data_ptr() + esz * op["dst_coff"]) if op["planes"] == 2 else None
-            work = work_n = bgl = bgn = bhi = blo = None
-            margin = -1
+            lists, field, margin = None, None, -1
             if oi in self.bg_idx:
                 bl = self.bg_idx.index(oi)
-                chi, clo = self.bg_field[bl]
-                work, work_n = L.ptr(self.bg_work[bl]), L.ptr(self.bg_counts[bl, 0:])
                 # the conv kernel's fill warps store the empty-frame response into the background strips a later
                 # launch reads
-                bgl, bgn = L.ptr(self.bg_bands[bl]), L.ptr(self.bg_band_counts[bl:])
-                bhi, blo = L.ptr(chi), L.ptr(clo)
-                margin = self.bg_margin[bl]
-            L.check(lib.b2s_conv2d_tc_ex2(
-                L.ptr(src[0]), L.ptr(src[1]), self.B, op["Hin"], op["Win"], op["cin"], L.ptr(op["w_hi"]),
-                L.ptr(op["w_lo"]), op["kh"], op["kw"], op["stride"], op["pad"], op["cout"], op["n_pad"],
-                L.ptr(op["scale"]), L.ptr(op["shift"]) if op["shift"] is not None else None,
-                1 if op["relu"] else 0, op["Hg"], op["Wg"], o_hi, o_lo, op["Hout"], op["Wout"],
-                1 if op["padded"] else 0, cdst, op["out_mul"], op["off_h"], op["off_w"], work, work_n, bgl, bgn, bhi, blo,
-                margin, BG_ROWS, L.ptr(self.status), st), "b2s_conv2d_tc_ex2(%s)" % op["kind"])
+                lists = (L.ptr(self.bg_work[bl]), L.ptr(self.bg_counts[bl, 0:]), L.ptr(self.bg_bands[bl]),
+                         L.ptr(self.bg_band_counts[bl:]))
+                field, margin = self.bg_field[bl], self.bg_margin[bl]
+            self._launch_conv(op, src, dst, self.B, lists, field, margin, st)
         if not marked_tail:
             self._mark("rpn_1x1")
         if self.tc_tail_fused:
@@ -894,60 +869,55 @@ class InferenceEngine:
             else:
                 self._launch_fused_tail(src, self.tc_heads, self.B, None, None, None, None, None, -1, st)
         if self.segments is not None:
-            self._mark("decode_filter")
-            segs = []
-            for g, pg in zip(self.segments, self.tc_prog["segments"]):
-                t = self.tc_seg_heads[g["name"]]
-                esz, S, offs = t.element_size(), pg["stride"], pg["offsets"]
-                bs = g["H"] * g["W"] * S
-                segs.append({"box": t.data_ptr() + offs[0] * esz, "cls": t.data_ptr() + offs[1] * esz,
-                             "dir": t.data_ptr() + offs[2] * esz if s.use_direction_classifier else None,
-                             "box_batch_stride": bs, "cls_batch_stride": bs, "dir_batch_stride": bs, "ch_stride": 1,
-                             "pix_stride": S, "a_loc": g["a_loc"], "H": g["H"], "W": g["W"], "anchor_base": g["base"]})
-            self._launch_decode_segments(segs, st)                                   # packed NHWC head records
-            self._launch_nms(st)
-            return
-        S = self.tc_head_stride
+            return [self._head_view(self.tc_seg_heads[g["name"]], g["H"], g["W"], offsets=pg["offsets"])
+                    for g, pg in zip(self.segments, self.tc_prog["segments"])]
+        return [self._head_view(self.tc_heads, self.fH, self.fW, offsets=self.tc_prog["heads"]["offsets"])]
+
+    def _head_view(self, heads, H, W, a_loc=None, offsets=None):
+        """one head map as the decode kernels read it: a tuple in _HEAD_VIEW order.  ``heads``: the (box, cls, dir or
+        None) NCHW conv outputs [B, a_loc * n, H, W]; or, with ``offsets``, a packed record map [B, H, W, S] whose box,
+        cls and dir channels start at offsets[0], [1] and [2]."""
+        s, HW = self.spec, H * W
+        if offsets is None:
+            box, cls, dirp = heads
+            return (box.data_ptr(), cls.data_ptr(), dirp.data_ptr() if dirp is not None else None,
+                    a_loc * self.code * HW, a_loc * s.num_class * HW, a_loc * s.num_direction_bins * HW, HW, 1)
+        S, esz = heads.shape[-1], heads.element_size()
+        box, cls, dirp = (heads.data_ptr() + o * esz for o in offsets[:3])
+        return (box, cls, dirp if s.use_direction_classifier else None, HW * S, HW * S, HW * S, 1, S)
+
+    def _launch_detect(self, heads, st):
+        """the head maps (one _head_view each, in anchor order) -> sigmoid + score threshold + box decode over all
+        anchors -> candidate lists (per frame, or per (class, frame)) -> NMS."""
+        L, lib, s = self._L, self.lib, self.spec
         self._mark("decode_filter")
-        offs = self.tc_prog["heads"]["offsets"]
-        heads = self.tc_heads
-        esz = heads.element_size()
-        box_p = ctypes_ptr(heads.data_ptr() + offs[0] * esz)
-        cls_p = ctypes_ptr(heads.data_ptr() + offs[1] * esz)
-        dir_p = ctypes_ptr(heads.data_ptr() + offs[2] * esz) if s.use_direction_classifier else None
-        bs = self.fH * self.fW * S
-        self._launch_decode(box_p, cls_p, dir_p, bs, bs, bs, 1, S, st)               # packed NHWC head records
-        self._launch_nms(st)
-
-    def _launch_decode(self, box_p, cls_p, dir_p, box_bs, cls_bs, dir_bs, ch_stride, pix_stride, st):
-        """sigmoid + score threshold + box decode over all anchors -> candidate lists (per frame, or per (class, frame))"""
-        L, lib, s = self._L, self.lib, self.spec
-        if self.mc:
+        if self.segments is not None:
+            # several head maps -> one candidate list per frame (global anchor ids; the single-class NMS branch)
+            segs = [dict(zip(_HEAD_VIEW, v), a_loc=g["a_loc"], H=g["H"], W=g["W"], anchor_base=g["base"])
+                    for v, g in zip(heads, self.segments)]
+            L.check(lib.b2s_decode_filter_segments(
+                L.head_segments(segs), len(segs), L.ptr(self.anchors),
+                L.ptr(self.anchors_mask) if self.use_mask else None, self.A, self.B, self.code, s.num_class,
+                s.num_direction_bins, self.score_thresh, L.ptr(self.cand_box), L.ptr(self.cand_score),
+                L.ptr(self.cand_label), L.ptr(self.cand_dir), L.ptr(self.cand_anchor), L.ptr(self.cand_count),
+                self.cand_cap, L.ptr(self.status), st), "b2s_decode_filter_segments")
+        elif self.mc:
             if self.use_mask:
-                raise RuntimeError("anchors_mask with the per-class NMS branch is ill-defined upstream (masking shifts the "
-                                   "anchors_range indices, voxelnet.py:432-439,492-501)")
+                raise RuntimeError("anchors_mask with the per-class NMS branch is ill-defined upstream (masking shifts "
+                                   "the anchors_range indices, voxelnet.py:432-439,492-501)")
             L.check(lib.b2s_decode_filter_multiclass(
-                box_p, cls_p, dir_p, box_bs, cls_bs, dir_bs, ch_stride, pix_stride, L.ptr(self.anchors), self.B,
-                self.a_loc, self.fH, self.fW, self.code, s.num_class, s.num_direction_bins, self.mc_lo, self.mc_hi,
-                self.mc_thresh, L.ptr(self.cand_box), L.ptr(self.cand_score), L.ptr(self.cand_label),
-                L.ptr(self.cand_dir), L.ptr(self.cand_anchor), L.ptr(self.cand_count), self.cand_cap,
-                L.ptr(self.status), st), "b2s_decode_filter_multiclass")
-            return
-        L.check(lib.b2s_decode_filter_strided(
-            box_p, cls_p, dir_p, box_bs, cls_bs, dir_bs, ch_stride, pix_stride, L.ptr(self.anchors),
-            L.ptr(self.anchors_mask) if self.use_mask else None, self.B, self.a_loc, self.fH, self.fW,
-            self.code, s.num_class, s.num_direction_bins, self.score_thresh, L.ptr(self.cand_box),
-            L.ptr(self.cand_score), L.ptr(self.cand_label), L.ptr(self.cand_dir), L.ptr(self.cand_anchor),
-            L.ptr(self.cand_count), self.cand_cap, L.ptr(self.status), st), "b2s_decode_filter_strided")
-
-    def _launch_decode_segments(self, segs, st):
-        """several head maps -> one candidate list per frame (global anchor ids; the single-class NMS branch)."""
-        L, lib, s = self._L, self.lib, self.spec
-        L.check(lib.b2s_decode_filter_segments(
-            L.head_segments(segs), len(segs), L.ptr(self.anchors), L.ptr(self.anchors_mask) if self.use_mask else None,
-            self.A, self.B, self.code, s.num_class, s.num_direction_bins, self.score_thresh, L.ptr(self.cand_box),
-            L.ptr(self.cand_score), L.ptr(self.cand_label), L.ptr(self.cand_dir), L.ptr(self.cand_anchor),
-            L.ptr(self.cand_count), self.cand_cap, L.ptr(self.status), st), "b2s_decode_filter_segments")
+                *heads[0], L.ptr(self.anchors), self.B, self.a_loc, self.fH, self.fW, self.code, s.num_class,
+                s.num_direction_bins, self.mc_lo, self.mc_hi, self.mc_thresh, L.ptr(self.cand_box),
+                L.ptr(self.cand_score), L.ptr(self.cand_label), L.ptr(self.cand_dir), L.ptr(self.cand_anchor),
+                L.ptr(self.cand_count), self.cand_cap, L.ptr(self.status), st), "b2s_decode_filter_multiclass")
+        else:
+            L.check(lib.b2s_decode_filter_strided(
+                *heads[0], L.ptr(self.anchors), L.ptr(self.anchors_mask) if self.use_mask else None, self.B,
+                self.a_loc, self.fH, self.fW, self.code, s.num_class, s.num_direction_bins, self.score_thresh,
+                L.ptr(self.cand_box), L.ptr(self.cand_score), L.ptr(self.cand_label), L.ptr(self.cand_dir),
+                L.ptr(self.cand_anchor), L.ptr(self.cand_count), self.cand_cap, L.ptr(self.status), st),
+                "b2s_decode_filter_strided")
+        self._launch_nms(st)
 
     def _launch_nms(self, st):
         L, lib, s = self._L, self.lib, self.spec
@@ -1007,7 +977,7 @@ class InferenceEngine:
         if self._mask_src == "area":
             n += 4                               # b2s_anchor_area_mask: scatter, scan_rows, scan_cols, lookup
         if self.is_pillars:
-            n += 1                               # b2s_pfn / b2s_pfn_ex
+            n += 1                               # b2s_pfn_ex
         for lyr in self.layers:
             if lyr["build_rb"]:
                 # subm_nbr / subm_ranked | mark, summary_scan, scan_sums, compact_words, nz_scan, scan_sums, emit,
@@ -1342,9 +1312,14 @@ class InferenceEngine:
         if getattr(self, "in_status", None) is not None:
             if int(self.in_status.item()):
                 raise RuntimeError("b2second engine: cropped clouds exceed the point buffer (max_points)")
-        if st & ~1:   # bit 1 (voxel overflow) is the reference's own drop-extra-voxels behaviour
-            raise RuntimeError("b2second engine: " + self._L.status_message(st))
+        self._raise_on_status(st)
         return st
+
+    def _raise_on_status(self, word):
+        """raise on a status word with a bit other than voxel overflow (bit 1: the reference's own drop-extra-voxels
+        behaviour)"""
+        if word & ~1:
+            raise RuntimeError("b2second engine: " + self._L.status_message(word))
 
     def detections(self, metadata=None, output="host"):
         """sync and convert to the reference's list-of-dicts (voxelnet.py:616-645).
@@ -1374,9 +1349,7 @@ class InferenceEngine:
         """the list of dicts from a read-back that has landed; raises on a status bit other than voxel overflow"""
         code, B = self.code, self.B
         meta = metadata if metadata is not None and len(metadata) > 0 else [None] * B
-        st = int(status_host[0])
-        if st & ~1:   # bit 1 (voxel overflow) is the reference's own drop-extra-voxels behaviour
-            raise RuntimeError("b2second engine: " + self._L.status_message(st))
+        self._raise_on_status(int(status_host[0]))
         cnt = rec_host[:, -1].round().to(torch.int64).tolist()
         out = []
         if output == "device":
