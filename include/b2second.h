@@ -267,6 +267,15 @@ int b2s_sparse_conv_tc_plan(const b2s_half *feat_hi, const b2s_half *feat_lo, in
                             int cap_out, const int *perm, const unsigned *tile_mask, const float *scale,
                             const float *shift, int relu, void *out_hi, b2s_half *out_lo, int out_stride, int cout,
                             unsigned *status_dev, void *stream);
+/* Half-precision mode (the `products` argument of the *_ex entry points below): products = 3 is the 3xF16 form of the
+ * entry point without it (hi/lo planes, three wgmma products per K step); products = 1 is the f16 mode: every operand
+ * is ONE fp16 plane (hi = fp16 round-to-nearest, saturating), every lo pointer must be NULL, and each K step is one
+ * f16 wgmma with fp32 accumulation.  b2s_sparse_conv_tc_plan_ex with products = 1 writes one fp16 plane in out_hi. */
+int b2s_sparse_conv_tc_plan_ex(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in, int cin,
+                               const b2s_half *w_hi, const b2s_half *w_lo, const int *nbr, int K, const int *num_out_dev,
+                               int cap_out, const int *perm, const unsigned *tile_mask, const float *scale,
+                               const float *shift, int relu, void *out_hi, b2s_half *out_lo, int out_stride, int cout,
+                               int products, unsigned *status_dev, void *stream);
 
 /* fp32 rows <-> fp16 hi/lo planes (hi = fp16 round-to-nearest, lo = fp16-rounded remainder; saturating).
  * split: x [rows, row_floats] -> out_channels halves per row and plane (>= row_floats, multiple of 8, zero padded), rows
@@ -277,6 +286,9 @@ int b2s_split_f16(const float *x, b2s_half *hi, b2s_half *lo, const int *num_row
                   int out_channels, int out_stride, void *stream);
 int b2s_merge_f16(const b2s_half *hi, const b2s_half *lo, float *x, const int *num_rows_dev, int cap_rows,
                   int row_floats, int in_stride, void *stream);
+/* b2s_split_f16 with products 3 (the same) or 1 (the f16 mode: lo NULL, only hi written) */
+int b2s_split_f16_ex(const float *x, b2s_half *hi, b2s_half *lo, const int *num_rows_dev, int cap_rows, int row_floats,
+                     int out_channels, int out_stride, int products, void *stream);
 /* b2s_split_f16 of x * 2^e with 2^e chosen on the device from max|x| over the live rows (the b2second.tc.pow2_scale
  * rule: max|x| over the finite elements, max|x| * 2^e in (2^12, 2^13], e clamped to [-126, 126]; 2^e = 1 when no
  * finite element is non-zero) -- for gradients, which are often far below the fp16 normal range.  Unlike b2s_split_f16
@@ -346,6 +358,10 @@ int b2s_to_bev_tc(const float *feat, const b2s_half *feat_hi, const b2s_half *fe
 int b2s_to_bev_tc_ex(const float *feat, const b2s_half *feat_hi, const b2s_half *feat_lo, int feat_stride,
                      const int *coors, const int *num_rows_dev, int cap_rows, int C, int batch, int D, int H, int W,
                      b2s_half *out_hi, b2s_half *out_lo, uint8_t *occupancy, void *stream);
+/* b2s_to_bev_tc_ex with products 3 (the same) or 1 (the f16 mode: feat_lo and out_lo NULL, one fp16 plane) */
+int b2s_to_bev_tc_ex2(const float *feat, const b2s_half *feat_hi, const b2s_half *feat_lo, int feat_stride,
+                      const int *coors, const int *num_rows_dev, int cap_rows, int C, int batch, int D, int H, int W,
+                      b2s_half *out_hi, b2s_half *out_lo, uint8_t *occupancy, int products, void *stream);
 
 /* ---- dense RPN convolution on the tensor pipe (second/pytorch/models/rpn.py:467-497 blocks, :264-299 deblocks,
  *      :386-391 heads): 3x3 stride-1 pad-1 (taps=9) or 1x1 (taps=1) conv + per-channel scale/shift (+ReLU).
@@ -401,6 +417,16 @@ int b2s_conv2d_tc_ex2(const b2s_half *in_hi, const b2s_half *in_lo, int batch, i
                       int off_w, const int *work_list, const int *work_count_dev, const int *bg_list,
                       const int *bg_count_dev, const b2s_half *bg_hi, const b2s_half *bg_lo, int bg_margin,
                       int list_rows, unsigned *status_dev, void *stream);
+/* b2s_conv2d_tc_ex2 with products 3 (the same; out_fp32 must be 0, out_lo == NULL selects the fp32 output) or 1 (the
+ * f16 mode: in_lo, w_lo, out_lo and bg_lo NULL; the output is one fp16 plane in out_hi, or with out_fp32 = 1 the fp32
+ * result, as for the packed heads) */
+int b2s_conv2d_tc_ex3(const b2s_half *in_hi, const b2s_half *in_lo, int batch, int Hin, int Win, int Cin,
+                      const b2s_half *w_hi, const b2s_half *w_lo, int kh, int kw, int stride, int pad, int Cout,
+                      int n_pad, const float *scale, const float *shift, int relu, int Hg, int Wg, void *out_hi,
+                      b2s_half *out_lo, int Hout, int Wout, int out_padded, int out_stride, int out_mul, int off_h,
+                      int off_w, const int *work_list, const int *work_count_dev, const int *bg_list,
+                      const int *bg_count_dev, const b2s_half *bg_hi, const b2s_half *bg_lo, int bg_margin,
+                      int list_rows, int products, int out_fp32, unsigned *status_dev, void *stream);
 
 /* ---- background tiles of the dense RPN ---------------------------------------------------------------
  * The output of layer l of a chain of 3x3 stride-1 pad-1 layers at pixel p depends on the BEV only inside the
@@ -460,6 +486,14 @@ int b2s_rpn_tail_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int B, int 
                        const b2s_half *w2_lo, int cout2, int n_pad2, const float *scale2, const float *shift2,
                        float *out, int out_stride, const int *work_list, const int *work_count, const int *bg_list,
                        const int *bg_count, const float *field, int margin, unsigned *status_dev, void *stream);
+/* b2s_rpn_tail_tc_ex with products 3 (the same) or 1 (the f16 mode: in_lo, w1_lo and w2_lo NULL; y is rounded to one
+ * fp16 plane before the heads) */
+int b2s_rpn_tail_tc_ex2(const b2s_half *in_hi, const b2s_half *in_lo, int B, int H, int W, int Cin, const b2s_half *w1_hi,
+                        const b2s_half *w1_lo, int Cmid, const float *scale1, const float *shift1, const b2s_half *w2_hi,
+                        const b2s_half *w2_lo, int cout2, int n_pad2, const float *scale2, const float *shift2,
+                        float *out, int out_stride, const int *work_list, const int *work_count, const int *bg_list,
+                        const int *bg_count, const float *field, int margin, int products, unsigned *status_dev,
+                        void *stream);
 
 /* ---- PointPillars feature net (single PFNLayer: Linear(F+5 -> Cout, no bias) + BN + ReLU + max) -- */
 int b2s_pfn(const float *points, int num_feat, const int *point_slots, const int *num_points_per_voxel,
@@ -520,6 +554,9 @@ int b2s_pfn_train_backward(const float *voxels, int num_rows, int max_points, in
  * zero padding torch applies at the crop edge, not the neighbouring pixels of src.  C % 8 == 0, 16-byte aligned planes. */
 int b2s_crop_nhwc(const b2s_half *src_hi, const b2s_half *src_lo, int batch, int H, int W, int C, int crop,
                   b2s_half *dst_hi, b2s_half *dst_lo, void *stream);
+/* b2s_crop_nhwc with products 3 (the same) or 1 (the f16 mode: src_lo and dst_lo NULL) */
+int b2s_crop_nhwc_ex(const b2s_half *src_hi, const b2s_half *src_lo, int batch, int H, int W, int C, int crop,
+                     b2s_half *dst_hi, b2s_half *dst_lo, int products, void *stream);
 
 /* ---- anchor-area mask (second/data/preprocess.py:345-357) ---------------------------------------- */
 /* mask_out [batch, num_anchors] uint8 = 1 where the anchor's BEV box holds more than `threshold` voxels.

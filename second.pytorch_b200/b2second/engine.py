@@ -19,6 +19,11 @@ buffers, so the whole frame batch is ONE CUDA graph:
       (rpn_impl="cudnn" keeps the torch modules as a cross-check: fp32, TF32 off)
   b2s_decode_filter_strided + b2s_nms (+ direction/range epilogue)   voxelnet.py:377-645
 
+precision="f16" is the half-precision mode: every tensor-pipe operand (sparse rows, BEV and RPN planes, weights) is ONE
+fp16 plane instead of a hi/lo pair, and each MMA is one f16 wgmma with fp32 accumulation (the ``*_ex`` entry points
+with products = 1).  Everything off the tensor pipe (voxelizer, VFE / PFN, the scatter's index work, decode, the anchor
+mask, NMS) is the fp32 code of the default mode, and the head outputs and detections stay float32.
+
 VoxelNetNuscenesMultiHead (net_multi_head.py:121-176) runs the same way with two head "segments": the large head's
 packed 1x1 convs on the concatenated map, and b2s_crop_nhwc of stage 0 -> three 3x3 convs -> the small head's packed
 1x1 convs; b2s_decode_filter_segments reads both records into ONE candidate list per frame, with global anchor ids.
@@ -30,7 +35,9 @@ Output per batch: ``det [B, post_max, code+2]`` (box, score, label) + ``det_coun
 record the multi-GPU path all-gathers (SURVEY.md §8e); ``det`` and ``det_count`` live in ONE buffer
 (``det_record [B, post_max*(code+2) + 1]``) so the all-gather needs no packing step.
 """
+import contextlib
 import ctypes
+import gc
 
 import numpy as np
 import torch
@@ -54,11 +61,43 @@ _HEAD_VIEW = ("box", "cls", "dir", "box_batch_stride", "cls_batch_stride", "dir_
 
 
 def _field_margin(hi, lo):
-    """the smallest m such that a layer's empty-frame response (halo-padded hi/lo planes [H+2, W+2, C]) holds, bit for
-    bit, its value at pixel (m, m) wherever it is at least m pixels from every border; -1 when no such interior exists.
-    The conv kernel stores that value into the background strips there instead of copying the field."""
+    """the smallest m such that a layer's empty-frame response (halo-padded hi/lo planes [H+2, W+2, C]; lo None in the
+    f16 mode) holds, bit for bit, its value at pixel (m, m) wherever it is at least m pixels from every border; -1 when
+    no such interior exists.  The conv kernel stores that value into the background strips there instead of copying
+    the field."""
     H, W = hi.shape[0] - 2, hi.shape[1] - 2
-    return _bits_margin(torch.cat([hi[1:H + 1, 1:W + 1], lo[1:H + 1, 1:W + 1]], -1).view(torch.int16))
+    planes = [hi] if lo is None else [hi, lo]
+    return _bits_margin(torch.cat([t[1:H + 1, 1:W + 1] for t in planes], -1).view(torch.int16))
+
+
+@contextlib.contextmanager
+def no_cyclic_gc():
+    """the block runs with Python's cyclic garbage collector off (restored after, also on an exception).  Used around a
+    CUDA graph capture: torch does not collect before capturing, and a CUDAGraph the collector frees inside the capture
+    (one of an engine dropped earlier and kept alive by a reference cycle) is destroyed mid-capture, which invalidates
+    the capture."""
+    on = gc.isenabled()
+    gc.disable()
+    try:
+        yield
+    finally:
+        if on:
+            gc.enable()
+
+
+# arithmetic modes of the tensor-pipe kernels: precision -> wgmma products per K step (the kernels' `products`)
+PRECISIONS = {"fp32": 3, "f16": 1}
+
+
+def check_precision(precision, sparse_impl="tc", rpn_impl="auto"):
+    """-> the kernels' product count for ``precision``; raises ValueError for an unknown precision and for the f16 mode
+    with the fp32 reference paths (sparse_impl="fma", rpn_impl="cudnn")"""
+    if precision not in PRECISIONS:
+        raise ValueError("precision must be one of %s, got %r" % (sorted(PRECISIONS), precision))
+    if precision == "f16" and (sparse_impl == "fma" or rpn_impl == "cudnn"):
+        raise ValueError("precision='f16' runs on the tensor pipe only: sparse_impl='fma' and rpn_impl='cudnn' are the "
+                         "fp32 reference paths")
+    return PRECISIONS[precision]
 
 
 def _record_margin(rec, n):
@@ -112,12 +151,15 @@ class _Streamed:
 class InferenceEngine:
     def __init__(self, net, batch_size=1, max_points=None, max_voxels=None, row_cap_factor=2.0,
                  cand_cap=None, use_cuda_graph=True, rpn_impl="auto", sparse_impl="tc", device=None,
-                 anchor_area_threshold=None):
+                 anchor_area_threshold=None, precision="fp32"):
         import spconv as sp                      # the CUDA drop-in: fails loudly if the library is missing
         assert not getattr(sp, "__oracle__", False), "the engine is the product path; it never runs on the oracle"
         self.sp = sp
         self.lib = sp._lib.load()
         self._L = sp._lib
+        # "fp32": 3xF16 (fp32-grade) tensor-pipe products; "f16": one fp16 plane per operand, one product
+        self.products = check_precision(precision, sparse_impl, rpn_impl)
+        self.precision = precision
         self.spec = s = net if isinstance(net, _spec.NetSpec) else _spec.spec_from_module(net, max_voxels)
         if max_voxels:
             s.max_voxels = int(max_voxels)
@@ -141,6 +183,9 @@ class InferenceEngine:
         if rpn_impl == "auto":
             rpn_impl = "tc" if _tc.supported(s.rpn, s.heads) else "cudnn"
         assert rpn_impl in ("tc", "cudnn")
+        if rpn_impl == "cudnn" and self.products == 1:
+            raise ValueError("precision='f16': this RPN has a layer b2s_conv2d_tc_ex3 does not cover, and rpn_impl="
+                             "'cudnn' is the fp32 reference path")
         if rpn_impl == "tc" and not _tc.supported(s.rpn, s.heads):
             raise ValueError("rpn_impl='tc': this RPN has a layer b2s_conv2d_tc_ex2 does not cover (channels % 64, "
                              "kernel > 4)")
@@ -195,7 +240,7 @@ class InferenceEngine:
             if lyr["tc"]:
                 wp = _tc.pack_sparse_weights(lyr["w"])
                 ws = _tc.pow2_scale(wp)
-                hi, lo = _tc.split_f16(wp, ws)
+                hi, lo = _tc.weight_planes(wp, ws, self.products)
                 base = lyr["scale"] if lyr["scale"] is not None else torch.ones(lyr["cout"], device=self.dev)
                 self._fill(lyr, "w_hi", hi)
                 self._fill(lyr, "w_lo", lo)
@@ -204,7 +249,9 @@ class InferenceEngine:
     def _rpn_plan(self):
         D, H, W = self.final_level.shape
         rpn, heads = self.spec.rpn, getattr(self.spec, "heads", None)
-        return _tc.plan_rpn(rpn, H, W) if heads is None else _tc.plan_rpn_multihead(rpn, dict(heads), H, W)
+        if heads is None:
+            return _tc.plan_rpn(rpn, H, W, products=self.products)
+        return _tc.plan_rpn_multihead(rpn, dict(heads), H, W, products=self.products)
 
     def _fill_tc_rpn(self):
         """every tensor-core RPN op's weight planes, epilogue scale and shift -- blocks, deblock sub-grids, packed head
@@ -229,7 +276,8 @@ class InferenceEngine:
         else:
             for old, new in zip(self.bg_field, fields):
                 for o, n in zip(old, new):
-                    o.copy_(n)
+                    if o is not None:
+                        o.copy_(n)
             self.tail_field.copy_(records)
         margins = ([_field_margin(hi, lo) for hi, lo in self.bg_field],
                    _record_margin(self.tail_field, self.tc_plan[-1]["cout"]))
@@ -276,7 +324,11 @@ class InferenceEngine:
         return lv
 
     def _hilo_rows(self, cap, c):
-        """interleaved fp16 rows [cap][hi c | lo c] -> (buffer, hi view, lo view, row stride in halves)."""
+        """interleaved fp16 rows [cap][hi c | lo c] -> (buffer, hi view, lo view, row stride in halves); in the f16 mode
+        rows [cap][c] of one plane, lo None."""
+        if self.products == 1:
+            buf = torch.zeros(cap, c, dtype=torch.float16, device=self.dev)
+            return buf, buf, None, c
         buf = torch.zeros(cap, 2, c, dtype=torch.float16, device=self.dev)
         return buf, buf[:, 0], buf[:, 1], 2 * c
 
@@ -416,8 +468,31 @@ class InferenceEngine:
         # pre-voxelised entry (the reference's own example dict): the caller's voxels land here
         self.in_voxels = None
 
+    # tensor-pipe entry points: the 3xF16 call of the default mode -> (its products-taking form, how many trailing
+    # arguments -- status, stream -- follow the inserted products arguments)
+    _F16_FORMS = {"b2s_conv2d_tc_ex2": ("b2s_conv2d_tc_ex3", 2),
+                  "b2s_sparse_conv_tc_plan": ("b2s_sparse_conv_tc_plan_ex", 2),
+                  "b2s_rpn_tail_tc_ex": ("b2s_rpn_tail_tc_ex2", 2), "b2s_to_bev_tc_ex": ("b2s_to_bev_tc_ex2", 1),
+                  "b2s_crop_nhwc": ("b2s_crop_nhwc_ex", 1), "b2s_split_f16": ("b2s_split_f16_ex", 1)}
+
+    def _tc_call(self, name, *args, f16=(), what=""):
+        """one tensor-pipe library call: ``name`` with ``args`` in the default mode, exactly as it has always been
+        called; in the f16 mode its products-taking form with products = 1 and then ``f16`` inserted before the
+        trailing status / stream arguments.  ``what`` follows the entry point's name in an error message."""
+        if self.products == 3:
+            return self._L.check(getattr(self.lib, name)(*args), name + what)
+        name1, tail = self._F16_FORMS[name]
+        args = args[:-tail] + (1,) + tuple(f16) + args[-tail:]
+        return self._L.check(getattr(self.lib, name1)(*args), name1 + what)
+
+    @property
+    def n_planes(self):
+        """fp16 planes per tensor-pipe operand: 2 (hi, lo) for precision "fp32", 1 for "f16"."""
+        return 2 if self.products == 3 else 1
+
     def _alloc_tc_rpn(self):
-        """buffers of the tensor-core RPN: NHWC halo-padded fp16 hi/lo planes (halo zero-filled once, never written)."""
+        """buffers of the tensor-core RPN: NHWC halo-padded fp16 hi/lo planes (halo zero-filled once, never written);
+        (hi, None) in the f16 mode."""
         dev, B = self.dev, self.B
         D, H, W = self.final_level.shape
         C = self.feat_final_c * D
@@ -433,8 +508,8 @@ class InferenceEngine:
         assert plan["in_channels"] == C, "BEV channels %d != RPN input %d" % (C, plan["in_channels"])
 
         def plane(h, w, c):
-            return (torch.zeros(B, h + 2, w + 2, c, dtype=torch.float16, device=dev),
-                    torch.zeros(B, h + 2, w + 2, c, dtype=torch.float16, device=dev))
+            return tuple(torch.zeros(B, h + 2, w + 2, c, dtype=torch.float16, device=dev) if i < self.n_planes else None
+                         for i in range(2))
         # the BEV planes are zero except at the pixels flagged in bev_occ (b2s_to_bev_tc_ex keeps that so from step
         # to step); nothing else writes them
         self.tc_bev = plane(H, W, C)
@@ -494,47 +569,47 @@ class InferenceEngine:
             if name not in planes:
                 h, w, c = shapes[name]
                 planes[name] = tuple(torch.zeros(1, h + 2, w + 2, c, dtype=torch.float16, device=self.dev)
-                                     for _ in range(2))
+                                     if i < self.n_planes else None for i in range(2))
             return planes[name]
         fields = []
         for oi in self.bg_idx:
             op = self.tc_plan[oi]
             src, dst = plane(op["src"]), plane(op["dst"])
             self._launch_conv(op, src, dst, 1, None, None, -1, st)
-            fields.append((dst[0][0, :, :, :op["cout"]].clone().contiguous(),
-                           dst[1][0, :, :, :op["cout"]].clone().contiguous()))
+            fields.append(tuple(t[0, :, :, :op["cout"]].clone().contiguous() if t is not None else None for t in dst))
         d = self.tc_plan[-2]
         records = torch.zeros(1, d["Hin"], d["Win"], self.tc_head_stride, dtype=torch.float32, device=self.dev)
         self._launch_fused_tail(plane(d["src"]), records, 1, None, None, None, None, None, -1, st)
         return fields, records[0]
 
     def _launch_conv(self, op, src, dst, batch, lists, field, margin, st):
-        """one b2s_conv2d_tc_ex2 launch of the tc_plan op ``op``: hi/lo planes ``src`` -> planes ``dst`` from the op's
-        channel offset on.  ``lists``: (strip work list, its count, background strip list, its count), or None for a
-        dense launch; ``field``: the (hi, lo) empty-frame response the background strips are stored from, or None."""
+        """one b2s_conv2d_tc_ex2 (f16 mode: _ex3) launch of the tc_plan op ``op``: hi/lo planes ``src`` -> planes
+        ``dst`` from the op's channel offset on (fp32 records for a "planes": 1 op; lo planes None in the f16 mode).
+        ``lists``: (strip work list, its count, background strip list, its count), or None for a dense launch;
+        ``field``: the (hi, lo) empty-frame response the background strips are stored from, or None."""
         L = self._L
         cdst = dst[0].shape[-1]                                   # channels per pixel of the destination map
         esz = dst[0].element_size()
         o_hi = ctypes_ptr(dst[0].data_ptr() + esz * op["dst_coff"])
-        o_lo = ctypes_ptr(dst[1].data_ptr() + esz * op["dst_coff"]) if op["planes"] == 2 else None
+        o_lo = None if op["planes"] == 1 or dst[1] is None else ctypes_ptr(dst[1].data_ptr() + esz * op["dst_coff"])
         work, work_n, bgl, bgn = lists or (None,) * 4
         bhi, blo = (L.ptr(field[0]), L.ptr(field[1])) if field is not None else (None, None)
-        L.check(self.lib.b2s_conv2d_tc_ex2(
-            L.ptr(src[0]), L.ptr(src[1]), batch, op["Hin"], op["Win"], op["cin"], L.ptr(op["w_hi"]),
-            L.ptr(op["w_lo"]), op["kh"], op["kw"], op["stride"], op["pad"], op["cout"], op["n_pad"],
+        self._tc_call(
+            "b2s_conv2d_tc_ex2", L.ptr(src[0]), L.ptr(src[1]), batch, op["Hin"], op["Win"], op["cin"],
+            L.ptr(op["w_hi"]), L.ptr(op["w_lo"]), op["kh"], op["kw"], op["stride"], op["pad"], op["cout"], op["n_pad"],
             L.ptr(op["scale"]), L.ptr(op["shift"]), 1 if op["relu"] else 0, op["Hg"], op["Wg"], o_hi, o_lo,
             op["Hout"], op["Wout"], 1 if op["padded"] else 0, cdst, op["out_mul"], op["off_h"], op["off_w"],
-            work, work_n, bgl, bgn, bhi, blo, margin, BG_ROWS, L.ptr(self.status), st),
-            "b2s_conv2d_tc_ex2(%s)" % op["kind"])
+            work, work_n, bgl, bgn, bhi, blo, margin, BG_ROWS, L.ptr(self.status), st,
+            f16=(1 if op["planes"] == 1 else 0,), what="(%s)" % op["kind"])    # f16: out_fp32 for the head records
 
     def _launch_fused_tail(self, src, out, batch, work, work_n, bgl, bgn, field, margin, st):
         L, lib = self._L, self.lib
         d, h = self.tc_plan[-2], self.tc_plan[-1]
-        L.check(lib.b2s_rpn_tail_tc_ex(
-            L.ptr(src[0]), L.ptr(src[1]), batch, d["Hin"], d["Win"], d["cin"], L.ptr(d["w_hi"]), L.ptr(d["w_lo"]),
-            d["cout"], L.ptr(d["scale"]), L.ptr(d["shift"]), L.ptr(h["w_hi"]), L.ptr(h["w_lo"]), h["cout"], h["n_pad"],
-            L.ptr(h["scale"]), L.ptr(h["shift"]), L.ptr(out), self.tc_head_stride, work, work_n, bgl, bgn,
-            L.ptr(field), margin, L.ptr(self.status), st), "b2s_rpn_tail_tc_ex")
+        self._tc_call(
+            "b2s_rpn_tail_tc_ex", L.ptr(src[0]), L.ptr(src[1]), batch, d["Hin"], d["Win"], d["cin"], L.ptr(d["w_hi"]),
+            L.ptr(d["w_lo"]), d["cout"], L.ptr(d["scale"]), L.ptr(d["shift"]), L.ptr(h["w_hi"]), L.ptr(h["w_lo"]),
+            h["cout"], h["n_pad"], L.ptr(h["scale"]), L.ptr(h["shift"]), L.ptr(out), self.tc_head_stride, work, work_n,
+            bgl, bgn, L.ptr(field), margin, L.ptr(self.status), st)
 
     def _feature_hw(self):
         if self.rpn_impl == "tc":
@@ -773,16 +848,15 @@ class InferenceEngine:
                 if lyr["tc"]:
                     if "in_split" in lyr:
                         _, hi, lo, stride = lyr["in_split"]
-                        L.check(lib.b2s_split_f16(L.ptr(feats), L.ptr(hi), L.ptr(lo), L.ptr(lin.n_dev), lin.cap,
-                                                  lyr["cin"], lyr["cin_tc"], stride, st), "b2s_split_f16")
+                        self._tc_call("b2s_split_f16", L.ptr(feats), L.ptr(hi), L.ptr(lo), L.ptr(lin.n_dev), lin.cap,
+                                      lyr["cin"], lyr["cin_tc"], stride, st)
                         hilo = (hi, lo, stride)
-                    L.check(lib.b2s_sparse_conv_tc_plan(
-                        L.ptr(hilo[0]), L.ptr(hilo[1]), hilo[2], lin.cap, lyr["cin_tc"], L.ptr(lyr["w_hi"]),
-                        L.ptr(lyr["w_lo"]), L.ptr(lyr["rb"]["nbr"]), lyr["K"], L.ptr(lout.n_dev), lout.cap,
-                        L.ptr(lyr["rb"].get("perm")), L.ptr(lyr["rb"].get("tile_mask")),
+                    self._tc_call(
+                        "b2s_sparse_conv_tc_plan", L.ptr(hilo[0]), L.ptr(hilo[1]), hilo[2], lin.cap, lyr["cin_tc"],
+                        L.ptr(lyr["w_hi"]), L.ptr(lyr["w_lo"]), L.ptr(lyr["rb"]["nbr"]), lyr["K"], L.ptr(lout.n_dev),
+                        lout.cap, L.ptr(lyr["rb"].get("perm")), L.ptr(lyr["rb"].get("tile_mask")),
                         L.ptr(lyr["scale_tc"]), L.ptr(lyr["shift"]), 1 if lyr["relu"] else 0, L.ptr(lyr["out_hi"]),
-                        L.ptr(lyr["out_lo"]), lyr["out_stride"], lyr["cout"], L.ptr(self.status), st),
-                        "b2s_sparse_conv_tc_plan")
+                        L.ptr(lyr["out_lo"]), lyr["out_stride"], lyr["cout"], L.ptr(self.status), st)
                     feats, hilo = None, (lyr["out_hi"], lyr["out_lo"], lyr["out_stride"])
                 else:
                     L.check(lib.b2s_sparse_conv(L.ptr(feats), lyr["cin"], L.ptr(lyr["w"]), L.ptr(lyr["rb"]["nbr"]),
@@ -826,9 +900,9 @@ class InferenceEngine:
         D, H, W = fl.shape
         self._mark("to_bev")
         feat, f_hi, f_lo, f_stride = (feats, None, None, 0) if hilo is None else (None,) + hilo
-        L.check(lib.b2s_to_bev_tc_ex(L.ptr(feat), L.ptr(f_hi), L.ptr(f_lo), f_stride, L.ptr(fl.coors), L.ptr(fl.n_dev),
-                                     fl.cap, self.feat_final_c, self.B, D, H, W, L.ptr(self.tc_bev[0]),
-                                     L.ptr(self.tc_bev[1]), L.ptr(self.bev_occ), st), "b2s_to_bev_tc_ex")
+        self._tc_call("b2s_to_bev_tc_ex", L.ptr(feat), L.ptr(f_hi), L.ptr(f_lo), f_stride, L.ptr(fl.coors),
+                      L.ptr(fl.n_dev), fl.cap, self.feat_final_c, self.B, D, H, W, L.ptr(self.tc_bev[0]),
+                      L.ptr(self.tc_bev[1]), L.ptr(self.bev_occ), st)
         self._mark("rpn")
         nl = len(self.bg_idx)
         if nl:
@@ -846,8 +920,8 @@ class InferenceEngine:
                 marked_tail = True
             src, dst = self.tc_bufs[op["src"]], self.tc_bufs[op["dst"]]
             if op["kind"] == "crop":                                  # small head input: stage 0 inside a zero halo
-                L.check(lib.b2s_crop_nhwc(L.ptr(src[0]), L.ptr(src[1]), self.B, op["Hin"], op["Win"], op["cin"],
-                                          op["crop"], L.ptr(dst[0]), L.ptr(dst[1]), st), "b2s_crop_nhwc")
+                self._tc_call("b2s_crop_nhwc", L.ptr(src[0]), L.ptr(src[1]), self.B, op["Hin"], op["Win"], op["cin"],
+                              op["crop"], L.ptr(dst[0]), L.ptr(dst[1]), st)
                 continue
             lists, field, margin = None, None, -1
             if oi in self.bg_idx:
@@ -1000,6 +1074,34 @@ class InferenceEngine:
             return n + 1 + 1 + 3 * (1 if self.mc_uniform else self.ncls) + 1      # ... + k_concat_classes
         return n + 1 + 1 + 3                     # to_bev, decode_filter(_segments), nms: select_sort + iou_mask + reduce
 
+    def fp16_plane_bytes(self):
+        """bytes of the fp16 operand planes this engine holds -- activations, BEV, weights, background fields -- as
+        {"hi": ..., "lo": ...}; the f16 mode allocates no lo planes, so an fp32-mode engine's "lo" is what it saves"""
+        seen, out = set(), {"hi": 0, "lo": 0}
+
+        def add(t, kind):
+            if isinstance(t, torch.Tensor) and t.dtype == torch.float16:
+                st = t.untyped_storage()
+                key = (st.data_ptr(), t.storage_offset(), tuple(t.shape))
+                if key not in seen:
+                    seen.add(key)
+                    out[kind] += t.numel() * 2
+        for lyr in getattr(self, "layers", []):
+            for split in (lyr.get("in_split"), (None, lyr.get("out_hi"), lyr.get("out_lo"))):
+                if split is not None:
+                    add(split[1], "hi")
+                    add(split[2], "lo")
+            add(lyr.get("w_hi"), "hi")
+            add(lyr.get("w_lo"), "lo")
+        if self.rpn_impl == "tc":
+            for pl in list(self.tc_bufs.values()) + list(getattr(self, "bg_field", [])):
+                add(pl[0], "hi")
+                add(pl[1], "lo")
+            for op in self.tc_plan:
+                add(op.get("w_hi"), "hi")
+                add(op.get("w_lo"), "lo")
+        return out
+
     def sparse_layer_stats(self):
         """sync; per sparse layer: rows in/out, pairs, algorithmic bytes and flops (SURVEY.md §8d formulas)."""
         out = []
@@ -1025,14 +1127,15 @@ class InferenceEngine:
             cin, cout, taps = op["cin"], op["cout"], op["taps"]
             px = self.B * op["Hg"] * op["Wg"]
             px_in = self.B * op["Hin"] * op["Win"]
-            out_b = 2 * 2 * px * cout if op["planes"] == 2 else 4 * px * cout
+            npl = self.n_planes
+            out_b = npl * 2 * px * cout if op["planes"] == 2 else 4 * px * cout
             frac = 1.0                        # share of the 8 x BG_ROWS output strips actually computed (the rest: background)
             if getattr(self, "bg_idx", None) and i in self.bg_idx:
                 frac = float(self.bg_counts[self.bg_idx.index(i), 0].item()) / self.bg_tiles
             out.append({"index": i, "kind": op["kind"], "v2": op["v2"], "cin": cin, "cout": cout, "taps": taps,
                         "tiles_computed_frac": frac,
                         "pixels": px, "flops": 2 * px * taps * cin * cout,
-                        "bytes": 2 * 2 * px_in * cin + out_b + 2 * 2 * taps * cin * op["n_pad"],
+                        "bytes": npl * 2 * px_in * cin + out_b + npl * 2 * taps * cin * op["n_pad"],
                         "bytes_fp32_algorithmic": 4 * (px_in * cin + px * cout + taps * cin * cout)})
         return out
 
@@ -1221,7 +1324,7 @@ class InferenceEngine:
                     torch.cuda.current_stream().wait_stream(side)
                     torch.cuda.synchronize()
                     g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g):
+                    with no_cyclic_gc(), torch.cuda.graph(g):
                         self._launch(mode, slot)
                     self._graphs[key] = g
             g.replay()

@@ -59,6 +59,9 @@ class FastPath:
         self.max_points = int(max_points)
         self.use_cuda_graph = use_cuda_graph
         self.engine_kw = engine_kw
+        from .engine import check_precision         # an unknown or refused precision raises here, not at the first call
+        check_precision(engine_kw.get("precision", "fp32"), engine_kw.get("sparse_impl", "tc"),
+                        engine_kw.get("rpn_impl", "auto"))
         self.spec = _spec.spec_from_module(net, max_voxels)      # raises UnsupportedNetwork for foreign layer patterns
         self.engines = {}
         self.stale = False           # the network's weights may have changed since the engines' operands were derived
@@ -212,7 +215,10 @@ class FastPath:
 
 
 def accelerate(net, **kw):
-    """re-bind ``net.forward`` to the fused engine (see module docstring); returns ``net``.
+    """re-bind ``net.forward`` to the fused engine (see module docstring); returns ``net``.  The keywords go to
+    ``FastPath`` and the engines it builds; ``precision="f16"`` selects the half-precision mode (one fp16 plane per
+    tensor-pipe operand, b2second.engine) and is checked here: an unknown precision, or "f16" with sparse_impl="fma" or
+    rpn_impl="cudnn", raises ValueError.
     ``net.b2s_fastpath`` is the FastPath object, ``net.b2s_reference_forward`` the original bound method.
 
     ``net.train`` is wrapped as well: ``train(False)`` / ``eval()`` set the modes exactly as before and then mark the

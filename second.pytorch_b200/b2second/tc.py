@@ -34,6 +34,13 @@ def split_f16(t, scale=1.0):
     return hi.contiguous(), lo.contiguous()
 
 
+def weight_planes(t, scale, products):
+    """the weight operand planes of a tensor-core kernel: (hi, lo) of split_f16 for products = 3 (3xF16), (hi, None)
+    for products = 1 (the f16 mode: one fp16 plane, bit for bit the hi plane of the 3xF16 split)"""
+    hi, lo = split_f16(t, scale)
+    return (hi, lo) if products == 3 else (hi, None)
+
+
 def merge_f16(hi, lo):
     return hi.float() + lo.float()
 
@@ -118,21 +125,22 @@ def _conv_out(n, k, s, pad):
     return (n + 2 * pad - k) // s + 1
 
 
-def plan_rpn(rpn, H, W, dry=False):
+def plan_rpn(rpn, H, W, dry=False, products=3):
     """RPNV2 (second/pytorch/models/rpn.py:469-497 blocks, :264-299 deblocks, :386-420 heads) on an H x W BEV map ->
     {"buffers": {name: (h, w, c)}, "ops": [conv op dicts in execution order], "heads": {...}}.
 
     Every op is one b2s_conv2d_tc_ex launch: conv k x k / stride / pad, or one (a, c) sub-grid of a k = s
     ConvTranspose2d; output channels are cut into slices of <= 128 (the kernel's n_pad) and `torch.cat` of the
-    deblock outputs is a channel offset into the shared "cat" buffer."""
-    bufs, ops, emit, (cur, h, w), _ = _plan_backbone(rpn, H, W, dry)
+    deblock outputs is a channel offset into the shared "cat" buffer.  ``products`` = 3: 3xF16 weight planes (w_hi,
+    w_lo); 1: the f16 mode, w_hi only (w_lo None)."""
+    bufs, ops, emit, (cur, h, w), _ = _plan_backbone(rpn, H, W, dry, products)
     heads = [rpn.conv_box, rpn.conv_cls] + ([rpn.conv_dir_cls] if rpn._use_direction_classifier else [])
     offs, stride_s = _emit_heads(emit, heads, cur, "heads", h, w)
     return {"buffers": bufs, "ops": ops, "in_channels": ops[0]["cin"],
             "heads": {"offsets": offs, "stride": stride_s, "H": h, "W": w}}
 
 
-def plan_rpn_multihead(rpn, heads, H, W, dry=False):
+def plan_rpn_multihead(rpn, heads, H, W, dry=False, products=3):
     """VoxelNetNuscenesMultiHead (second/pytorch/models/net_multi_head.py:121-176) on an H x W BEV map: the RPNNoHead
     backbone up to the concatenated map, then
       large head: its 1x1 box | cls | dir convs packed into one fp32 record per pixel of the concat map ("heads_large");
@@ -141,7 +149,7 @@ def plan_rpn_multihead(rpn, heads, H, W, dry=False):
     ``heads`` = {"large": module, "small": module}.  Records wider than 128 channels are two launches (dst_coff 0 / 128).
     -> {"buffers", "ops", "in_channels", "stage0", "crop", "segments": [{"name", "buffer", "offsets", "stride", "H", "W",
     "a_loc"}, large first]} -- the order of the reference's torch.cat, hence of the anchors."""
-    bufs, ops, emit, (cur, h, w), (s0, h0, w0) = _plan_backbone(rpn, H, W, dry)
+    bufs, ops, emit, (cur, h, w), (s0, h0, w0) = _plan_backbone(rpn, H, W, dry, products)
     segs = []
 
     def packed(m, src, name, hh, ww):
@@ -195,7 +203,7 @@ def _emit_heads(emit, heads, src, dst, h, w):
     return offs, stride_s
 
 
-def _plan_backbone(rpn, H, W, dry):
+def _plan_backbone(rpn, H, W, dry, products=3):
     """blocks + deblocks of an RPN (RPNV2 or RPNNoHead) -> (buffers, ops, emit, (output buffer, h, w),
     (stage-0 buffer, h, w))."""
     bufs, ops = {}, []
@@ -219,7 +227,7 @@ def _plan_backbone(rpn, H, W, dry):
                 # weights pre-scaled by a power of two (exact), undone by the epilogue scale
                 wp = _pad_rows(w_t_co_ci[:, c0:c1].float(), n_pad)
                 ws = pow2_scale(wp)
-                d["w_hi"], d["w_lo"] = split_f16(wp, ws)
+                d["w_hi"], d["w_lo"] = weight_planes(wp, ws, products)
                 d["w_scale"] = ws
                 base = torch.ones(c1 - c0, dtype=torch.float32, device=wp.device) if scale is None \
                     else scale[c0:c1].float()

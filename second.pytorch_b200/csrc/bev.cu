@@ -42,8 +42,10 @@ __global__ void k_to_bev(const float *__restrict__ feat, const int *__restrict__
     }
 }
 
-// tensor-core RPN input: NHWC + one-pixel zero halo, fp16 hi/lo planes (3xF16 split).  The rows come either as fp32
-// (PointPillars: the PFN output) or already split (the last sparse layer's hi/lo planes, row stride feat_stride halves).
+// tensor-core RPN input: NHWC + one-pixel zero halo, fp16 hi/lo planes (3xF16 split; P = 1: the hi plane only, the
+// f16 mode).  The rows come either as fp32 (PointPillars: the PFN output) or already split (the last sparse layer's
+// hi/lo planes, row stride feat_stride halves).
+template <int P>
 __global__ void k_to_bev_tc(const float *__restrict__ feat, const __half *__restrict__ feat_hi,
                             const __half *__restrict__ feat_lo, int feat_stride, const int *__restrict__ coors,
                             const int *__restrict__ n_dev, int cap_rows, int C, int batch, int D, int H, int W,
@@ -64,16 +66,18 @@ __global__ void k_to_bev_tc(const float *__restrict__ feat, const __half *__rest
         if (feat) {
             const uint32_t pk = b2s_tc::split_f16(__ldg(&feat[gid]));
             out_hi[idx] = __ushort_as_half((unsigned short)(pk & 0xFFFFu));
-            out_lo[idx] = __ushort_as_half((unsigned short)(pk >> 16));
+            if constexpr (P == 3) out_lo[idx] = __ushort_as_half((unsigned short)(pk >> 16));
         } else {
             out_hi[idx] = feat_hi[(size_t)row * feat_stride + c];
-            out_lo[idx] = feat_lo[(size_t)row * feat_stride + c];
+            if constexpr (P == 3) out_lo[idx] = feat_lo[(size_t)row * feat_stride + c];
         }
     }
 }
 
 // the pixels the previous step flagged in `occ` back to zero in both planes (CV 16-byte vectors per pixel), and their
-// flags cleared: each warp reads the flags of 32 pixels and zeroes the flagged ones one pixel at a time
+// flags cleared: each warp reads the flags of 32 pixels and zeroes the flagged ones one pixel at a time (P = 1: the hi
+// plane only)
+template <int P>
 __global__ void k_bev_clear(uint8_t *__restrict__ occ, int batch, int H, int W, int CV, uint4 *__restrict__ out_hi,
                             uint4 *__restrict__ out_lo)
 {
@@ -90,7 +94,7 @@ __global__ void k_bev_clear(uint8_t *__restrict__ occ, int batch, int H, int W, 
             const size_t o = ((size_t)(row + row / H * 2 + 1) * (W + 2) + (px % W) + 1) * CV;
             for (int v = lane; v < CV; v += 32) {
                 out_hi[o + v] = make_uint4(0u, 0u, 0u, 0u);
-                out_lo[o + v] = make_uint4(0u, 0u, 0u, 0u);
+                if constexpr (P == 3) out_lo[o + v] = make_uint4(0u, 0u, 0u, 0u);
             }
         }
     }
@@ -156,7 +160,8 @@ k_pfn(const float *__restrict__ points, int F, const int *__restrict__ slots, co
 }
 
 // interior window [c, H-c) x [c, W-c) of a halo-padded map [B, H+2, W+2, C] -> [B, Ho+2, Wo+2, C] whose halo is
-// written as zero; 16-byte vectors (C % 8 == 0)
+// written as zero; 16-byte vectors (C % 8 == 0); P = 1: the hi plane only
+template <int P>
 __global__ void k_crop_nhwc(const uint4 *__restrict__ src_hi, const uint4 *__restrict__ src_lo, int batch, int H, int W,
                             int CV, int c, uint4 *__restrict__ dst_hi, uint4 *__restrict__ dst_lo)
 {
@@ -175,10 +180,10 @@ __global__ void k_crop_nhwc(const uint4 *__restrict__ src_hi, const uint4 *__res
             // dst interior pixel (y-1, x-1) = src pixel (y-1+c, x-1+c) = padded src (y+c, x+c)
             const size_t s = (((size_t)b * (H + 2) + (y + c)) * (W + 2) + (x + c)) * CV + v;
             hi = __ldg(&src_hi[s]);
-            lo = __ldg(&src_lo[s]);
+            if constexpr (P == 3) lo = __ldg(&src_lo[s]);
         }
         dst_hi[gid] = hi;
-        dst_lo[gid] = lo;
+        if constexpr (P == 3) dst_lo[gid] = lo;
     }
 }
 
@@ -229,7 +234,7 @@ extern "C" int b2s_to_bev_tc(const float *feat, const b2s_half *feat_hi, const b
     B2S_CUDA_OK(cudaMemsetAsync(out_lo, 0, sizeof(__half) * total, stream));
     if (occupancy) B2S_CUDA_OK(cudaMemsetAsync(occupancy, 0, (size_t)batch * H * W, stream));
     if (cap_rows > 0) {
-        k_to_bev_tc<<<bounded_grid((long long)cap_rows * C), kThreads, 0, stream>>>(
+        k_to_bev_tc<3><<<bounded_grid((long long)cap_rows * C), kThreads, 0, stream>>>(
             feat, reinterpret_cast<const __half *>(feat_hi), reinterpret_cast<const __half *>(feat_lo), feat_stride, coors,
             num_rows_dev, cap_rows, C, batch, D, H, W, reinterpret_cast<__half *>(out_hi),
             reinterpret_cast<__half *>(out_lo), occupancy);
@@ -238,27 +243,48 @@ extern "C" int b2s_to_bev_tc(const float *feat, const b2s_half *feat_hi, const b
     return 0;
 }
 
-extern "C" int b2s_to_bev_tc_ex(const float *feat, const b2s_half *feat_hi, const b2s_half *feat_lo, int feat_stride,
-                                const int *coors, const int *num_rows_dev, int cap_rows, int C, int batch, int D, int H,
-                                int W, b2s_half *out_hi, b2s_half *out_lo, uint8_t *occupancy, void *stream_)
+// products = 3: hi/lo planes; products = 1 (the f16 mode): feat_lo and out_lo must be NULL, one fp16 plane
+extern "C" int b2s_to_bev_tc_ex2(const float *feat, const b2s_half *feat_hi, const b2s_half *feat_lo, int feat_stride,
+                                 const int *coors, const int *num_rows_dev, int cap_rows, int C, int batch, int D, int H,
+                                 int W, b2s_half *out_hi, b2s_half *out_lo, uint8_t *occupancy, int products,
+                                 void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(products == 3 || (products == 1 && feat_lo == nullptr && out_lo == nullptr),
+                "b2s_to_bev_tc_ex: products must be 3 (hi/lo planes) or 1 (f16, no lo planes)");
     B2S_REQUIRE(C >= 1 && batch >= 1 && D >= 1 && H >= 1 && W >= 1, "b2s_to_bev_tc_ex: bad sizes");
-    B2S_REQUIRE((feat != nullptr) != (feat_hi != nullptr && feat_lo != nullptr),
+    B2S_REQUIRE((feat != nullptr) != (feat_hi != nullptr && (feat_lo != nullptr || products == 1)),
                 "b2s_to_bev_tc_ex: pass either fp32 rows or hi/lo fp16 rows");
     B2S_REQUIRE(occupancy != nullptr && (C * D) % 8 == 0 && ((uintptr_t)out_hi & 15) == 0 && ((uintptr_t)out_lo & 15) == 0,
                 "b2s_to_bev_tc_ex: needs the occupancy map, C*D a multiple of 8 and 16-byte aligned planes");
-    k_bev_clear<<<bounded_grid((long long)batch * H * W), kThreads, 0, stream>>>(
-        occupancy, batch, H, W, C * D / 8, reinterpret_cast<uint4 *>(out_hi), reinterpret_cast<uint4 *>(out_lo));
+    const int grid_clear = bounded_grid((long long)batch * H * W), grid_rows = bounded_grid((long long)cap_rows * C);
+    const __half *fh = reinterpret_cast<const __half *>(feat_hi), *fl = reinterpret_cast<const __half *>(feat_lo);
+    __half *oh = reinterpret_cast<__half *>(out_hi), *ol = reinterpret_cast<__half *>(out_lo);
+    if (products == 1)
+        k_bev_clear<1><<<grid_clear, kThreads, 0, stream>>>(occupancy, batch, H, W, C * D / 8,
+                                                            reinterpret_cast<uint4 *>(oh), nullptr);
+    else
+        k_bev_clear<3><<<grid_clear, kThreads, 0, stream>>>(occupancy, batch, H, W, C * D / 8,
+                                                            reinterpret_cast<uint4 *>(oh), reinterpret_cast<uint4 *>(ol));
     B2S_LAUNCH_OK();
     if (cap_rows > 0) {
-        k_to_bev_tc<<<bounded_grid((long long)cap_rows * C), kThreads, 0, stream>>>(
-            feat, reinterpret_cast<const __half *>(feat_hi), reinterpret_cast<const __half *>(feat_lo), feat_stride, coors,
-            num_rows_dev, cap_rows, C, batch, D, H, W, reinterpret_cast<__half *>(out_hi),
-            reinterpret_cast<__half *>(out_lo), occupancy);
+        if (products == 1)
+            k_to_bev_tc<1><<<grid_rows, kThreads, 0, stream>>>(feat, fh, nullptr, feat_stride, coors, num_rows_dev,
+                                                               cap_rows, C, batch, D, H, W, oh, nullptr, occupancy);
+        else
+            k_to_bev_tc<3><<<grid_rows, kThreads, 0, stream>>>(feat, fh, fl, feat_stride, coors, num_rows_dev, cap_rows,
+                                                               C, batch, D, H, W, oh, ol, occupancy);
         B2S_LAUNCH_OK();
     }
     return 0;
+}
+
+extern "C" int b2s_to_bev_tc_ex(const float *feat, const b2s_half *feat_hi, const b2s_half *feat_lo, int feat_stride,
+                                const int *coors, const int *num_rows_dev, int cap_rows, int C, int batch, int D, int H,
+                                int W, b2s_half *out_hi, b2s_half *out_lo, uint8_t *occupancy, void *stream)
+{
+    return b2s_to_bev_tc_ex2(feat, feat_hi, feat_lo, feat_stride, coors, num_rows_dev, cap_rows, C, batch, D, H, W,
+                             out_hi, out_lo, occupancy, 3, stream);
 }
 
 extern "C" int b2s_pfn(const float *points, int num_feat, const int *point_slots,
@@ -292,19 +318,33 @@ extern "C" int b2s_pfn_ex(const float *points, int num_feat, const int *point_sl
                                      max_points, weight, scale, shift, cout, vx, vy, x_offset, y_offset, out, stream);
 }
 
-extern "C" int b2s_crop_nhwc(const b2s_half *src_hi, const b2s_half *src_lo, int batch, int H, int W, int C, int crop,
-                             b2s_half *dst_hi, b2s_half *dst_lo, void *stream_)
+// products = 3: hi/lo planes; products = 1 (the f16 mode): src_lo and dst_lo must be NULL, one fp16 plane
+extern "C" int b2s_crop_nhwc_ex(const b2s_half *src_hi, const b2s_half *src_lo, int batch, int H, int W, int C, int crop,
+                                b2s_half *dst_hi, b2s_half *dst_lo, int products, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(products == 3 || (products == 1 && src_lo == nullptr && dst_lo == nullptr),
+                "b2s_crop_nhwc: products must be 3 (hi/lo planes) or 1 (f16, no lo planes)");
     B2S_REQUIRE(batch >= 1 && H >= 1 && W >= 1 && crop >= 0 && H - 2 * crop >= 1 && W - 2 * crop >= 1,
                 "b2s_crop_nhwc: bad sizes (the window [crop, H-crop) x [crop, W-crop) must be non-empty)");
     B2S_REQUIRE(C % 8 == 0 && ((uintptr_t)src_hi & 15) == 0 && ((uintptr_t)src_lo & 15) == 0 &&
                     ((uintptr_t)dst_hi & 15) == 0 && ((uintptr_t)dst_lo & 15) == 0,
                 "b2s_crop_nhwc: C must be a multiple of 8 and the planes 16-byte aligned");
     const long long total = (long long)batch * (H - 2 * crop + 2) * (W - 2 * crop + 2) * (C / 8);
-    k_crop_nhwc<<<bounded_grid(total), kThreads, 0, stream>>>(
-        reinterpret_cast<const uint4 *>(src_hi), reinterpret_cast<const uint4 *>(src_lo), batch, H, W, C / 8, crop,
-        reinterpret_cast<uint4 *>(dst_hi), reinterpret_cast<uint4 *>(dst_lo));
+    if (products == 1)
+        k_crop_nhwc<1><<<bounded_grid(total), kThreads, 0, stream>>>(
+            reinterpret_cast<const uint4 *>(src_hi), nullptr, batch, H, W, C / 8, crop, reinterpret_cast<uint4 *>(dst_hi),
+            nullptr);
+    else
+        k_crop_nhwc<3><<<bounded_grid(total), kThreads, 0, stream>>>(
+            reinterpret_cast<const uint4 *>(src_hi), reinterpret_cast<const uint4 *>(src_lo), batch, H, W, C / 8, crop,
+            reinterpret_cast<uint4 *>(dst_hi), reinterpret_cast<uint4 *>(dst_lo));
     B2S_LAUNCH_OK();
     return 0;
+}
+
+extern "C" int b2s_crop_nhwc(const b2s_half *src_hi, const b2s_half *src_lo, int batch, int H, int W, int C, int crop,
+                             b2s_half *dst_hi, b2s_half *dst_lo, void *stream)
+{
+    return b2s_crop_nhwc_ex(src_hi, src_lo, batch, H, W, C, crop, dst_hi, dst_lo, 3, stream);
 }

@@ -23,6 +23,10 @@
 // The ring's full/empty mbarriers let the loads of the next K blocks (and of the next tile) run under the MMAs.
 //
 // Every mbarrier wait is bounded: on a (never expected) protocol error the kernel traps instead of hanging the GPU.
+//
+// P = products per K step: 3 is the 3xF16 split above; 1 is the f16 mode (b2s_conv2d_tc_ex3 with products = 1): one
+// fp16 plane per operand, so a stage holds the A and B hi tiles only, each K step is one wgmma A_hi*B_hi, and the
+// epilogue writes one rounded fp16 plane, or with F32_OUT the fp32 result (P = 3 reads that from out_lo == NULL).
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -50,14 +54,41 @@ struct ConvParams {
     int *status;
 };
 
-template <int N, int STAGES>
+// The statements of the 3xF16 instances are kept as they were (their SASS is unchanged by the f16 instances): what
+// only the 3xF16 form does goes through these helpers, which compile to nothing for the f16 form.
+template <bool ON>
+__device__ __forceinline__ void tma_load_4d_if(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2,
+                                               int c3)
+{
+    if constexpr (ON) tma_load_4d(dst, map, bar, c0, c1, c2, c3);
+}
+template <bool ON>
+__device__ __forceinline__ void tma_load_3d_if(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2)
+{
+    if constexpr (ON) tma_load_3d(dst, map, bar, c0, c1, c2);
+}
+template <bool ON>
+__device__ __forceinline__ void store_u32_if(__half *dst, uint32_t v)
+{
+    if constexpr (ON) *reinterpret_cast<uint32_t *>(dst) = v;
+}
+// the epilogue writes fp16 planes: 3xF16 when out_lo is given, f16 unless the instance writes fp32
+template <int P, bool F32_OUT>
+__device__ __forceinline__ bool f16_planes_out(const __half *out_lo)
+{
+    if constexpr (P == 3) return out_lo != nullptr;
+    else return !F32_OUT;
+}
+
+template <int N, int STAGES, int P, bool F32_OUT>
 __global__ void __launch_bounds__(kThreads, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
           const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
           const ConvParams p)
 {
     constexpr uint32_t B_TILE_BYTES = N * BLOCK_K * ELEM_BYTES;
-    constexpr uint32_t STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
+    static_assert(P == 3 || P == 1, "products per K step: 3 (3xF16) or 1 (f16)");
+    constexpr uint32_t STAGE_BYTES = P == 3 ? 2 * A_TILE_BYTES + 2 * B_TILE_BYTES : A_TILE_BYTES + B_TILE_BYTES;
     constexpr int R = N / 2;                 // accumulator registers per thread (64 rows x N per warpgroup)
     // The tensor core's fp32 accumulate is not round-to-nearest: one long accumulation chain (432 MMAs for a 3x3x128
     // tap stack) carries a systematic ~2e-5 relative error.  So the reduction is cut into short chains of CHAIN K
@@ -104,11 +135,13 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ 
                     mbar_wait(&bar_empty[stage], phase ^ 1);
                     uint8_t *st = smem + (size_t)stage * STAGE_BYTES;
                     mbar_arrive_expect_tx(&bar_full[stage], STAGE_BYTES);
+                    // 3xF16: [A_hi | A_lo | B_hi | B_lo]; f16: [A_hi | B_hi]
                     tma_load_4d(st, &map_a_hi, &bar_full[stage], chunk * BLOCK_K, w0 + dx, h0 + dy, b);
-                    tma_load_4d(st + A_TILE_BYTES, &map_a_lo, &bar_full[stage], chunk * BLOCK_K, w0 + dx, h0 + dy, b);
-                    tma_load_3d(st + 2 * A_TILE_BYTES, &map_b_hi, &bar_full[stage], chunk * BLOCK_K, 0, tap);
-                    tma_load_3d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_b_lo, &bar_full[stage], chunk * BLOCK_K, 0,
-                                tap);
+                    tma_load_4d_if<P == 3>(st + A_TILE_BYTES, &map_a_lo, &bar_full[stage], chunk * BLOCK_K, w0 + dx,
+                                           h0 + dy, b);
+                    tma_load_3d(st + (P == 3 ? 2 : 1) * A_TILE_BYTES, &map_b_hi, &bar_full[stage], chunk * BLOCK_K, 0, tap);
+                    tma_load_3d_if<P == 3>(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_b_lo, &bar_full[stage],
+                                           chunk * BLOCK_K, 0, tap);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
@@ -134,16 +167,26 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ 
                 for (int chunk = 0; chunk < kb_chain; ++chunk) {
                     mbar_wait(&bar_full[stage], phase);          // TMA bytes have landed
                     const uint32_t sa = smem0 + (uint32_t)stage * STAGE_BYTES;
-                    const uint64_t a_hi = make_desc_sw128(sa + a_off), a_lo = make_desc_sw128(sa + A_TILE_BYTES + a_off);
-                    const uint64_t b_hi = make_desc_sw128(sa + 2 * A_TILE_BYTES);
-                    const uint64_t b_lo = make_desc_sw128(sa + 2 * A_TILE_BYTES + B_TILE_BYTES);
-                    wgmma_fence();
+                    if constexpr (P == 3) {
+                        const uint64_t a_hi = make_desc_sw128(sa + a_off), a_lo = make_desc_sw128(sa + A_TILE_BYTES + a_off);
+                        const uint64_t b_hi = make_desc_sw128(sa + 2 * A_TILE_BYTES);
+                        const uint64_t b_lo = make_desc_sw128(sa + 2 * A_TILE_BYTES + B_TILE_BYTES);
+                        wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
-                        const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);   // +32 B per K step
-                        wgmma_ss<N>(acc, a_lo + koff, b_hi + koff, (chunk | k) != 0);
-                        wgmma_ss<N>(acc, a_hi + koff, b_lo + koff, 1);
-                        wgmma_ss<N>(acc, a_hi + koff, b_hi + koff, 1);
+                        for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+                            const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);   // +32 B per K step
+                            wgmma_ss<N>(acc, a_lo + koff, b_hi + koff, (chunk | k) != 0);
+                            wgmma_ss<N>(acc, a_hi + koff, b_lo + koff, 1);
+                            wgmma_ss<N>(acc, a_hi + koff, b_hi + koff, 1);
+                        }
+                    } else {
+                        const uint64_t a_hi = make_desc_sw128(sa + a_off), b_hi = make_desc_sw128(sa + A_TILE_BYTES);
+                        wgmma_fence();
+#pragma unroll
+                        for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+                            const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                            wgmma_ss<N>(acc, a_hi + koff, b_hi + koff, (chunk | k) != 0);
+                        }
                     }
                     wgmma_commit();
                     wgmma_wait_all();
@@ -174,12 +217,12 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ 
                     float x0 = fmaf(sum[4 * j + 2 * rh], s_scale[c], s_shift[c]);
                     float x1 = fmaf(sum[4 * j + 2 * rh + 1], s_scale[c + 1], s_shift[c + 1]);
                     if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-                    if (p.out_lo) {
+                    if (f16_planes_out<P, F32_OUT>(p.out_lo)) {
                         range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
                         const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
                         *reinterpret_cast<uint32_t *>(reinterpret_cast<__half *>(p.out_hi) + gpix * p.out_stride + c) =
                             __byte_perm(p0, p1, 0x5410);
-                        *reinterpret_cast<uint32_t *>(p.out_lo + gpix * p.out_stride + c) = __byte_perm(p0, p1, 0x7632);
+                        store_u32_if<P == 3>(p.out_lo + gpix * p.out_stride + c, __byte_perm(p0, p1, 0x7632));
                     } else {
                         *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out_hi) + gpix * p.out_stride + c) =
                             make_float2(x0, x1);
@@ -191,15 +234,15 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ 
     }
 }
 
-template <int N, int STAGES>
+template <int N, int STAGES, int P, bool F32_OUT = false>
 int launch(const CUtensorMap &a_hi, const CUtensorMap &a_lo, const CUtensorMap &b_hi, const CUtensorMap &b_lo,
            const ConvParams &p, int num_sms, cudaStream_t stream)
 {
-    constexpr size_t stage = 2 * A_TILE_BYTES + 2 * (size_t)N * BLOCK_K * ELEM_BYTES;
+    constexpr size_t stage = (P == 3 ? 2 : 1) * (A_TILE_BYTES + (size_t)N * BLOCK_K * ELEM_BYTES);
     size_t smem = stage * STAGES + 1024;
-    B2S_SMEM_OPT_IN((k_conv_tc<N, STAGES>), smem);
+    B2S_SMEM_OPT_IN((k_conv_tc<N, STAGES, P, F32_OUT>), smem);
     int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-    k_conv_tc<N, STAGES><<<grid, kThreads, smem, stream>>>(a_hi, a_lo, b_hi, b_lo, p);
+    k_conv_tc<N, STAGES, P, F32_OUT><<<grid, kThreads, smem, stream>>>(a_hi, a_lo, b_hi, b_lo, p);
     B2S_LAUNCH_OK();
     return 0;
 }
@@ -211,7 +254,7 @@ int b2s_conv3x3_tc2(const __half *in_hi, const __half *in_lo, int B, int H, int 
                     const __half *w_lo, int Cout, const float *scale, const float *shift, int relu, __half *out_hi,
                     __half *out_lo, int out_stride, const int *work_list, const int *work_count, const int *bg_list,
                     const int *bg_count, const __half *bg_hi, const __half *bg_lo, int bg_margin, int list_rows,
-                    int *status, int num_sms, cudaStream_t stream);
+                    int products, int *status, int num_sms, cudaStream_t stream);
 
 // General form (include/b2second.h).  Input: halo-padded fp16 hi/lo planes [B, Hin+2, Win+2, Cin].  One GEMM pixel
 // (h, w) of the Hg x Wg grid reads input pixels (h*stride + dy - pad, w*stride + dx - pad), dy < kh, dx < kw, and is
@@ -222,27 +265,38 @@ int b2s_conv3x3_tc2(const __half *in_hi, const __half *in_lo, int B, int H, int 
 // work_list / bg_list name output strips 8 wide and list_rows (8, 4 or 2) high (b2s_rpn_block_plan,
 // b2s_rpn_strip_plan).  bg_margin >= 0: the field bg_hi/bg_lo equals its value at pixel (bg_margin, bg_margin)
 // wherever it is at least bg_margin pixels from every border, and background strips there are stored from that value.
-extern "C" int b2s_conv2d_tc_ex2(const b2s_half *in_hi_, const b2s_half *in_lo_, int B, int Hin, int Win, int Cin,
+//
+// products = 3: 3xF16 (hi/lo planes; out_lo == NULL: fp32 output).  products = 1: the f16 mode -- every lo pointer
+// (in_lo, w_lo, out_lo, bg_lo) must be NULL, the output is one fp16 plane in out_hi, or the fp32 result when out_fp32
+// is 1 (out_fp32 must be 0 with products = 3, where out_lo says it).
+extern "C" int b2s_conv2d_tc_ex3(const b2s_half *in_hi_, const b2s_half *in_lo_, int B, int Hin, int Win, int Cin,
                                  const b2s_half *w_hi_, const b2s_half *w_lo_, int kh, int kw, int stride, int pad,
                                  int Cout, int n_pad, const float *scale, const float *shift, int relu, int Hg, int Wg,
                                  void *out_hi, b2s_half *out_lo_, int Hout, int Wout, int out_padded, int out_stride,
                                  int out_mul, int off_h, int off_w, const int *work_list, const int *work_count_dev,
                                  const int *bg_list, const int *bg_count_dev, const b2s_half *bg_hi,
-                                 const b2s_half *bg_lo, int bg_margin, int list_rows, unsigned *status_dev,
-                                 void *stream_)
+                                 const b2s_half *bg_lo, int bg_margin, int list_rows, int products, int out_fp32,
+                                 unsigned *status_dev, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     const __half *in_hi = reinterpret_cast<const __half *>(in_hi_), *in_lo = reinterpret_cast<const __half *>(in_lo_);
     const __half *w_hi = reinterpret_cast<const __half *>(w_hi_), *w_lo = reinterpret_cast<const __half *>(w_lo_);
     __half *out_lo = reinterpret_cast<__half *>(out_lo_);
     const int taps = kh * kw;
+    B2S_REQUIRE(products == 3 || products == 1, "b2s_conv2d_tc: products must be 3 (3xF16) or 1 (f16)");
+    B2S_REQUIRE(products == 3 ? out_fp32 == 0
+                              : (in_lo == nullptr && w_lo == nullptr && out_lo == nullptr && bg_lo == nullptr &&
+                                 (out_fp32 == 0 || out_fp32 == 1)),
+                "b2s_conv2d_tc: products = 1 takes no lo planes and out_fp32 0 or 1; products = 3 takes out_fp32 = 0");
+    // fp16 plane output: hi/lo (products 3, out_lo given) or one plane (products 1, out_fp32 0)
+    const bool f16_out = products == 3 ? out_lo != nullptr : out_fp32 == 0;
     B2S_REQUIRE(kh >= 1 && kw >= 1 && taps <= 16 && stride >= 1 && stride <= 4 && (pad == 0 || pad == 1),
                 "b2s_conv2d_tc: kernel up to 4x4 (16 taps), stride 1..4, pad 0 or 1");
     B2S_REQUIRE(Cin % BLOCK_K == 0 && Cin >= BLOCK_K, "b2s_conv2d_tc: Cin must be a multiple of 64");
     B2S_REQUIRE(n_pad >= Cout && Cout % 4 == 0 && out_stride >= Cout && out_stride % 4 == 0,
                 "b2s_conv2d_tc: Cout/out_stride must be multiples of 4, n_pad >= Cout");
-    B2S_REQUIRE(out_lo == nullptr || (Cout % 8 == 0 && out_stride % 8 == 0 && ((uintptr_t)out_hi & 15) == 0 &&
-                                      ((uintptr_t)out_lo & 15) == 0),
+    B2S_REQUIRE(!f16_out || (Cout % 8 == 0 && out_stride % 8 == 0 && ((uintptr_t)out_hi & 15) == 0 &&
+                             ((uintptr_t)out_lo & 15) == 0),
                 "b2s_conv2d_tc: fp16 plane output needs Cout, out_stride multiples of 8 and 16-byte aligned pointers");
     B2S_REQUIRE(B >= 1 && Hin >= 1 && Win >= 1 && Hg >= 1 && Wg >= 1 && out_mul >= 1, "b2s_conv2d_tc: bad sizes");
     B2S_REQUIRE((Hg - 1) * out_mul + off_h < Hout && (Wg - 1) * out_mul + off_w < Wout && off_h >= 0 && off_w >= 0,
@@ -250,20 +304,21 @@ extern "C" int b2s_conv2d_tc_ex2(const b2s_half *in_hi_, const b2s_half *in_lo_,
     const int num_sms = num_sms_current();
     // 3x3 stride 1 pad 1, n_pad 128, hi/lo halo-padded output on the same grid: the weights-stationary N=256
     // kernel (conv_tc2.cu).  Every other shape runs k_conv_tc below.
-    const bool v2 = kh == 3 && kw == 3 && stride == 1 && pad == 1 && n_pad == 128 && out_lo != nullptr &&
+    const bool v2 = kh == 3 && kw == 3 && stride == 1 && pad == 1 && n_pad == 128 && f16_out &&
                     out_padded && out_mul == 1 && off_h == 0 && off_w == 0 && Hg == Hin && Wg == Win && Hout == Hin &&
                     Wout == Win;
     B2S_REQUIRE(work_list == nullptr || (v2 && work_count_dev != nullptr),
                 "b2s_conv2d_tc: a strip work list is only taken by the 3x3 stride-1 128-channel kernel");
     B2S_REQUIRE(work_list == nullptr || list_rows == 8 || list_rows == 4 || list_rows == 2,
                 "b2s_conv2d_tc: work-list strips are 8, 4 or 2 rows high");
-    B2S_REQUIRE(bg_list == nullptr || (work_list != nullptr && bg_count_dev != nullptr && bg_hi != nullptr && bg_lo != nullptr),
+    B2S_REQUIRE(bg_list == nullptr || (work_list != nullptr && bg_count_dev != nullptr && bg_hi != nullptr &&
+                                       (bg_lo != nullptr || products == 1)),
                 "b2s_conv2d_tc: a background-block list needs the work list, its count and the constant's hi/lo planes");
     if (v2)
         return b2s_conv3x3_tc2(in_hi, in_lo, B, Hin, Win, Cin, w_hi, w_lo, Cout, scale, shift, relu,
                                reinterpret_cast<__half *>(out_hi), out_lo, out_stride, work_list, work_count_dev, bg_list,
                                bg_count_dev, reinterpret_cast<const __half *>(bg_hi), reinterpret_cast<const __half *>(bg_lo),
-                               bg_margin, list_rows, (int *)status_dev, num_sms, stream);
+                               bg_margin, list_rows, products, (int *)status_dev, num_sms, stream);
     CUtensorMap a_hi, a_lo, b_hi, b_lo;
     {
         cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)(Win + 2), (cuuint64_t)(Hin + 2), (cuuint64_t)B};
@@ -272,14 +327,17 @@ extern "C" int b2s_conv2d_tc_ex2(const b2s_half *in_hi_, const b2s_half *in_lo_,
         // the box TRAVERSES stride*TILE pixels and keeps every stride-th one: TILE_W x TILE_H pixels land in smem
         cuuint32_t box[4] = {BLOCK_K, (cuuint32_t)(TILE_W * stride), (cuuint32_t)(TILE_H * stride), 1};
         cuuint32_t es[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-        if (make_map(&a_hi, in_hi, 4, dims, str, box, es) || make_map(&a_lo, in_lo, 4, dims, str, box, es)) return -1;
+        if (make_map(&a_hi, in_hi, 4, dims, str, box, es) ||
+            (products == 3 && make_map(&a_lo, in_lo, 4, dims, str, box, es)))
+            return -1;
     }
     {
         // weights [taps][n_pad][Cin] (rows >= Cout are zero)
         cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)n_pad, (cuuint64_t)taps};
         cuuint64_t str[2] = {(cuuint64_t)Cin * ELEM_BYTES, (cuuint64_t)n_pad * Cin * ELEM_BYTES};
         cuuint32_t box[3] = {BLOCK_K, (cuuint32_t)n_pad, 1};
-        if (make_map(&b_hi, w_hi, 3, dims, str, box) || make_map(&b_lo, w_lo, 3, dims, str, box)) return -1;
+        if (make_map(&b_hi, w_hi, 3, dims, str, box) || (products == 3 && make_map(&b_lo, w_lo, 3, dims, str, box)))
+            return -1;
     }
     ConvParams p;
     p.B = B; p.H = Hg; p.W = Wg; p.Cin = Cin; p.Cout = Cout; p.taps = taps; p.relu = relu;
@@ -290,14 +348,46 @@ extern "C" int b2s_conv2d_tc_ex2(const b2s_half *in_hi_, const b2s_half *in_lo_,
     p.Hout = Hout; p.Wout = Wout; p.out_mul = out_mul; p.off_h = off_h; p.off_w = off_w;
     p.out_padded = out_padded; p.out_stride = out_stride;
     p.scale = scale; p.shift = shift; p.out_hi = out_hi; p.out_lo = out_lo; p.status = (int *)status_dev;
-    switch (n_pad) {
-        case 128: return launch<128, 3>(a_hi, a_lo, b_hi, b_lo, p, num_sms, stream);
-        case 64: return launch<64, 4>(a_hi, a_lo, b_hi, b_lo, p, num_sms, stream);
-        case 32: return launch<32, 4>(a_hi, a_lo, b_hi, b_lo, p, num_sms, stream);
-        default: break;
+    if (products == 1 && f16_out) {
+        switch (n_pad) {
+            case 128: return launch<128, 3, 1>(a_hi, a_hi, b_hi, b_hi, p, num_sms, stream);
+            case 64: return launch<64, 4, 1>(a_hi, a_hi, b_hi, b_hi, p, num_sms, stream);
+            case 32: return launch<32, 4, 1>(a_hi, a_hi, b_hi, b_hi, p, num_sms, stream);
+            default: break;
+        }
+    } else if (products == 1) {
+        switch (n_pad) {
+            case 128: return launch<128, 3, 1, true>(a_hi, a_hi, b_hi, b_hi, p, num_sms, stream);
+            case 64: return launch<64, 4, 1, true>(a_hi, a_hi, b_hi, b_hi, p, num_sms, stream);
+            case 32: return launch<32, 4, 1, true>(a_hi, a_hi, b_hi, b_hi, p, num_sms, stream);
+            default: break;
+        }
+    } else {
+        switch (n_pad) {
+            case 128: return launch<128, 3, 3>(a_hi, a_lo, b_hi, b_lo, p, num_sms, stream);
+            case 64: return launch<64, 4, 3>(a_hi, a_lo, b_hi, b_lo, p, num_sms, stream);
+            case 32: return launch<32, 4, 3>(a_hi, a_lo, b_hi, b_lo, p, num_sms, stream);
+            default: break;
+        }
     }
     b2s_set_error("b2s_conv2d_tc: n_pad=%d not built (32, 64, 128)", n_pad);
     return -2;
+}
+
+// the 3xF16 form
+extern "C" int b2s_conv2d_tc_ex2(const b2s_half *in_hi, const b2s_half *in_lo, int B, int Hin, int Win, int Cin,
+                                 const b2s_half *w_hi, const b2s_half *w_lo, int kh, int kw, int stride, int pad,
+                                 int Cout, int n_pad, const float *scale, const float *shift, int relu, int Hg, int Wg,
+                                 void *out_hi, b2s_half *out_lo, int Hout, int Wout, int out_padded, int out_stride,
+                                 int out_mul, int off_h, int off_w, const int *work_list, const int *work_count_dev,
+                                 const int *bg_list, const int *bg_count_dev, const b2s_half *bg_hi,
+                                 const b2s_half *bg_lo, int bg_margin, int list_rows, unsigned *status_dev,
+                                 void *stream)
+{
+    return b2s_conv2d_tc_ex3(in_hi, in_lo, B, Hin, Win, Cin, w_hi, w_lo, kh, kw, stride, pad, Cout, n_pad, scale, shift,
+                             relu, Hg, Wg, out_hi, out_lo, Hout, Wout, out_padded, out_stride, out_mul, off_h, off_w,
+                             work_list, work_count_dev, bg_list, bg_count_dev, bg_hi, bg_lo, bg_margin, list_rows, 3, 0,
+                             status_dev, stream);
 }
 
 // the same with the lists of b2s_rpn_block_plan (8x8 blocks)

@@ -27,6 +27,10 @@
 // constant interior value from registers, copied near the border; independently of the work items), 3 weight TMA
 // producer, 4-11 two consumer warpgroups (MMA, epilogue).  The kernel is bound by the bytes it reads from L2, so the
 // fill reading nothing for interior strips is worth as much as the MMAs it skips.
+//
+// P = products per K step: 3 (3xF16, above) or 1 (the f16 mode): one fp16 plane per operand, so a stage holds the hi
+// windows only, the weight ring carries hi planes only (its six slots are then two whole (dx, chunk) groups), each K
+// step is one wgmma, and the epilogue and the background fill write the hi plane only.
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -43,15 +47,17 @@ constexpr uint32_t W_PLANE_BYTES = 128 * BLOCK_K * ELEM_BYTES;             // 16
 constexpr int X_STAGES = 2, W_STAGES = 6;
 static_assert(ATOM_BYTES == 1024, "window rows are whole swizzle atoms");
 
-// shared-memory geometry for strips of R rows: S = 8 / R strips per warpgroup tile
-template <int R>
+// shared-memory geometry for strips of R rows: S = 8 / R strips per warpgroup tile; P products per K step
+template <int R, int P>
 struct StripGeom {
     static_assert(R == 8 || R == 4 || R == 2, "strip heights 8, 4 and 2 are built");
+    static_assert(P == 3 || P == 1, "products per K step: 3 (3xF16) or 1 (f16)");
     static constexpr int S = 8 / R;
+    static constexpr int PLANES = P == 3 ? 2 : 1;                          // operand planes: hi, lo
     static constexpr uint32_t DY_BYTES = S * ATOM_BYTES;                    // one window row of all S strips
     static constexpr uint32_t X_TILE_BYTES = (R + 2) * DY_BYTES;           // one warpgroup tile's windows, one plane
     static constexpr uint32_t X_PLANE_BYTES = 2 * X_TILE_BYTES;            // hi or lo: both tiles of a pair
-    static constexpr uint32_t X_STAGE_BYTES = 2 * X_PLANE_BYTES;           // R = 8: 40 KB, R = 2: 64 KB
+    static constexpr uint32_t X_STAGE_BYTES = PLANES * X_PLANE_BYTES;      // 3xF16, R = 8: 40 KB, R = 2: 64 KB
     static constexpr size_t SMEM_BYTES = (size_t)X_STAGES * X_STAGE_BYTES + (size_t)W_STAGES * W_PLANE_BYTES + 1024;
 };
 
@@ -85,13 +91,13 @@ __device__ __forceinline__ void strip_origin(const Conv2Params &p, int id, int &
     b = id / (p.strips_w * p.strips_h);
 }
 
-template <int R>
+template <int R, int P>
 __global__ void __launch_bounds__(kThreads2, 1)
 k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
               const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
               const Conv2Params p)
 {
-    using G = StripGeom<R>;
+    using G = StripGeom<R, P>;
     constexpr int S = G::S;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -146,8 +152,9 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                             for (int r = 0; r < (S == 1 ? 1 : R + 2); ++r) {
                                 tma_load_4d(dst + r * G::DY_BYTES, &map_x_hi, &bar_xfull[xs], chunk * BLOCK_K, x0,
                                             h0[j] + r, bb[j]);
-                                tma_load_4d(dst + G::X_PLANE_BYTES + r * G::DY_BYTES, &map_x_lo, &bar_xfull[xs],
-                                            chunk * BLOCK_K, x0, h0[j] + r, bb[j]);
+                                if constexpr (P == 3)
+                                    tma_load_4d(dst + G::X_PLANE_BYTES + r * G::DY_BYTES, &map_x_lo, &bar_xfull[xs],
+                                                chunk * BLOCK_K, x0, h0[j] + r, bb[j]);
                             }
                         }
                         if (++xs == X_STAGES) { xs = 0; xph ^= 1; }
@@ -163,7 +170,7 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                 for (int dx = 0; dx < 3; ++dx)
                     for (int chunk = 0; chunk < kchunks; ++chunk)
                         for (int dy = 0; dy < 3; ++dy)
-                            for (int pl = 0; pl < 2; ++pl) {           // hi plane, then lo plane
+                            for (int pl = 0; pl < G::PLANES; ++pl) {   // hi plane, then lo plane
                                 mbar_wait(&bar_wempty[ws], wph ^ 1);
                                 mbar_arrive_expect_tx(&bar_wfull[ws], W_PLANE_BYTES);
                                 tma_load_3d(smem_w + (size_t)ws * W_PLANE_BYTES, pl ? &map_w_lo : &map_w_hi,
@@ -191,7 +198,7 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                 if (m >= 0) {
                     const size_t cpix = (size_t)(m + 1) * (p.W + 2) + (m + 1);
                     ch = __ldg(reinterpret_cast<const uint4 *>(p.bg_hi + cpix * p.Cout + chunk * 8));
-                    cl = __ldg(reinterpret_cast<const uint4 *>(p.bg_lo + cpix * p.Cout + chunk * 8));
+                    if constexpr (P == 3) cl = __ldg(reinterpret_cast<const uint4 *>(p.bg_lo + cpix * p.Cout + chunk * 8));
                 }
                 for (int i0 = blockIdx.x * NF; i0 < n_bg; i0 += gridDim.x * NF) {
 #pragma unroll
@@ -213,19 +220,28 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                             const uint4 *fh = reinterpret_cast<const uint4 *>(p.bg_hi + fpix * p.Cout + chunk * 8);
                             const uint4 *fl = reinterpret_cast<const uint4 *>(p.bg_lo + fpix * p.Cout + chunk * 8);
                             oh[u] = reinterpret_cast<uint4 *>(p.out_hi + opix * p.out_stride + chunk * 8);
-                            ol[u] = reinterpret_cast<uint4 *>(p.out_lo + opix * p.out_stride + chunk * 8);
+                            if constexpr (P == 3) {
+                                ol[u] = reinterpret_cast<uint4 *>(p.out_lo + opix * p.out_stride + chunk * 8);
 #pragma unroll
-                            for (int r = 0; r < R; ++r)
-                                if (r < rows[u]) {
-                                    if (inner[u]) { vh[u][r] = ch; vl[u][r] = cl; }
-                                    else { vh[u][r] = __ldg(fh + r * fstep); vl[u][r] = __ldg(fl + r * fstep); }
-                                }
+                                for (int r = 0; r < R; ++r)
+                                    if (r < rows[u]) {
+                                        if (inner[u]) { vh[u][r] = ch; vl[u][r] = cl; }
+                                        else { vh[u][r] = __ldg(fh + r * fstep); vl[u][r] = __ldg(fl + r * fstep); }
+                                    }
+                            } else {
+#pragma unroll
+                                for (int r = 0; r < R; ++r)
+                                    if (r < rows[u]) vh[u][r] = inner[u] ? ch : __ldg(fh + r * fstep);
+                            }
                         }
 #pragma unroll
                         for (int u = 0; u < U; ++u)
 #pragma unroll
                             for (int r = 0; r < R; ++r)
-                                if (r < rows[u]) { oh[u][r * ostep] = vh[u][r]; ol[u][r * ostep] = vl[u][r]; }
+                                if (r < rows[u]) {
+                                    if constexpr (P == 3) { oh[u][r * ostep] = vh[u][r]; ol[u][r * ostep] = vl[u][r]; }
+                                    else oh[u][r * ostep] = vh[u][r];
+                                }
                     }
                 }
             }
@@ -246,6 +262,24 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                 const uint32_t sx = sx0 + (uint32_t)xs * G::X_STAGE_BYTES + (uint32_t)cg * G::X_TILE_BYTES;
 #pragma unroll 1
                 for (int dy = 0; dy < 3; ++dy) {
+                    if constexpr (P == 1) {
+                        mbar_wait(&bar_wfull[ws], wph);
+                        const uint64_t x_hi = make_desc_sw128(sx + dy * G::DY_BYTES);
+                        const uint64_t w_hi = make_desc_sw128(sw0 + (uint32_t)ws * W_PLANE_BYTES);
+                        wgmma_fence();
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) {
+                            const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                            wgmma_ss<128>(acc, x_hi + koff, w_hi + koff, (dy | k) != 0);
+                        }
+                        wgmma_commit();
+                        wgmma_wait_all();
+                        wgmma_fence_operands<64>(acc);
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&bar_wempty[ws]);
+                        if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
+                        continue;
+                    }
                     int ws2 = ws + 1;
                     uint32_t wph2 = wph;
                     if (ws2 == W_STAGES) { ws2 = 0; wph2 ^= 1; }
@@ -297,7 +331,7 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                 const int h = h0 + a / S, w = w0 + (lane >> 2);
                 if (h >= p.H || w >= p.W) continue;
                 const size_t pix = ((size_t)b * (p.H + 2) + (h + 1)) * (p.W + 2) + (w + 1);
-                __half *oh = p.out_hi + pix * p.out_stride, *ol = p.out_lo + pix * p.out_stride;
+                __half *oh = p.out_hi + pix * p.out_stride, *ol = P == 3 ? p.out_lo + pix * p.out_stride : nullptr;
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
                     const int c = 8 * j + 2 * (lane & 3);
@@ -308,7 +342,7 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
                     range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
                     const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
                     *reinterpret_cast<uint32_t *>(oh + c) = __byte_perm(p0, p1, 0x5410);
-                    *reinterpret_cast<uint32_t *>(ol + c) = __byte_perm(p0, p1, 0x7632);
+                    if constexpr (P == 3) *reinterpret_cast<uint32_t *>(ol + c) = __byte_perm(p0, p1, 0x7632);
                 }
             }
             if (range_bad && p.status) atomicOr(p.status, B2S_STATUS_F16_RANGE);
@@ -316,11 +350,11 @@ k_conv3x3_tc2(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constan
     }
 }
 
-template <int R>
+template <int R, int P>
 int launch_tc2(const __half *in_hi, const __half *in_lo, const __half *w_hi, const __half *w_lo, Conv2Params &p,
                int num_sms, cudaStream_t stream)
 {
-    using G = StripGeom<R>;
+    using G = StripGeom<R, P>;
     CUtensorMap x_hi, x_lo, m_w_hi, m_w_lo;
     {
         const int B = p.B, H = p.H, W = p.W, Cin = p.Cin;
@@ -329,34 +363,37 @@ int launch_tc2(const __half *in_hi, const __half *in_lo, const __half *w_hi, con
                              (cuuint64_t)(H + 2) * (W + 2) * Cin * ELEM_BYTES};
         // S = 1: a strip's whole (R+2)-row window is one box; else one box per window row (rows are interleaved)
         cuuint32_t box[4] = {BLOCK_K, STRIP_W, G::S == 1 ? (cuuint32_t)(R + 2) : 1u, 1};
-        if (make_map(&x_hi, in_hi, 4, dims, str, box) || make_map(&x_lo, in_lo, 4, dims, str, box)) return -1;
+        if (make_map(&x_hi, in_hi, 4, dims, str, box) || make_map(&x_lo, P == 3 ? in_lo : in_hi, 4, dims, str, box))
+            return -1;
     }
     {
         cuuint64_t dims[3] = {(cuuint64_t)p.Cin, 128, 9};
         cuuint64_t str[2] = {(cuuint64_t)p.Cin * ELEM_BYTES, (cuuint64_t)128 * p.Cin * ELEM_BYTES};
         cuuint32_t box[3] = {BLOCK_K, 128, 1};
-        if (make_map(&m_w_hi, w_hi, 3, dims, str, box) || make_map(&m_w_lo, w_lo, 3, dims, str, box)) return -1;
+        if (make_map(&m_w_hi, w_hi, 3, dims, str, box) || make_map(&m_w_lo, P == 3 ? w_lo : w_hi, 3, dims, str, box))
+            return -1;
     }
     p.strips_h = (p.H + R - 1) / R;
     p.strips_w = (p.W + STRIP_W - 1) / STRIP_W;
     p.num_strips = p.B * p.strips_h * p.strips_w;
-    B2S_SMEM_OPT_IN(k_conv3x3_tc2<R>, G::SMEM_BYTES);
+    B2S_SMEM_OPT_IN((k_conv3x3_tc2<R, P>), G::SMEM_BYTES);
     const int max_pairs = (p.num_strips + 2 * G::S - 1) / (2 * G::S);
     const int grid = max_pairs < num_sms ? max_pairs : num_sms;     // (with a work list some CTAs may only fill)
-    k_conv3x3_tc2<R><<<grid, kThreads2, G::SMEM_BYTES, stream>>>(x_hi, x_lo, m_w_hi, m_w_lo, p);
+    k_conv3x3_tc2<R, P><<<grid, kThreads2, G::SMEM_BYTES, stream>>>(x_hi, x_lo, m_w_hi, m_w_lo, p);
     B2S_LAUNCH_OK();
     return 0;
 }
 
 }  // namespace
 
-// called by b2s_conv2d_tc_ex2 (conv_tc.cu) for taps == 9, n_pad == 128, halo-padded hi/lo output; work_list / bg_list
-// name 8 x list_rows strips (list_rows 8, 4 or 2); dense launches (no work list) run 8 x 8 blocks
+// called by b2s_conv2d_tc_ex3 (conv_tc.cu) for taps == 9, n_pad == 128, halo-padded fp16 plane output; work_list /
+// bg_list name 8 x list_rows strips (list_rows 8, 4 or 2); dense launches (no work list) run 8 x 8 blocks; products 3
+// (hi/lo planes) or 1 (hi planes only)
 int b2s_conv3x3_tc2(const __half *in_hi, const __half *in_lo, int B, int H, int W, int Cin, const __half *w_hi,
                     const __half *w_lo, int Cout, const float *scale, const float *shift, int relu, __half *out_hi,
                     __half *out_lo, int out_stride, const int *work_list, const int *work_count, const int *bg_list,
                     const int *bg_count, const __half *bg_hi, const __half *bg_lo, int bg_margin, int list_rows,
-                    int *status, int num_sms, cudaStream_t stream)
+                    int products, int *status, int num_sms, cudaStream_t stream)
 {
     Conv2Params p;
     p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.relu = relu;
@@ -365,7 +402,12 @@ int b2s_conv3x3_tc2(const __half *in_hi, const __half *in_lo, int B, int H, int 
     p.bg_margin = (bg_list && bg_margin >= 0 && 2 * bg_margin < H && 2 * bg_margin < W) ? bg_margin : -1;
     p.out_stride = out_stride;
     p.scale = scale; p.shift = shift; p.out_hi = out_hi; p.out_lo = out_lo; p.status = status;
-    if (work_list && list_rows == 2) return launch_tc2<2>(in_hi, in_lo, w_hi, w_lo, p, num_sms, stream);
-    if (work_list && list_rows == 4) return launch_tc2<4>(in_hi, in_lo, w_hi, w_lo, p, num_sms, stream);
-    return launch_tc2<8>(in_hi, in_lo, w_hi, w_lo, p, num_sms, stream);
+    if (products == 1) {
+        if (work_list && list_rows == 2) return launch_tc2<2, 1>(in_hi, in_lo, w_hi, w_lo, p, num_sms, stream);
+        if (work_list && list_rows == 4) return launch_tc2<4, 1>(in_hi, in_lo, w_hi, w_lo, p, num_sms, stream);
+        return launch_tc2<8, 1>(in_hi, in_lo, w_hi, w_lo, p, num_sms, stream);
+    }
+    if (work_list && list_rows == 2) return launch_tc2<2, 3>(in_hi, in_lo, w_hi, w_lo, p, num_sms, stream);
+    if (work_list && list_rows == 4) return launch_tc2<4, 3>(in_hi, in_lo, w_hi, w_lo, p, num_sms, stream);
+    return launch_tc2<8, 3>(in_hi, in_lo, w_hi, w_lo, p, num_sms, stream);
 }

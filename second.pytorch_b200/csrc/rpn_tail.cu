@@ -21,6 +21,10 @@
 //   warpgroups 1, 2   consumers: warpgroup g owns tile pixels 64g .. 64g+63 through GEMM 1, the y epilogue, GEMM 2
 //                     and the record stores
 // With a work list, TMA and consumers walk the listed tiles only (a tile id = (b * tiles_h + th) * tiles_w + tw).
+//
+// P = products per K step: 3 (3xF16, above) or 1 (the f16 mode): x and both weight sets are single fp16 planes (half
+// the shared memory), GEMM 1 is one wgmma per K step, y is rounded to one fp16 plane, and GEMM 2 is one register-A
+// wgmma per K step.
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -35,13 +39,20 @@ constexpr int N1 = 128;                   // GEMM 1 N (= channels of y)
 constexpr int N2 = 32;                    // GEMM 2 N (packed head channels, zero padded)
 constexpr int kThreads = 384;             // 1 producer warpgroup + 2 consumer warpgroups
 constexpr int XS = 2 * KB;                // x ring slots (one K block of one tile each)
-constexpr uint32_t W1_KB_BYTES = 2 * N1 * BLOCK_K * ELEM_BYTES;        // hi + lo of one K block: 32 KB
-constexpr uint32_t W2_KB_BYTES = 2 * N2 * BLOCK_K * ELEM_BYTES;        // hi + lo of one K block of the head weights: 8 KB
-constexpr uint32_t X_STAGE_BYTES = 2 * A_TILE_BYTES;                   // hi + lo of one K block of x: 32 KB
-constexpr uint32_t OFF_W1 = 0, OFF_W2 = OFF_W1 + KB * W1_KB_BYTES, OFF_X = OFF_W2 + KB * W2_KB_BYTES;
-constexpr size_t SMEM_BYTES = OFF_X + XS * X_STAGE_BYTES + 1024;
-static_assert((OFF_W2 % 1024) == 0 && (OFF_X % 1024) == 0 && (W2_KB_BYTES / 2) % 1024 == 0,
-              "operand tiles are 1024-byte aligned (SWIZZLE_128B)");
+
+// shared-memory layout for P products per K step (PL = 2 planes for 3xF16, 1 for f16)
+template <int P>
+struct TailGeom {
+    static_assert(P == 3 || P == 1, "products per K step: 3 (3xF16) or 1 (f16)");
+    static constexpr int PL = P == 3 ? 2 : 1;
+    static constexpr uint32_t W1_KB_BYTES = PL * N1 * BLOCK_K * ELEM_BYTES;   // hi + lo of one K block: 32 KB
+    static constexpr uint32_t W2_KB_BYTES = PL * N2 * BLOCK_K * ELEM_BYTES;   // ... of the head weights: 8 KB
+    static constexpr uint32_t X_STAGE_BYTES = PL * A_TILE_BYTES;              // hi + lo of one K block of x: 32 KB
+    static constexpr uint32_t OFF_W1 = 0, OFF_W2 = OFF_W1 + KB * W1_KB_BYTES, OFF_X = OFF_W2 + KB * W2_KB_BYTES;
+    static constexpr size_t SMEM_BYTES = OFF_X + XS * X_STAGE_BYTES + 1024;
+    static_assert((OFF_W2 % 1024) == 0 && (OFF_X % 1024) == 0 && (N2 * BLOCK_K * ELEM_BYTES) % 1024 == 0,
+                  "operand tiles are 1024-byte aligned (SWIZZLE_128B)");
+};
 
 struct TailParams {
     int B, H, W, tiles_h, tiles_w, num_tiles;
@@ -56,12 +67,16 @@ struct TailParams {
                                          // pixels from every border; < 0: no such promise
 };
 
+template <int P>
 __global__ void __launch_bounds__(kThreads, 1)
 k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
            const __grid_constant__ CUtensorMap map_w1_hi, const __grid_constant__ CUtensorMap map_w1_lo,
            const __grid_constant__ CUtensorMap map_w2_hi, const __grid_constant__ CUtensorMap map_w2_lo,
            const TailParams p)
 {
+    using G = TailGeom<P>;
+    constexpr uint32_t W1_KB_BYTES = G::W1_KB_BYTES, W2_KB_BYTES = G::W2_KB_BYTES, X_STAGE_BYTES = G::X_STAGE_BYTES;
+    constexpr uint32_t OFF_W1 = G::OFF_W1, OFF_W2 = G::OFF_W2, OFF_X = G::OFF_X;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     __shared__ __align__(8) uint64_t bar_w, bar_xfull[XS], bar_xempty[XS];
@@ -93,9 +108,11 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
             mbar_arrive_expect_tx(&bar_w, KB * (W1_KB_BYTES + W2_KB_BYTES));
             for (int kb = 0; kb < KB; ++kb) {
                 tma_load_3d(smem + OFF_W1 + kb * W1_KB_BYTES, &map_w1_hi, &bar_w, kb * BLOCK_K, 0, 0);
-                tma_load_3d(smem + OFF_W1 + kb * W1_KB_BYTES + W1_KB_BYTES / 2, &map_w1_lo, &bar_w, kb * BLOCK_K, 0, 0);
+                if constexpr (P == 3)
+                    tma_load_3d(smem + OFF_W1 + kb * W1_KB_BYTES + W1_KB_BYTES / 2, &map_w1_lo, &bar_w, kb * BLOCK_K, 0, 0);
                 tma_load_3d(smem + OFF_W2 + kb * W2_KB_BYTES, &map_w2_hi, &bar_w, kb * BLOCK_K, 0, 0);
-                tma_load_3d(smem + OFF_W2 + kb * W2_KB_BYTES + W2_KB_BYTES / 2, &map_w2_lo, &bar_w, kb * BLOCK_K, 0, 0);
+                if constexpr (P == 3)
+                    tma_load_3d(smem + OFF_W2 + kb * W2_KB_BYTES + W2_KB_BYTES / 2, &map_w2_lo, &bar_w, kb * BLOCK_K, 0, 0);
             }
             int u = 0;                                                 // K blocks of x loaded so far: slot u % XS, its (u / XS)-th use
             for (int i = blockIdx.x; i < n_work; i += gridDim.x) {
@@ -108,7 +125,7 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
                     uint8_t *st = smem + OFF_X + slot * X_STAGE_BYTES;
                     mbar_arrive_expect_tx(&bar_xfull[slot], X_STAGE_BYTES);
                     tma_load_4d(st, &map_x_hi, &bar_xfull[slot], kb * BLOCK_K, w0, h0, b);
-                    tma_load_4d(st + A_TILE_BYTES, &map_x_lo, &bar_xfull[slot], kb * BLOCK_K, w0, h0, b);
+                    if constexpr (P == 3) tma_load_4d(st + A_TILE_BYTES, &map_x_lo, &bar_xfull[slot], kb * BLOCK_K, w0, h0, b);
                 }
             }
         }
@@ -156,15 +173,23 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
                 mbar_wait(&bar_xfull[slot], (uint32_t)(((u + kb) / XS) & 1));
                 const uint32_t xa = smem0 + OFF_X + slot * X_STAGE_BYTES + a_off;
                 const uint32_t wb = smem0 + OFF_W1 + kb * W1_KB_BYTES;
-                const uint64_t a_hi = make_desc_sw128(xa), a_lo = make_desc_sw128(xa + A_TILE_BYTES);
-                const uint64_t b_hi = make_desc_sw128(wb), b_lo = make_desc_sw128(wb + W1_KB_BYTES / 2);
+                const uint64_t a_hi = make_desc_sw128(xa), b_hi = make_desc_sw128(wb);
                 wgmma_fence();
+                if constexpr (P == 3) {
+                    const uint64_t a_lo = make_desc_sw128(xa + A_TILE_BYTES), b_lo = make_desc_sw128(wb + W1_KB_BYTES / 2);
 #pragma unroll
-                for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
-                    const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
-                    wgmma_ss<N1>(d1, a_lo + koff, b_hi + koff, (kb | k) != 0);
-                    wgmma_ss<N1>(d1, a_hi + koff, b_lo + koff, 1);
-                    wgmma_ss<N1>(d1, a_hi + koff, b_hi + koff, 1);
+                    for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+                        const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                        wgmma_ss<N1>(d1, a_lo + koff, b_hi + koff, (kb | k) != 0);
+                        wgmma_ss<N1>(d1, a_hi + koff, b_lo + koff, 1);
+                        wgmma_ss<N1>(d1, a_hi + koff, b_hi + koff, 1);
+                    }
+                } else {
+#pragma unroll
+                    for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+                        const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                        wgmma_ss<N1>(d1, a_hi + koff, b_hi + koff, (kb | k) != 0);
+                    }
                 }
                 wgmma_commit();
             }
@@ -188,7 +213,7 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
                 range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
                 const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
                 yh[i] = __byte_perm(p0, p1, 0x5410);
-                yl[i] = __byte_perm(p0, p1, 0x7632);
+                if constexpr (P == 3) yl[i] = __byte_perm(p0, p1, 0x7632);
             }
             // ---- GEMM 2: D2 = y * W2^T (A from registers)
             float d2[N2 / 2];
@@ -198,10 +223,15 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
                 const int kb = s / (BLOCK_K / MMA_K), k = s % (BLOCK_K / MMA_K);
                 const uint32_t wb = smem0 + OFF_W2 + kb * W2_KB_BYTES;
                 const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
-                const uint64_t b_hi = make_desc_sw128(wb) + koff, b_lo = make_desc_sw128(wb + W2_KB_BYTES / 2) + koff;
-                wgmma_rs<N2>(d2, &yl[4 * s], b_hi, s != 0);
-                wgmma_rs<N2>(d2, &yh[4 * s], b_lo, 1);
-                wgmma_rs<N2>(d2, &yh[4 * s], b_hi, 1);
+                const uint64_t b_hi = make_desc_sw128(wb) + koff;
+                if constexpr (P == 3) {
+                    const uint64_t b_lo = make_desc_sw128(wb + W2_KB_BYTES / 2) + koff;
+                    wgmma_rs<N2>(d2, &yl[4 * s], b_hi, s != 0);
+                    wgmma_rs<N2>(d2, &yh[4 * s], b_lo, 1);
+                    wgmma_rs<N2>(d2, &yh[4 * s], b_hi, 1);
+                } else {
+                    wgmma_rs<N2>(d2, &yh[4 * s], b_hi, s != 0);
+                }
             }
             wgmma_commit();
             wgmma_wait_all();
@@ -231,14 +261,18 @@ k_rpn_tail(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__
 
 // in: halo-padded hi/lo planes [B, H+2, W+2, 128]; w1: [128][128] (y channel, x channel), w2: [n_pad][128] (rows >= cout2
 // zero), both K-major hi/lo planes pre-scaled by a power of two folded into scale1 / scale2; out: fp32 [B, H, W, out_stride].
-extern "C" int b2s_rpn_tail_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int B, int H, int W, int Cin,
-                                  const b2s_half *w1_hi, const b2s_half *w1_lo, int Cmid, const float *scale1,
-                                  const float *shift1, const b2s_half *w2_hi, const b2s_half *w2_lo, int cout2,
-                                  int n_pad2, const float *scale2, const float *shift2, float *out, int out_stride,
-                                  const int *work_list, const int *work_count, const int *bg_list, const int *bg_count,
-                                  const float *field, int margin, unsigned *status_dev, void *stream_)
+// products = 3: 3xF16; products = 1: the f16 mode, in_lo, w1_lo and w2_lo must be NULL.
+extern "C" int b2s_rpn_tail_tc_ex2(const b2s_half *in_hi, const b2s_half *in_lo, int B, int H, int W, int Cin,
+                                   const b2s_half *w1_hi, const b2s_half *w1_lo, int Cmid, const float *scale1,
+                                   const float *shift1, const b2s_half *w2_hi, const b2s_half *w2_lo, int cout2,
+                                   int n_pad2, const float *scale2, const float *shift2, float *out, int out_stride,
+                                   const int *work_list, const int *work_count, const int *bg_list, const int *bg_count,
+                                   const float *field, int margin, int products, unsigned *status_dev, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(products == 3 || (products == 1 && in_lo == nullptr && w1_lo == nullptr && w2_lo == nullptr),
+                "b2s_rpn_tail_tc: products must be 3 (3xF16) or 1 (f16, no lo planes)");
+    const bool three = products == 3;
     B2S_REQUIRE(Cin == C && Cmid == N1, "b2s_rpn_tail_tc: built for a 128 -> 128 deblock (got %d -> %d)", Cin, Cmid);
     B2S_REQUIRE(n_pad2 == N2 && cout2 >= 4 && cout2 <= n_pad2 && cout2 % 4 == 0 && out_stride >= cout2 && out_stride % 4 == 0,
                 "b2s_rpn_tail_tc: up to 32 packed head channels (multiple of 4), out_stride a multiple of 4");
@@ -252,19 +286,21 @@ extern "C" int b2s_rpn_tail_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, 
         cuuint64_t str[3] = {(cuuint64_t)C * ELEM_BYTES, (cuuint64_t)(W + 2) * C * ELEM_BYTES,
                              (cuuint64_t)(H + 2) * (W + 2) * C * ELEM_BYTES};
         cuuint32_t box[4] = {BLOCK_K, TILE_W, TILE_H, 1};
-        if (make_map(&x_hi, in_hi, 4, dims, str, box) || make_map(&x_lo, in_lo, 4, dims, str, box)) return -1;
+        if (make_map(&x_hi, in_hi, 4, dims, str, box) || (three && make_map(&x_lo, in_lo, 4, dims, str, box))) return -1;
     }
     {
         cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)N1, 1};
         cuuint64_t str[2] = {(cuuint64_t)C * ELEM_BYTES, (cuuint64_t)N1 * C * ELEM_BYTES};
         cuuint32_t box[3] = {BLOCK_K, N1, 1};
-        if (make_map(&m1_hi, w1_hi, 3, dims, str, box) || make_map(&m1_lo, w1_lo, 3, dims, str, box)) return -1;
+        if (make_map(&m1_hi, w1_hi, 3, dims, str, box) || (three && make_map(&m1_lo, w1_lo, 3, dims, str, box)))
+            return -1;
     }
     {
         cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)n_pad2, 1};
         cuuint64_t str[2] = {(cuuint64_t)C * ELEM_BYTES, (cuuint64_t)n_pad2 * C * ELEM_BYTES};
         cuuint32_t box[3] = {BLOCK_K, (cuuint32_t)n_pad2, 1};
-        if (make_map(&m2_hi, w2_hi, 3, dims, str, box) || make_map(&m2_lo, w2_lo, 3, dims, str, box)) return -1;
+        if (make_map(&m2_hi, w2_hi, 3, dims, str, box) || (three && make_map(&m2_lo, w2_lo, 3, dims, str, box)))
+            return -1;
     }
     TailParams p;
     p.B = B; p.H = H; p.W = W;
@@ -278,10 +314,28 @@ extern "C" int b2s_rpn_tail_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, 
     p.margin = (bg_list && margin >= 0 && 2 * margin < H && 2 * margin < W) ? margin : -1;
     const int num_sms = num_sms_current();
     const int grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-    B2S_SMEM_OPT_IN(k_rpn_tail, SMEM_BYTES);
-    k_rpn_tail<<<grid, kThreads, SMEM_BYTES, stream>>>(x_hi, x_lo, m1_hi, m1_lo, m2_hi, m2_lo, p);
+    if (three) {
+        B2S_SMEM_OPT_IN(k_rpn_tail<3>, TailGeom<3>::SMEM_BYTES);
+        k_rpn_tail<3><<<grid, kThreads, TailGeom<3>::SMEM_BYTES, stream>>>(x_hi, x_lo, m1_hi, m1_lo, m2_hi, m2_lo, p);
+    } else {
+        B2S_SMEM_OPT_IN(k_rpn_tail<1>, TailGeom<1>::SMEM_BYTES);
+        k_rpn_tail<1><<<grid, kThreads, TailGeom<1>::SMEM_BYTES, stream>>>(x_hi, x_hi, m1_hi, m1_hi, m2_hi, m2_hi, p);
+    }
     B2S_LAUNCH_OK();
     return 0;
+}
+
+// the 3xF16 form
+extern "C" int b2s_rpn_tail_tc_ex(const b2s_half *in_hi, const b2s_half *in_lo, int B, int H, int W, int Cin,
+                                  const b2s_half *w1_hi, const b2s_half *w1_lo, int Cmid, const float *scale1,
+                                  const float *shift1, const b2s_half *w2_hi, const b2s_half *w2_lo, int cout2,
+                                  int n_pad2, const float *scale2, const float *shift2, float *out, int out_stride,
+                                  const int *work_list, const int *work_count, const int *bg_list, const int *bg_count,
+                                  const float *field, int margin, unsigned *status_dev, void *stream)
+{
+    return b2s_rpn_tail_tc_ex2(in_hi, in_lo, B, H, W, Cin, w1_hi, w1_lo, Cmid, scale1, shift1, w2_hi, w2_lo, cout2, n_pad2,
+                               scale2, shift2, out, out_stride, work_list, work_count, bg_list, bg_count, field, margin, 3,
+                               status_dev, stream);
 }
 
 extern "C" int b2s_rpn_tail_tc(const b2s_half *in_hi, const b2s_half *in_lo, int B, int H, int W, int Cin,

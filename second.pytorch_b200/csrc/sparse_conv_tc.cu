@@ -29,6 +29,10 @@
 //               Consumers only wait on full stages and release them: a consumer warp that also issued the weights
 //               would wait for the OTHER warpgroup to release each stage, tying the two together on every K block
 //               (that cost 25-35 % of the time of every layer but the last, 3x1x1 one, on H100).
+//
+// P = products per K block: 3 (3xF16, above) or 1 (the f16 mode, b2s_sparse_conv_tc_plan_ex with products = 1): one
+// fp16 plane per operand, so the gather copies hi rows only, a stage holds [A_hi | W_hi], each K step is one wgmma
+// A_hi*W_hi of width N, and the epilogue writes one rounded fp16 plane.
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -91,8 +95,8 @@ __device__ __forceinline__ uint32_t kb_mask_of(uint32_t offsets, int num_kb)
     return m ? m : 1u;
 }
 
-// CIN in {8, 16, 32, 64}; COUT in {16, 32, 64}
-template <int CIN, int COUT>
+// CIN in {8, 16, 32, 64}; COUT in {16, 32, 64}; P in {3, 1}
+template <int CIN, int COUT, int P>
 __global__ void __launch_bounds__(kThreads, 1)
 k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
                  const SpParams p)
@@ -107,12 +111,13 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
     constexpr int CHAIN_KB = PACK > 1 ? 2 : GROUP;            // K blocks per accumulation chain (short chains)
     constexpr uint32_t CHAIN_BITS = (1u << CHAIN_KB) - 1u;
     constexpr uint32_t B_TILE_BYTES = N * BLOCK_K * ELEM_BYTES;
-    constexpr uint32_t STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
+    static_assert(P == 3 || P == 1, "products per K block: 3 (3xF16) or 1 (f16)");
+    constexpr uint32_t STAGE_BYTES = P == 3 ? 2 * A_TILE_BYTES + 2 * B_TILE_BYTES : A_TILE_BYTES + B_TILE_BYTES;
     // B-operand concatenation: the stage holds W_hi (N rows) directly followed by W_lo (N rows), so ONE wgmma with
     // N' = 2N computes A_hi*W_hi (accumulator columns [0,N)) and A_hi*W_lo (columns [N,2N)); a second one (N' = N, the
     // first half of the same accumulator registers) adds A_lo*W_hi into columns [0,N).  8 instead of 12 MMAs per K block
     // for the same products.  The drain adds the two halves.
-    constexpr int R = N;                                      // accumulator registers per thread: 64 rows x 2N
+    constexpr int R = P == 3 ? N : N / 2;                     // accumulator registers per thread: 64 rows x 2N (x N)
     static_assert(N % 16 == 0 && B_TILE_BYTES % 1024 == 0, "wgmma N / swizzle atoms");
 
     extern __shared__ uint8_t smem_raw[];
@@ -162,7 +167,7 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
         const int ko = (int)chunk / CPO;                       // offset inside the pack this lane's chunk belongs to
         const char *src_base = reinterpret_cast<const char *>(p.in_hi) + (((int)chunk % CPO) * 16);
         asm volatile("" : "+l"(src_base));                     // one 64-bit register (not base + lane part re-added per copy)
-        const long long lo_delta = reinterpret_cast<const char *>(p.in_lo) - reinterpret_cast<const char *>(p.in_hi);
+        const long long lo_delta = P == 3 ? reinterpret_cast<const char *>(p.in_lo) - reinterpret_cast<const char *>(p.in_hi) : 0;
         const uint32_t row_bytes = (uint32_t)p.in_stride * ELEM_BYTES;       // rows_in * row_bytes < 2^32 (checked on the host)
         const int grid = (int)gridDim.x;
         const int *__restrict__ nbr = p.nbr;
@@ -253,11 +258,28 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
             // the K block's weights: its expect_tx arrival is the "+ 1" of the stage's bar_full count
             if (half == 0 && lane == 0) {
                 uint8_t *st = smem + (size_t)my_stage * STAGE_BYTES;
-                mbar_arrive_expect_tx(&bar_full[my_stage], 2 * B_TILE_BYTES);
-                tma_load_3d(st + 2 * A_TILE_BYTES, &map_w_hi, &bar_full[my_stage], 0, 0, kb_cur);
-                tma_load_3d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_w_lo, &bar_full[my_stage], 0, 0, kb_cur);
+                if constexpr (P == 3) {
+                    mbar_arrive_expect_tx(&bar_full[my_stage], 2 * B_TILE_BYTES);
+                    tma_load_3d(st + 2 * A_TILE_BYTES, &map_w_hi, &bar_full[my_stage], 0, 0, kb_cur);
+                    tma_load_3d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_w_lo, &bar_full[my_stage], 0, 0, kb_cur);
+                } else {
+                    mbar_arrive_expect_tx(&bar_full[my_stage], B_TILE_BYTES);
+                    tma_load_3d(st + A_TILE_BYTES, &map_w_hi, &bar_full[my_stage], 0, 0, kb_cur);
+                }
             }
-            if (lo_delta == (long long)(CIN * ELEM_BYTES)) {
+            if constexpr (P == 1) {
+                // hi rows only
+#pragma unroll
+                for (int i = 0; i < RI; ++i) {
+                    const char *g = src_base + (unsigned long long)(uint32_t)max(nb_cur[i], 0) * row_bytes;
+                    asm volatile(
+                        "{\n\t.reg .pred p;\n\t"
+                        "setp.ne.b32 p, %3, 0;\n\t"
+                        "@p cp.async.cg.shared.global [%0], [%1], 16, %2;\n\t}"
+                        ::"r"(sa + ((i & 1) ? dst_odd : dst_even) + (uint32_t)i * 512u), "l"(g), "r"((valid >> i & 1u) << 4),
+                          "r"(need & (1u << i)) : "memory");
+                }
+            } else if (lo_delta == (long long)(CIN * ELEM_BYTES)) {
                 // interleaved rows [hi Cin | lo Cin]: the lo copy is the hi address + an immediate
 #pragma unroll
                 for (int i = 0; i < RI; ++i) {
@@ -317,7 +339,7 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
         const uint32_t a_off = (uint32_t)cg * 64u * 128u;
         int stage = 0;
         uint32_t phase = 0;
-        float acc[R], sum[R / 2];
+        float acc[R], sum[N / 2];
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             uint32_t kbm = tile_kbm(tile);
             // bit set = this K block is the last one of its accumulation chain present in the tile
@@ -327,7 +349,7 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
                 if (m_) ce |= 0x80000000u >> __clz(m_);
             }
 #pragma unroll
-            for (int j = 0; j < R / 2; ++j) sum[j] = 0.f;
+            for (int j = 0; j < N / 2; ++j) sum[j] = 0.f;
             uint32_t fresh = 1;                                 // the next MMA opens an accumulation chain
             while (kbm) {
                 const uint32_t low = kbm & (0u - kbm);
@@ -335,14 +357,24 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
                 mbar_wait(&bar_full[stage], phase);
                 fence_proxy_async();                            // gathered rows were written by cp.async (generic proxy)
                 const uint32_t sa = smem0 + (uint32_t)stage * STAGE_BYTES;
-                const uint64_t a_hi = make_desc_sw128(sa + a_off), a_lo = make_desc_sw128(sa + A_TILE_BYTES + a_off);
-                const uint64_t b_hl = make_desc_sw128(sa + 2 * A_TILE_BYTES);   // [W_hi; W_lo], 2N rows
-                wgmma_fence();
+                if constexpr (P == 3) {
+                    const uint64_t a_hi = make_desc_sw128(sa + a_off), a_lo = make_desc_sw128(sa + A_TILE_BYTES + a_off);
+                    const uint64_t b_hl = make_desc_sw128(sa + 2 * A_TILE_BYTES);   // [W_hi; W_lo], 2N rows
+                    wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
-                    const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
-                    wgmma_ss<2 * N>(acc, a_hi + koff, b_hl + koff, (fresh && k == 0) ? 0u : 1u);
-                    wgmma_ss<N>(acc, a_lo + koff, b_hl + koff, 1);
+                    for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+                        const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                        wgmma_ss<2 * N>(acc, a_hi + koff, b_hl + koff, (fresh && k == 0) ? 0u : 1u);
+                        wgmma_ss<N>(acc, a_lo + koff, b_hl + koff, 1);
+                    }
+                } else {
+                    const uint64_t a_hi = make_desc_sw128(sa + a_off), b_hi = make_desc_sw128(sa + A_TILE_BYTES);
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+                        const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                        wgmma_ss<N>(acc, a_hi + koff, b_hi + koff, (fresh && k == 0) ? 0u : 1u);
+                    }
                 }
                 wgmma_commit();
                 wgmma_wait_all();
@@ -353,9 +385,14 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 fresh = (ce & low) ? 1u : 0u;
                 if (fresh) {
-                    // columns [0,N) hold A_hi*W_hi + A_lo*W_hi, the same columns of the second half A_hi*W_lo
+                    if constexpr (P == 3) {
+                        // columns [0,N) hold A_hi*W_hi + A_lo*W_hi, the same columns of the second half A_hi*W_lo
 #pragma unroll
-                    for (int j = 0; j < R / 2; ++j) sum[j] = __fadd_rn(__fadd_rn(sum[j], acc[j]), acc[R / 2 + j]);
+                        for (int j = 0; j < R / 2; ++j) sum[j] = __fadd_rn(__fadd_rn(sum[j], acc[j]), acc[R / 2 + j]);
+                    } else {
+#pragma unroll
+                        for (int j = 0; j < R; ++j) sum[j] = __fadd_rn(sum[j], acc[j]);
+                    }
                 }
             }
             // epilogue: rows m0 = 64 cg + 16 wl + lane/4 and m0 + 8 of the tile, per 8-column block j the channel pair
@@ -372,12 +409,12 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
                     float x0 = fmaf(sum[4 * j + 2 * rh], s_scale[c], s_shift[c]);
                     float x1 = fmaf(sum[4 * j + 2 * rh + 1], s_scale[c + 1], s_shift[c + 1]);
                     if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-                    if (p.out_lo) {
+                    if (P == 1 || p.out_lo) {
                         range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
                         const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
                         const size_t o = (size_t)row * p.out_stride + c;
                         *reinterpret_cast<uint32_t *>(reinterpret_cast<__half *>(p.out_hi) + o) = __byte_perm(p0, p1, 0x5410);
-                        *reinterpret_cast<uint32_t *>(p.out_lo + o) = __byte_perm(p0, p1, 0x7632);
+                        if constexpr (P == 3) *reinterpret_cast<uint32_t *>(p.out_lo + o) = __byte_perm(p0, p1, 0x7632);
                     } else {
                         *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out_hi) + (size_t)row * N + c) = make_float2(x0, x1);
                     }
@@ -388,15 +425,15 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
     }
 }
 
-template <int CIN, int COUT>
+template <int CIN, int COUT, int P>
 int launch(const CUtensorMap &w_hi, const CUtensorMap &w_lo, const SpParams &p, int num_sms, cudaStream_t stream)
 {
-    constexpr size_t stage = 2 * A_TILE_BYTES + 2 * (size_t)COUT * BLOCK_K * ELEM_BYTES;
+    constexpr size_t stage = (P == 3 ? 2 : 1) * (A_TILE_BYTES + (size_t)COUT * BLOCK_K * ELEM_BYTES);
     size_t smem = stage * STAGES + 1024;
-    B2S_SMEM_OPT_IN((k_sparse_conv_tc<CIN, COUT>), smem);
+    B2S_SMEM_OPT_IN((k_sparse_conv_tc<CIN, COUT, P>), smem);
     int tiles_cap = (p.cap_out + BLOCK_M - 1) / BLOCK_M;
     int grid = tiles_cap < num_sms ? tiles_cap : num_sms;
-    k_sparse_conv_tc<CIN, COUT><<<grid, kThreads, smem, stream>>>(w_hi, w_lo, p);
+    k_sparse_conv_tc<CIN, COUT, P><<<grid, kThreads, smem, stream>>>(w_hi, w_lo, p);
     B2S_LAUNCH_OK();
     return 0;
 }
@@ -410,19 +447,25 @@ extern "C" int b2s_sparse_conv_tc_supported(int cin, int cout)
 
 // Weight layout: Cin = 64: [K][Cout][64]; Cin < 64 (8, 16, 32): packed [ceil(K / (64/Cin))][Cout][64] with column
 // (offset-in-pack * Cin + cin) and zero columns for offsets >= K (b2second/tc.py: pack_sparse_weights).
-extern "C" int b2s_sparse_conv_tc_plan(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in, int cin,
-                                       const b2s_half *w_hi, const b2s_half *w_lo, const int *nbr, int K,
-                                       const int *num_out_dev, int cap_out, const int *perm, const unsigned *tile_mask,
-                                       const float *scale, const float *shift, int relu, void *out_hi, b2s_half *out_lo,
-                                       int out_stride, int cout, unsigned *status_dev, void *stream_)
+// products = 3: 3xF16 hi/lo planes (out_lo == NULL: fp32 rows).  products = 1: the f16 mode -- feat_lo, w_lo and
+// out_lo must be NULL, and the output is one fp16 plane in out_hi.
+extern "C" int b2s_sparse_conv_tc_plan_ex(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in,
+                                          int cin, const b2s_half *w_hi, const b2s_half *w_lo, const int *nbr, int K,
+                                          const int *num_out_dev, int cap_out, const int *perm, const unsigned *tile_mask,
+                                          const float *scale, const float *shift, int relu, void *out_hi,
+                                          b2s_half *out_lo, int out_stride, int cout, int products, unsigned *status_dev,
+                                          void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(products == 3 || (products == 1 && feat_lo == nullptr && w_lo == nullptr && out_lo == nullptr),
+                "b2s_sparse_conv_tc: products must be 3 (3xF16) or 1 (f16, no lo planes)");
+    if (products == 1) feat_lo = feat_hi;           // (alignment checks below; the f16 kernel never reads it)
     B2S_REQUIRE(b2s_sparse_conv_tc_supported(cin, cout),
                 "b2s_sparse_conv_tc: built for Cin in {8, 16, 32, 64}, Cout in {16, 32, 64} (others: b2s_sparse_conv)");
     B2S_REQUIRE(K >= 1 && K <= 27 && cap_out >= 0 && rows_in >= 0, "b2s_sparse_conv_tc: K must be 1..27");
     B2S_REQUIRE(in_stride >= cin && in_stride % 8 == 0 && ((uintptr_t)feat_hi & 15) == 0 && ((uintptr_t)feat_lo & 15) == 0,
                 "b2s_sparse_conv_tc: input rows must be 16-byte aligned (in_stride multiple of 8 halves)");
-    B2S_REQUIRE(out_lo == nullptr || (out_stride >= cout && out_stride % 8 == 0 && ((uintptr_t)out_hi & 15) == 0 &&
+    B2S_REQUIRE((products == 3 && out_lo == nullptr) || (out_stride >= cout && out_stride % 8 == 0 && ((uintptr_t)out_hi & 15) == 0 &&
                                       ((uintptr_t)out_lo & 15) == 0),
                 "b2s_sparse_conv_tc: output rows must be 16-byte aligned (out_stride multiple of 8 halves)");
     B2S_REQUIRE((unsigned long long)rows_in * (unsigned long long)in_stride * ELEM_BYTES < (1ull << 32),
@@ -436,7 +479,8 @@ extern "C" int b2s_sparse_conv_tc_plan(const b2s_half *feat_hi, const b2s_half *
         cuuint64_t dims[3] = {BLOCK_K, (cuuint64_t)cout, nkb};
         cuuint64_t str[2] = {BLOCK_K * ELEM_BYTES, (cuuint64_t)cout * BLOCK_K * ELEM_BYTES};
         cuuint32_t box[3] = {BLOCK_K, (cuuint32_t)cout, 1};
-        if (make_map(&m_hi, w_hi, 3, dims, str, box) || make_map(&m_lo, w_lo, 3, dims, str, box)) return -1;
+        if (make_map(&m_hi, w_hi, 3, dims, str, box) || (products == 3 && make_map(&m_lo, w_lo, 3, dims, str, box)))
+            return -1;
     }
     SpParams p;
     p.in_hi = reinterpret_cast<const __half *>(feat_hi); p.in_lo = reinterpret_cast<const __half *>(feat_lo);
@@ -444,12 +488,27 @@ extern "C" int b2s_sparse_conv_tc_plan(const b2s_half *feat_hi, const b2s_half *
     p.nbr = nbr; p.n_out_dev = num_out_dev; p.cap_out = cap_out; p.K = K;
     p.perm = perm; p.tile_mask = tile_mask;
     p.relu = relu; p.scale = scale; p.shift = shift; p.out_hi = out_hi; p.out_lo = reinterpret_cast<__half *>(out_lo);
-#define B2S_TC_CASE(CI, CO) if (cin == CI && cout == CO) return launch<CI, CO>(m_hi, m_lo, p, num_sms, stream);
+#define B2S_TC_CASE(CI, CO)                                                                         \
+    if (cin == CI && cout == CO)                                                                    \
+        return products == 1 ? launch<CI, CO, 1>(m_hi, m_hi, p, num_sms, stream)                    \
+                             : launch<CI, CO, 3>(m_hi, m_lo, p, num_sms, stream);
     B2S_TC_CASE(64, 64) B2S_TC_CASE(64, 32) B2S_TC_CASE(64, 16) B2S_TC_CASE(32, 64) B2S_TC_CASE(32, 32) B2S_TC_CASE(32, 16)
     B2S_TC_CASE(16, 64) B2S_TC_CASE(16, 32) B2S_TC_CASE(16, 16) B2S_TC_CASE(8, 64) B2S_TC_CASE(8, 32) B2S_TC_CASE(8, 16)
 #undef B2S_TC_CASE
     b2s_set_error("b2s_sparse_conv_tc: Cin=%d Cout=%d not built", cin, cout);
     return -2;
+}
+
+// the 3xF16 form
+extern "C" int b2s_sparse_conv_tc_plan(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in, int cin,
+                                       const b2s_half *w_hi, const b2s_half *w_lo, const int *nbr, int K,
+                                       const int *num_out_dev, int cap_out, const int *perm, const unsigned *tile_mask,
+                                       const float *scale, const float *shift, int relu, void *out_hi, b2s_half *out_lo,
+                                       int out_stride, int cout, unsigned *status_dev, void *stream)
+{
+    return b2s_sparse_conv_tc_plan_ex(feat_hi, feat_lo, in_stride, rows_in, cin, w_hi, w_lo, nbr, K, num_out_dev, cap_out,
+                                      perm, tile_mask, scale, shift, relu, out_hi, out_lo, out_stride, cout, 3, status_dev,
+                                      stream);
 }
 
 extern "C" int b2s_sparse_conv_tc(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in, int cin,

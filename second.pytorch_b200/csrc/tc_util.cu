@@ -6,7 +6,9 @@
 
 namespace {
 
-// one thread per (row, 8-channel group of the OUTPUT row): reads up to 8 floats, writes 16 bytes per plane
+// one thread per (row, 8-channel group of the OUTPUT row): reads up to 8 floats, writes 16 bytes per plane (P = 1: the
+// hi plane only)
+template <int P>
 __global__ void k_split_f16(const float *__restrict__ x, __half *__restrict__ hi, __half *__restrict__ lo,
                             const int *__restrict__ n_rows_dev, int cap_rows, int row_floats, int out_channels,
                             int out_stride)
@@ -27,7 +29,7 @@ __global__ void k_split_f16(const float *__restrict__ x, __half *__restrict__ hi
             l[j] = __byte_perm(pa, pb, 0x7632);
         }
         *reinterpret_cast<uint4 *>(hi + row * out_stride + c0) = make_uint4(h[0], h[1], h[2], h[3]);
-        *reinterpret_cast<uint4 *>(lo + row * out_stride + c0) = make_uint4(l[0], l[1], l[2], l[3]);
+        if constexpr (P == 3) *reinterpret_cast<uint4 *>(lo + row * out_stride + c0) = make_uint4(l[0], l[1], l[2], l[3]);
     }
 }
 
@@ -56,20 +58,34 @@ inline int grid_for(long long items)
 // x [rows, row_floats] fp32 -> hi = fp16(x), lo = fp16(x - hi): out_channels halves per row and plane (>= row_floats,
 // multiple of 8; columns past row_floats are written as zeros), rows out_stride halves apart (>= out_channels,
 // multiple of 8 -- e.g. 2*out_channels for interleaved [row][hi | lo] storage).  rows = *num_rows_dev (NULL: cap_rows).
-extern "C" int b2s_split_f16(const float *x, b2s_half *hi, b2s_half *lo, const int *num_rows_dev, int cap_rows,
-                             int row_floats, int out_channels, int out_stride, void *stream_)
+// products = 1 (the f16 mode): lo must be NULL, only hi = fp16(x) is written.
+extern "C" int b2s_split_f16_ex(const float *x, b2s_half *hi, b2s_half *lo, const int *num_rows_dev, int cap_rows,
+                                int row_floats, int out_channels, int out_stride, int products, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(products == 3 || (products == 1 && lo == nullptr),
+                "b2s_split_f16: products must be 3 (hi/lo planes) or 1 (f16, no lo plane)");
     B2S_REQUIRE(row_floats >= 1 && out_channels >= row_floats && out_channels % 8 == 0 && out_stride >= out_channels &&
                     out_stride % 8 == 0 && cap_rows >= 0,
                 "b2s_split_f16: out_channels / out_stride must be multiples of 8, out_stride >= out_channels >= row_floats");
     B2S_REQUIRE(((uintptr_t)hi & 15) == 0 && ((uintptr_t)lo & 15) == 0, "b2s_split_f16: planes must be 16-byte aligned");
     const long long items = (long long)cap_rows * (out_channels / 8);
     if (items == 0) return 0;
-    k_split_f16<<<grid_for(items), 256, 0, stream>>>(x, reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo),
-                                                     num_rows_dev, cap_rows, row_floats, out_channels, out_stride);
+    if (products == 1)
+        k_split_f16<1><<<grid_for(items), 256, 0, stream>>>(x, reinterpret_cast<__half *>(hi), nullptr, num_rows_dev,
+                                                            cap_rows, row_floats, out_channels, out_stride);
+    else
+        k_split_f16<3><<<grid_for(items), 256, 0, stream>>>(x, reinterpret_cast<__half *>(hi),
+                                                            reinterpret_cast<__half *>(lo), num_rows_dev, cap_rows,
+                                                            row_floats, out_channels, out_stride);
     B2S_LAUNCH_OK();
     return 0;
+}
+
+extern "C" int b2s_split_f16(const float *x, b2s_half *hi, b2s_half *lo, const int *num_rows_dev, int cap_rows,
+                             int row_floats, int out_channels, int out_stride, void *stream)
+{
+    return b2s_split_f16_ex(x, hi, lo, num_rows_dev, cap_rows, row_floats, out_channels, out_stride, 3, stream);
 }
 
 // hi/lo rows of in_stride halves -> x [rows, row_floats] fp32 = hi + lo (exact).  row_floats even.

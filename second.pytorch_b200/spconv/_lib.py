@@ -50,6 +50,8 @@ SIGNATURES = {
     "b2s_pfn_ex": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
                            c_void_p, c_int, c_float, c_float, c_float, c_float, c_int, c_void_p, c_void_p]),
     "b2s_crop_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "b2s_crop_nhwc_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                 c_void_p]),
     "b2s_decode_filter": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                   c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                   c_int, c_void_p, c_void_p]),
@@ -61,7 +63,11 @@ SIGNATURES = {
     "b2s_sparse_conv_tc_plan": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                         c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                         c_int, c_int, c_void_p, c_void_p]),
+    "b2s_sparse_conv_tc_plan_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                           c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                           c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b2s_split_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "b2s_split_f16_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "b2s_merge_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b2s_split_f16_autoscale": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
                                         c_void_p]),
@@ -91,6 +97,8 @@ SIGNATURES = {
                               c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2s_to_bev_tc_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                  c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2s_to_bev_tc_ex2": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                  c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "b2s_rpn_strip_bands": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p]),
     "b2s_rpn_bg_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -109,11 +117,19 @@ SIGNATURES = {
                                   c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                   c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                   c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "b2s_conv2d_tc_ex3": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
+                                  c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                  c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b2s_rpn_tail_tc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                 c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "b2s_rpn_tail_tc_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
                                    c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "b2s_rpn_tail_tc_ex2": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                    c_void_p]),
     "b2s_decode_filter_strided": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_longlong, ctypes.c_longlong,
                                           ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                           c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
