@@ -393,12 +393,10 @@ class InferenceEngine:
                 rb["tile_mask"] = torch.zeros((cap_rb + 127) // 128, dtype=torch.int32, device=dev)
                 rb["row_mask"] = torch.zeros(cap_rb, dtype=torch.int32, device=dev)    # written by the rulebook builder
                 rb["perm"] = torch.zeros(cap_rb, dtype=torch.int32, device=dev)
-            # tensor-pipe core (csrc/sparse_conv_tc.cu): the library says which (Cin, Cout) it was built for;
-            # 3-/4-feature input layers are zero-padded to 8 channels.  Everything else: fp32 FMA core.
-            cin_tc = _tc.sparse_tc_cin(ls["cin"])
+            # tensor-pipe core (csrc/sparse_conv_tc.cu) where tc.sparse_tc_channels allows; else fp32 FMA core
+            cin_tc = _tc.sparse_tc_channels(self.lib, ls["cin"], ls["cout"], K) if self.sparse_impl == "tc" else None
             lyr["cin_tc"] = cin_tc
-            lyr["tc"] = bool(self.sparse_impl == "tc" and cin_tc is not None and
-                             self.lib.b2s_sparse_conv_tc_supported(cin_tc, ls["cout"]))
+            lyr["tc"] = cin_tc is not None
             self.layers.append(lyr)
         # a level's coordinate hash is only built when some SubM rulebook still looks rows up by hash
         for lyr in self.layers:

@@ -59,6 +59,16 @@ def sparse_tc_cin(cin):
     return None
 
 
+def sparse_tc_channels(lib, cin, cout, K):
+    """input width the tensor-core sparse kernel sees for a (cin -> cout, K offsets) layer -- sparse_tc_cin(cin) -- or
+    None when the layer runs on the fp32 FMA kernel (b2s_sparse_conv): a width the library was not built for
+    (b2s_sparse_conv_tc_supported) or more than 27 kernel offsets, which only the FMA kernel covers."""
+    cin_tc = sparse_tc_cin(cin)
+    if cin_tc is None or K > 27 or not lib.b2s_sparse_conv_tc_supported(cin_tc, cout):
+        return None
+    return cin_tc
+
+
 def wants_tile_plan(subm, K):
     """whether a rulebook gets a tile plan (csrc/sparse_plan.cu: rows grouped by neighbourhood shape + per-tile offset
     masks) for b2s_sparse_conv_tc_plan.  SubM rulebooks with more than 3 offsets do: an ``indice_key`` shares them

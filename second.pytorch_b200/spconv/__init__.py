@@ -319,6 +319,33 @@ def _pack_tc_weights(w, transpose=False, flip=False):
     return hi, lo, sc[0:1], sc[1:2]
 
 
+def _conv_tc(x, w, table, K, n_dev, n_out, plan, scale, shift, relu, out, out_lo=None):
+    """one b2s_sparse_conv_tc_plan launch for the first n_out rows of `table`: fp16 input planes x = (hi, lo, row stride)
+    as wide as Cin, packed weight planes w = (hi, lo), plan = ops.tile_plan's (perm, tile_mask); `out` as wide as Cout
+    is fp32 rows, or with `out_lo` the hi plane of fp16 hi/lo rows.  -> the status word, None when there are no rows."""
+    if n_out == 0:
+        return None
+    (hi, lo, stride), (w_hi, w_lo), (perm, tmask) = x, w, plan
+    status = torch.zeros(1, dtype=torch.int32, device=out.device)
+    _lib.check(_lib.load().b2s_sparse_conv_tc_plan(
+        _lib.ptr(hi), _lib.ptr(lo), stride, hi.shape[0], hi.shape[1], _lib.ptr(w_hi), _lib.ptr(w_lo), _lib.ptr(table), K,
+        _lib.ptr(n_dev), n_out, _lib.ptr(perm), _lib.ptr(tmask), _lib.ptr(scale), _lib.ptr(shift), int(relu),
+        _lib.ptr(out), _lib.ptr(out_lo), out.stride(0), out.shape[1], _lib.ptr(status), _lib.stream()),
+        "b2s_sparse_conv_tc_plan")
+    return status
+
+
+def _conv_fma(x, w, table, n_dev, n_out, scale, shift, relu, out):
+    """one b2s_sparse_conv launch (fp32 FMA) over `table` for its first n_out rows: fp32 rows x through w [K, Cin, Cout]
+    into out [n_out, Cout]"""
+    if n_out == 0:
+        return
+    K, cin, cout = w.shape
+    _lib.check(_lib.load().b2s_sparse_conv(_lib.ptr(x), cin, _lib.ptr(w), _lib.ptr(table), K, _lib.ptr(n_dev), n_out,
+                                           _lib.ptr(scale), _lib.ptr(shift), int(relu), _lib.ptr(out), cout,
+                                           _lib.stream()), "b2s_sparse_conv")
+
+
 def _triple(v):
     if isinstance(v, (list, tuple, np.ndarray)):
         assert len(v) == 3
@@ -419,11 +446,8 @@ class SparseConvolution(SparseModule):
             _lib.require_cuda(feats, "SparseConvTensor.features")
             out._features = _SparseConvFunction.apply(feats.contiguous().float(), self.weight, self.bias, self, rb)
             return out
-        from b2second import tc as _tc
-        cin_tc = _tc.sparse_tc_cin(self.in_channels)
-        use_tc = (USE_TENSOR_CORES and cin_tc is not None
-                  and bool(lib.b2s_sparse_conv_tc_supported(cin_tc, self.out_channels)))
-        if use_tc:
+        cin_tc = self._wgrad_tc_cin(lib, K)
+        if cin_tc is not None:
             # tensor pipe (wgmma, 3xF16 split): fp16 hi/lo rows in, fp16 hi/lo rows out
             if input._hilo is not None and input._hilo[0].shape[1] == cin_tc:
                 hi, lo, stride = input._hilo
@@ -442,29 +466,18 @@ class SparseConvolution(SparseModule):
             scale_tc = inv if scale is None else (scale / ws).contiguous()
             obuf = torch.empty(max(n_out, 1), 2, self.out_channels, dtype=torch.float16, device=dev)
             o_hi, o_lo = obuf[:, 0], obuf[:, 1]
-            if n_out > 0:
-                status = torch.zeros(1, dtype=torch.int32, device=dev)
-                perm, tmask = ops.tile_plan(rb)        # SubM rulebooks: K blocks no row of a tile needs are skipped
-                _lib.check(lib.b2s_sparse_conv_tc_plan(
-                    _lib.ptr(hi), _lib.ptr(lo), stride, hi.shape[0], cin_tc, _lib.ptr(w_hi), _lib.ptr(w_lo),
-                    _lib.ptr(rb.nbr), K, _lib.ptr(rb.num_out_dev), n_out, _lib.ptr(perm), _lib.ptr(tmask),
-                    _lib.ptr(scale_tc), _lib.ptr(shift), 1 if relu else 0, _lib.ptr(o_hi), _lib.ptr(o_lo),
-                    2 * self.out_channels, self.out_channels, _lib.ptr(status), _lib.stream()), "b2s_sparse_conv_tc_plan")
-                out._status = status
+            # SubM rulebooks get a tile plan: K blocks no row of a tile needs are skipped
+            out._status = _conv_tc((hi, lo, stride), (w_hi, w_lo), rb.nbr, K, rb.num_out_dev, n_out, ops.tile_plan(rb),
+                                   scale_tc, shift, relu, o_hi, o_lo)
             out._hilo = (o_hi[:n_out], o_lo[:n_out], 2 * self.out_channels)
             out._keep = obuf
             return out
         feats = input.features
         _lib.require_cuda(feats, "SparseConvTensor.features")
         feats = feats.contiguous().float()
-        out_feats = torch.empty(n_out, self.out_channels, dtype=torch.float32, device=dev)
+        out._features = torch.empty(n_out, self.out_channels, dtype=torch.float32, device=dev)
         w = self.weight.detach().float().contiguous().view(K, self.in_channels, self.out_channels)
-        if n_out > 0:
-            _lib.check(lib.b2s_sparse_conv(_lib.ptr(feats), self.in_channels, _lib.ptr(w), _lib.ptr(rb.nbr), K,
-                                           _lib.ptr(rb.num_out_dev), n_out, _lib.ptr(scale), _lib.ptr(shift),
-                                           1 if relu else 0, _lib.ptr(out_feats), self.out_channels,
-                                           _lib.stream()), "b2s_sparse_conv")
-        out._features = out_feats
+        _conv_fma(feats, w, rb.nbr, rb.num_out_dev, n_out, scale, shift, relu, out._features)
         return out
 
     # ---- training (b2second.training.enable_sparse_backward sets _b2s_backward) --------------------------------------
@@ -488,28 +501,18 @@ class SparseConvolution(SparseModule):
             hi, lo, stride, inv_x = split.planes()
             w_hi, w_lo, ws, inv = self._tc_weights(cin_tc)
             scale = inv * inv_x                                        # powers of two: exact, no host sync
-            status = torch.zeros(1, dtype=torch.int32, device=dev)
-            perm, tmask = ops.tile_plan(rb)
-            _lib.check(lib.b2s_sparse_conv_tc_plan(
-                _lib.ptr(hi), _lib.ptr(lo), stride, hi.shape[0], cin_tc, _lib.ptr(w_hi), _lib.ptr(w_lo),
-                _lib.ptr(rb.nbr), K, _lib.ptr(rb.num_out_dev), n_out, _lib.ptr(perm), _lib.ptr(tmask), _lib.ptr(scale),
-                _lib.ptr(shift), 0, _lib.ptr(out), None, self.out_channels, self.out_channels, _lib.ptr(status),
-                _lib.stream()), "b2s_sparse_conv_tc_plan")
+            _conv_tc((hi, lo, stride), (w_hi, w_lo), rb.nbr, K, rb.num_out_dev, n_out, ops.tile_plan(rb), scale, shift,
+                     False, out)
             return out, split
         w = self.weight.detach().float().contiguous().view(K, self.in_channels, self.out_channels)
-        _lib.check(lib.b2s_sparse_conv(_lib.ptr(feats), self.in_channels, _lib.ptr(w), _lib.ptr(rb.nbr), K,
-                                       _lib.ptr(rb.num_out_dev), n_out, None, _lib.ptr(shift), 0, _lib.ptr(out),
-                                       self.out_channels, _lib.stream()), "b2s_sparse_conv")
+        _conv_fma(feats, w, rb.nbr, rb.num_out_dev, n_out, None, shift, False, out)
         return out, None
 
     def _wgrad_tc_cin(self, lib, K):
-        """channel count of the tensor-pipe forward / weight gradient (the input padded to 8), or None: fp32 kernels"""
+        """channel count of the tensor-pipe forward / weight gradient (the input padded to 8, tc.sparse_tc_channels), or
+        None: fp32 kernels"""
         from b2second import tc as _tc
-        cin_tc = _tc.sparse_tc_cin(self.in_channels)
-        if (USE_TENSOR_CORES and cin_tc is not None and K <= 27
-                and bool(lib.b2s_sparse_conv_tc_supported(cin_tc, self.out_channels))):
-            return cin_tc
-        return None
+        return _tc.sparse_tc_channels(lib, self.in_channels, self.out_channels, K) if USE_TENSOR_CORES else None
 
     def _dgrad_weights(self, w, flip):
         """packed fp16 hi/lo planes of W'[k] = W[k]^T (flip: W[K-1-k]^T) for the tensor-pipe input gradient, with their
@@ -538,28 +541,23 @@ class SparseConvolution(SparseModule):
             return torch.zeros(n_in, cin, dtype=torch.float32, device=dev)
         flip = rb.subm and all(k % 2 == 1 for k in rb.ksize)
         if flip:
-            table, n_dev, (perm, tmask) = rb.nbr, rb.num_out_dev, ops.tile_plan(rb)
+            table, n_dev, plan = rb.nbr, rb.num_out_dev, ops.tile_plan(rb)
         else:
-            table, perm, tmask = ops.transpose_rulebook(rb, n_in), None, None
+            table, plan = ops.transpose_rulebook(rb, n_in), (None, None)
             n_dev = torch.tensor([n_in], dtype=torch.int32, device=dev)
         dx = torch.empty(n_in, cin, dtype=torch.float32, device=dev)
-        if (USE_TENSOR_CORES and K <= 27 and _tc.sparse_tc_cin(cout) == cout
-                and bool(lib.b2s_sparse_conv_tc_supported(cout, cin))):
+        # the contraction runs Cout -> Cin; dY is not padded, so it takes the tensor pipe only at an unpadded width
+        if USE_TENSOR_CORES and _tc.sparse_tc_channels(lib, cout, cin, K) == cout:
             # dY goes onto the tensor pipe scaled by a power of two picked on the device (gradients are often far below
             # the fp16 normal range); the kernel's epilogue scale undoes both that and the weights' scale
             w_hi, w_lo, ws = self._dgrad_weights(weight, flip)
             g_hi, g_lo, g_stride, inv = (split or _GradSplit(dy)).planes()
             scale = (inv / ws).expand(cin).contiguous()
-            status = torch.zeros(1, dtype=torch.int32, device=dev)
-            _lib.check(lib.b2s_sparse_conv_tc_plan(
-                _lib.ptr(g_hi), _lib.ptr(g_lo), g_stride, g_hi.shape[0], cout, _lib.ptr(w_hi), _lib.ptr(w_lo),
-                _lib.ptr(table), K, _lib.ptr(n_dev), n_in, _lib.ptr(perm), _lib.ptr(tmask), _lib.ptr(scale), None, 0,
-                _lib.ptr(dx), None, cin, cin, _lib.ptr(status), _lib.stream()), "b2s_sparse_conv_tc_plan")
+            _conv_tc((g_hi, g_lo, g_stride), (w_hi, w_lo), table, K, n_dev, n_in, plan, scale, None, False, dx)
             return dx
         w = weight.detach().float().reshape(K, cin, cout)
         wt = (w.flip(0) if flip else w).transpose(1, 2).contiguous()        # [K, Cout, Cin]
-        _lib.check(lib.b2s_sparse_conv(_lib.ptr(dy), cout, _lib.ptr(wt), _lib.ptr(table), K, _lib.ptr(n_dev), n_in, None,
-                                       None, 0, _lib.ptr(dx), cin, _lib.stream()), "b2s_sparse_conv")
+        _conv_fma(dy, wt, table, n_dev, n_in, None, None, False, dx)
         return dx
 
     def _wgrad(self, feats, dy, rb, split=None, x_split=None):
