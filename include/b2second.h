@@ -95,7 +95,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 214
+#define B2S_VERSION 215
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -276,6 +276,13 @@ int b2s_sparse_conv_tc_plan_ex(const b2s_half *feat_hi, const b2s_half *feat_lo,
                                int cap_out, const int *perm, const unsigned *tile_mask, const float *scale,
                                const float *shift, int relu, void *out_hi, b2s_half *out_lo, int out_stride, int cout,
                                int products, unsigned *status_dev, void *stream);
+/* the same with out_fp32: with products = 1 and out_fp32 = 1 the output is fp32 rows [cap_out, cout] in out_hi (the
+ * training forward and input gradient of the f16 mode); out_fp32 must be 0 with products = 3 (out_lo NULL says it). */
+int b2s_sparse_conv_tc_plan_ex2(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in, int cin,
+                                const b2s_half *w_hi, const b2s_half *w_lo, const int *nbr, int K, const int *num_out_dev,
+                                int cap_out, const int *perm, const unsigned *tile_mask, const float *scale,
+                                const float *shift, int relu, void *out_hi, b2s_half *out_lo, int out_stride, int cout,
+                                int products, int out_fp32, unsigned *status_dev, void *stream);
 
 /* fp32 rows <-> fp16 hi/lo planes (hi = fp16 round-to-nearest, lo = fp16-rounded remainder; saturating).
  * split: x [rows, row_floats] -> out_channels halves per row and plane (>= row_floats, multiple of 8, zero padded), rows
@@ -297,6 +304,11 @@ int b2s_split_f16_ex(const float *x, b2s_half *hi, b2s_half *lo, const int *num_
  * sync. */
 int b2s_split_f16_autoscale(const float *x, b2s_half *hi, b2s_half *lo, const int *num_rows_dev, int cap_rows,
                             int row_floats, int out_channels, int out_stride, float *scale_dev, void *stream);
+/* b2s_split_f16_autoscale with products 3 (the same) or 1 (the f16 mode: lo NULL, only hi written, bit-equal to the hi
+ * plane of products = 3; the same scale) */
+int b2s_split_f16_autoscale_ex(const float *x, b2s_half *hi, b2s_half *lo, const int *num_rows_dev, int cap_rows,
+                               int row_floats, int out_channels, int out_stride, float *scale_dev, int products,
+                               void *stream);
 
 /* ---- sparse convolution backward (training) ------------------------------------------------------ */
 /* Input gradient (dgrad) is the forward contraction on a transposed table, computed by b2s_sparse_conv /
@@ -331,6 +343,14 @@ int b2s_sparse_conv_wgrad_tc(const b2s_half *feat_hi, const b2s_half *feat_lo, i
                              int K, const int *num_out_dev, int cap_out, const int *perm, const unsigned *tile_mask,
                              const float *scale_dev, float *dweight, void *workspace, size_t workspace_bytes,
                              void *stream);
+/* b2s_sparse_conv_wgrad_tc with products 3 (the same) or 1 (the f16 mode: feat_lo and dout_lo NULL, one X_hi^T * dY_hi
+ * product per k16 step; staging moves half the bytes).  The workspace (b2s_sparse_conv_wgrad_tc_workspace_bytes), the
+ * tile_mask skipping and the fixed-order slab sums are those of products = 3. */
+int b2s_sparse_conv_wgrad_tc_ex(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in, int cin,
+                                const b2s_half *dout_hi, const b2s_half *dout_lo, int dout_stride, int cout,
+                                const int *nbr, int K, const int *num_out_dev, int cap_out, const int *perm,
+                                const unsigned *tile_mask, const float *scale_dev, float *dweight, void *workspace,
+                                size_t workspace_bytes, int products, void *stream);
 
 /* ---- dense BEV map ----------------------------------------------------------------------------- */
 #define B2S_LAYOUT_NCHW 0 /* out[b, c*D+z, y, x]  (== dense() [B,C,D,H,W] viewed [B,C*D,H,W]) */
@@ -966,6 +986,9 @@ int b2s_train_metrics(const float *cls_preds, int num_class, const void *labels,
  * then the pack and split); no sync. */
 int b2s_pack_sparse_weights(const float *w, int K, int cin, int cout, int transpose, int flip, b2s_half *hi,
                             b2s_half *lo, float *scale_dev, void *stream);
+/* with products 3 (the same) or 1 (the f16 mode: lo NULL, only hi written, bit-equal to the hi plane of products = 3) */
+int b2s_pack_sparse_weights_ex(const float *w, int K, int cin, int cout, int transpose, int flip, b2s_half *hi,
+                               b2s_half *lo, float *scale_dev, int products, void *stream);
 
 /* ---- dense RPN training: 3x3 stride-1 pad-1 convolutions on the tensor pipe (csrc/conv_train.cu) ------------------
  * Forward y = conv(x, W) and input gradient dX = conv(dY, W') with W'[tap] = W[8 - tap]^T are b2s_conv2d_tc_ex
@@ -978,6 +1001,9 @@ int b2s_pack_sparse_weights(const float *w, int K, int cin, int cout, int transp
  * B2S_STATUS_F16_RANGE (status_dev may be NULL).  A memset, two kernels. */
 int b2s_split_halo_f16_autoscale(const float *x, int layout, int batch, int C, int H, int W, b2s_half *hi, b2s_half *lo,
                                  float *scale_dev, unsigned *status_dev, void *stream);
+/* with products 3 (the same) or 1 (the f16 mode: lo NULL, only hi written, bit-equal to the hi plane of products = 3) */
+int b2s_split_halo_f16_autoscale_ex(const float *x, int layout, int batch, int C, int H, int W, b2s_half *hi,
+                                    b2s_half *lo, float *scale_dev, unsigned *status_dev, int products, void *stream);
 /* torch weight w [cout, cin, 3, 3] fp32 -> the b2s_conv2d_tc_ex weight planes, scaled by the power of two s with
  * max|w| * s in (2^12, 2^13] (as b2s_pack_sparse_weights, non-finite weights and the clamp included; scale_dev [3]:
  * [0] = s, [1] = 1/s, [2] scratch).
@@ -987,6 +1013,9 @@ int b2s_split_halo_f16_autoscale(const float *x, int layout, int batch, int C, i
  * multiples of 64.  The epilogue scale of a launch is (the input planes' 2^-e) * (1/s). */
 int b2s_pack_conv2d_weights(const float *w, int cout, int cin, int transpose, b2s_half *hi, b2s_half *lo,
                             float *scale_dev, void *stream);
+/* with products 3 (the same) or 1 (the f16 mode: lo NULL, only hi written, bit-equal to the hi plane of products = 3) */
+int b2s_pack_conv2d_weights_ex(const float *w, int cout, int cin, int transpose, b2s_half *hi, b2s_half *lo,
+                               float *scale_dev, int products, void *stream);
 /* dW[co][ci][ky][kx] = sum_px dY[px][co] * X[px + (ky - 1, kx - 1)][ci] for a 3x3 stride-1 pad-1 conv, in torch's layout
  * [Cout, Cin, 3, 3] fp32, from the halo planes of b2s_split_halo_f16_autoscale (x [B, H+2, W+2, Cin], dout
  * [B, H+2, W+2, Cout], both halos zero), times both planes' 2^-e (x_scale_dev[0] * dout_scale_dev[0], applied as one
@@ -998,6 +1027,13 @@ int b2s_conv2d_wgrad_tc(const b2s_half *x_hi, const b2s_half *x_lo, const b2s_ha
                         int batch, int H, int W, int Cin, int Cout, const float *x_scale_dev,
                         const float *dout_scale_dev, float *dweight, void *workspace, size_t workspace_bytes,
                         void *stream);
+/* b2s_conv2d_wgrad_tc with products 3 (the same) or 1 (the f16 mode: x_lo and dout_lo NULL, one dY_hi*X_hi product per
+ * tap and k16 step; a stage holds the hi planes only).  The same workspace and slab order.  The forward and the input
+ * gradient of the f16 mode are b2s_conv2d_tc_ex3 launches with products = 1 and out_fp32 = 1. */
+int b2s_conv2d_wgrad_tc_ex(const b2s_half *x_hi, const b2s_half *x_lo, const b2s_half *dout_hi, const b2s_half *dout_lo,
+                           int batch, int H, int W, int Cin, int Cout, const float *x_scale_dev,
+                           const float *dout_scale_dev, float *dweight, void *workspace, size_t workspace_bytes,
+                           int products, void *stream);
 
 /* ---- BatchNorm + ReLU in training (csrc/bn_train.cu) --------------------------------------------------------------
  * y = relu(BatchNorm(x)) as torch.nn.BatchNorm1d / BatchNorm2d.forward in train() (affine, track_running_stats, a

@@ -18,6 +18,12 @@ Conv3x3TC, all on the caller's stream without a host sync (the layer can be capt
             the packed weights (b2s_pack_conv2d_weights), fp32 NHWC out, returned as a channels_last NCHW tensor;
   backward  dY -> halo planes of dY * 2^ey -> dX through b2s_conv2d_tc_ex with W'[tap] = W[8 - tap]^T, and dW through
             b2s_conv2d_wgrad_tc from the saved X planes and the dY planes.
+
+``enable(net, products=1)`` (``training.enable_rpn_training(net, precision="f16")``) runs the same layers in the f16 mode:
+every plane is the hi plane alone (the ``*_ex`` splits and packs with products = 1), the forward and input gradient are
+b2s_conv2d_tc_ex3 launches with products = 1 and fp32 output, and the weight gradient is b2s_conv2d_wgrad_tc_ex with
+products = 1 -- one f16 wgmma product per MAC instead of three.  The product count is stored per conv
+(``_b2s_products``).
 """
 import types
 
@@ -91,11 +97,13 @@ def _pad_forward(self, x):
     return x if _active(self._b2s_rpn_conv, x) else nn.ZeroPad2d.forward(self, x)
 
 
-def enable(net):
-    """rebind the covered layers under ``net.rpn`` (or ``net`` itself when it has no ``rpn``); idempotent, never raises
-    on a layer it does not cover.  Returns ``net``."""
+def enable(net, products=3):
+    """rebind the covered layers under ``net.rpn`` (or ``net`` itself when it has no ``rpn``) with ``products`` tensor-pipe
+    products per MAC (3: 3xF16, 1: the f16 mode); idempotent apart from the product count, which a second call sets;
+    never raises on a layer it does not cover.  Returns ``net``."""
     rpn = getattr(net, "rpn", net)
     for conv, pad in select(rpn):
+        conv._b2s_products = products
         if getattr(conv, "_b2s_rpn_train", False):
             continue
         if pad is not None:
@@ -108,9 +116,9 @@ def enable(net):
 
 # ---- planes and weights --------------------------------------------------------------------------------------------
 
-def split_halo(t, status=None):
+def split_halo(t, status=None, products=3):
     """fp32 map [B, C, H, W] (contiguous or channels_last) -> (hi, lo) fp16 [B, H+2, W+2, C] planes of t * 2^e with a zero
-    halo, and 2^-e as a [1] device tensor."""
+    halo, and 2^-e as a [1] device tensor.  products = 1: the hi plane only, lo is None."""
     L, lib = _lib()
     B, C, H, W = (int(v) for v in t.shape)
     if t.is_contiguous():
@@ -119,18 +127,24 @@ def split_halo(t, status=None):
         layout = LAYOUT_NHWC
     else:
         t, layout = t.contiguous(), LAYOUT_NCHW
-    planes = torch.empty(2, B, H + 2, W + 2, C, dtype=torch.float16, device=t.device)
     sc = torch.empty(2, dtype=torch.float32, device=t.device)
+    if products == 1:
+        hi = torch.empty(B, H + 2, W + 2, C, dtype=torch.float16, device=t.device)
+        L.check(lib.b2s_split_halo_f16_autoscale_ex(L.ptr(t), layout, B, C, H, W, L.ptr(hi), None, L.ptr(sc),
+                                                    L.ptr(status), 1, L.stream()), "b2s_split_halo_f16_autoscale_ex")
+        return hi, None, sc[:1]
+    planes = torch.empty(2, B, H + 2, W + 2, C, dtype=torch.float16, device=t.device)
     L.check(lib.b2s_split_halo_f16_autoscale(L.ptr(t), layout, B, C, H, W, L.ptr(planes[0]), L.ptr(planes[1]),
                                              L.ptr(sc), L.ptr(status), L.stream()), "b2s_split_halo_f16_autoscale")
     return planes[0], planes[1], sc[:1]
 
 
-def pack_weights(conv, transpose):
+def pack_weights(conv, transpose, products=3):
     """the b2s_conv2d_tc_ex weight planes of ``conv`` ([G, 9, n_pad, n_in] hi / lo) and 1/s as a [1] device tensor,
-    cached on the weight's (data_ptr, _version) like the sparse convs' planes."""
+    cached on the weight's (data_ptr, _version) and the product count like the sparse convs' planes (products = 1: the
+    hi plane only, lo None)."""
     w = conv.weight
-    key = (w.data_ptr(), w._version, str(w.device), transpose)
+    key = (w.data_ptr(), w._version, str(w.device), transpose, products)
     cache = conv.__dict__.setdefault("_b2s_rpn_planes", {})
     hit = cache.get(transpose)
     if hit is not None and hit[0] == key:
@@ -138,11 +152,18 @@ def pack_weights(conv, transpose):
     L, lib = _lib()
     cout, cin = int(w.shape[0]), int(w.shape[1])
     n_in, n_out = (cout, cin) if transpose else (cin, cout)
-    planes = torch.empty(2, (n_out + 127) // 128, 9, min(n_out, 128), n_in, dtype=torch.float16, device=w.device)
+    planes = torch.empty(2 if products == 3 else 1, (n_out + 127) // 128, 9, min(n_out, 128), n_in, dtype=torch.float16,
+                         device=w.device)
     sc = torch.empty(3, dtype=torch.float32, device=w.device)
     wd = w.detach()
     if not wd.is_contiguous():
         wd = wd.contiguous()
+    if products == 1:
+        L.check(lib.b2s_pack_conv2d_weights_ex(L.ptr(wd), cout, cin, int(transpose), L.ptr(planes[0]), None, L.ptr(sc),
+                                               1, L.stream()), "b2s_pack_conv2d_weights_ex")
+        val = (planes[0], None, sc[1:2])
+        cache[transpose] = (key, val)
+        return val
     L.check(lib.b2s_pack_conv2d_weights(L.ptr(wd), cout, cin, int(transpose), L.ptr(planes[0]), L.ptr(planes[1]),
                                         L.ptr(sc), L.stream()), "b2s_pack_conv2d_weights")
     val = (planes[0], planes[1], sc[1:2])
@@ -150,15 +171,22 @@ def pack_weights(conv, transpose):
     return val
 
 
-def conv3x3(x_hi, x_lo, x_scale, w_hi, w_lo, w_inv, B, H, W, cin, cout):
+def conv3x3(x_hi, x_lo, x_scale, w_hi, w_lo, w_inv, B, H, W, cin, cout, products=3):
     """3x3 stride-1 pad-1 conv of halo planes -> fp32 [B, H, W, cout]: one b2s_conv2d_tc_ex launch per 128 output
-    channels, epilogue scale = (input's 2^-e) * (weights' 1/s), computed on the device."""
+    channels, epilogue scale = (input's 2^-e) * (weights' 1/s), computed on the device.  products = 1: single planes
+    (x_lo, w_lo None) through b2s_conv2d_tc_ex3 with products = 1 and fp32 output."""
     L, lib = _lib()
     out = torch.empty(B, H, W, cout, dtype=torch.float32, device=x_hi.device)
     n_pad = int(w_hi.shape[2])
     epi = (x_scale * w_inv).expand(n_pad).contiguous()
     for g in range(int(w_hi.shape[0])):
         cg = min(128, cout - 128 * g)
+        if products == 1:
+            L.check(lib.b2s_conv2d_tc_ex3(
+                L.ptr(x_hi), None, B, H, W, cin, L.ptr(w_hi[g]), None, 3, 3, 1, 1, cg, n_pad, L.ptr(epi), None, 0, H, W,
+                L.ptr(out[..., 128 * g:]), None, H, W, 0, cout, 1, 0, 0, None, None, None, None, None, None, -1, 8, 1, 1,
+                None, L.stream()), "b2s_conv2d_tc_ex3")
+            continue
         L.check(lib.b2s_conv2d_tc_ex(
             L.ptr(x_hi), L.ptr(x_lo), B, H, W, cin, L.ptr(w_hi[g]), L.ptr(w_lo[g]), 3, 3, 1, 1, cg, n_pad, L.ptr(epi),
             None, 0, H, W, L.ptr(out[..., 128 * g:]), None, H, W, 0, cout, 1, 0, 0, None, None, None, None, None, None,
@@ -166,11 +194,16 @@ def conv3x3(x_hi, x_lo, x_scale, w_hi, w_lo, w_inv, B, H, W, cin, cout):
     return out
 
 
-def wgrad(x_hi, x_lo, x_scale, g_hi, g_lo, g_scale, B, H, W, cin, cout):
+def wgrad(x_hi, x_lo, x_scale, g_hi, g_lo, g_scale, B, H, W, cin, cout, products=3):
     L, lib = _lib()
     dw = torch.empty(cout, cin, 3, 3, dtype=torch.float32, device=x_hi.device)
     nbytes = int(lib.b2s_conv2d_wgrad_tc_workspace_bytes(B, H, W, cin, cout))
     ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=x_hi.device)
+    if products == 1:
+        L.check(lib.b2s_conv2d_wgrad_tc_ex(L.ptr(x_hi), None, L.ptr(g_hi), None, B, H, W, cin, cout, L.ptr(x_scale),
+                                           L.ptr(g_scale), L.ptr(dw), L.ptr(ws), nbytes, 1, L.stream()),
+                "b2s_conv2d_wgrad_tc_ex")
+        return dw
     L.check(lib.b2s_conv2d_wgrad_tc(L.ptr(x_hi), L.ptr(x_lo), L.ptr(g_hi), L.ptr(g_lo), B, H, W, cin, cout,
                                     L.ptr(x_scale), L.ptr(g_scale), L.ptr(dw), L.ptr(ws), nbytes, L.stream()),
             "b2s_conv2d_wgrad_tc")
@@ -186,24 +219,27 @@ class Conv3x3TC(torch.autograd.Function):
         cout = int(weight.shape[0])
         if cin != conv.in_channels:
             raise RuntimeError("Conv3x3TC: input has %d channels, the conv takes %d" % (cin, conv.in_channels))
-        x_hi, x_lo, x_scale = split_halo(x)
-        w_hi, w_lo, w_inv = pack_weights(conv, False)
-        y = conv3x3(x_hi, x_lo, x_scale, w_hi, w_lo, w_inv, B, H, W, cin, cout)
+        # the product count goes to the helpers only in the f16 mode: the default mode calls them as it always has
+        kw = {} if getattr(conv, "_b2s_products", 3) == 3 else {"products": 1}
+        x_hi, x_lo, x_scale = split_halo(x, **kw)
+        w_hi, w_lo, w_inv = pack_weights(conv, False, **kw)
+        y = conv3x3(x_hi, x_lo, x_scale, w_hi, w_lo, w_inv, B, H, W, cin, cout, **kw)
         ctx.save_for_backward(x_hi, x_lo, x_scale)
-        ctx.conv, ctx.shape = conv, (B, cin, H, W, cout)
+        ctx.conv, ctx.shape, ctx.kw = conv, (B, cin, H, W, cout), kw
         return y.permute(0, 3, 1, 2)                    # NCHW view of NHWC storage: channels_last
 
     @staticmethod
     def backward(ctx, dy):
         x_hi, x_lo, x_scale = ctx.saved_tensors
         B, cin, H, W, cout = ctx.shape
+        kw = ctx.kw
         if not (dy.is_contiguous() or dy.is_contiguous(memory_format=torch.channels_last)):
             dy = dy.contiguous(memory_format=torch.channels_last)
-        g_hi, g_lo, g_scale = split_halo(dy)
+        g_hi, g_lo, g_scale = split_halo(dy, **kw)
         dx = dw = None
         if ctx.needs_input_grad[0]:
-            wt_hi, wt_lo, wt_inv = pack_weights(ctx.conv, True)
-            dx = conv3x3(g_hi, g_lo, g_scale, wt_hi, wt_lo, wt_inv, B, H, W, cout, cin).permute(0, 3, 1, 2)
+            wt_hi, wt_lo, wt_inv = pack_weights(ctx.conv, True, **kw)
+            dx = conv3x3(g_hi, g_lo, g_scale, wt_hi, wt_lo, wt_inv, B, H, W, cout, cin, **kw).permute(0, 3, 1, 2)
         if ctx.needs_input_grad[1]:
-            dw = wgrad(x_hi, x_lo, x_scale, g_hi, g_lo, g_scale, B, H, W, cin, cout)
+            dw = wgrad(x_hi, x_lo, x_scale, g_hi, g_lo, g_scale, B, H, W, cin, cout, **kw)
         return dx, dw, None

@@ -17,6 +17,10 @@
 //
 // L2 -> SM bytes per pixel: 3 * (Cin/64) * ceil(Cout/128) jobs, each reading X hi/lo (2 x 128 B x 10/8 for the window
 // halo) and dY hi/lo (2 x 2 B x min(Cout, 128)); 5.0 KB at 128 -> 128 against 9 KB if each tap re-read both operands.
+//
+// P = products per k16 step: 3 (3xF16, above) or 1 (the f16 mode, the *_ex entry points with products = 1): one fp16
+// plane per operand.  The split writes the hi plane only; the weight gradient's stage holds [X_hi window | dY_hi blocks]
+// (half the bytes, 2.5 KB per pixel at 128 -> 128) and each tap's chain is 4 dY_hi*X_hi MMAs.
 #include <cuda_fp16.h>
 
 #include "autoscale.cuh"
@@ -48,7 +52,8 @@ inline int num_slabs(int B, int H, int W) { return (num_strips(B, H, W) + WS_SLA
 // fp32 map [B, C, H, W] (layout NCHW) or [B, H, W, C] (NHWC) -> x * 2^e as fp16 hi/lo planes [B, H+2, W+2, C] with a zero
 // halo.  One thread per (padded pixel, 8 channels); for NCHW consecutive threads take consecutive pixels of one channel
 // group, so the reads of each channel row are coalesced.  A non-finite element goes through as itself
-// (split_f16_keep_nonfinite) and raises B2S_STATUS_F16_RANGE.
+// (split_f16_keep_nonfinite) and raises B2S_STATUS_F16_RANGE.  P = 1: the hi plane only.
+template <int P>
 __global__ void k_split_halo(const float *__restrict__ x, int layout, int B, int C, int H, int W, __half *__restrict__ hi,
                              __half *__restrict__ lo, float *__restrict__ scale_dev, unsigned *__restrict__ status)
 {
@@ -97,7 +102,7 @@ __global__ void k_split_halo(const float *__restrict__ x, int layout, int B, int
             l4 = make_uint4(l[0], l[1], l[2], l[3]);
         }
         *reinterpret_cast<uint4 *>(hi + pix * C + g * 8) = h4;
-        *reinterpret_cast<uint4 *>(lo + pix * C + g * 8) = l4;
+        if constexpr (P == 3) *reinterpret_cast<uint4 *>(lo + pix * C + g * 8) = l4;
     }
     if (nonfinite && status) atomicOr(status, B2S_STATUS_F16_RANGE);
 }
@@ -137,11 +142,15 @@ __device__ __forceinline__ void strip_origin(const WgradParams &p, int id, int &
     b = id / (p.strips_w * p.strips_h);
 }
 
+template <int P>
 __global__ void __launch_bounds__(WS_THREADS, 1)
 k_conv2d_wgrad_tc(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
                   const __grid_constant__ CUtensorMap map_g_hi, const __grid_constant__ CUtensorMap map_g_lo,
                   const WgradParams p)
 {
+    static_assert(P == 3 || P == 1, "products per k16 step: 3 (3xF16) or 1 (f16)");
+    constexpr uint32_t SB = P == 3 ? STAGE_BYTES : XWIN_BYTES + 2 * DY_BYTES;   // P = 1: X_hi, dY_hi x 2 blocks
+    constexpr uint32_t XB = (P == 3 ? 2 : 1) * XWIN_BYTES, GB = (P == 3 ? 2 : 1) * DY_BYTES;   // X window, dY block
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     __shared__ __align__(8) uint64_t bar_full[WS_STAGES], bar_empty[WS_STAGES];
@@ -162,22 +171,22 @@ k_conv2d_wgrad_tc(const __grid_constant__ CUtensorMap map_x_hi, const __grid_con
         if (lane == 0) {
             int st = 0;
             uint32_t ph = 0;
-            const uint32_t bytes = 2 * XWIN_BYTES + 2 * co_blocks * DY_BYTES;
+            const uint32_t bytes = XB + co_blocks * GB;
             for (int id = s0; id < s1; ++id) {
                 int h0, w0, b;
                 strip_origin(p, id, h0, w0, b);
                 mbar_wait(&bar_empty[st], ph ^ 1);
-                uint8_t *dst = smem + (size_t)st * STAGE_BYTES;
+                uint8_t *dst = smem + (size_t)st * SB;
                 mbar_arrive_expect_tx(&bar_full[st], bytes);
                 // padded coordinates: output pixel (h, w) of tap (ky, kx) reads X at (h + ky, w + kx), dY at (h+1, w+1);
                 // boxes past the padded map are zero-filled, and past-the-edge dY pixels are halo or fill: zero terms
                 tma_load_4d(dst, &map_x_hi, &bar_full[st], cib * 64, w0 + dx, h0, b);
-                tma_load_4d(dst + XWIN_BYTES, &map_x_lo, &bar_full[st], cib * 64, w0 + dx, h0, b);
+                if constexpr (P == 3) tma_load_4d(dst + XWIN_BYTES, &map_x_lo, &bar_full[st], cib * 64, w0 + dx, h0, b);
                 for (int q = 0; q < co_blocks; ++q) {
                     const int co = (2 * cop + q) * 64;
-                    uint8_t *gd = dst + 2 * XWIN_BYTES + q * 2 * DY_BYTES;
+                    uint8_t *gd = dst + XB + q * GB;
                     tma_load_4d(gd, &map_g_hi, &bar_full[st], co, w0 + 1, h0 + 1, b);
-                    tma_load_4d(gd + DY_BYTES, &map_g_lo, &bar_full[st], co, w0 + 1, h0 + 1, b);
+                    if constexpr (P == 3) tma_load_4d(gd + DY_BYTES, &map_g_lo, &bar_full[st], co, w0 + 1, h0 + 1, b);
                 }
                 if (++st == WS_STAGES) { st = 0; ph ^= 1; }
             }
@@ -196,20 +205,22 @@ k_conv2d_wgrad_tc(const __grid_constant__ CUtensorMap map_x_hi, const __grid_con
         for (int id = s0; id < s1; ++id) {
             mbar_wait(&bar_full[st], ph);
             if (active) {
-                const uint32_t sx = sm0 + (uint32_t)st * STAGE_BYTES;
-                const uint32_t sg = sx + 2 * XWIN_BYTES + (uint32_t)cg * 2 * DY_BYTES;
+                const uint32_t sx = sm0 + (uint32_t)st * SB;
+                const uint32_t sg = sx + XB + (uint32_t)cg * GB;
 #pragma unroll
                 for (int ky = 0; ky < 3; ++ky) {
                     wgmma_fence();
 #pragma unroll
                     for (int k = 0; k < WS_R / 2; ++k) {          // k16 step = strip rows 2k, 2k + 1
                         const uint64_t g_hi = make_desc_mn_sw128(sg + 2 * k * ATOM);
-                        const uint64_t g_lo = make_desc_mn_sw128(sg + DY_BYTES + 2 * k * ATOM);
                         const uint64_t x_hi = make_desc_mn_sw128(sx + (ky + 2 * k) * ATOM);
-                        const uint64_t x_lo = make_desc_mn_sw128(sx + XWIN_BYTES + (ky + 2 * k) * ATOM);
                         wgmma_mn64(acc, g_hi, x_hi, k != 0);
-                        wgmma_mn64(acc, g_hi, x_lo, 1);
-                        wgmma_mn64(acc, g_lo, x_hi, 1);
+                        if constexpr (P == 3) {
+                            const uint64_t g_lo = make_desc_mn_sw128(sg + DY_BYTES + 2 * k * ATOM);
+                            const uint64_t x_lo = make_desc_mn_sw128(sx + XWIN_BYTES + (ky + 2 * k) * ATOM);
+                            wgmma_mn64(acc, g_hi, x_lo, 1);
+                            wgmma_mn64(acc, g_lo, x_hi, 1);
+                        }
                     }
                     wgmma_commit();
                     wgmma_wait_all();
@@ -270,10 +281,15 @@ int make_plane_map(CUtensorMap *m, const void *base, int B, int H, int W, int C,
 
 }  // namespace
 
-extern "C" int b2s_split_halo_f16_autoscale(const float *x, int layout, int batch, int C, int H, int W, b2s_half *hi,
-                                            b2s_half *lo, float *scale_dev, unsigned *status_dev, void *stream_)
+// products = 1: lo must be NULL, only the hi plane is written (the same bits as the hi plane of products = 3)
+extern "C" int b2s_split_halo_f16_autoscale_ex(const float *x, int layout, int batch, int C, int H, int W, b2s_half *hi,
+                                               b2s_half *lo, float *scale_dev, unsigned *status_dev, int products,
+                                               void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(products == 3 || (products == 1 && lo == nullptr),
+                "b2s_split_halo_f16_autoscale: products must be 3 (hi/lo planes) or 1 (f16, no lo plane)");
+    if (products == 1) lo = hi;                       // (the checks below; never written)
     B2S_REQUIRE(layout == B2S_LAYOUT_NCHW || layout == B2S_LAYOUT_NHWC, "b2s_split_halo_f16_autoscale: bad layout");
     B2S_REQUIRE(batch >= 1 && C >= 8 && C % 8 == 0 && H >= 1 && W >= 1,
                 "b2s_split_halo_f16_autoscale: bad sizes (C must be a multiple of 8)");
@@ -286,10 +302,21 @@ extern "C" int b2s_split_halo_f16_autoscale(const float *x, int layout, int batc
     const long long n = (long long)batch * C * H * W;
     k_absmax<<<grid_for(n), kThreads, 0, stream>>>(x, nullptr, 1, (int)n, reinterpret_cast<unsigned *>(scale_dev + 1));
     B2S_LAUNCH_OK();
-    k_split_halo<<<grid_for((long long)batch * (H + 2) * (W + 2) * (C / 8)), kThreads, 0, stream>>>(
-        x, layout, batch, C, H, W, reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo), scale_dev, status_dev);
+    if (products == 1)
+        k_split_halo<1><<<grid_for((long long)batch * (H + 2) * (W + 2) * (C / 8)), kThreads, 0, stream>>>(
+            x, layout, batch, C, H, W, reinterpret_cast<__half *>(hi), nullptr, scale_dev, status_dev);
+    else
+        k_split_halo<3><<<grid_for((long long)batch * (H + 2) * (W + 2) * (C / 8)), kThreads, 0, stream>>>(
+            x, layout, batch, C, H, W, reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo), scale_dev,
+            status_dev);
     B2S_LAUNCH_OK();
     return 0;
+}
+
+extern "C" int b2s_split_halo_f16_autoscale(const float *x, int layout, int batch, int C, int H, int W, b2s_half *hi,
+                                            b2s_half *lo, float *scale_dev, unsigned *status_dev, void *stream)
+{
+    return b2s_split_halo_f16_autoscale_ex(x, layout, batch, C, H, W, hi, lo, scale_dev, status_dev, 3, stream);
 }
 
 extern "C" size_t b2s_conv2d_wgrad_tc_workspace_bytes(int batch, int H, int W, int Cin, int Cout)
@@ -298,12 +325,17 @@ extern "C" size_t b2s_conv2d_wgrad_tc_workspace_bytes(int batch, int H, int W, i
     return sizeof(float) * (size_t)num_slabs(batch, H, W) * 9 * Cin * Cout;
 }
 
-extern "C" int b2s_conv2d_wgrad_tc(const b2s_half *x_hi, const b2s_half *x_lo, const b2s_half *dout_hi,
-                                   const b2s_half *dout_lo, int batch, int H, int W, int Cin, int Cout,
-                                   const float *x_scale_dev, const float *dout_scale_dev, float *dweight,
-                                   void *workspace, size_t workspace_bytes, void *stream_)
+// products = 3: the 3xF16 form (b2s_conv2d_wgrad_tc).  products = 1: the f16 mode -- x_lo and dout_lo must be NULL;
+// one dY_hi*X_hi product per tap and k16 step, the same workspace.
+extern "C" int b2s_conv2d_wgrad_tc_ex(const b2s_half *x_hi, const b2s_half *x_lo, const b2s_half *dout_hi,
+                                      const b2s_half *dout_lo, int batch, int H, int W, int Cin, int Cout,
+                                      const float *x_scale_dev, const float *dout_scale_dev, float *dweight,
+                                      void *workspace, size_t workspace_bytes, int products, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(products == 3 || (products == 1 && x_lo == nullptr && dout_lo == nullptr),
+                "b2s_conv2d_wgrad_tc: products must be 3 (3xF16) or 1 (f16, no lo planes)");
+    if (products == 1) { x_lo = x_hi; dout_lo = dout_hi; }   // (the checks below; never read)
     B2S_REQUIRE(Cin >= 64 && Cin % 64 == 0 && (Cout == 64 || Cout == 128 || Cout == 256),
                 "b2s_conv2d_wgrad_tc: Cin must be a multiple of 64 and Cout 64, 128 or 256");
     B2S_REQUIRE(batch >= 1 && H >= 1 && W >= 1, "b2s_conv2d_wgrad_tc: bad sizes");
@@ -317,8 +349,10 @@ extern "C" int b2s_conv2d_wgrad_tc(const b2s_half *x_hi, const b2s_half *x_lo, c
     B2S_REQUIRE(workspace_bytes >= b2s_conv2d_wgrad_tc_workspace_bytes(batch, H, W, Cin, Cout),
                 "b2s_conv2d_wgrad_tc: workspace too small (b2s_conv2d_wgrad_tc_workspace_bytes)");
     CUtensorMap mx_hi, mx_lo, mg_hi, mg_lo;
-    if (make_plane_map(&mx_hi, x_hi, batch, H, W, Cin, WS_R + 2) || make_plane_map(&mx_lo, x_lo, batch, H, W, Cin, WS_R + 2) ||
-        make_plane_map(&mg_hi, dout_hi, batch, H, W, Cout, WS_R) || make_plane_map(&mg_lo, dout_lo, batch, H, W, Cout, WS_R))
+    if (make_plane_map(&mx_hi, x_hi, batch, H, W, Cin, WS_R + 2) || make_plane_map(&mg_hi, dout_hi, batch, H, W, Cout, WS_R))
+        return -1;
+    if (products == 3 && (make_plane_map(&mx_lo, x_lo, batch, H, W, Cin, WS_R + 2) ||
+                          make_plane_map(&mg_lo, dout_lo, batch, H, W, Cout, WS_R)))
         return -1;
     WgradParams p;
     p.B = batch; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout;
@@ -329,12 +363,28 @@ extern "C" int b2s_conv2d_wgrad_tc(const b2s_half *x_hi, const b2s_half *x_lo, c
     p.co_pairs = (Cout + 127) / 128;
     p.partial = reinterpret_cast<float *>(workspace);
     const int slabs = num_slabs(batch, H, W);
-    B2S_SMEM_OPT_IN(k_conv2d_wgrad_tc, WS_SMEM);
-    k_conv2d_wgrad_tc<<<dim3(slabs, 3 * p.ci_blocks * p.co_pairs), WS_THREADS, WS_SMEM, stream>>>(mx_hi, mx_lo, mg_hi,
-                                                                                                  mg_lo, p);
+    if (products == 1) {
+        constexpr size_t smem1 = (size_t)WS_STAGES * (XWIN_BYTES + 2 * DY_BYTES) + 1024;
+        B2S_SMEM_OPT_IN(k_conv2d_wgrad_tc<1>, smem1);
+        k_conv2d_wgrad_tc<1><<<dim3(slabs, 3 * p.ci_blocks * p.co_pairs), WS_THREADS, smem1, stream>>>(mx_hi, mx_hi,
+                                                                                                      mg_hi, mg_hi, p);
+    } else {
+        B2S_SMEM_OPT_IN(k_conv2d_wgrad_tc<3>, WS_SMEM);
+        k_conv2d_wgrad_tc<3><<<dim3(slabs, 3 * p.ci_blocks * p.co_pairs), WS_THREADS, WS_SMEM, stream>>>(mx_hi, mx_lo,
+                                                                                                        mg_hi, mg_lo, p);
+    }
     B2S_LAUNCH_OK();
     k_conv2d_wgrad_reduce<<<grid_for(9ll * Cin * Cout), kThreads, 0, stream>>>(p.partial, slabs, Cin, Cout, x_scale_dev,
                                                                                dout_scale_dev, dweight);
     B2S_LAUNCH_OK();
     return 0;
+}
+
+extern "C" int b2s_conv2d_wgrad_tc(const b2s_half *x_hi, const b2s_half *x_lo, const b2s_half *dout_hi,
+                                   const b2s_half *dout_lo, int batch, int H, int W, int Cin, int Cout,
+                                   const float *x_scale_dev, const float *dout_scale_dev, float *dweight,
+                                   void *workspace, size_t workspace_bytes, void *stream)
+{
+    return b2s_conv2d_wgrad_tc_ex(x_hi, x_lo, dout_hi, dout_lo, batch, H, W, Cin, Cout, x_scale_dev, dout_scale_dev,
+                                  dweight, workspace, workspace_bytes, 3, stream);
 }

@@ -32,7 +32,8 @@
 //
 // P = products per K block: 3 (3xF16, above) or 1 (the f16 mode, b2s_sparse_conv_tc_plan_ex with products = 1): one
 // fp16 plane per operand, so the gather copies hi rows only, a stage holds [A_hi | W_hi], each K step is one wgmma
-// A_hi*W_hi of width N, and the epilogue writes one rounded fp16 plane.
+// A_hi*W_hi of width N, and the epilogue writes one rounded fp16 plane, or with out_fp32 (b2s_sparse_conv_tc_plan_ex2,
+// the training forward and input gradient) fp32 rows as the 3xF16 form does without out_lo.
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -75,6 +76,7 @@ struct SpParams {
     const float *scale, *shift;
     void *out_hi;                // fp16 hi plane, or (out_lo == NULL) fp32 rows [cap_out, COUT]
     __half *out_lo;
+    int out_fp32;                // P = 1: fp32 rows in out_hi instead of one fp16 plane
 };
 
 // K blocks a tile needs, from its offset mask: bit j = K block j (offsets j*PACK .. j*PACK+PACK-1).  Never empty:
@@ -409,7 +411,7 @@ k_sparse_conv_tc(const __grid_constant__ CUtensorMap map_w_hi, const __grid_cons
                     float x0 = fmaf(sum[4 * j + 2 * rh], s_scale[c], s_shift[c]);
                     float x1 = fmaf(sum[4 * j + 2 * rh + 1], s_scale[c + 1], s_shift[c + 1]);
                     if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-                    if (P == 1 || p.out_lo) {
+                    if ((P == 1 && !p.out_fp32) || p.out_lo) {
                         range_bad |= (fabsf(x0) > 65504.f) | (fabsf(x1) > 65504.f);
                         const uint32_t p0 = split_f16(x0), p1 = split_f16(x1);
                         const size_t o = (size_t)row * p.out_stride + c;
@@ -448,24 +450,27 @@ extern "C" int b2s_sparse_conv_tc_supported(int cin, int cout)
 // Weight layout: Cin = 64: [K][Cout][64]; Cin < 64 (8, 16, 32): packed [ceil(K / (64/Cin))][Cout][64] with column
 // (offset-in-pack * Cin + cin) and zero columns for offsets >= K (b2second/tc.py: pack_sparse_weights).
 // products = 3: 3xF16 hi/lo planes (out_lo == NULL: fp32 rows).  products = 1: the f16 mode -- feat_lo, w_lo and
-// out_lo must be NULL, and the output is one fp16 plane in out_hi.
-extern "C" int b2s_sparse_conv_tc_plan_ex(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in,
-                                          int cin, const b2s_half *w_hi, const b2s_half *w_lo, const int *nbr, int K,
-                                          const int *num_out_dev, int cap_out, const int *perm, const unsigned *tile_mask,
-                                          const float *scale, const float *shift, int relu, void *out_hi,
-                                          b2s_half *out_lo, int out_stride, int cout, int products, unsigned *status_dev,
-                                          void *stream_)
+// out_lo must be NULL, and the output is one fp16 plane in out_hi, or fp32 rows [cap_out, cout] when out_fp32 is 1
+// (out_fp32 must be 0 with products = 3, where out_lo says it).
+extern "C" int b2s_sparse_conv_tc_plan_ex2(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in,
+                                           int cin, const b2s_half *w_hi, const b2s_half *w_lo, const int *nbr, int K,
+                                           const int *num_out_dev, int cap_out, const int *perm,
+                                           const unsigned *tile_mask, const float *scale, const float *shift, int relu,
+                                           void *out_hi, b2s_half *out_lo, int out_stride, int cout, int products,
+                                           int out_fp32, unsigned *status_dev, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     B2S_REQUIRE(products == 3 || (products == 1 && feat_lo == nullptr && w_lo == nullptr && out_lo == nullptr),
                 "b2s_sparse_conv_tc: products must be 3 (3xF16) or 1 (f16, no lo planes)");
+    B2S_REQUIRE(products == 3 ? out_fp32 == 0 : (out_fp32 == 0 || out_fp32 == 1),
+                "b2s_sparse_conv_tc: out_fp32 must be 0 or 1 with products = 1 and 0 with products = 3");
     if (products == 1) feat_lo = feat_hi;           // (alignment checks below; the f16 kernel never reads it)
     B2S_REQUIRE(b2s_sparse_conv_tc_supported(cin, cout),
                 "b2s_sparse_conv_tc: built for Cin in {8, 16, 32, 64}, Cout in {16, 32, 64} (others: b2s_sparse_conv)");
     B2S_REQUIRE(K >= 1 && K <= 27 && cap_out >= 0 && rows_in >= 0, "b2s_sparse_conv_tc: K must be 1..27");
     B2S_REQUIRE(in_stride >= cin && in_stride % 8 == 0 && ((uintptr_t)feat_hi & 15) == 0 && ((uintptr_t)feat_lo & 15) == 0,
                 "b2s_sparse_conv_tc: input rows must be 16-byte aligned (in_stride multiple of 8 halves)");
-    B2S_REQUIRE((products == 3 && out_lo == nullptr) || (out_stride >= cout && out_stride % 8 == 0 && ((uintptr_t)out_hi & 15) == 0 &&
+    B2S_REQUIRE((products == 3 && out_lo == nullptr) || out_fp32 == 1 || (out_stride >= cout && out_stride % 8 == 0 && ((uintptr_t)out_hi & 15) == 0 &&
                                       ((uintptr_t)out_lo & 15) == 0),
                 "b2s_sparse_conv_tc: output rows must be 16-byte aligned (out_stride multiple of 8 halves)");
     B2S_REQUIRE((unsigned long long)rows_in * (unsigned long long)in_stride * ELEM_BYTES < (1ull << 32),
@@ -488,6 +493,7 @@ extern "C" int b2s_sparse_conv_tc_plan_ex(const b2s_half *feat_hi, const b2s_hal
     p.nbr = nbr; p.n_out_dev = num_out_dev; p.cap_out = cap_out; p.K = K;
     p.perm = perm; p.tile_mask = tile_mask;
     p.relu = relu; p.scale = scale; p.shift = shift; p.out_hi = out_hi; p.out_lo = reinterpret_cast<__half *>(out_lo);
+    p.out_fp32 = out_fp32;
 #define B2S_TC_CASE(CI, CO)                                                                         \
     if (cin == CI && cout == CO)                                                                    \
         return products == 1 ? launch<CI, CO, 1>(m_hi, m_hi, p, num_sms, stream)                    \
@@ -497,6 +503,18 @@ extern "C" int b2s_sparse_conv_tc_plan_ex(const b2s_half *feat_hi, const b2s_hal
 #undef B2S_TC_CASE
     b2s_set_error("b2s_sparse_conv_tc: Cin=%d Cout=%d not built", cin, cout);
     return -2;
+}
+
+extern "C" int b2s_sparse_conv_tc_plan_ex(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in,
+                                          int cin, const b2s_half *w_hi, const b2s_half *w_lo, const int *nbr, int K,
+                                          const int *num_out_dev, int cap_out, const int *perm, const unsigned *tile_mask,
+                                          const float *scale, const float *shift, int relu, void *out_hi,
+                                          b2s_half *out_lo, int out_stride, int cout, int products, unsigned *status_dev,
+                                          void *stream)
+{
+    return b2s_sparse_conv_tc_plan_ex2(feat_hi, feat_lo, in_stride, rows_in, cin, w_hi, w_lo, nbr, K, num_out_dev,
+                                       cap_out, perm, tile_mask, scale, shift, relu, out_hi, out_lo, out_stride, cout,
+                                       products, 0, status_dev, stream);
 }
 
 // the 3xF16 form

@@ -165,7 +165,9 @@ __global__ void k_from_bev(const float *__restrict__ dmap, const int *__restrict
 }
 
 // one thread per 8 columns of a packed row: out[kb, o, p * n_in' + i] = L[kb * P + p, i, o] * s, zero past K and n_in
-// (tc.pack_sparse_weights), split into hi / lo.  s is the float32 the host path multiplies by: float(2.0 ** e).
+// (tc.pack_sparse_weights), split into hi / lo (P = 1: hi only).  s is the float32 the host path multiplies by:
+// float(2.0 ** e).
+template <int P>
 __global__ void k_pack_sparse_weights(const float *__restrict__ w, int K, int cin, int cout, int transpose, int flip,
                                       int n_in, int n_in_pad, int n_out, int nkb, __half *__restrict__ hi,
                                       __half *__restrict__ lo, float *__restrict__ scale_dev)
@@ -202,13 +204,15 @@ __global__ void k_pack_sparse_weights(const float *__restrict__ w, int K, int ci
             l[j] = __byte_perm(pa, pb, 0x7632);
         }
         *reinterpret_cast<uint4 *>(hi + row * b2s_tc::BLOCK_K + c0) = make_uint4(h[0], h[1], h[2], h[3]);
-        *reinterpret_cast<uint4 *>(lo + row * b2s_tc::BLOCK_K + c0) = make_uint4(l[0], l[1], l[2], l[3]);
+        if constexpr (P == 3)
+            *reinterpret_cast<uint4 *>(lo + row * b2s_tc::BLOCK_K + c0) = make_uint4(l[0], l[1], l[2], l[3]);
     }
 }
 
 // dense 3x3 weights, one thread per 8 columns of a packed row: out[g, tap, o, i] = L[tap][g * 128 + o][i] * s with
 // L[tap][o][i] = W[o][i][tap] (transpose 0: the forward) or W[i][o][8 - tap] (transpose 1: the input gradient), W the
 // torch weight [cout, cin, 3, 3]; rows past n_out of the last group are zero.  s as in k_pack_sparse_weights.
+template <int P>
 __global__ void k_pack_conv2d_weights(const float *__restrict__ w, int cout, int cin, int transpose, int n_in,
                                       int n_out, int n_pad, int groups, __half *__restrict__ hi, __half *__restrict__ lo,
                                       float *__restrict__ scale_dev)
@@ -244,10 +248,11 @@ __global__ void k_pack_conv2d_weights(const float *__restrict__ w, int cout, int
             l[j] = __byte_perm(pa, pb, 0x7632);
         }
         *reinterpret_cast<uint4 *>(hi + row * n_in + c0) = make_uint4(h[0], h[1], h[2], h[3]);
-        *reinterpret_cast<uint4 *>(lo + row * n_in + c0) = make_uint4(l[0], l[1], l[2], l[3]);
+        if constexpr (P == 3) *reinterpret_cast<uint4 *>(lo + row * n_in + c0) = make_uint4(l[0], l[1], l[2], l[3]);
     }
 }
 
+template <int P>
 __global__ void k_split_f16_scaled(const float *__restrict__ x, __half *__restrict__ hi, __half *__restrict__ lo,
                                    const int *__restrict__ n_rows_dev, int cap_rows, int row_floats, int out_channels,
                                    int out_stride, float *__restrict__ scale_dev)
@@ -271,7 +276,7 @@ __global__ void k_split_f16_scaled(const float *__restrict__ x, __half *__restri
             l[j] = __byte_perm(pa, pb, 0x7632);
         }
         *reinterpret_cast<uint4 *>(hi + row * out_stride + c0) = make_uint4(h[0], h[1], h[2], h[3]);
-        *reinterpret_cast<uint4 *>(lo + row * out_stride + c0) = make_uint4(l[0], l[1], l[2], l[3]);
+        if constexpr (P == 3) *reinterpret_cast<uint4 *>(lo + row * out_stride + c0) = make_uint4(l[0], l[1], l[2], l[3]);
     }
 }
 
@@ -287,6 +292,11 @@ __global__ void k_split_f16_scaled(const float *__restrict__ x, __half *__restri
 // in the K block -- known from tile_mask, or found while staging -- contributes exact zeros and is skipped, so results are
 // bit-identical with and without tile_mask.  The slab partials go to the workspace; the reduce launch adds them in
 // order, multiplies by *scale_dev and unpacks into [K, Cin, Cout].
+//
+// P = products per k16 step: 3 (3xF16, above) or 1 (the f16 mode, b2s_sparse_conv_wgrad_tc_ex with products = 1): one
+// fp16 plane per operand, so staging moves the hi rows only (half the bytes), the smem holds [A_hi | B_hi], each k16
+// step is one wgmma A_hi*B_hi of width N, and the chain's accumulator (64 x N) is drained as it is.  The partials have
+// the same layout, so the workspace is the same.
 constexpr int WT_CHUNK = 64;
 constexpr int WT_THREADS = 128;
 
@@ -295,7 +305,7 @@ __device__ __forceinline__ uint32_t sw128_off(int m, int r)
     return (uint32_t)(m * 128 + ((((r >> 3) ^ (m & 7)) << 4) | ((r & 7) << 1)));
 }
 
-template <int CIN, int COUT>
+template <int CIN, int COUT, int P>
 __global__ void __launch_bounds__(WT_THREADS)
 k_wgrad_tc(const __half *__restrict__ x_hi, const __half *__restrict__ x_lo, int in_stride,
            const __half *__restrict__ g_hi, const __half *__restrict__ g_lo, int g_stride, const int *__restrict__ nbr,
@@ -306,10 +316,12 @@ k_wgrad_tc(const __half *__restrict__ x_hi, const __half *__restrict__ x_lo, int
     constexpr int N = COUT;
     constexpr int PACK = b2s_tc::BLOCK_K / CIN;
     constexpr int A_BYTES = 64 * 128;
-    constexpr int R = N;                                     // accumulator registers: 64 rows x 2N columns
+    static_assert(P == 3 || P == 1, "products per k16 step: 3 (3xF16) or 1 (f16)");
+    constexpr int R = P == 3 ? N : N / 2;                    // accumulator registers: 64 rows x 2N (x N) columns
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t *sa_hi = smem, *sa_lo = smem + A_BYTES, *sb = smem + 2 * A_BYTES;   // sb: [B_hi (N rows); B_lo (N rows)]
+    // P = 3: sb = [B_hi (N rows); B_lo (N rows)]; P = 1: [A_hi | B_hi]
+    uint8_t *sa_hi = smem, *sa_lo = smem + A_BYTES, *sb = smem + (P == 3 ? 2 : 1) * A_BYTES;
     __shared__ int s_row[WT_CHUNK];
 
     const int n_out = min(*n_out_dev, cap_out);
@@ -321,9 +333,9 @@ k_wgrad_tc(const __half *__restrict__ x_hi, const __half *__restrict__ x_lo, int
     const uint32_t all_offsets = K >= 32 ? 0xffffffffu : ((1u << K) - 1u);
     const uint32_t pack_bits = (((1u << PACK) - 1u) << (kb * PACK)) & all_offsets;
 
-    float acc[R], sum[R / 2];
+    float acc[R], sum[N / 2];
 #pragma unroll
-    for (int j = 0; j < R / 2; ++j) sum[j] = 0.f;
+    for (int j = 0; j < N / 2; ++j) sum[j] = 0.f;
 
     for (int c0 = pos0; c0 < pos_end; c0 += WT_CHUNK) {
         if (tile_mask && !(__ldg(&tile_mask[c0 / BLOCK_M]) & pack_bits)) continue;   // uniform: no row needs the block
@@ -339,51 +351,85 @@ k_wgrad_tc(const __half *__restrict__ x_hi, const __half *__restrict__ x_lo, int
             const int k = kb * PACK + m0 / CIN, ci0 = m0 % CIN;
             const int row = s_row[r];
             const int src = (row >= 0 && k < K) ? __ldg(&nbr[(size_t)row * K + k]) : -1;
-            uint4 h = make_uint4(0, 0, 0, 0), l = make_uint4(0, 0, 0, 0);
-            if (src >= 0) {
-                h = __ldg(reinterpret_cast<const uint4 *>(x_hi + (size_t)src * in_stride + ci0));
-                l = __ldg(reinterpret_cast<const uint4 *>(x_lo + (size_t)src * in_stride + ci0));
-                have = 1;
-            }
-            const uint16_t *hh = reinterpret_cast<const uint16_t *>(&h), *ll = reinterpret_cast<const uint16_t *>(&l);
+            if constexpr (P == 3) {
+                uint4 h = make_uint4(0, 0, 0, 0), l = make_uint4(0, 0, 0, 0);
+                if (src >= 0) {
+                    h = __ldg(reinterpret_cast<const uint4 *>(x_hi + (size_t)src * in_stride + ci0));
+                    l = __ldg(reinterpret_cast<const uint4 *>(x_lo + (size_t)src * in_stride + ci0));
+                    have = 1;
+                }
+                const uint16_t *hh = reinterpret_cast<const uint16_t *>(&h), *ll = reinterpret_cast<const uint16_t *>(&l);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                *reinterpret_cast<uint16_t *>(sa_hi + sw128_off(m0 + j, r)) = hh[j];
-                *reinterpret_cast<uint16_t *>(sa_lo + sw128_off(m0 + j, r)) = ll[j];
+                for (int j = 0; j < 8; ++j) {
+                    *reinterpret_cast<uint16_t *>(sa_hi + sw128_off(m0 + j, r)) = hh[j];
+                    *reinterpret_cast<uint16_t *>(sa_lo + sw128_off(m0 + j, r)) = ll[j];
+                }
+            } else {
+                uint4 h = make_uint4(0, 0, 0, 0);
+                if (src >= 0) {
+                    h = __ldg(reinterpret_cast<const uint4 *>(x_hi + (size_t)src * in_stride + ci0));
+                    have = 1;
+                }
+                const uint16_t *hh = reinterpret_cast<const uint16_t *>(&h);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) *reinterpret_cast<uint16_t *>(sa_hi + sw128_off(m0 + j, r)) = hh[j];
             }
         }
         // B = dY^T: (row r, 8 consecutive output channels) per item
         for (int v = tid; v < WT_CHUNK * (N / 8); v += WT_THREADS) {
             const int r = v / (N / 8), n0 = (v % (N / 8)) * 8;
             const int row = s_row[r];
-            uint4 h = make_uint4(0, 0, 0, 0), l = make_uint4(0, 0, 0, 0);
-            if (row >= 0) {
-                h = __ldg(reinterpret_cast<const uint4 *>(g_hi + (size_t)row * g_stride + n0));
-                l = __ldg(reinterpret_cast<const uint4 *>(g_lo + (size_t)row * g_stride + n0));
-            }
-            const uint16_t *hh = reinterpret_cast<const uint16_t *>(&h), *ll = reinterpret_cast<const uint16_t *>(&l);
+            if constexpr (P == 3) {
+                uint4 h = make_uint4(0, 0, 0, 0), l = make_uint4(0, 0, 0, 0);
+                if (row >= 0) {
+                    h = __ldg(reinterpret_cast<const uint4 *>(g_hi + (size_t)row * g_stride + n0));
+                    l = __ldg(reinterpret_cast<const uint4 *>(g_lo + (size_t)row * g_stride + n0));
+                }
+                const uint16_t *hh = reinterpret_cast<const uint16_t *>(&h), *ll = reinterpret_cast<const uint16_t *>(&l);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                *reinterpret_cast<uint16_t *>(sb + sw128_off(n0 + j, r)) = hh[j];
-                *reinterpret_cast<uint16_t *>(sb + sw128_off(N + n0 + j, r)) = ll[j];
+                for (int j = 0; j < 8; ++j) {
+                    *reinterpret_cast<uint16_t *>(sb + sw128_off(n0 + j, r)) = hh[j];
+                    *reinterpret_cast<uint16_t *>(sb + sw128_off(N + n0 + j, r)) = ll[j];
+                }
+            } else {
+                uint4 h = make_uint4(0, 0, 0, 0);
+                if (row >= 0) h = __ldg(reinterpret_cast<const uint4 *>(g_hi + (size_t)row * g_stride + n0));
+                const uint16_t *hh = reinterpret_cast<const uint16_t *>(&h);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) *reinterpret_cast<uint16_t *>(sb + sw128_off(n0 + j, r)) = hh[j];
             }
         }
         fence_proxy_async();                                  // st.shared (generic proxy) -> wgmma operand reads
         if (!__syncthreads_or(have)) continue;                // no neighbour in the chunk: exact zeros, nothing to add
-        const uint64_t a_hi = make_desc_sw128(smem_u32(sa_hi)), a_lo = make_desc_sw128(smem_u32(sa_lo));
-        const uint64_t b_hl = make_desc_sw128(smem_u32(sb));
-        wgmma_fence();
+        if constexpr (P == 3) {
+            const uint64_t a_hi = make_desc_sw128(smem_u32(sa_hi)), a_lo = make_desc_sw128(smem_u32(sa_lo));
+            const uint64_t b_hl = make_desc_sw128(smem_u32(sb));
+            wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < WT_CHUNK / MMA_K; ++k) {
-            const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
-            wgmma_ss<2 * N>(acc, a_hi + koff, b_hl + koff, k == 0 ? 0u : 1u);
-            wgmma_ss<N>(acc, a_lo + koff, b_hl + koff, 1);
+            for (int k = 0; k < WT_CHUNK / MMA_K; ++k) {
+                const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                wgmma_ss<2 * N>(acc, a_hi + koff, b_hl + koff, k == 0 ? 0u : 1u);
+                wgmma_ss<N>(acc, a_lo + koff, b_hl + koff, 1);
+            }
+        } else {
+            const uint64_t a_hi = make_desc_sw128(smem_u32(sa_hi)), b_hi = make_desc_sw128(smem_u32(sb));
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < WT_CHUNK / MMA_K; ++k) {
+                const uint64_t koff = (uint64_t)((k * MMA_K * ELEM_BYTES) >> 4);
+                wgmma_ss<N>(acc, a_hi + koff, b_hi + koff, k == 0 ? 0u : 1u);
+            }
         }
         wgmma_commit();
         wgmma_wait_all();
         wgmma_fence_operands<R>(acc);
+        if constexpr (P == 3) {
 #pragma unroll
-        for (int j = 0; j < R / 2; ++j) sum[j] = __fadd_rn(__fadd_rn(sum[j], acc[j]), acc[R / 2 + j]);
+            for (int j = 0; j < R / 2; ++j) sum[j] = __fadd_rn(__fadd_rn(sum[j], acc[j]), acc[R / 2 + j]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < R; ++j) sum[j] = __fadd_rn(sum[j], acc[j]);
+        }
         __syncthreads();                                      // the next chunk overwrites the operand tiles
     }
     float *dst = partial + ((size_t)slab * num_kb + kb) * 64 * N;
@@ -417,14 +463,14 @@ __global__ void k_wgrad_tc_reduce(const float *__restrict__ partial, int num_kb,
     }
 }
 
-template <int CIN, int COUT>
+template <int CIN, int COUT, int P>
 int launch_wgrad_tc(const __half *x_hi, const __half *x_lo, int in_stride, const __half *g_hi, const __half *g_lo,
                     int g_stride, const int *nbr, int K, const int *n_out_dev, int cap_out, const int *perm,
                     const unsigned *tile_mask, float *partial, cudaStream_t stream)
 {
-    constexpr size_t smem = 2 * 64 * 128 + 2 * COUT * 128 + 1024;
+    constexpr size_t smem = (P == 3 ? 2 : 1) * (64 * 128 + COUT * 128) + 1024;
     const int num_kb = (K + (64 / CIN) - 1) / (64 / CIN);
-    k_wgrad_tc<CIN, COUT><<<dim3(num_slabs(cap_out), num_kb), WT_THREADS, smem, stream>>>(
+    k_wgrad_tc<CIN, COUT, P><<<dim3(num_slabs(cap_out), num_kb), WT_THREADS, smem, stream>>>(
         x_hi, x_lo, in_stride, g_hi, g_lo, g_stride, nbr, K, n_out_dev, cap_out, perm, tile_mask, partial);
     B2S_LAUNCH_OK();
     return 0;
@@ -473,13 +519,19 @@ extern "C" size_t b2s_sparse_conv_wgrad_tc_workspace_bytes(int cap_out, int K, i
     return sizeof(float) * (size_t)num_slabs(cap_out) * ((K + pack - 1) / pack) * 64 * cout;
 }
 
-extern "C" int b2s_sparse_conv_wgrad_tc(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in,
-                                        int cin, const b2s_half *dout_hi, const b2s_half *dout_lo, int dout_stride,
-                                        int cout, const int *nbr, int K, const int *num_out_dev, int cap_out,
-                                        const int *perm, const unsigned *tile_mask, const float *scale_dev,
-                                        float *dweight, void *workspace, size_t workspace_bytes, void *stream_)
+// products = 3: the 3xF16 form (b2s_sparse_conv_wgrad_tc).  products = 1: the f16 mode -- feat_lo and dout_lo must be
+// NULL; X_hi^T * dY_hi, the same workspace.
+extern "C" int b2s_sparse_conv_wgrad_tc_ex(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in,
+                                           int cin, const b2s_half *dout_hi, const b2s_half *dout_lo, int dout_stride,
+                                           int cout, const int *nbr, int K, const int *num_out_dev, int cap_out,
+                                           const int *perm, const unsigned *tile_mask, const float *scale_dev,
+                                           float *dweight, void *workspace, size_t workspace_bytes, int products,
+                                           void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(products == 3 || (products == 1 && feat_lo == nullptr && dout_lo == nullptr),
+                "b2s_sparse_conv_wgrad_tc: products must be 3 (3xF16) or 1 (f16, no lo planes)");
+    if (products == 1) { feat_lo = feat_hi; dout_lo = dout_hi; }   // (alignment checks below; never read)
     B2S_REQUIRE(b2s_sparse_conv_tc_supported(cin, cout),
                 "b2s_sparse_conv_wgrad_tc: built for Cin in {8, 16, 32, 64}, Cout in {16, 32, 64} (others: "
                 "b2s_sparse_conv_wgrad)");
@@ -500,8 +552,10 @@ extern "C" int b2s_sparse_conv_wgrad_tc(const b2s_half *feat_hi, const b2s_half 
     int rc = -2;
 #define B2S_WT_CASE(CI, CO)                                                                                         \
     if (cin == CI && cout == CO)                                                                                    \
-        rc = launch_wgrad_tc<CI, CO>(xh, xl, in_stride, gh, gl, dout_stride, nbr, K, num_out_dev, cap_out, perm,     \
-                                     tile_mask, partial, stream);
+        rc = products == 1 ? launch_wgrad_tc<CI, CO, 1>(xh, nullptr, in_stride, gh, nullptr, dout_stride, nbr, K,    \
+                                                        num_out_dev, cap_out, perm, tile_mask, partial, stream)      \
+                           : launch_wgrad_tc<CI, CO, 3>(xh, xl, in_stride, gh, gl, dout_stride, nbr, K, num_out_dev, \
+                                                        cap_out, perm, tile_mask, partial, stream);
     B2S_WT_CASE(64, 64) B2S_WT_CASE(64, 32) B2S_WT_CASE(64, 16) B2S_WT_CASE(32, 64) B2S_WT_CASE(32, 32)
     B2S_WT_CASE(32, 16) B2S_WT_CASE(16, 64) B2S_WT_CASE(16, 32) B2S_WT_CASE(16, 16) B2S_WT_CASE(8, 64)
     B2S_WT_CASE(8, 32) B2S_WT_CASE(8, 16)
@@ -513,6 +567,17 @@ extern "C" int b2s_sparse_conv_wgrad_tc(const b2s_half *feat_hi, const b2s_half 
                                                                 num_out_dev, cap_out, scale_dev, dweight);
     B2S_LAUNCH_OK();
     return 0;
+}
+
+extern "C" int b2s_sparse_conv_wgrad_tc(const b2s_half *feat_hi, const b2s_half *feat_lo, int in_stride, int rows_in,
+                                        int cin, const b2s_half *dout_hi, const b2s_half *dout_lo, int dout_stride,
+                                        int cout, const int *nbr, int K, const int *num_out_dev, int cap_out,
+                                        const int *perm, const unsigned *tile_mask, const float *scale_dev,
+                                        float *dweight, void *workspace, size_t workspace_bytes, void *stream)
+{
+    return b2s_sparse_conv_wgrad_tc_ex(feat_hi, feat_lo, in_stride, rows_in, cin, dout_hi, dout_lo, dout_stride, cout,
+                                       nbr, K, num_out_dev, cap_out, perm, tile_mask, scale_dev, dweight, workspace,
+                                       workspace_bytes, 3, stream);
 }
 
 extern "C" int b2s_rulebook_transpose(const int *nbr, const int *num_out_dev, int cap_out, int K, int *nbrT, int cap_in,
@@ -541,10 +606,14 @@ extern "C" int b2s_from_bev(const float *dmap, const int *coors, const int *num_
     return 0;
 }
 
-extern "C" int b2s_split_f16_autoscale(const float *x, b2s_half *hi, b2s_half *lo, const int *num_rows_dev, int cap_rows,
-                                       int row_floats, int out_channels, int out_stride, float *scale_dev, void *stream_)
+// products = 1: lo must be NULL, only the hi plane is written (the same bits as the hi plane of products = 3)
+extern "C" int b2s_split_f16_autoscale_ex(const float *x, b2s_half *hi, b2s_half *lo, const int *num_rows_dev,
+                                          int cap_rows, int row_floats, int out_channels, int out_stride,
+                                          float *scale_dev, int products, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(products == 3 || (products == 1 && lo == nullptr),
+                "b2s_split_f16_autoscale: products must be 3 (hi/lo planes) or 1 (f16, no lo plane)");
     B2S_REQUIRE(row_floats >= 1 && out_channels >= row_floats && out_channels % 8 == 0 && out_stride >= out_channels &&
                     out_stride % 8 == 0 && cap_rows >= 0,
                 "b2s_split_f16_autoscale: out_channels / out_stride must be multiples of 8, out_stride >= out_channels >= "
@@ -560,17 +629,33 @@ extern "C" int b2s_split_f16_autoscale(const float *x, b2s_half *hi, b2s_half *l
         B2S_LAUNCH_OK();
     }
     // one CTA at least: it writes scale_dev[0] even when there are no rows
-    k_split_f16_scaled<<<grid_for((long long)cap_rows * (out_channels / 8)), kThreads, 0, stream>>>(
-        x, reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo), num_rows_dev, cap_rows, row_floats,
-        out_channels, out_stride, scale_dev);
+    if (products == 1)
+        k_split_f16_scaled<1><<<grid_for((long long)cap_rows * (out_channels / 8)), kThreads, 0, stream>>>(
+            x, reinterpret_cast<__half *>(hi), nullptr, num_rows_dev, cap_rows, row_floats, out_channels, out_stride,
+            scale_dev);
+    else
+        k_split_f16_scaled<3><<<grid_for((long long)cap_rows * (out_channels / 8)), kThreads, 0, stream>>>(
+            x, reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo), num_rows_dev, cap_rows, row_floats,
+            out_channels, out_stride, scale_dev);
     B2S_LAUNCH_OK();
     return 0;
 }
 
-extern "C" int b2s_pack_sparse_weights(const float *w, int K, int cin, int cout, int transpose, int flip, b2s_half *hi,
-                                       b2s_half *lo, float *scale_dev, void *stream_)
+extern "C" int b2s_split_f16_autoscale(const float *x, b2s_half *hi, b2s_half *lo, const int *num_rows_dev, int cap_rows,
+                                       int row_floats, int out_channels, int out_stride, float *scale_dev, void *stream)
+{
+    return b2s_split_f16_autoscale_ex(x, hi, lo, num_rows_dev, cap_rows, row_floats, out_channels, out_stride, scale_dev,
+                                      3, stream);
+}
+
+// products = 1: lo must be NULL, only the hi plane is written (the same bits as the hi plane of products = 3)
+extern "C" int b2s_pack_sparse_weights_ex(const float *w, int K, int cin, int cout, int transpose, int flip, b2s_half *hi,
+                                          b2s_half *lo, float *scale_dev, int products, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(products == 3 || (products == 1 && lo == nullptr),
+                "b2s_pack_sparse_weights: products must be 3 (hi/lo planes) or 1 (f16, no lo plane)");
+    if (products == 1) lo = hi;                       // (the checks below; never written)
     const int n_in = transpose ? cout : cin, n_out = transpose ? cin : cout;
     const int n_in_pad = n_in <= 8 ? 8 : n_in;
     B2S_REQUIRE(K >= 1 && cin >= 1 && cout >= 1 && n_in >= 1 && (n_in_pad == 8 || n_in_pad == 16 || n_in_pad == 32 ||
@@ -586,17 +671,32 @@ extern "C" int b2s_pack_sparse_weights(const float *w, int K, int cin, int cout,
     B2S_CUDA_OK(cudaMemsetAsync(scale_dev + 2, 0, sizeof(float), stream));
     k_absmax<<<grid_for(n), kThreads, 0, stream>>>(w, nullptr, 1, (int)n, reinterpret_cast<unsigned *>(scale_dev + 2));
     B2S_LAUNCH_OK();
-    k_pack_sparse_weights<<<grid_for((long long)nkb * n_out * (b2s_tc::BLOCK_K / 8)), kThreads, 0, stream>>>(
-        w, K, cin, cout, transpose, flip ? 1 : 0, n_in, n_in_pad, n_out, nkb, reinterpret_cast<__half *>(hi),
-        reinterpret_cast<__half *>(lo), scale_dev);
+    if (products == 1)
+        k_pack_sparse_weights<1><<<grid_for((long long)nkb * n_out * (b2s_tc::BLOCK_K / 8)), kThreads, 0, stream>>>(
+            w, K, cin, cout, transpose, flip ? 1 : 0, n_in, n_in_pad, n_out, nkb, reinterpret_cast<__half *>(hi), nullptr,
+            scale_dev);
+    else
+        k_pack_sparse_weights<3><<<grid_for((long long)nkb * n_out * (b2s_tc::BLOCK_K / 8)), kThreads, 0, stream>>>(
+            w, K, cin, cout, transpose, flip ? 1 : 0, n_in, n_in_pad, n_out, nkb, reinterpret_cast<__half *>(hi),
+            reinterpret_cast<__half *>(lo), scale_dev);
     B2S_LAUNCH_OK();
     return 0;
 }
 
-extern "C" int b2s_pack_conv2d_weights(const float *w, int cout, int cin, int transpose, b2s_half *hi, b2s_half *lo,
-                                       float *scale_dev, void *stream_)
+extern "C" int b2s_pack_sparse_weights(const float *w, int K, int cin, int cout, int transpose, int flip, b2s_half *hi,
+                                       b2s_half *lo, float *scale_dev, void *stream)
+{
+    return b2s_pack_sparse_weights_ex(w, K, cin, cout, transpose, flip, hi, lo, scale_dev, 3, stream);
+}
+
+// products = 1: lo must be NULL, only the hi plane is written (the same bits as the hi plane of products = 3)
+extern "C" int b2s_pack_conv2d_weights_ex(const float *w, int cout, int cin, int transpose, b2s_half *hi, b2s_half *lo,
+                                          float *scale_dev, int products, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    B2S_REQUIRE(products == 3 || (products == 1 && lo == nullptr),
+                "b2s_pack_conv2d_weights: products must be 3 (hi/lo planes) or 1 (f16, no lo plane)");
+    if (products == 1) lo = hi;                       // (the checks below; never written)
     B2S_REQUIRE(cout >= 1 && cin >= 1 && cout % 64 == 0 && cin % 64 == 0,
                 "b2s_pack_conv2d_weights: cin and cout must be multiples of 64");
     B2S_REQUIRE(transpose == 0 || transpose == 1, "b2s_pack_conv2d_weights: transpose must be 0 or 1");
@@ -610,9 +710,19 @@ extern "C" int b2s_pack_conv2d_weights(const float *w, int cout, int cin, int tr
     B2S_CUDA_OK(cudaMemsetAsync(scale_dev + 2, 0, sizeof(float), stream));
     k_absmax<<<grid_for(n), kThreads, 0, stream>>>(w, nullptr, 1, (int)n, reinterpret_cast<unsigned *>(scale_dev + 2));
     B2S_LAUNCH_OK();
-    k_pack_conv2d_weights<<<grid_for((long long)groups * 9 * n_pad * (n_in / 8)), kThreads, 0, stream>>>(
-        w, cout, cin, transpose, n_in, n_out, n_pad, groups, reinterpret_cast<__half *>(hi),
-        reinterpret_cast<__half *>(lo), scale_dev);
+    if (products == 1)
+        k_pack_conv2d_weights<1><<<grid_for((long long)groups * 9 * n_pad * (n_in / 8)), kThreads, 0, stream>>>(
+            w, cout, cin, transpose, n_in, n_out, n_pad, groups, reinterpret_cast<__half *>(hi), nullptr, scale_dev);
+    else
+        k_pack_conv2d_weights<3><<<grid_for((long long)groups * 9 * n_pad * (n_in / 8)), kThreads, 0, stream>>>(
+            w, cout, cin, transpose, n_in, n_out, n_pad, groups, reinterpret_cast<__half *>(hi),
+            reinterpret_cast<__half *>(lo), scale_dev);
     B2S_LAUNCH_OK();
     return 0;
+}
+
+extern "C" int b2s_pack_conv2d_weights(const float *w, int cout, int cin, int transpose, b2s_half *hi, b2s_half *lo,
+                                       float *scale_dev, void *stream)
+{
+    return b2s_pack_conv2d_weights_ex(w, cout, cin, transpose, hi, lo, scale_dev, 3, stream);
 }

@@ -169,22 +169,22 @@ class _SparseConvFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, feats, weight, bias, conv, rb):
-        ctx.conv, ctx.rb = conv, rb
+        ctx.conv, ctx.rb, ctx.products = conv, rb, conv._b2s_products
         ctx.save_for_backward(feats, weight)
-        out, ctx.x_split = conv._forward_rows(feats, rb)
+        out, ctx.x_split = conv._forward_rows(feats, rb, ctx.products)
         return out
 
     @staticmethod
     def backward(ctx, dy):
         feats, weight = ctx.saved_tensors
-        conv, rb = ctx.conv, ctx.rb
+        conv, rb, products = ctx.conv, ctx.rb, ctx.products
         dy = dy.contiguous().float()
-        split = _GradSplit(dy)
+        split = _GradSplit(dy, products=products)
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
-            dx = conv._dgrad(dy, weight, rb, feats.shape[0], split)
+            dx = conv._dgrad(dy, weight, rb, feats.shape[0], split, products)
         if ctx.needs_input_grad[1]:
-            dw = conv._wgrad(feats, dy, rb, split, ctx.x_split).view_as(weight)
+            dw = conv._wgrad(feats, dy, rb, split, ctx.x_split, products).view_as(weight)
         if ctx.needs_input_grad[2]:
             db = dy.sum(0)
         return dx, dw, db, None, None
@@ -193,12 +193,23 @@ class _SparseConvFunction(torch.autograd.Function):
 class _GradSplit:
     """fp32 rows [n, c] as fp16 hi/lo planes of `channels` (>= c, zero padded) halves, scaled by a power of two picked on
     the device (b2s_split_f16_autoscale), made on first use -- dY shared by the tensor-pipe dgrad and wgrad, and X for the
-    wgrad: (hi, lo, row stride in halves, 2^-e as a [1] device tensor)."""
+    wgrad: (hi, lo, row stride in halves, 2^-e as a [1] device tensor).  products = 1 (the f16 mode): the hi plane only,
+    lo is None."""
 
-    def __init__(self, t, channels=None):
-        self.t, self.channels, self._planes = t, channels, None
+    def __init__(self, t, channels=None, products=3):
+        self.t, self.channels, self.products, self._planes = t, channels, products, None
 
     def planes(self):
+        if self._planes is None and self.products == 1:
+            t = self.t
+            n, c = t.shape
+            cp = self.channels or c
+            hi = torch.empty(max(n, 1), cp, dtype=torch.float16, device=t.device)
+            sc = torch.empty(2, dtype=torch.float32, device=t.device)
+            _lib.check(_lib.load().b2s_split_f16_autoscale_ex(_lib.ptr(t), _lib.ptr(hi), None, None, n, c, cp, cp,
+                                                              _lib.ptr(sc), 1, _lib.stream()),
+                       "b2s_split_f16_autoscale_ex")
+            self._planes = (hi, None, cp, sc[:1])
         if self._planes is None:
             t = self.t
             n, c = t.shape
@@ -300,33 +311,47 @@ class SparseSequential(SparseModule):
         return input
 
 
-def _pack_tc_weights(w, transpose=False, flip=False):
+def _pack_tc_weights(w, transpose=False, flip=False, products=3):
     """fp32 weight [K, Cin, Cout] -> (hi, lo, s, 1/s): the fp16 planes of W[k] (transpose: W[k]^T, flip: W[K-1-k]^T) in
     the tensor-core kernel's packed layout, pre-scaled by the power of two s of b2second.tc.pow2_scale, with s and 1/s as
     [1] device tensors.  b2s_pack_sparse_weights reduces max|w| on the device, so nothing is read on the host; the
     planes and the scale are bit for bit tc.split_f16(tc.pack_sparse_weights(...), tc.pow2_scale(...)) for finite weights
-    (a non-finite weight is packed as itself, not saturated)."""
+    (a non-finite weight is packed as itself, not saturated).  products = 1 (the f16 mode): the hi plane only, lo is
+    None."""
     lib = _lib.load()
     K, cin, cout = (int(v) for v in w.shape)
     n_in, n_out = (cout, cin) if transpose else (cin, cout)
     n_in_pad = 8 if n_in <= 8 else n_in
     pack = 64 // n_in_pad
     hi = torch.empty((K + pack - 1) // pack, n_out, 64, dtype=torch.float16, device=w.device)
-    lo = torch.empty_like(hi)
     sc = torch.empty(3, dtype=torch.float32, device=w.device)
+    if products == 1:
+        _lib.check(lib.b2s_pack_sparse_weights_ex(_lib.ptr(w), K, cin, cout, int(transpose), int(flip), _lib.ptr(hi), None,
+                                                  _lib.ptr(sc), 1, _lib.stream()), "b2s_pack_sparse_weights_ex")
+        return hi, None, sc[0:1], sc[1:2]
+    lo = torch.empty_like(hi)
     _lib.check(lib.b2s_pack_sparse_weights(_lib.ptr(w), K, cin, cout, int(transpose), int(flip), _lib.ptr(hi),
                                            _lib.ptr(lo), _lib.ptr(sc), _lib.stream()), "b2s_pack_sparse_weights")
     return hi, lo, sc[0:1], sc[1:2]
 
 
-def _conv_tc(x, w, table, K, n_dev, n_out, plan, scale, shift, relu, out, out_lo=None):
+def _conv_tc(x, w, table, K, n_dev, n_out, plan, scale, shift, relu, out, out_lo=None, products=3):
     """one b2s_sparse_conv_tc_plan launch for the first n_out rows of `table`: fp16 input planes x = (hi, lo, row stride)
     as wide as Cin, packed weight planes w = (hi, lo), plan = ops.tile_plan's (perm, tile_mask); `out` as wide as Cout
-    is fp32 rows, or with `out_lo` the hi plane of fp16 hi/lo rows.  -> the status word, None when there are no rows."""
+    is fp32 rows, or with `out_lo` the hi plane of fp16 hi/lo rows.  -> the status word, None when there are no rows.
+    products = 1 (the f16 training mode): single planes (the lo entries None) and fp32 rows out, through
+    b2s_sparse_conv_tc_plan_ex2."""
     if n_out == 0:
         return None
     (hi, lo, stride), (w_hi, w_lo), (perm, tmask) = x, w, plan
     status = torch.zeros(1, dtype=torch.int32, device=out.device)
+    if products == 1:
+        _lib.check(_lib.load().b2s_sparse_conv_tc_plan_ex2(
+            _lib.ptr(hi), None, stride, hi.shape[0], hi.shape[1], _lib.ptr(w_hi), None, _lib.ptr(table), K,
+            _lib.ptr(n_dev), n_out, _lib.ptr(perm), _lib.ptr(tmask), _lib.ptr(scale), _lib.ptr(shift), int(relu),
+            _lib.ptr(out), None, out.stride(0), out.shape[1], 1, 1, _lib.ptr(status), _lib.stream()),
+            "b2s_sparse_conv_tc_plan_ex2")
+        return status
     _lib.check(_lib.load().b2s_sparse_conv_tc_plan(
         _lib.ptr(hi), _lib.ptr(lo), stride, hi.shape[0], hi.shape[1], _lib.ptr(w_hi), _lib.ptr(w_lo), _lib.ptr(table), K,
         _lib.ptr(n_dev), n_out, _lib.ptr(perm), _lib.ptr(tmask), _lib.ptr(scale), _lib.ptr(shift), int(relu),
@@ -388,17 +413,19 @@ class SparseConvolution(SparseModule):
             bound = 1 / math.sqrt(fan_in)
             nn.init.uniform_(self.bias, -bound, bound)
 
-    def _tc_weights(self, cin_tc):
+    def _tc_weights(self, cin_tc, products=3):
         """fp16 hi/lo planes of the (power-of-two scaled) weight in the tensor-core kernel's layout, the scale as a [1]
-        device tensor and its inverse per output channel; cached until the parameter changes."""
+        device tensor and its inverse per output channel; cached until the parameter or the product count changes
+        (products = 1: the hi plane only, lo None)."""
         w = self.weight
-        key = (w.data_ptr(), w._version, str(w.device))
+        key = (w.data_ptr(), w._version, str(w.device), products)
         cached = getattr(self, "_b2s_tc_w", None)
         if cached is None or cached[0] != key:
             K = int(np.prod(self.kernel_size))
             with torch.no_grad():
-                hi, lo, ws, inv = _pack_tc_weights(w.detach().float().contiguous().view(K, self.in_channels,
-                                                                                        self.out_channels))
+                wk = w.detach().float().contiguous().view(K, self.in_channels, self.out_channels)
+                # the 3xF16 call keeps its form (products is passed only in the f16 mode)
+                hi, lo, ws, inv = _pack_tc_weights(wk) if products == 3 else _pack_tc_weights(wk, products=products)
                 inv = inv.expand(self.out_channels).contiguous()
             cached = (key, hi, lo, ws, inv)
             self._b2s_tc_w = cached
@@ -480,14 +507,17 @@ class SparseConvolution(SparseModule):
         _conv_fma(feats, w, rb.nbr, rb.num_out_dev, n_out, scale, shift, relu, out._features)
         return out
 
-    # ---- training (b2second.training.enable_sparse_backward sets _b2s_backward) --------------------------------------
+    # ---- training (b2second.training.enable_sparse_backward sets _b2s_backward and _b2s_products) ---------------------
     _b2s_backward = False
+    _b2s_products = 3       # tensor-pipe products per MAC in training: 3 (3xF16, fp32-grade) or 1 (the f16 mode)
 
-    def _forward_rows(self, feats, rb):
+    def _forward_rows(self, feats, rb, products=None):
         """(fp32 output rows [n_out, Cout] (+ bias) from fp32 input rows, the _GradSplit of X or None) on the kernel the
         inference path would pick (tensor pipe with fp32 output, or b2s_sparse_conv).  On the tensor pipe X is split
         under its own power-of-two scale, as in the backward: unscaled, an activation above 65504 would saturate and one
-        below 2^-3 keep only 2^-25 absolute precision.  The split is kept for the weight gradient."""
+        below 2^-3 keep only 2^-25 absolute precision.  The split is kept for the weight gradient.  products: the
+        tensor-pipe product count (None: the module's _b2s_products)."""
+        products = self._b2s_products if products is None else products
         lib = _lib.load()
         K, n_out = rb.K, rb.num_out
         dev = feats.device
@@ -497,12 +527,12 @@ class SparseConvolution(SparseModule):
             return out, None
         cin_tc = self._wgrad_tc_cin(lib, K)
         if cin_tc is not None:
-            split = _GradSplit(feats, cin_tc)
+            split = _GradSplit(feats, cin_tc, products)
             hi, lo, stride, inv_x = split.planes()
-            w_hi, w_lo, ws, inv = self._tc_weights(cin_tc)
+            w_hi, w_lo, ws, inv = self._tc_weights(cin_tc, products)
             scale = inv * inv_x                                        # powers of two: exact, no host sync
             _conv_tc((hi, lo, stride), (w_hi, w_lo), rb.nbr, K, rb.num_out_dev, n_out, ops.tile_plan(rb), scale, shift,
-                     False, out)
+                     False, out, products=products)
             return out, split
         w = self.weight.detach().float().contiguous().view(K, self.in_channels, self.out_channels)
         _conv_fma(feats, w, rb.nbr, rb.num_out_dev, n_out, None, shift, False, out)
@@ -514,26 +544,28 @@ class SparseConvolution(SparseModule):
         from b2second import tc as _tc
         return _tc.sparse_tc_channels(lib, self.in_channels, self.out_channels, K) if USE_TENSOR_CORES else None
 
-    def _dgrad_weights(self, w, flip):
+    def _dgrad_weights(self, w, flip, products=3):
         """packed fp16 hi/lo planes of W'[k] = W[k]^T (flip: W[K-1-k]^T) for the tensor-pipe input gradient, with their
-        power-of-two scale as a [1] device tensor; cached until the weight changes (one scale measurement per weight
-        version)."""
-        key = (w.data_ptr(), w._version, str(w.device), flip)
+        power-of-two scale as a [1] device tensor; cached until the weight or the product count changes (one scale
+        measurement per weight version; products = 1: the hi plane only, lo None)."""
+        key = (w.data_ptr(), w._version, str(w.device), flip, products)
         cached = getattr(self, "_b2s_tc_wt", None)
         if cached is None or cached[0] != key:
             K = int(np.prod(self.kernel_size))
             with torch.no_grad():
                 wk = w.detach().float().contiguous().view(K, self.in_channels, self.out_channels)
-                hi, lo, ws, _ = _pack_tc_weights(wk, transpose=True, flip=flip)
+                hi, lo, ws, _ = (_pack_tc_weights(wk, transpose=True, flip=flip) if products == 3 else
+                                 _pack_tc_weights(wk, transpose=True, flip=flip, products=products))
             cached = (key, hi, lo, ws)
             self._b2s_tc_wt = cached
         return cached[1:]
 
-    def _dgrad(self, dy, weight, rb, n_in, split=None):
+    def _dgrad(self, dy, weight, rb, n_in, split=None, products=None):
         """input gradient [n_in, Cin] = the forward contraction of dY [n_out, Cout] over the transposed table with
         W'[k] = W[k]^T.  A SubM table with odd kernel sizes is its own transpose under k <-> K-1-k (same table, same tile
         plan, W'[k] = W[K-1-k]^T); any other table is transposed once (ops.transpose_rulebook)."""
         from b2second import tc as _tc
+        products = self._b2s_products if products is None else products
         lib = _lib.load()
         K, cin, cout, n_out = rb.K, self.in_channels, self.out_channels, rb.num_out
         dev = dy.device
@@ -544,40 +576,50 @@ class SparseConvolution(SparseModule):
             table, n_dev, plan = rb.nbr, rb.num_out_dev, ops.tile_plan(rb)
         else:
             table, plan = ops.transpose_rulebook(rb, n_in), (None, None)
-            n_dev = torch.tensor([n_in], dtype=torch.int32, device=dev)
+            n_dev = rb.nbrT_rows_dev                    # cached with the table: no host copy, the backward can be captured
         dx = torch.empty(n_in, cin, dtype=torch.float32, device=dev)
         # the contraction runs Cout -> Cin; dY is not padded, so it takes the tensor pipe only at an unpadded width
         if USE_TENSOR_CORES and _tc.sparse_tc_channels(lib, cout, cin, K) == cout:
             # dY goes onto the tensor pipe scaled by a power of two picked on the device (gradients are often far below
             # the fp16 normal range); the kernel's epilogue scale undoes both that and the weights' scale
-            w_hi, w_lo, ws = self._dgrad_weights(weight, flip)
-            g_hi, g_lo, g_stride, inv = (split or _GradSplit(dy)).planes()
+            w_hi, w_lo, ws = self._dgrad_weights(weight, flip, products)
+            g_hi, g_lo, g_stride, inv = (split or _GradSplit(dy, products=products)).planes()
             scale = (inv / ws).expand(cin).contiguous()
-            _conv_tc((g_hi, g_lo, g_stride), (w_hi, w_lo), table, K, n_dev, n_in, plan, scale, None, False, dx)
+            _conv_tc((g_hi, g_lo, g_stride), (w_hi, w_lo), table, K, n_dev, n_in, plan, scale, None, False, dx,
+                     products=products)
             return dx
         w = weight.detach().float().reshape(K, cin, cout)
         wt = (w.flip(0) if flip else w).transpose(1, 2).contiguous()        # [K, Cout, Cin]
         _conv_fma(dy, wt, table, n_dev, n_in, None, None, False, dx)
         return dx
 
-    def _wgrad(self, feats, dy, rb, split=None, x_split=None):
+    def _wgrad(self, feats, dy, rb, split=None, x_split=None, products=None):
         """weight gradient [K, Cin, Cout] = sum over output rows of X[nbr[o,k]]^T dY[o]: b2s_sparse_conv_wgrad_tc on the
         tensor pipe, b2s_sparse_conv_wgrad (fp32 FMA) otherwise.  On the tensor pipe both operands are split under their
         own power-of-two scale (b2s_split_f16_autoscale; X's split is the forward's when given): unscaled, a small
         activation would keep only 2^-25 absolute precision, which a weight gradient of few pairs would see; rows are
-        reduced in the forward's tile-plan order."""
+        reduced in the forward's tile-plan order.  products = 1 (the f16 mode): b2s_sparse_conv_wgrad_tc_ex on the hi
+        planes."""
+        products = self._b2s_products if products is None else products
         lib = _lib.load()
         K, cin, cout, n_out = rb.K, self.in_channels, self.out_channels, rb.num_out
         dev = dy.device
         cin_tc = self._wgrad_tc_cin(lib, K)
         if cin_tc is not None and n_out > 0 and feats.shape[0] > 0:
-            x_hi, x_lo, x_stride, inv_x = (x_split or _GradSplit(feats, cin_tc)).planes()
-            g_hi, g_lo, g_stride, inv_g = (split or _GradSplit(dy)).planes()
+            x_hi, x_lo, x_stride, inv_x = (x_split or _GradSplit(feats, cin_tc, products)).planes()
+            g_hi, g_lo, g_stride, inv_g = (split or _GradSplit(dy, products=products)).planes()
             scale = inv_x * inv_g                                      # powers of two: exact
             perm, tmask = ops.tile_plan(rb)
             dw = torch.empty(K, cin_tc, cout, dtype=torch.float32, device=dev)
             ws_bytes = lib.b2s_sparse_conv_wgrad_tc_workspace_bytes(n_out, K, cin_tc, cout)
             work = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+            if products == 1:
+                _lib.check(lib.b2s_sparse_conv_wgrad_tc_ex(
+                    _lib.ptr(x_hi), None, x_stride, x_hi.shape[0], cin_tc, _lib.ptr(g_hi), None, g_stride, cout,
+                    _lib.ptr(rb.nbr.contiguous()), K, _lib.ptr(rb.num_out_dev), n_out, _lib.ptr(perm), _lib.ptr(tmask),
+                    _lib.ptr(scale), _lib.ptr(dw), _lib.ptr(work), ws_bytes, 1, _lib.stream()),
+                    "b2s_sparse_conv_wgrad_tc_ex")
+                return dw if cin_tc == cin else dw[:, :cin].contiguous()
             _lib.check(lib.b2s_sparse_conv_wgrad_tc(
                 _lib.ptr(x_hi), _lib.ptr(x_lo), x_stride, x_hi.shape[0], cin_tc, _lib.ptr(g_hi), _lib.ptr(g_lo), g_stride,
                 cout, _lib.ptr(rb.nbr.contiguous()), K, _lib.ptr(rb.num_out_dev), n_out, _lib.ptr(perm), _lib.ptr(tmask),

@@ -66,11 +66,16 @@ SIGNATURES = {
     "b2s_sparse_conv_tc_plan_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                            c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                            c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "b2s_sparse_conv_tc_plan_ex2": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                            c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                            c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b2s_split_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b2s_split_f16_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "b2s_merge_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b2s_split_f16_autoscale": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
                                         c_void_p]),
+    "b2s_split_f16_autoscale_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                           c_int, c_void_p]),
     "b2s_rulebook_transpose": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "b2s_sparse_conv_wgrad_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "b2s_sparse_conv_wgrad": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
@@ -79,6 +84,9 @@ SIGNATURES = {
     "b2s_sparse_conv_wgrad_tc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
                                          c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_size_t, c_void_p]),
+    "b2s_sparse_conv_wgrad_tc_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
+                                            c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_size_t, c_int, c_void_p]),
     "b2s_pfn_train_workspace_bytes": (c_size_t, [c_int]),
     "b2s_pfn_train_forward": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_int, c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_float, c_float,
@@ -195,6 +203,13 @@ SIGNATURES = {
                                   c_void_p, c_size_t, c_void_p, c_void_p]),
     "b2s_pack_sparse_weights": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                         c_void_p]),
+    "b2s_pack_sparse_weights_ex": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_int, c_void_p]),
+    "b2s_split_halo_f16_autoscale_ex": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                                c_void_p, c_void_p, c_int, c_void_p]),
+    "b2s_pack_conv2d_weights_ex": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "b2s_conv2d_wgrad_tc_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                       c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
     "b2s_split_halo_f16_autoscale": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                              c_void_p, c_void_p]),
     "b2s_pack_conv2d_weights": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -28,7 +28,7 @@ def _pow2_at_least(n):
 class Rulebook:
     """output-stationary rulebook: ``nbr[o,k]`` = input row feeding output row ``o`` via offset ``k`` (-1: none)."""
     __slots__ = ("out_indices", "nbr", "num_out", "num_out_dev", "out_hash", "K", "out_shape", "subm", "row_mask", "ksize", "plan",
-                 "nbrT")
+                 "nbrT", "nbrT_rows_dev")
 
     # tuple-style access keeps code written against upstream's (outids, indices, pairs, pair_num, shape) working
     def __iter__(self):
@@ -52,6 +52,7 @@ def build_rulebook(x, ksize, stride, padding, dilation, subm):
     rb.ksize = [int(k) for k in ksize]
     rb.plan = None
     rb.nbrT = None
+    rb.nbrT_rows_dev = None
     if subm:
         keys, vals, cap = x._locator()
         nbr = torch.empty(max(n_in, 1), K, dtype=torch.int32, device=dev)
@@ -119,13 +120,15 @@ def tile_plan(rb):
 
 def transpose_rulebook(rb, n_in):
     """input-side table of a rulebook, ``nbrT [n_in, K]``: ``nbrT[i, k] = o`` where ``nbr[o, k] = i`` (-1: none) --
-    what the input gradient of a strided conv gathers through.  Built on first use and cached on the rulebook."""
+    what the input gradient of a strided conv gathers through.  Built on first use and cached on the rulebook, with its
+    row count n_in as a [1] device tensor (``rb.nbrT_rows_dev``), so a backward makes no host copy and can be captured."""
     if rb.nbrT is None or rb.nbrT.shape[0] != n_in:
         lib = _lib.load()
         nbrT = torch.empty(max(n_in, 1), rb.K, dtype=torch.int32, device=rb.nbr.device)
         _lib.check(lib.b2s_rulebook_transpose(_lib.ptr(rb.nbr.contiguous()), _lib.ptr(rb.num_out_dev), rb.num_out, rb.K,
                                               _lib.ptr(nbrT), n_in, None, _lib.stream()), "b2s_rulebook_transpose")
         rb.nbrT = nbrT[:n_in]
+        rb.nbrT_rows_dev = torch.tensor([n_in], dtype=torch.int32, device=rb.nbr.device)
     return rb.nbrT
 
 
