@@ -73,7 +73,8 @@
  *                       torch.nn.utils.clip_grad_norm_, OptimWrapper.step (torchplus/train/fastai_optim.py:154-167) over
  *                       torch.optim.Adam (second/pytorch/builder/optimizer_builder.py:68-87) and zero_grad
  *   b2s_train_metrics   VoxelNet.update_metrics (second/pytorch/models/voxelnet.py:654-679, torchplus/metrics.py) and the
- *                       log figures of train.py:335-373
+ *                       log figures of train.py:335-373; b2s_train_metrics_count / _finish split it so the counts of
+ *                       several data-parallel ranks can be added in between (train.py:203-204 multi_gpu)
  *   b2s_pack_sparse_weights
  *                       the tensor-core weight planes of a sparse conv in training (tc.pack_sparse_weights, pow2_scale,
  *                       split_f16 in SparseConvolution._tc_weights / _dgrad_weights) on the device
@@ -973,6 +974,37 @@ int b2s_train_metrics(const float *cls_preds, int num_class, const void *labels,
                       const float *cls_pos_loss, const float *cls_neg_loss, const float *dir_loss,
                       const b2s_metrics_buffers *buffers, float *record, void *workspace, size_t workspace_bytes,
                       unsigned *status_dev, void *stream);
+/* The same step in two halves, so the counts of several shares of a batch (one per data-parallel rank) can be added
+ * before the buffers are updated.  b2s_train_metrics_count takes b2s_train_metrics' inputs and writes this share's
+ * count record, float32 [B2S_METRICS_COUNT_HEAD + 2 * num_thresholds]: */
+#define B2S_METRICS_CNT_FRAMES 0        /* batch */
+#define B2S_METRICS_CNT_CORRECT 1       /* anchors with pred == label (Accuracy's total) */
+#define B2S_METRICS_CNT_CARED 2         /* cared anchors */
+#define B2S_METRICS_CNT_POS 3           /* cared anchors with label > 0 */
+#define B2S_METRICS_CNT_NUM_POS 4       /* labels > 0 in frame 0 (0 when has_frame0 is 0) */
+#define B2S_METRICS_CNT_NUM_NEG 5       /* labels == 0 in frame 0 (0 when has_frame0 is 0) */
+#define B2S_METRICS_CNT_NUM_ANCHORS 6   /* anchors_mask set in frame 0 (0 when has_frame0 is 0) */
+#define B2S_METRICS_CNT_CLS_LOSS 7      /* *cls_loss */
+#define B2S_METRICS_CNT_LOC_LOSS 8      /* *loc_loss */
+#define B2S_METRICS_CNT_CLS_POS 9       /* *cls_pos_loss (0 when NULL) */
+#define B2S_METRICS_CNT_CLS_NEG 10      /* *cls_neg_loss (0 when NULL) */
+#define B2S_METRICS_CNT_DIR 11          /* *dir_loss (0 when NULL) */
+#define B2S_METRICS_CNT_LOC_ELEM 12     /* [B2S_METRICS_MAX_CODE]: loc_loss_elem[:, :, j] summed (float64, rounded once) */
+#define B2S_METRICS_COUNT_HEAD 20       /* then tp[T] and fp[T]: cared positives / negatives scored above each threshold */
+/* Every count is an integer below 2^24, so the float32 records of several shares add exactly.  Summed over W shares,
+ * the five loss slots hold W times the replica mean, which b2s_train_metrics_finish scales back by loss_scale (1/W).
+ * b2s_train_metrics_finish reads such a (possibly summed) record on the device, updates the running buffers in the
+ * reference's order and writes the record b2s_train_metrics writes; with loss_scale 1, count followed by finish on one
+ * share is b2s_train_metrics bit for bit.  loc_elem of the log record is the summed slot over the summed frame count.
+ * No sync; finish needs no workspace. */
+int b2s_train_metrics_count(const float *cls_preds, int num_class, const void *labels, int labels_int64,
+                            const uint8_t *cared, int batch, int num_anchors, const b2s_metrics_params *params,
+                            const float *cls_loss, const float *loc_loss, const float *loc_loss_elem, int code_size,
+                            const uint8_t *anchors_mask, const float *cls_pos_loss, const float *cls_neg_loss,
+                            const float *dir_loss, int has_frame0, float *counts, void *workspace,
+                            size_t workspace_bytes, unsigned *status_dev, void *stream);
+int b2s_train_metrics_finish(const float *counts, const b2s_metrics_params *params, float loss_scale,
+                             const b2s_metrics_buffers *buffers, float *record, void *stream);
 
 /* ---- sparse conv weights on the tensor pipe (b2second/tc.py: pack_sparse_weights, pow2_scale, split_f16) -------- */
 /* w [K, cin, cout] float32 (spconv's layout) -> the fp16 hi/lo planes b2s_sparse_conv_tc(_plan) takes as its B operand,

@@ -106,6 +106,18 @@ def draw(rs, settings, num_gt_per_frame, num_points_per_frame):
         num_gt=[int(v) for v in num_gt_per_frame], num_points=[int(v) for v in num_points_per_frame])
 
 
+def select(draws, start, stop):
+    """-> the Draws of frames ``start .. stop - 1`` of ``draws``: a data-parallel rank's share of draws made for the
+    whole batch in single-process order, so the augmentation does not depend on the number of ranks."""
+    g = np.cumsum([0] + list(draws.num_gt))
+    p = np.cumsum([0] + list(draws.num_points))
+    return Draws(
+        loc_noise=None if draws.loc_noise is None else draws.loc_noise[g[start]:g[stop]],
+        rot_noise=None if draws.rot_noise is None else draws.rot_noise[g[start]:g[stop]],
+        frame=draws.frame[start:stop], perm=None if draws.perm is None else draws.perm[p[start]:p[stop]],
+        num_gt=list(draws.num_gt[start:stop]), num_points=list(draws.num_points[start:stop]))
+
+
 def _to_device(a, device, dtype):
     t = torch.from_numpy(np.ascontiguousarray(a, dtype=dtype))
     if t.numel() == 0:

@@ -214,6 +214,14 @@ def draw(rs, state, gt_names_per_frame):
                       offsets=np.asarray(offs, np.int32))
 
 
+def select(candidates, start, stop):
+    """-> the Candidates of frames ``start .. stop - 1``: a data-parallel rank's share of candidates drawn for the whole
+    batch in single-process order, so the sampling does not depend on the number of ranks."""
+    o = candidates.offsets
+    return Candidates(objects=candidates.objects[o[start]:o[stop]], group=candidates.group[o[start]:o[stop]],
+                      offsets=(o[start:stop + 1] - o[start]).astype(np.int32))
+
+
 # ------------------------------------------------------------------------------------------------ device
 class SampleResult(dict):
     """device outputs of ``sample_batch``: points float32 [P + CP, F], point_offsets int32 [B+1], boxes [G + C, ndim],

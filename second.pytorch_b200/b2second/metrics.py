@@ -18,6 +18,7 @@ conditionals, so ``state_dict()`` and checkpoints are unchanged.  ``plan`` reads
 attribute names; sigmoid scores with background encoded as zeros (what every config uses) are covered, anything else
 raises ``spec.UnsupportedNetwork``.
 """
+import ctypes
 import types
 
 import numpy as np
@@ -110,6 +111,7 @@ class MetricsPlan:
         self.num_class = num_class
         self.last_status = None
         self._params = None
+        self._count_log = (0, [False] * 3)
 
     def params(self):
         """b2s_metrics_params as a ctypes structure (host memory, read by the call)."""
@@ -139,11 +141,9 @@ class MetricsPlan:
             setattr(b, name, t.data_ptr())
         return b
 
-    def update_metrics_async(self, cls_loss, loc_loss, cls_preds, labels, sampled, ret_dict=None, anchors_mask=None):
-        """launch one step's metrics (VoxelNet.update_metrics' arguments: the reduced cls / loc losses, cls_preds,
-        labels, and the 0/1 weights ``sampled`` -- the loss's ``cared``); -> MetricsHandle.  ``ret_dict`` (the loss
-        dict) and ``anchors_mask`` (the example's, if any) add train.py's log figures.  No host synchronisation."""
-        L, lib = _lib()
+    def _inputs(self, cls_loss, loc_loss, cls_preds, labels, sampled, ret_dict, anchors_mask):
+        """the launch arguments of one share's metrics, checked: the b2s_train_metrics(_count) inputs after num_anchors"""
+        L, _ = _lib()
         B = int(cls_preds.shape[0])
         C = self.num_class
         cls = cls_preds.detach()
@@ -152,7 +152,6 @@ class MetricsPlan:
             raise TypeError("cls_preds must be float32, got %s" % cls.dtype)
         cls = cls.contiguous().view(B, -1, C)
         A = int(cls.shape[1])
-        dev = cls.device
         if labels.dtype not in (torch.int32, torch.int64):
             labels = labels.to(torch.int64)
         labels = labels.contiguous().view(B, A)
@@ -181,23 +180,80 @@ class MetricsPlan:
             tensors.append(("anchors_mask", mask))
         for name, t in tensors:
             L.require_cuda(t, name)
+        sc = [extra[k].view(-1)[:1] if extra[k] is not None else None
+              for k in ("cls_pos_loss", "cls_neg_loss", "dir_loss_reduced")]
+        args = [L.ptr(cls), C, L.ptr(labels), int(labels.dtype == torch.int64), L.ptr(cared), B, A,
+                ctypes.byref(self.params()), L.ptr(scal[0]), L.ptr(scal[1]), L.ptr(loc_elem), code, L.ptr(mask),
+                L.ptr(sc[0]), L.ptr(sc[1]), L.ptr(sc[2])]
+        keep = (cls, labels, cared, scal, extra, mask)
+        return args, keep, cls.device, B, A, code, [s is not None for s in sc]
+
+    def update_metrics_async(self, cls_loss, loc_loss, cls_preds, labels, sampled, ret_dict=None, anchors_mask=None):
+        """launch one step's metrics (VoxelNet.update_metrics' arguments: the reduced cls / loc losses, cls_preds,
+        labels, and the 0/1 weights ``sampled`` -- the loss's ``cared``); -> MetricsHandle.  ``ret_dict`` (the loss
+        dict) and ``anchors_mask`` (the example's, if any) add train.py's log figures.  No host synchronisation.
+
+        Under data parallelism (``b2second.dist.enable_data_parallel(net)``) the arguments are this rank's share: its
+        count record is summed over the ranks (one all-reduce) before the buffers are updated, so every rank's buffers
+        and record are those of the whole batch, with the replica-mean losses and the global frame 0's figures."""
+        dp = getattr(self.net, "b2s_data_parallel", None)
+        if dp is not None:
+            counts = self.count(cls_loss, loc_loss, cls_preds, labels, sampled, ret_dict, anchors_mask,
+                                has_frame0=dp.rank == 0)
+            dp.all_reduce_sum(counts)
+            return self.finish(counts, 1.0 / dp.world)
+        L, lib = _lib()
+        args, keep, dev, B, A, code, have = self._inputs(cls_loss, loc_loss, cls_preds, labels, sampled, ret_dict,
+                                                          anchors_mask)
         T = len(self.thresholds)
         record = torch.empty(L.METRICS_RECORD_HEAD + 2 * T, dtype=torch.float32, device=dev)
         status = torch.zeros(1, dtype=torch.int32, device=dev)
         ws_bytes = lib.b2s_train_metrics_workspace_bytes(B, A)
         ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
         bufs = self._buffers(dev)
-        sc = [extra[k].view(-1)[:1] if extra[k] is not None else None
-              for k in ("cls_pos_loss", "cls_neg_loss", "dir_loss_reduced")]
-        import ctypes
         with torch.cuda.device(dev):
-            L.check(lib.b2s_train_metrics(
-                L.ptr(cls), C, L.ptr(labels), int(labels.dtype == torch.int64), L.ptr(cared), B, A,
-                ctypes.byref(self.params()), L.ptr(scal[0]), L.ptr(scal[1]), L.ptr(loc_elem), code, L.ptr(mask),
-                L.ptr(sc[0]), L.ptr(sc[1]), L.ptr(sc[2]), ctypes.byref(bufs), L.ptr(record), L.ptr(ws), ws_bytes,
-                L.ptr(status), L.stream()), "b2s_train_metrics")
+            L.check(lib.b2s_train_metrics(*args, ctypes.byref(bufs), L.ptr(record), L.ptr(ws), ws_bytes,
+                                          L.ptr(status), L.stream()), "b2s_train_metrics")
         self.last_status = status        # device word; nonzero: a label outside [-1, num_class]
-        return MetricsHandle(self, record, status, code, [s is not None for s in sc])
+        return MetricsHandle(self, record, status, code, have)
+
+    def count(self, cls_loss, loc_loss, cls_preds, labels, sampled, ret_dict=None, anchors_mask=None, has_frame0=True):
+        """the first half of ``update_metrics_async`` on one share of a batch: -> its count record (device float32
+        [METRICS_COUNT_HEAD + 2 * T], include/b2second.h B2S_METRICS_CNT_*).  Records of several shares add exactly;
+        ``has_frame0`` False leaves the frame-0 figures zero, for shares that do not hold the batch's first frame."""
+        L, lib = _lib()
+        args, keep, dev, B, A, code, have = self._inputs(cls_loss, loc_loss, cls_preds, labels, sampled, ret_dict,
+                                                          anchors_mask)
+        T = len(self.thresholds)
+        counts = torch.empty(L.METRICS_COUNT_HEAD + 2 * T, dtype=torch.float32, device=dev)
+        status = torch.zeros(1, dtype=torch.int32, device=dev)
+        ws_bytes = lib.b2s_train_metrics_workspace_bytes(B, A)
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            L.check(lib.b2s_train_metrics_count(*args, int(bool(has_frame0)), L.ptr(counts), L.ptr(ws), ws_bytes,
+                                                L.ptr(status), L.stream()), "b2s_train_metrics_count")
+        self.last_status = status
+        self._count_log = (code, have)       # which log fields the last count's inputs held
+        return counts
+
+    def finish(self, counts, loss_scale=1.0):
+        """the second half: update the running buffers from a (summed) count record, the five loss slots scaled by
+        ``loss_scale`` (1/W for a sum over W ranks); -> MetricsHandle.  No host synchronisation."""
+        L, lib = _lib()
+        L.require_cuda(counts, "counts")
+        T = len(self.thresholds)
+        if counts.dtype != torch.float32 or counts.numel() != L.METRICS_COUNT_HEAD + 2 * T:
+            raise ValueError("counts must be a float32 count record of %d entries" % (L.METRICS_COUNT_HEAD + 2 * T))
+        dev = counts.device
+        counts = counts.contiguous()
+        record = torch.empty(L.METRICS_RECORD_HEAD + 2 * T, dtype=torch.float32, device=dev)
+        bufs = self._buffers(dev)
+        with torch.cuda.device(dev):
+            L.check(lib.b2s_train_metrics_finish(L.ptr(counts), ctypes.byref(self.params()), float(loss_scale),
+                                                 ctypes.byref(bufs), L.ptr(record), L.stream()),
+                    "b2s_train_metrics_finish")
+        code, have = self._count_log
+        return MetricsHandle(self, record, self.last_status, code, have)
 
     def update_metrics(self, cls_loss, loc_loss, cls_preds, labels, sampled):
         """VoxelNet.update_metrics: the reference's dict of Python floats, read with one device-to-host copy."""

@@ -35,6 +35,11 @@ The kernels write parameters through raw pointers, so after every call ``step`` 
 parameter: the drop-in's weight caches (packed fp16 planes, folded batch norms) are keyed on it.  Replaying a captured
 step does not run that host code; bump the versions (``opt.touch()``) before the next forward.
 
+Data-parallel training (``b2second.dist.enable_data_parallel``): ``plan(..., data_parallel=handle)`` makes ``step``
+enqueue one all-reduce of the flat gradient bucket (``sum_r (1/W) * g_r``) on the current stream before the clip, so
+every rank clips, decays and steps on the same averaged gradient.  The gradients are views of that bucket and stay
+so (zeroed in place), hence ``step(set_to_none=True)`` is refused there.
+
 ``state_dict`` / ``load_state_dict`` use ``torch.optim.Adam``'s format, so a checkpoint written by the reference's
 ``OptimWrapper`` resumes here and the other way round.
 """
@@ -233,20 +238,25 @@ def parameter_groups(net):
     return list(groups)
 
 
-def plan(net, optimizer_cfg, total_step):
-    """-> OptimPlan for ``net``, the optimizer block (see ``settings``) and ``train_config.steps``."""
-    return OptimPlan(settings(optimizer_cfg), parameter_groups(net), total_step)
+def plan(net, optimizer_cfg, total_step, data_parallel=None):
+    """-> OptimPlan for ``net``, the optimizer block (see ``settings``) and ``train_config.steps``; ``data_parallel``:
+    the handle of ``b2second.dist.enable_data_parallel(net)``, to all-reduce the gradients in every ``step``."""
+    return OptimPlan(settings(optimizer_cfg), parameter_groups(net), total_step, data_parallel=data_parallel)
 
 
 class OptimPlan:
     """the optimizer of one network (see ``plan``)."""
 
-    def __init__(self, s: OptimSettings, groups, total_step):
+    def __init__(self, s: OptimSettings, groups, total_step, data_parallel=None):
         self.settings = s
         self.groups = groups
         self.params = [p for g in groups for p in g]
         if not self.params:
             raise ValueError("no trainable parameter")
+        if data_parallel is not None and [id(p) for p in data_parallel.params] != [id(p) for p in self.params]:
+            raise ValueError("the data-parallel handle was made for other parameters (enable_data_parallel(net) on "
+                             "the same network)")
+        self.data_parallel = data_parallel
         dev = self.params[0].device
         for p in self.params:
             if p.dtype != torch.float32:
@@ -309,7 +319,12 @@ class OptimPlan:
 
     def step(self, set_to_none=False):
         """one training step's clip, decay, Adam update, schedule advance and zero_grad; -> the gradient norm before
-        clipping (device float32 scalar).  No host synchronisation."""
+        clipping (device float32 scalar).  No host synchronisation.  Under data parallelism the gradients are first
+        averaged over the ranks, and ``set_to_none`` is refused (it would detach them from the bucket)."""
+        dp = self.data_parallel
+        if dp is not None and set_to_none:
+            raise ValueError("step(set_to_none=True) would detach the gradients from the data-parallel bucket; "
+                             "zero them in place (set_to_none=False)")
         L, lib = _lib()
         L.require_cuda(self.params[0], "parameters")
         grads = [p.grad for p in self.params]
@@ -324,6 +339,8 @@ class OptimPlan:
         n = len(self.params)
         base = t["ptrs"].data_ptr()
         with torch.cuda.device(self.device):
+            if dp is not None:
+                dp.all_reduce_grads()
             L.check(lib.b2s_optim_step(
                 ctypes.c_void_p(base), ctypes.c_void_p(base + 8 * n), ctypes.c_void_p(base + 16 * n),
                 ctypes.c_void_p(base + 24 * n), n, L.ptr(t["chunks"]), t["num_chunks"], L.ptr(self.hyper),

@@ -32,6 +32,9 @@ The training targets ``VoxelNet.loss`` reads (labels, reg_targets, importance) c
 for a whole batch (``targets.plan(net.target_assigner, feature_map_size).assign_batch(...)``), after
 ``b2second.inputs.anchor_area_mask``, and the loss they feed runs in csrc/loss.cu through ``b2second.loss`` (the
 focal, smooth-L1 and direction terms and their gradient); see INTEGRATION.md, Training.
+
+Several GPUs: ``enable_data_parallel(net)`` trains one process per GPU with the reference's ``--multi_gpu``
+(``torch.nn.DataParallel``) semantics; see b2second.dist.
 """
 
 
@@ -86,3 +89,11 @@ def enable_bn_relu_training(net):
     state-dict keys and ``eval()`` are unchanged; idempotent.  Returns ``net``."""
     from . import bn_train
     return bn_train.enable(net)
+
+
+def enable_data_parallel(net, group=None):
+    """train ``net`` data-parallel, one process per GPU over an NCCL process group, with the reference's
+    ``torch.nn.DataParallel`` step (b2second.dist.enable_data_parallel); -> the handle ``optim.plan(...,
+    data_parallel=)`` takes."""
+    from . import dist
+    return dist.enable_data_parallel(net, group)

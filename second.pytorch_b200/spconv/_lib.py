@@ -201,6 +201,10 @@ SIGNATURES = {
     "b2s_train_metrics": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                   c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                   c_void_p, c_size_t, c_void_p, c_void_p]),
+    "b2s_train_metrics_count": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                        c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "b2s_train_metrics_finish": (c_int, [c_void_p, c_void_p, ctypes.c_float, c_void_p, c_void_p, c_void_p]),
     "b2s_pack_sparse_weights": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                         c_void_p]),
     "b2s_pack_sparse_weights_ex": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
@@ -244,6 +248,10 @@ METRICS_RECORD_HEAD = 19      # B2S_METRICS_RECORD_HEAD; the B2S_METRICS_REC_* s
 METRICS_REC = ("rpn_acc", "cls_loss", "cls_loss_rt", "loc_loss", "loc_loss_rt", "cls_pos_rt", "cls_neg_rt", "dir_rt",
                "num_pos", "num_neg", "num_anchors")
 METRICS_REC_LOC_ELEM = 11     # B2S_METRICS_REC_LOC_ELEM
+METRICS_COUNT_HEAD = 20       # B2S_METRICS_COUNT_HEAD; the B2S_METRICS_CNT_* slots in order:
+METRICS_CNT = ("frames", "correct", "cared", "pos", "num_pos", "num_neg", "num_anchors", "cls_loss", "loc_loss",
+               "cls_pos", "cls_neg", "dir")
+METRICS_CNT_LOC_ELEM = 12     # B2S_METRICS_CNT_LOC_ELEM
 
 
 class MetricsParams(ctypes.Structure):
