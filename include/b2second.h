@@ -62,6 +62,9 @@
  *                       noise_per_object_v3_, random_flip, global_rotation_v2 / scaling_v2 / translate_, the range
  *                       filter, limit_period and the point shuffle (second/core/preprocess.py:153-164,244-273,450-476,
  *                       582-678,749-800,803-899), for a batch of frames
+ *   b2s_augment_draws   the random numbers of that augmentation (noise_per_object_v3_'s noises, random_flip,
+ *                       global_rotation_v2 / scaling_v2 / translate_ and np.random.shuffle(points)), from a seeded
+ *                       Philox stream keyed by (seed, step) and counted by frame instead of numpy's global stream
  *   b2s_db_sample       ground-truth database sampling of prep_pointcloud (second/data/preprocess.py:210-249):
  *                       DataBaseSamplerV2.sample_all / sample_class_v2 collision rejection (second/core/sample_ops.py:
  *                       95-285), points_in_rbbox point removal and the concatenation, for a batch of frames
@@ -96,7 +99,7 @@
 extern "C" {
 #endif
 
-#define B2S_VERSION 215
+#define B2S_VERSION 216
 
 /* status bits raised in *status_dev */
 #define B2S_STATUS_VOXEL_OVERFLOW 1u   /* more voxels than max_voxels (extra voxels dropped, as spconv) */
@@ -806,6 +809,43 @@ int b2s_augment(const float *points, int num_points, int num_feat, const int *po
                 const float *range_host, float *points_out, int *point_box, void *boxes_out, int *gt_offsets_out,
                 int *classes_out, float *importance_out, int *src_out, int *selected, void *workspace,
                 size_t workspace_bytes, unsigned *status_dev, void *stream);
+
+/* ---- device draws of the training augmentation ------------------------------------------------------------------ */
+/* The random numbers b2s_augment reads, drawn on the device instead of from numpy's stream: noise_per_object_v3_'s
+ * loc_noises and rot_noises, random_flip's choices, global_rotation_v2's and global_scaling_v2's uniforms and
+ * global_translate_'s normals (second/core/preprocess.py:582-678,749-800,885-899), and preprocess.py's
+ * np.random.shuffle(points).  Every value is a function of (seed, *step_dev, frame, stream, index):
+ *   block function Philox4x64-10 (numpy.random.Philox's), key (seed, step), counter (frame, stream, index, 0) with
+ *   frame = frame_base + b for batch-local frame b; u(w) = (w >> 11) 2^-53; a uniform on [lo, hi) is lo + (hi - lo) u;
+ *   normals by Box-Muller from words (wa, wb): r = sqrt(-2 ln(1 - u(wa))), t = 2 pi u(wb), the pair (r cos t, r sin t).
+ *   loc_noise[g, t] (box b of its frame, try t): block (f, 0, 100 b + t), normals (w0, w1) -> n0, n1 and (w2, w3) ->
+ *   n2 (the cos term), times loc_std; rot_noise[g, t]: uniform(rot_noise) from w0 of block (f, 1, 100 b + t).
+ *   frame_params[b] (b2s_augment's layout): block (f, 2, 0, 0): flip_x = u(w0) < 0.5, flip_y = u(w1) < 0.5 (each only
+ *   where random_flip_x / _y is set), angle = uniform(rotation) from w2, scale = uniform(scaling) from w3; when a
+ *   translate_std is nonzero, translate = 1 and block (f, 2, 1, 0)'s normals as loc_noise's times (translate_std[0],
+ *   translate_std[1], translate_std[0]) (global_translate_ draws z with std[0]); otherwise translate = 0, t = 0.
+ *   perm: the frame-local permutation pi of a frame of n points: k >= 1 the smallest with 4^k >= n, x < 4^k split
+ *   into (L, R) = (x >> k, x & (2^k - 1)), 4 rounds (L, R) <- (R, L ^ (w0 of block (f, 3, r, R) & (2^k - 1))) for
+ *   r = 0..3, repeated while the result is >= n; perm[point_offsets[b] + i] = pi(i); n <= 1 keeps the identity.
+ * Each row finds its frame by searching gt_offsets / point_offsets [batch + 1] (device); rows outside every frame, or
+ * in a frame whose range is malformed, get zeros.  loc_noise [num_gt, B2S_AUGMENT_NUM_TRY, 3] and rot_noise [num_gt,
+ * B2S_AUGMENT_NUM_TRY] float64 are written when params_host->object_noise (else may be NULL); frame_params [batch, 8]
+ * float64; perm int32 [num_points], or NULL: no shuffle.  step_dev: uint64 device counter, read by every kernel of the
+ * call and advanced by one at its end, so a captured call draws the next step at every replay.  No host sync, no
+ * atomics; deterministic.  Four kernels at most. */
+#define B2S_AUGMENT_NUM_TRY 100
+typedef struct {
+    double loc_std[3];          /* groundtruth_localization_noise_std */
+    double rot_noise[2];        /* groundtruth_rotation_uniform_noise */
+    double rotation[2];         /* global_rotation_uniform_noise */
+    double scaling[2];          /* global_scaling_uniform_noise */
+    double translate_std[3];    /* global_translate_noise_std */
+    int object_noise;           /* 1: noise_per_object_v3_ draws (b2second.augment.object_noise_enabled) */
+    int random_flip_x, random_flip_y;
+} b2s_augment_draw_params;
+int b2s_augment_draws(uint64_t seed, uint64_t *step_dev, uint64_t frame_base, int batch, const int *gt_offsets,
+                      int num_gt, const int *point_offsets, int num_points, const b2s_augment_draw_params *params_host,
+                      double *loc_noise, double *rot_noise, double *frame_params, int *perm, void *stream);
 
 /* ---- training ground-truth database sampling (second/data/preprocess.py:210-249) ----------------------------- */
 /* The device half of DataBaseSamplerV2.sample_all without group sampling, per-object rotation or random crop, for

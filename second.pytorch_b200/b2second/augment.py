@@ -10,18 +10,27 @@ Steps, in the reference's order: noise_per_object_v3_ with 100 tries (second/cor
 boxes outside the class mask, random_flip, global_rotation_v2, global_scaling_v2, global_translate_ (:749-800, 885-899),
 filter_gt_box_outside_range_by_center (:153-164), limit_period(0.5, 2 pi) and np.random.shuffle(points).
 
-Random numbers never come from the device: ``draw`` consumes a numpy RandomState exactly as the reference's functions
-do, frame after frame, so a caller that samples the ground-truth database on the host first and then calls ``draw`` on
-the same state gets the reference's augmentation.  Arithmetic follows the reference's dtypes (float32 points, float32
-or float64 boxes, float64 draws); values that pass through the reference's BLAS matmuls (per-object and global
-rotation) agree to a few float32 ulp, everything else bit for bit, and every decision (selected try, point-in-box,
-range filter) is the reference's away from exact ties.
+Random numbers come from one of two sources.  ``draw`` (the default) consumes a numpy RandomState exactly as the
+reference's functions do, frame after frame, so a caller that samples the ground-truth database on the host first and
+then calls ``draw`` on the same state gets the reference's augmentation.  ``DeviceDrawer`` (opt-in) draws them on the
+device (csrc/augment_draws.cu) from a seeded Philox4x64-10 stream keyed by (seed, step) and counted by frame, with no
+host work per frame and no host sync; its draws are reproducible from (seed, step), do not depend on how frames are
+split over calls or data-parallel ranks, and replay inside a CUDA graph (INTEGRATION.md states the contract):
+
+    dd = augment.DeviceDrawer(seed, "cuda")                                      # once; dd.step is the checkpoint
+    d = dd.draw(cfg.augment, gt_offsets, point_offsets, G, P, frame_base=rank * B)  # device, per batch
+
+Arithmetic follows the reference's dtypes (float32 points, float32 or float64 boxes, float64 draws); values that pass
+through the reference's BLAS matmuls (per-object and global rotation) agree to a few float32 ulp, everything else bit
+for bit, and every decision (selected try, point-in-box, range filter) is the reference's away from exact ties.
 Refused (spec.UnsupportedNetwork), as no config uses them: a per-object global rotation range
 (``global_random_rotation_range_per_object`` wider than 1e-3, noise_per_box_v2_) and ``use_group_id``.
 Left on the host: database sampling and the row selections before augmentation (remove_environment, remove_unknown,
 min_num_of_points_in_gt, the frustum crop, remove_outside_points); ``gt_valid`` and the packed inputs carry them.
 """
 import ctypes
+import math
+import operator
 from dataclasses import dataclass
 from typing import List, Optional
 
@@ -51,7 +60,8 @@ def object_noise_enabled(s):
 
 @dataclass
 class Draws:
-    """the random numbers of one batch, in the reference's terms (host numpy arrays).
+    """the random numbers of one batch, in the reference's terms: host numpy arrays from ``draw``, or CUDA tensors from
+    ``DeviceDrawer.draw`` (whose num_gt and num_points are None: the counts stay on the device).
     loc_noise [G, 100, 3] / rot_noise [G, 100] float64 (None when the object noise returns early); frame [B, 8]
     float64: flip_y, flip_x, translate (0/1, as applied), rotation angle, scale, tx, ty, tz; perm [P] int32 frame-local
     source rows (None when not shuffling)."""
@@ -108,7 +118,10 @@ def draw(rs, settings, num_gt_per_frame, num_points_per_frame):
 
 def select(draws, start, stop):
     """-> the Draws of frames ``start .. stop - 1`` of ``draws``: a data-parallel rank's share of draws made for the
-    whole batch in single-process order, so the augmentation does not depend on the number of ranks."""
+    whole batch in single-process order, so the augmentation does not depend on the number of ranks.  Device draws
+    are refused: a rank draws its own frames with ``DeviceDrawer.draw(..., frame_base=start)`` instead."""
+    if isinstance(draws.frame, torch.Tensor):
+        raise ValueError("select takes host draws; DeviceDrawer.draw's frame_base gives a rank its frames' draws")
     g = np.cumsum([0] + list(draws.num_gt))
     p = np.cumsum([0] + list(draws.num_points))
     return Draws(
@@ -123,6 +136,15 @@ def _to_device(a, device, dtype):
     if t.numel() == 0:
         return torch.empty(t.shape, dtype=t.dtype, device=device)
     return t.pin_memory().to(device, non_blocking=True)
+
+
+def _draw_input(a, device, dtype):
+    """one array of a Draws as b2s_augment reads it: host arrays are copied, DeviceDrawer's tensors used as they are"""
+    if isinstance(a, torch.Tensor):
+        if a.device != device or a.dtype != dtype:
+            raise ValueError("device draws must be %s on %s, got %s on %s" % (dtype, device, a.dtype, a.device))
+        return a.contiguous()
+    return _to_device(a, device, np.float64 if dtype == torch.float64 else np.int32)
 
 
 class AugmentPlan:
@@ -140,7 +162,8 @@ class AugmentPlan:
         """augment a batch without a host sync.
         points CUDA float32 [P, F] packed frame after frame, point_offsets CUDA int32 [B+1]; gt_boxes CUDA float32 or
         float64 [G, 7 or 9], gt_offsets CUDA int32 [B+1]; gt_valid CUDA bool [G] (the class mask); gt_classes CUDA int
-        [G]; importance CUDA float [G] or None; draws: ``draw``'s result for these frames.
+        [G]; importance CUDA float [G] or None; draws: ``draw``'s result for these frames (copied to the device) or
+        ``DeviceDrawer.draw``'s (read in place, so one CUDA graph can capture both calls).
         -> {"points": float32 [P, F] (frame rows in shuffled order), "boxes": [G, ndim] of the input dtype, "gt_offsets":
         int32 [B+1], "classes": int32 [G], "importance": float32 [G], "src_row": int32 [G]}: the kept boxes packed in
         input order, rows past gt_offsets[B] zero (src_row -1).  with_debug adds "selected" (int32 [G], the try each input box
@@ -162,8 +185,9 @@ class AugmentPlan:
         B = int(point_offsets.shape[0]) - 1
         if B < 1 or int(gt_offsets.shape[0]) != B + 1:
             raise ValueError("point_offsets and gt_offsets must both hold batch + 1 >= 2 entries")
-        if len(draws.num_gt) != B or draws.frame.shape[0] != B:
-            raise ValueError("draws were made for %d frames, the batch has %d" % (len(draws.num_gt), B))
+        frames = draws.frame.shape[0] if draws.num_gt is None else len(draws.num_gt)
+        if frames != B or draws.frame.shape[0] != B:
+            raise ValueError("draws were made for %d frames, the batch has %d" % (frames, B))
         P, F = int(points.shape[0]), int(points.shape[1])
         G, ndim = int(gt_boxes.shape[0]), int(gt_boxes.shape[1])
         if self.object_noise and draws.loc_noise is None:
@@ -180,10 +204,10 @@ class AugmentPlan:
         cls = gt_classes.to(torch.int32).contiguous()
         imp = importance.to(torch.float32).contiguous() if importance is not None else None
         noise = self.object_noise and G > 0
-        loc = _to_device(draws.loc_noise, device, np.float64) if noise else None
-        rot = _to_device(draws.rot_noise, device, np.float64) if noise else None
-        frame = _to_device(draws.frame, device, np.float64)
-        perm = _to_device(draws.perm, device, np.int32) if draws.perm is not None else None
+        loc = _draw_input(draws.loc_noise, device, torch.float64) if noise else None
+        rot = _draw_input(draws.rot_noise, device, torch.float64) if noise else None
+        frame = _draw_input(draws.frame, device, torch.float64)
+        perm = _draw_input(draws.perm, device, torch.int32) if draws.perm is not None else None
         pts_out = torch.empty_like(points)
         boxes_out = torch.empty_like(gt_boxes)
         offs_out = torch.empty(B + 1, dtype=torch.int32, device=device)
@@ -251,6 +275,11 @@ class AugmentPlan:
 
 def plan(settings, point_cloud_range, class_names):
     """-> AugmentPlan.  settings: b2second.config.AugmentSettings (``cfg.augment``)."""
+    _check_settings(settings)
+    return AugmentPlan(settings, point_cloud_range, class_names)
+
+
+def _check_settings(settings):
     grot = list(settings.global_random_rotation_range_per_object)
     if len(grot) != 2:
         raise ValueError("global_random_rotation_range_per_object must hold two values, got %r" % (grot,))
@@ -265,4 +294,94 @@ def plan(settings, point_cloud_range, class_names):
         if len(getattr(settings, key)) != n and not (key == "global_translate_noise_std" and
                                                      not settings.global_translate_noise_std):
             raise ValueError("%s must hold %d values, got %r" % (key, n, getattr(settings, key)))
-    return AugmentPlan(settings, point_cloud_range, class_names)
+
+
+def draw_params(settings):
+    """-> spconv._lib.AugmentDrawParams: the settings of b2s_augment_draws.  Refuses what ``plan`` refuses, and what
+    ``draw``'s numpy calls reject: a negative std (numpy.random.normal) or a bound that is not finite (uniform)."""
+    _check_settings(settings)
+    s = settings
+    tstd = [float(v) for v in s.global_translate_noise_std] or [0.0, 0.0, 0.0]
+    std = [float(v) for v in s.groundtruth_localization_noise_std]
+    # the translation's z normal uses std[0] (global_translate_), so std[2] only decides whether it happens
+    for key, v in (("groundtruth_localization_noise_std", std), ("global_translate_noise_std", tstd[:2]),
+                   ("groundtruth_rotation_uniform_noise", s.groundtruth_rotation_uniform_noise),
+                   ("global_rotation_uniform_noise", s.global_rotation_uniform_noise),
+                   ("global_scaling_uniform_noise", s.global_scaling_uniform_noise)):
+        if not all(math.isfinite(float(x)) for x in v):
+            raise ValueError("%s must be finite, got %r" % (key, list(v)))
+        if key.endswith("_std") and any(x < 0 for x in v):
+            raise ValueError("%s must be >= 0, got %r" % (key, list(v)))
+    from spconv import _lib as L
+    d = lambda v: (ctypes.c_double * len(v))(*[float(x) for x in v])   # noqa: E731
+    return L.AugmentDrawParams(d(std), d(s.groundtruth_rotation_uniform_noise), d(s.global_rotation_uniform_noise),
+                               d(s.global_scaling_uniform_noise), d(tstd), int(object_noise_enabled(s)),
+                               int(bool(s.random_flip_x)), int(bool(s.random_flip_y)))
+
+
+class DeviceDrawer:
+    """the augmentation's random numbers drawn on the device (csrc/augment_draws.cu, b2s_augment_draws): an opt-in
+    alternative to ``draw`` whose every value is a function of (seed, step, frame, stream, index) through Philox4x64-10
+    (numpy.random.Philox's block function).  INTEGRATION.md states the contract.
+
+    ``step`` is a uint64 counter in device memory: every ``draw`` keys its numbers with it and advances it by one on
+    the device, so a CUDA graph that captures ``draw`` (with ``augment_batch``) draws the next step at every replay.
+    A checkpoint that saves ``seed`` and ``step`` and restores them resumes the same stream."""
+
+    def __init__(self, seed, device):
+        seed = operator.index(seed)
+        if not 0 <= seed < 2 ** 64:
+            raise ValueError("seed must be in [0, 2**64), got %d" % seed)
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise ValueError("DeviceDrawer draws on a CUDA device, got %s" % device)
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        self.seed, self.device = seed, device
+        self._step = torch.zeros(1, dtype=torch.int64, device=device)     # the uint64 word's bits
+
+    @property
+    def step(self):
+        """the step the next ``draw`` uses (reading it waits for the device: meant for checkpoints)"""
+        return int(self._step.item()) % 2 ** 64
+
+    @step.setter
+    def step(self, value):
+        value = operator.index(value)
+        if not 0 <= value < 2 ** 64:
+            raise ValueError("step must be in [0, 2**64), got %d" % value)
+        self._step.fill_(value - 2 ** 64 if value >= 2 ** 63 else value)
+
+    def draw(self, settings, gt_offsets, point_offsets, num_boxes, num_points, frame_base=0):
+        """-> Draws of CUDA tensors (num_gt = num_points = None) for the frames frame_base + b, b < B, whose boxes and
+        points gt_offsets / point_offsets (CUDA int [B+1]) delimit; num_boxes / num_points: their totals G and P (the
+        shapes of loc_noise / rot_noise and perm).  No host sync."""
+        params = draw_params(settings)
+        L, lib = _lib()
+        L.require_cuda(gt_offsets, "gt_offsets")
+        L.require_cuda(point_offsets, "point_offsets")
+        if gt_offsets.device != self.device or point_offsets.device != self.device:
+            raise ValueError("the offsets must be on %s, got %s and %s" % (self.device, gt_offsets.device,
+                                                                           point_offsets.device))
+        B = int(gt_offsets.shape[0]) - 1
+        if gt_offsets.dim() != 1 or point_offsets.shape != gt_offsets.shape or B < 1:
+            raise ValueError("gt_offsets and point_offsets must both hold batch + 1 >= 2 entries")
+        G, P, frame_base = operator.index(num_boxes), operator.index(num_points), operator.index(frame_base)
+        if G < 0 or P < 0 or G >= 2 ** 31 or P >= 2 ** 31:
+            raise ValueError("num_boxes and num_points must be in [0, 2**31), got %d and %d" % (G, P))
+        if not 0 <= frame_base <= 2 ** 64 - 1 - B:
+            raise ValueError("frame_base must be in [0, 2**64 - batch], got %d" % frame_base)
+        goff = gt_offsets.to(torch.int32).contiguous()
+        poff = point_offsets.to(torch.int32).contiguous()
+        dev = self.device
+        noise = bool(params.object_noise)
+        loc = torch.empty((G, NUM_TRY, 3), dtype=torch.float64, device=dev) if noise else None
+        rot = torch.empty((G, NUM_TRY), dtype=torch.float64, device=dev) if noise else None
+        frame = torch.empty((B, 8), dtype=torch.float64, device=dev)
+        perm = torch.empty(P, dtype=torch.int32, device=dev) if settings.shuffle_points else None
+        with torch.cuda.device(dev):
+            L.check(lib.b2s_augment_draws(
+                self.seed, L.ptr(self._step), frame_base, B, L.ptr(goff), G, L.ptr(poff), P, ctypes.byref(params),
+                L.ptr(loc) if (noise and G) else None, L.ptr(rot) if (noise and G) else None, L.ptr(frame),
+                L.ptr(perm) if (perm is not None and P) else None, L.stream()), "b2s_augment_draws")
+        return Draws(loc_noise=loc, rot_noise=rot, frame=frame, perm=perm, num_gt=None, num_points=None)

@@ -181,6 +181,8 @@ SIGNATURES = {
                             c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
                             c_void_p, c_void_p]),
+    "b2s_augment_draws": (c_int, [ctypes.c_uint64, c_void_p, ctypes.c_uint64, c_int, c_void_p, c_int, c_void_p, c_int,
+                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2s_db_sample_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b2s_db_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
@@ -221,6 +223,14 @@ SIGNATURES = {
     "b2s_conv2d_wgrad_tc": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
+
+class AugmentDrawParams(ctypes.Structure):
+    """b2s_augment_draw_params (include/b2second.h): the settings of b2s_augment_draws, passed by host pointer."""
+    _fields_ = [("loc_std", ctypes.c_double * 3), ("rot_noise", ctypes.c_double * 2),
+                ("rotation", ctypes.c_double * 2), ("scaling", ctypes.c_double * 2),
+                ("translate_std", ctypes.c_double * 3), ("object_noise", c_int), ("random_flip_x", c_int),
+                ("random_flip_y", c_int)]
+
 
 OPTIM_CHUNK = 4096       # B2S_OPTIM_CHUNK
 OPTIM_HYPER_COLS = 5     # B2S_OPTIM_HYPER_COLS

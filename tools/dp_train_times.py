@@ -1,5 +1,5 @@
 """data-parallel training step times (CUDA events) at 1, 2, 4 and 8 GPUs:
-python -m torch.distributed.run --nproc-per-node N tools/dp_train_times.py [steps] [frames_per_rank]
+python -m torch.distributed.run --nproc-per-node N tools/dp_train_times.py [steps] [frames_per_rank] [--draws device]
 
 One process per GPU, NCCL.  For every world size W in (1, 2, 4, 8) up to N, ranks 0 .. W-1 form a group and train
 car.fhd and pointpillars xyres_16, in the fp32 and f16 training modes, with b2second.training.enable_data_parallel: the
@@ -8,11 +8,16 @@ backward -> optimizer step (with the gradient all-reduce) -> metrics (with the c
 (dbsample.draw, augment.draw) are made for the global batch of W * B frames in single-process order and each rank keeps
 its frames' draws (dbsample.select, augment.select), so the data does not depend on W; the frames' box and point
 counts the augmentation draws need are all-gathered (one small collective next to the pipeline's one host read).
+With --draws device every configuration is also measured, right after the numpy path, with the augmentation's draws
+made on the device (augment.DeviceDrawer): each rank draws only its own frames, with frame_base = rank * B, and reads
+only its own counts, so that path has no all-gather.  The database sampler draws from its own numpy state in both
+paths, so both see the same frames.
 
 Rank 0 prints one JSON line: per configuration, mode and W the step time (ms, CUDA events over the timed steps, after
 warm-up ones), frames/s over the global batch, the scaling efficiency (frames/s over W times the one-GPU frames/s), and
 the gradient all-reduce's share of the step (CUDA events around it); with rank 0's card, its power limit and its SM
 clock sampled during the run."""
+import argparse
 import contextlib
 import os
 import sys
@@ -45,7 +50,7 @@ def build(name, precision, dev):
 class Pipeline:
     """the input side of one rank: the global batch's frames and ground truths (host), the object database"""
 
-    def __init__(self, name, net, root, world, rank, B, dev, group):
+    def __init__(self, name, net, root, world, rank, B, dev, group, draws):
         self.cfg = cfg = config.get_config(name)
         self.net, self.world, self.rank, self.B, self.dev, self.group = net, world, rank, B, dev, group
         rng = np.random.default_rng(0)
@@ -77,14 +82,20 @@ class Pipeline:
                        t(np.concatenate([f[1] for f in mine])),
                        t(np.arange(0, 10 * B + 1, 10, dtype=np.int32)), t(np.ones(10 * B, bool)),
                        t(np.ones(10 * B, np.int32)), None)
-        self.rs = np.random.RandomState(1)
+        # one state per sampler, so both draw paths sample the same database objects and counts every step
+        self.db_rs, self.aug_rs = np.random.RandomState(1), np.random.RandomState(2)
         self.anchors = torch.from_numpy(net.anchors().reshape(-1, 7)).to(dev)[None].repeat(B, 1, 1)
         self.counts = torch.zeros(world, 2 * B, dtype=torch.int64, device=dev)
+        self.drawer = augment.DeviceDrawer(1, dev) if draws == "device" else None
 
     def example(self):
         cfg, B, lo = self.cfg, self.B, self.rank * self.B
-        cand = dbsample.draw(self.rs, self.ds.state, [f[2] for f in self.frames])
+        cand = dbsample.draw(self.db_rs, self.ds.state, [f[2] for f in self.frames])
         s = self.ds.sample_batch(*self.inputs, dbsample.select(cand, lo, lo + B))
+        if self.drawer is not None:
+            nb, npts = s.counts()                          # the pipeline's host read, this rank's frames only
+            d = self.drawer.draw(cfg.augment, s["gt_offsets"], s["point_offsets"], sum(nb), sum(npts), frame_base=lo)
+            return self.finish(s, self.ap.augment_batch(*s.augment_inputs(nb, npts), d))
         mine = torch.cat([torch.diff(s["gt_offsets"]), torch.diff(s["point_offsets"])]).to(torch.int64)
         if self.world > 1:
             dist.all_gather_into_tensor(self.counts, mine, group=self.group)
@@ -92,8 +103,11 @@ class Pipeline:
             self.counts[0].copy_(mine)
         c = self.counts.cpu().numpy()                      # the pipeline's host read
         nb, npts = c[:, :B].reshape(-1).tolist(), c[:, B:].reshape(-1).tolist()
-        d = augment.select(augment.draw(self.rs, cfg.augment, nb, npts), lo, lo + B)
-        a = self.ap.augment_batch(*s.augment_inputs(nb[lo:lo + B], npts[lo:lo + B]), d)
+        d = augment.select(augment.draw(self.aug_rs, cfg.augment, nb, npts), lo, lo + B)
+        return self.finish(s, self.ap.augment_batch(*s.augment_inputs(nb[lo:lo + B], npts[lo:lo + B]), d))
+
+    def finish(self, s, a):
+        cfg, B = self.cfg, self.B
         res = self.gen.generate_device(a["points"], cfg.max_voxels, frame_offsets=s["point_offsets"], batch=B)
         n = int(res["num_voxels"][0].item())
         ex = {"voxels": res["voxels"][:n], "num_points": res["num_points_per_voxel"][:n],
@@ -116,11 +130,11 @@ def step(p, opt):
                                          ex["labels"], ret["cared"], ret, mask)
 
 
-def measure(name, precision, world, rank, B, steps, warmup, group, dev, root):
+def measure(name, precision, world, rank, B, steps, warmup, group, dev, root, draws):
     net = build(name, precision, dev)
     dp = training.enable_data_parallel(net, group)
     opt = optim.plan(net, orf.ONE_CYCLE, warmup + steps + 1, data_parallel=dp)
-    p = Pipeline(name, net, root, world, rank, B, dev, group)
+    p = Pipeline(name, net, root, world, rank, B, dev, group, draws)
     for _ in range(warmup):
         step(p, opt)
     torch.cuda.synchronize()
@@ -134,8 +148,14 @@ def measure(name, precision, world, rank, B, steps, warmup, group, dev, root):
 
 
 def main():
-    steps = int(sys.argv[1]) if len(sys.argv) > 1 else 10
-    B = int(sys.argv[2]) if len(sys.argv) > 2 else 2
+    ap = argparse.ArgumentParser()
+    ap.add_argument("steps", type=int, nargs="?", default=10)
+    ap.add_argument("frames_per_rank", type=int, nargs="?", default=2)
+    ap.add_argument("--draws", choices=("numpy", "device"), default="numpy",
+                    help="device: also measure every configuration with augment.DeviceDrawer, after the numpy path")
+    args = ap.parse_args(sys.argv[1:])
+    steps, B = args.steps, args.frames_per_rank
+    sources = ("numpy", "device") if args.draws == "device" else ("numpy",)
     warmup = 3
     local = int(os.environ.get("LOCAL_RANK", "0"))
     _measure.require_gpu("dp_train_times")
@@ -152,18 +172,21 @@ def main():
     with tempfile.TemporaryDirectory() as root, sampling as clk:
         for name in CONFIGS:
             for precision in MODES:
-                base = None
+                base = {}
                 for w in worlds:
-                    if rank < w:
-                        ms, ar = measure(name, precision, w, rank, B, steps, warmup, groups[w], dev, root)
-                        fps = w * B * 1e3 / ms
-                        base = fps if w == 1 else base
-                        if rank == 0:
-                            rows.append({"config": name, "precision": precision, "gpus": w, "frames_per_rank": B,
-                                         "step_ms": round(ms, 3), "frames_per_s": round(fps, 2),
-                                         "scaling_efficiency": round(fps / (w * base), 3),
-                                         "allreduce_ms": round(ar, 3), "allreduce_share": round(ar / ms, 4)})
-                    dist.barrier()
+                    for src in sources:
+                        if rank < w:
+                            ms, ar = measure(name, precision, w, rank, B, steps, warmup, groups[w], dev, root, src)
+                            fps = w * B * 1e3 / ms
+                            if w == 1:                     # only rank 0 reads base: ranks > 0 never run W = 1
+                                base[src] = fps
+                            if rank == 0:
+                                rows.append({"config": name, "precision": precision, "draws": src, "gpus": w,
+                                             "frames_per_rank": B, "step_ms": round(ms, 3),
+                                             "frames_per_s": round(fps, 2),
+                                             "scaling_efficiency": round(fps / (w * base[src]), 3),
+                                             "allreduce_ms": round(ar, 3), "allreduce_share": round(ar / ms, 4)})
+                        dist.barrier()
     if rank == 0:
         _measure.report("dp_train_times", rows, clk, steps=steps, warmup=warmup, processes=size)
     dist.destroy_process_group()
